@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- frame-pairs/sec of the rgbdslam_v2 frame-pair hot path (ORB Hamming brute-force match +
-RANSAC SE(3)) on B200, BASELINE.json config C2: a batch of 256 synthetic frame pairs, 1000 ORB keypoints
+RANSAC SE(3)) on H100, BASELINE.json config C2: a batch of 256 synthetic frame pairs, 1000 ORB keypoints
 per frame, per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
 
@@ -16,6 +16,9 @@ One "step" = Node::matchNodePair (node.cpp:1305) for every pair of the batch thr
   cpu_baseline : the CPU oracle (plain-C port of the reference path) on this box's host cores.
 --impl reference times that CPU oracle as the reference arm (the reference itself cannot be built: ROS /
 Qt / PCL / g2o / OpenCV-C++ are absent -- see DESIGN.md).
+--steps K times exactly K steps.  --dump-outputs DIR writes the pair results of the last timed step (the records a caller of
+rgbdslam_b200_match_pairs receives, one DIR/pair_<field>.npy per field, float32 / float64); the inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,7 +46,7 @@ ALGO_BYTES_PER_PAIR = (N_KP + N_KP) * 32 + N_KP * 8  # SURVEY.md section 8(d): 7
 # one string for both arms (the driver compares config.workload of `ours` and `reference`)
 WORKLOAD = (f"C2: {PAIRS_PER_GPU} frame pairs x {N_KP} ORB kp per GPU, Hamming BF match + 4-pt RANSAC "
             "(200 hypotheses, max_matches 300), synthetic feature-level pairs (rgbdslam_v2_b200/synth.py make_batch)")
-MIN_TIMED_MS = 50.0  # the timed regions cover at least this much device time whatever --steps says
+MIN_TIMED_MS = 50.0  # the rendered-frame C2 sub-measurement times at least this much device time
 
 
 def measured_peaks():
@@ -51,7 +54,7 @@ def measured_peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not a measured figure)"
 
 
 class ClockSampler:
@@ -147,34 +150,22 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm), "source": "nvidia-smi"}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE tc_hamming_expand_kernel launch on this workload, from the committed
-# `ncu --set full` capture: 16.48 MB read + 0 written (the 2 MB of results stay in L2 for the selection kernel) against 18.4 MB
-# algorithmic -- the kernel expands the 32-byte descriptors to MMA operands in shared memory itself.  (Round 1 read a resident
-# +-1 int8 expansion instead: 139.3 MB per launch, 7.6 x the algorithmic bytes.)
-NCU_DRAM_BYTES_PER_LAUNCH = 16479744
-NCU_TRAFFIC_SOURCE = "profiles/r2_final_c2_kernels_ncu_full.txt (ncu --set full, 1 launch, C2 batch)"
-# tcgen05.mma.kind::i8 M128 N128 K32 issued back to back on all 148 SMs, no epilogue (tools/microbench/tc_peaks.cu on this pool's
-# B200s, profiles/r2_v7_tc_peaks.json): 64.0 cycles per MMA = 4514.7 TOP/s at the 1.86 GHz the SMs hold under that load
-INT8_MMA_MEASURED_TOPS = 4514.7
-
-
 def tensor_roofline(kernel_ms: float) -> dict:
     """The match kernel against the tensor roofline: exact +-1 int8 GEMM, 2 * Nq * Nt * 256 integer ops per pair.  Peak:
-    dense int8 = 2 x the dense bf16 rate on B200 (4.5 vs 2.25 POP/s nominal), scaled from the MEASURED bf16 number."""
+    dense int8 = 2 x the dense bf16 rate on H100 (1979 vs 989 TOP/s in the data sheet), scaled from a measured bf16 number
+    when MEASURED_PEAKS.json provides one."""
     ops = 2.0 * N_KP * N_KP * 256 * PAIRS_PER_GPU
     achieved = ops / (kernel_ms * 1e-3) / 1e12
-    peak = 2.0 * 1701.0
-    src = "2 x nominal-ratio of fallback bf16 1701 TF/s"
+    peak = 1979.0
+    src = "H100 SXM data sheet, dense int8 (700 W card; not a measured figure)"
     try:
         with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "MEASURED_PEAKS.json")) as f:
             peak = 2.0 * float(json.load(f)["bf16_tflops"])
-            src = "2 x MEASURED_PEAKS.json bf16_tflops (int8 dense = 2 x bf16 dense on sm_100)"
+            src = "2 x MEASURED_PEAKS.json bf16_tflops (int8 dense = 2 x bf16 dense on sm_90)"
     except Exception:
         pass
     return {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TOP/s (int8)", "frac": achieved / peak, "peak_source": src,
-            "ops_counted": "algorithmic 2 * Nq * Nt * 256 per pair (the ninth, column-index k-step and the padding to 128-row tiles are overhead)",
-            "int8_mma_issue_peak": INT8_MMA_MEASURED_TOPS, "frac_of_int8_mma_issue_peak": achieved / INT8_MMA_MEASURED_TOPS,
-            "int8_mma_issue_peak_source": "tools/microbench/tc_peaks.cu (profiles/r2_v7_tc_peaks.json): tcgen05.mma.kind::i8 alone, 64.0 cycles per M128 N128 K32"}
+            "ops_counted": "algorithmic 2 * Nq * Nt * 256 per pair (the ninth, column-index k-step and the padding to 128-row tiles are overhead)"}
 
 
 def make_workload(rank: int):
@@ -241,8 +232,9 @@ def run_reference(args, rank, world):
     for _ in range(max(args.warmup, 3)):
         oracle_run(b, 0, cores)
     times = []
+    last_res = None
     for _ in range(args.steps):
-        dt, _ = oracle_run(b, 0, cores)
+        dt, last_res = oracle_run(b, 0, cores)
         times.append(dt)
     tot = sum(times)
     value = PAIRS_PER_GPU * args.steps / tot
@@ -259,6 +251,19 @@ def run_reference(args, rank, world):
         "gpu_launches": 0,
     }
     emit(out)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_res)
+
+
+def dump_outputs(out_dir: str, res: np.ndarray):
+    """One DIR/pair_<field>.npy per field of the pair result records (float64 for integers and doubles, float32 for floats)."""
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name in res.dtype.names:
+        if name.endswith("_"):
+            continue  # padding
+        a = res[name]
+        np.save(d / f"pair_{name}.npy", a.astype(np.float32 if a.dtype == np.float32 else np.float64))
 
 
 def fe_device(fe):
@@ -401,14 +406,14 @@ def bench_c3(fe, local_rank, cpu=True):
     from rgbdslam_v2_b200 import synth
     rng = np.random.default_rng(33)
     out = {"workload": f"C3: {C3_PAIRS} frame pairs x {C3_KP} SIFT-128 descriptors per frame (synthetic SIFT-like rows, 50 % of the "
-                       "newer frame's features are noisy copies of the older frame's), exact 2-NN via bf16 tcgen05 GEMM + fp32 re-rank, "
+                       "newer frame's features are noisy copies of the older frame's), exact 2-NN via bf16 wgmma GEMM + fp32 re-rank, "
                        "ratio 0.95 / uniqueness, 4-pt RANSAC"}
-    peak_bf16 = 1701.0
+    peak_bf16 = 989.0
     try:
         peak_bf16 = float(json.loads((ROOT / "MEASURED_PEAKS.json").read_text())["bf16_tflops"])
         out["peak_source"] = "MEASURED_PEAKS.json bf16_tflops (burst)"
     except Exception:
-        out["peak_source"] = "fallback 1701 TF/s"
+        out["peak_source"] = "H100 SXM data sheet, dense bf16 989 TF/s (700 W card; not a measured figure)"
     for kind, matcher in (("sift", 0), ("siftgpu", 1)):
         fe.set_sift_matcher(matcher)
         pairs = [synth.make_pair_sift(9000 + k, C3_KP, overlap=0.5, kind=kind) for k in range(C3_PAIRS)]
@@ -636,11 +641,9 @@ def run_ours(args, rank, local_rank, world):
     torch.cuda.set_stream(stream)
     fe.set_stream(stream.cuda_stream)
 
-    # Two independent batches (A/B) alternate between two pipeline slots: their resident inputs (2 x 156 MB of node
-    # data incl. the int8 operands) exceed the 126 MB L2, so no explicit flush is needed between steps, and the
-    # host->device copies / latency-bound RANSAC phases of step k+1 overlap the kernels of step k.
-    # batches in flight (measured, 200 steps: depth 3 / 4 / 5 / 7 -> 1.62 / 1.71 / 1.75 / 1.73 M pairs/s on one GPU; with the
-    # per-step all-gather every batch also waits for the slowest rank: 2 GPUs, depth 4 / 6 -> 3.20 / 3.37 M pairs/s)
+    # DEPTH independent batches alternate between DEPTH pipeline slots: the resident node data of one batch alone is larger
+    # than the 50 MB L2, so no explicit flush is needed between steps, and the host->device copies / latency-bound RANSAC
+    # phases of step k+1 overlap the kernels of step k.
     DEPTH = int(os.environ.get("RB200_BENCH_DEPTH", "5" if world == 1 else "6"))
     sets = []
     for j in range(DEPTH):
@@ -736,23 +739,9 @@ def run_ours(args, rank, local_rank, world):
     if rank == 0:
         sampler.start()
 
-    # ---- timed: device-resident inputs, pipelined over DEPTH slots ------------------------------------
-    # --steps K is timed as R back-to-back blocks of K steps so that the region covers >= MIN_TIMED_MS (20 steps of 0.15 ms
-    # are four pipeline turn-overs); per-step numbers divide by K * R.  R comes from a short probe, identical on every rank.
-    run_steps(submit_resident, max(args.steps, DEPTH))  # first region of this size: the exchange buffers are allocated here
-    torch.cuda.synchronize()
-    p0 = time.perf_counter()
-    run_steps(submit_resident, max(args.steps, DEPTH))
-    torch.cuda.synchronize()
-    probe = torch.tensor([(time.perf_counter() - p0) / max(args.steps, DEPTH)], dtype=torch.float64, device="cuda")
-    if world > 1:
-        dist.all_reduce(probe, op=dist.ReduceOp.MAX)
-    # a short probe region over-estimates the step (pipeline ramp, the exchange): never fewer steps than MIN_TIMED_MS of the
-    # fastest step this code has measured (0.12 ms), or the fixed costs of a region dominate it (the first 2- and 8-GPU lines of
-    # round 2 timed 6 and 41 ms)
-    repeats = max(1, int(np.ceil(MIN_TIMED_MS * 1e-3 / (float(probe.item()) * args.steps))),
-                  int(np.ceil(MIN_TIMED_MS / (0.12 * args.steps))))
-    timed_steps = args.steps * repeats
+    # ---- timed: device-resident inputs, pipelined over DEPTH slots: exactly --steps steps ------------------------------
+    timed_steps = args.steps
+    run_steps(submit_resident, timed_steps)  # first region of this size: the exchange buffers are allocated here
     reserve_exchange(timed_steps)
     launches0 = fe.launch_count
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -774,6 +763,7 @@ def run_ours(args, rank, local_rank, world):
         dist.all_reduce(total_ms, op=dist.ReduceOp.MAX)
     total_ms = float(total_ms.item())
     n_valid = int((res_np["id1"] >= 0).sum())
+    last_step_results = sets[(timed_steps - 1) % DEPTH]["res"].copy()  # the later regions reuse the result buffers
 
     # ---- timed: end to end through the host-buffer C ABI (pinned host buffers in, host results out) -----
     barrier()
@@ -788,9 +778,8 @@ def run_ours(args, rank, local_rank, world):
     e2e_total = float(e2e_total.item())
 
     # ---- reference point: the same step, one at a time (synchronous API, L2 flushed before every step) ----
-    # READ a 256 MiB buffer (> 126 MB L2): the lines it leaves behind are clean.  (A memset flush leaves 126 MB of dirty lines
-    # whose write-back lands inside the timed kernels: the cold Hamming launch then measures 86 us instead of the 53 us the
-    # ncu launch list -- which invalidates the caches between kernels -- shows for the same cold launch.)
+    # READ a 256 MiB buffer (> 50 MB L2): the lines it leaves behind are clean (a memset flush would leave dirty lines whose
+    # write-back lands inside the timed kernels).
     flush = torch.zeros(64 * 1024 * 1024, dtype=torch.int32, device="cuda")
     sync_ms, sync_ham, sync_dev = [], [], []
     for k in range(3 + min(args.steps, 10)):
@@ -830,16 +819,15 @@ def run_ours(args, rank, local_rank, world):
             "ms_per_step": total_ms / timed_steps, "timed_steps": timed_steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u8 descriptors (exact integer Hamming) + f32 fit + f64 Mahalanobis", "data": "synthetic",
             "config": {"workload": WORKLOAD,
-                       "l2": f"inputs larger than L2: {DEPTH} alternating batches = {DEPTH} x 156 MB resident node data (126 MB L2); "
+                       "l2": f"inputs larger than L2: {DEPTH} alternating batches = {DEPTH} x 156 MB resident node data (50 MB L2); "
                              "the synchronous reference point flushes L2 (a 256 MiB read) before every step",
                        "pipeline": f"{DEPTH} batches in flight on {DEPTH} library streams (rgbdslam_b200_match_pairs_submit / _wait)",
                        "pairs_per_gpu": PAIRS_PER_GPU,
                        "exchange": "none (1 GPU)" if world == 1 else f"ONE ncclAllGather of the {world} x {timed_steps} x {PAIRS_PER_GPU} edge records (120 B) of the region at its end (rgbdslam_b200_allgather_edges), inside the timed region",
                        "edges_gathered": None if comm is None else int((local_edges["all"]["id1"] >= 0).sum()),
-                       "valid_edges_rank0": n_valid, "wall_ms_per_step_incl_flush": 1e3 * wall_resident / timed_steps,
-                       "repeats": f"{repeats} x --steps {args.steps} timed back to back (>= {MIN_TIMED_MS:.0f} ms per timed region)"},
+                       "valid_edges_rank0": n_valid, "wall_ms_per_step_incl_flush": 1e3 * wall_resident / timed_steps},
             "roofline": {"bound": "hbm", "kernel": "hamming_match", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": NCU_DRAM_BYTES_PER_LAUNCH, "traffic_source": NCU_TRAFFIC_SOURCE, "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": ALGO_BYTES_PER_PAIR * PAIRS_PER_GPU, "kernel_ms": ham,
                          "kernel_share_of_step": ham / statistics.mean(sync_dev),
                          "kernel_ms_when_pipelined": statistics.mean(ham_ms),
@@ -897,6 +885,8 @@ def run_ours(args, rank, local_rank, world):
             agree = int(((ores["id1"] >= 0) == (res_np["id1"] >= 0)).sum())
             out["config"]["oracle_agreement_valid_flags"] = f"{agree}/{PAIRS_PER_GPU}"
         emit(out)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_step_results)
     if comm is not None:
         fe.comm_destroy(comm)
     fe.close()
@@ -916,14 +906,17 @@ def emit(out: dict):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)  # 200 x 0.16 ms: long enough that one scheduling hiccup does not halve the number
+    ap.add_argument("--steps", type=int, default=200, help="timed steps (exactly this many)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-c4", action="store_true", help="skip the 2000-frame sequence (config C4) sub-measurement")
     ap.add_argument("--c4-frames", type=int, default=C4_FRAMES)
     ap.add_argument("--no-c3", action="store_true", help="skip the SIFT-128 (config C3) sub-measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the pair results of the last timed step as DIR/pair_<field>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

@@ -137,7 +137,7 @@ int rgbdslam_b200_set_stream(void* cuda_stream);
 /* Block until all work queued by the library has finished. */
 int rgbdslam_b200_synchronize(void);
 
-/* Which kernel computes the Hamming brute-force stage: 0 = SIMT popcount kernel (cross-check); 1 (default) = tcgen05 kind::i8
+/* Which kernel computes the Hamming brute-force stage: 0 = SIMT popcount kernel (cross-check); 1 (default) = wgmma s8
  * tensor-core GEMM with arg-max epilogue, the 32-byte descriptors expanded to int8 operands inside the kernel.  Both are exact
  * and give identical results (DESIGN.md 4.1); other values are rejected. */
 int rgbdslam_b200_set_hamming_path(int path);

@@ -1,4 +1,4 @@
-"""rgbdslam_v2_b200 -- B200-native (sm_100a) re-implementation of the rgbdslam_v2 frame-pair hot path.
+"""rgbdslam_v2_b200 -- H100-native (sm_90a) re-implementation of the rgbdslam_v2 frame-pair hot path.
 
 The product is the C-ABI shared library ``librgbdslam_b200.so`` (see ``include/rgbdslam_b200.h``) built from
 ``csrc/``.  This package is the thin Python host mirror used by tests and ``bench.py``; it binds the library

@@ -94,7 +94,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     if not p.exists():
         raise LibraryMissingError(
             f"{p} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  rgbdslam_v2_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  rgbdslam_v2_b200 has no CPU fallback.")
     lib = C.CDLL(str(p))
     u64, i64, i32p = C.c_uint64, C.c_int64, C.POINTER(C.c_int32)
     vp = C.c_void_p
@@ -225,7 +225,7 @@ class Frontend:
         self._check(self.lib.rgbdslam_b200_set_stream(stream_ptr))
 
     def set_hamming_path(self, path: int):
-        """1 = tcgen05 int8 tensor-core GEMM (default), 0 = SIMT popcount."""
+        """1 = wgmma int8 tensor-core GEMM (default), 0 = SIMT popcount."""
         self._check(self.lib.rgbdslam_b200_set_hamming_path(path))
 
     def set_sift_matcher(self, matcher: int):

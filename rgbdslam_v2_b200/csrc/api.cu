@@ -539,8 +539,8 @@ int rgbdslam_b200_init(int device, const rgbdslam_b200_params* p) {
   cudaDeviceProp prop;
   e = cudaGetDeviceProperties(&prop, device);
   if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceProperties");
-  if (prop.major != 10) {
-    set_error(std::string("this build targets sm_100a (B200); device is ") + prop.name);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error(std::string("this build targets sm_90a (H100); device is ") + prop.name);
     return RGBDSLAM_B200_ERR_CUDA;
   }
   if (!s.inited) {
@@ -699,7 +699,7 @@ int rgbdslam_b200_set_sift_matcher(int matcher) {
 int rgbdslam_b200_set_hamming_path(int path) {
   std::lock_guard<std::mutex> lk(g_state.mu);
   if (path < 0 || path > 1) {
-    set_error("set_hamming_path: 0 = SIMT popcount (cross-check), 1 = tcgen05 int8 GEMM (default)");
+    set_error("set_hamming_path: 0 = SIMT popcount (cross-check), 1 = wgmma int8 GEMM (default)");
     return RGBDSLAM_B200_ERR_ARG;
   }
   g_state.hamming_path = path;

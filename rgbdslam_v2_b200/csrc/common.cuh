@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host definitions for the sm_100a front-end kernels.
+// common.cuh -- shared device/host definitions for the sm_90a front-end kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

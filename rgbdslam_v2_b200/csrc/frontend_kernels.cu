@@ -1,4 +1,4 @@
-// frontend_kernels.cu -- sm_100a kernels of the frame-pair hot path:
+// frontend_kernels.cu -- sm_90a kernels of the frame-pair hot path:
 //   hamming_simt_kernel    : bruteForceSearchORB (features.cpp:168-182) for every query row of every pair
 //   select_matches_kernel  : hd<128 filter, jitter distance, sort, keepStrongestMatches (node.cpp:572-573,674,1127)
 //   ransac_hyp_kernel      : one warp per RANSAC hypothesis (node.cpp:1130-1169) -- sample 4, weighted Kabsch

@@ -1,19 +1,21 @@
-// hamming_tc.cu -- brute-force descriptor matching on the 5th-gen tensor cores (tcgen05, sm_100a).
+// hamming_tc.cu -- brute-force descriptor matching on the Hopper tensor cores (wgmma, sm_90a).
 //
 // bruteForceSearchORB (features.cpp:168-182) for all query rows of all pairs, exact:
 //   for two 256-bit descriptors a, b read as +-1 vectors:  a . b = 256 - 2 * hamming(a, b)   (exact in int32)
 //   => argmin_j hd(q_i, t_j)  ==  argmax_j (Q T^T)_ij, ties -> lowest j  (features.cpp:176 strict <).
-// The N x M distance matrix is therefore an int8 GEMM with a row-arg-max epilogue: tcgen05.mma.kind::i8, M = 128 (queries ->
-// TMEM lanes), N = 128 (train rows -> TMEM columns), K = 32 per instruction, int32 accumulators in TMEM, double buffered so the
-// epilogue of tile n overlaps the MMAs of tile n+1.  Operand tiles use the UMMA canonical K-major no-swizzle shared-memory
-// layout in 128-row tiles of 32 KiB:  tile[row_group 16][k_chunk 16][row_in_group 8][16 B]  (conflict-free 8 x 16 B core matrices).
+// The N x M distance matrix is therefore an int8 GEMM with a row-arg-max epilogue.  A work item is 256 queries of one pair
+// against all train rows of the other node, in 128-row train tiles; each of four warp groups owns 64 query rows and issues
+// wgmma.mma_async m64n128 (K = 32 bytes per instruction) with the accumulators in registers (64 per thread).  Operand tiles
+// use the canonical K-major no-swizzle ("interleave") shared-memory layout:
+//   tile[row_group][k_chunk 16][row_in_group 8][16 B]   (8 x 16 B core matrices, 2048 B per 8-row group)
 //
 // Two kernels:
-//  * tc_hamming_expand_kernel -- the ORB path: producer warps expand the 32-byte descriptors to +-64 operands straight into
-//    shared memory, a ninth k-step carries the column index, two MMA-issuing warps, VIMNMX3 epilogue (see its own header below);
+//  * tc_hamming_expand_kernel -- the ORB path: the threads expand the 32-byte descriptors to +-64 operands straight into shared
+//    memory, a ninth k-step carries the column index, and the expansion of train tile n+1 runs while the MMAs of tile n execute;
 //  * tc_match256_kernel<1|2>  -- the float-descriptor matchers (bf16 RootSIFT scores / SiftGPU's u8 dot products): operand
-//    tiles resident in HBM in the layout above, each staged by ONE cp.async.bulk completing on an mbarrier.
-#include <cstdio>
+//    tiles resident in HBM in the layout above, each staged by ONE cp.async.bulk completing on an mbarrier, one producer warp
+//    and four consumer warp groups that run independently of each other (one group's epilogue overlaps another's MMAs).
+#include <type_traits>
 
 #include "kernels.h"
 
@@ -45,370 +47,260 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
-// mbarrier wait with a watchdog for the kernels under development (-DRB200_HANG_DEBUG): a wait that spins for ~1 s reports which
-// role was waiting on which barrier and traps, so that a pipeline bug surfaces as an error with a message instead of a hung GPU.
-__device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-#ifdef RB200_HANG_DEBUG
-__device__ __noinline__ void mbar_wait_dbg(uint32_t bar, uint32_t parity, int tag, int a, int b) {
-  const long long t0 = clock64();
-  while (!mbar_try(bar, parity)) {
-    if (clock64() - t0 > 2000000000ll) {
-      printf("HANG block %d thread %d tag %d (%d, %d) bar %u parity %u\n", blockIdx.x, threadIdx.x, tag, a, b, bar, parity);
-      __trap();
-    }
-  }
-}
-#define RB200_WAIT(bar, parity, tag, a, b) mbar_wait_dbg(bar, parity, tag, a, b)
-#else
-#define RB200_WAIT(bar, parity, tag, a, b) mbar_wait(bar, parity)
-#endif
 __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-// Pull a block of global memory into L2 ahead of its bulk copy (no shared memory, no completion tracking).
-__device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_i8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// One lane of a fully converged warp (elect.sync): the way to issue tcgen05 / bulk-copy instructions from warp-uniform code.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "elect.sync _|p, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// UMMA shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"):
+// wgmma shared-memory matrix descriptor, K-major, no swizzle ("interleave"):
 //   bits [0,14)  start address >> 4
-//   bits [16,30) leading-dimension byte offset >> 4  = distance between the two 8x16 B core matrices of
-//                one K=32 B step                      = 128 B  (k_chunk stride of the tile layout)
-//   bits [32,46) stride-dimension byte offset >> 4   = distance between consecutive 8-row groups = 2048 B
-//   bits [46,48) descriptor version = 1 (Blackwell);  bits [61,64) layout type = 0 (no swizzle)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(128u >> 4) << 16) | ((uint64_t)(2048u >> 4) << 32) |
-         (1ull << 46);
+//   bits [16,30) leading-dimension byte offset >> 4 = distance between the two 8 x 16 B core matrices of one K = 32 B step
+//   bits [32,46) stride-dimension byte offset >> 4  = distance between consecutive 8-row groups
+//   base offset 0, layout type 0 (interleave)
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-constexpr uint32_t kTileA = 128 * 256;   // 32 KiB: 128 rows x 256 B of operand data
-constexpr int kNoBest = (int)0x80000000;
+// The 64 accumulator registers of an m64n128 wgmma.  Element j of thread t of the warp group holds
+//   row 16 (t / 32) + (t % 32) / 4 + 8 ((j / 2) % 2),  column 8 (j / 4) + 2 (t % 4) + j % 2.
+#define RB_WG_D                                                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, " \
+  "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "   \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define RB_WG_OPS(C, d)                                                                                                  \
+  C(d[0]), C(d[1]), C(d[2]), C(d[3]), C(d[4]), C(d[5]), C(d[6]), C(d[7]), C(d[8]), C(d[9]), C(d[10]), C(d[11]), C(d[12]),  \
+      C(d[13]), C(d[14]), C(d[15]), C(d[16]), C(d[17]), C(d[18]), C(d[19]), C(d[20]), C(d[21]), C(d[22]), C(d[23]),     \
+      C(d[24]), C(d[25]), C(d[26]), C(d[27]), C(d[28]), C(d[29]), C(d[30]), C(d[31]), C(d[32]), C(d[33]), C(d[34]),     \
+      C(d[35]), C(d[36]), C(d[37]), C(d[38]), C(d[39]), C(d[40]), C(d[41]), C(d[42]), C(d[43]), C(d[44]), C(d[45]),     \
+      C(d[46]), C(d[47]), C(d[48]), C(d[49]), C(d[50]), C(d[51]), C(d[52]), C(d[53]), C(d[54]), C(d[55]), C(d[56]),     \
+      C(d[57]), C(d[58]), C(d[59]), C(d[60]), C(d[61]), C(d[62]), C(d[63])
 
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t acc) {
+// D (+)= A B^T, s8 x s8 -> s32 (ORB), M64 N128 K32
+__device__ __forceinline__ void wgmma_s8(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(acc)
-      : "memory");
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 " RB_WG_D ", %64, %65, p;\n}\n"
+      : RB_WG_OPS("+r", d)
+      : "l"(da), "l"(db), "r"(acc));
 }
+// u8 x u8 -> s32 (SiftGPU matcher), M64 N128 K32
+__device__ __forceinline__ void wgmma_acc(uint32_t (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 " RB_WG_D ", %64, %65, p;\n}\n"
+      : RB_WG_OPS("+r", d)
+      : "l"(da), "l"(db), "r"(acc));
+}
+// bf16 x bf16 -> f32 (RootSIFT scores), M64 N128 K16 (32 bytes of K per instruction as well)
+__device__ __forceinline__ void wgmma_acc(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " RB_WG_D ", %64, %65, p, 1, 1, 0, 0;\n}\n"
+      : RB_WG_OPS("+f", d)
+      : "l"(da), "l"(db), "r"(acc));
+}
+#undef RB_WG_OPS
+#undef RB_WG_D
+
+constexpr int kNoBest = (int)0x80000000;
+constexpr uint32_t kGroupStride = 2048;     // bytes per 8-row group of a 256-byte-row operand tile
+constexpr uint32_t kWgRows = 64 * 256;      // 16 KiB: the 64 query rows of one warp group
+constexpr uint32_t kA256 = 256 * 256;       // 64 KiB: the 256 query rows of a work item
+constexpr uint32_t kB128 = 128 * 256;       // 32 KiB: one train tile
 
 // ---------------------------------------------------------------------------------------------
-// Variant with a 256-query A block per work item (two M=128 accumulator halves) and 128-row B tiles:
-//   smem  : A 2 x 64 KiB (double buffered across items) + B 2 x 32 KiB
-//   TMEM  : [stage 2][half 2][128 columns]  (512 columns)
-//   L2->SM traffic per 256 queries: 64 KiB + nt/128 * 32 KiB  (1.8x less than the 128-query kernel, whose operand
-//   fetch rate -- not the tensor pipe -- limits it: ncu shows 42 % tensor-pipe activity at ~29 B/clk/SM)
-//   warps : 0 = bulk-copy producer, 1 = MMA issuer, 2..9 = epilogue (warp group g drains half g)
-constexpr uint32_t kA256 = 256 * 256;  // 64 KiB
-constexpr uint32_t kB128 = 128 * 256;  // 32 KiB
-// Ring depths: the query block (A, 64 KiB) is double-buffered across items, the train tiles (B, 32 KiB) stream through
-// a 3-deep ring -- one tile feeds ~1.1 k cycles of MMA, an L2 / HBM fetch takes longer than that, so two stages stall
-// the tensor pipe on every tile (measured 61 us vs 75 us for the shallower variants).  224 KiB + barriers <= 227 KiB.
-#ifndef RB200_TC_L2_PREFETCH
-#define RB200_TC_L2_PREFETCH 0  // measured: no gain (bench `value` 1.50-1.52 M with, 1.54-1.59 M pairs/s without)
-#endif
-#ifndef RB200_TC256_ASTAGES
-#define RB200_TC256_ASTAGES 2
-#endif
-#ifndef RB200_TC256_BSTAGES
-#define RB200_TC256_BSTAGES 3
-#endif
-constexpr int kASt = RB200_TC256_ASTAGES, kBSt = RB200_TC256_BSTAGES;
-constexpr uint32_t kSmem256Bars = kASt * kA256 + kBSt * kB128;
-constexpr uint32_t kTc256SmemBytes = kSmem256Bars + 256;
+// Float-descriptor matchers.  Warps 0-15: four consumer warp groups (64 query rows each), warp 16: bulk-copy producer.
+// smem: A (the item's 256 query rows, 64 KiB) + a 3-deep ring of 32 KiB train tiles + barriers.
+constexpr int kBSt = 3;
+constexpr int kTc256ConsumerWarps = 16;
+constexpr int kTc256Threads = (kTc256ConsumerWarps + 1) * 32;  // 544
+constexpr uint32_t kTc256BarsOff = kA256 + kBSt * kB128;
+constexpr uint32_t kTc256SmemBytes = kTc256BarsOff + 128;
 static_assert(kTc256SmemBytes <= 232448, "tc_match256: shared memory over the 227 KiB per-CTA limit");
-// barrier slots
-constexpr int kBarAFull = 0, kBarAEmpty = kASt, kBarBFull = 2 * kASt, kBarBEmpty = 2 * kASt + kBSt,
-              kBarAccFull = 2 * kASt + 2 * kBSt, kBarAccEmpty = kBarAccFull + 2, kBarCount = kBarAccEmpty + 2;
-static_assert(kBarCount * 8 <= 192, "barrier area");
-constexpr int kTc256Threads = 320;
-constexpr uint32_t kIdescI8_N128 = (2u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-constexpr uint32_t kIdescU8_N128 = (2u << 4) | ((128u >> 3) << 17) | ((128u >> 4) << 24);  // a/b format 0 = unsigned 8-bit
-constexpr uint32_t kIdescBF16_N128 = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
+constexpr int kBarAFull = 0, kBarAEmpty = 1, kBarBFull = 2, kBarBEmpty = 2 + kBSt;  // 8 barriers
 
-#ifdef RB200_PROFILE_TC
-// [role: loader, MMA issuer, epilogue warps][cycles waiting on A, on B, on accumulators, total, participants]
-__device__ unsigned long long g_tc_prof[3][8];
-extern "C" int rb200_debug_tc_profile(unsigned long long* out24, int reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out24, g_tc_prof, sizeof(unsigned long long) * 24);
-  if (e == cudaSuccess && reset) {
-    unsigned long long z[24] = {0};
-    e = cudaMemcpyToSymbol(g_tc_prof, z, sizeof(z));
+// top-4 of one query row, ordered by (score descending, column ascending)
+struct Top4 {
+  float s0 = -3.0e38f, s1 = -3.0e38f, s2 = -3.0e38f, s3 = -3.0e38f;
+  int i0 = -1, i1 = -1, i2 = -1, i3 = -1;
+  __device__ static bool ahead(float s, int i, float t, int j) { return s > t || (s == t && i < j); }
+  __device__ __forceinline__ void insert(float sc, int col) {
+    if (!ahead(sc, col, s3, i3)) return;
+    if (ahead(sc, col, s2, i2)) {
+      s3 = s2; i3 = i2;
+      if (ahead(sc, col, s1, i1)) {
+        s2 = s1; i2 = i1;
+        if (ahead(sc, col, s0, i0)) { s1 = s0; i1 = i0; s0 = sc; i0 = col; }
+        else { s1 = sc; i1 = col; }
+      } else { s2 = sc; i2 = col; }
+    } else { s3 = sc; i3 = col; }
   }
-  return (int)e;
-}
-#endif
+  // merge with the list of the lane `mask` away (the four lanes of a quad share a row)
+  __device__ __forceinline__ void merge_xor(int mask) {
+    const float t0 = __shfl_xor_sync(0xffffffffu, s0, mask), t1 = __shfl_xor_sync(0xffffffffu, s1, mask),
+                t2 = __shfl_xor_sync(0xffffffffu, s2, mask), t3 = __shfl_xor_sync(0xffffffffu, s3, mask);
+    const int j0 = __shfl_xor_sync(0xffffffffu, i0, mask), j1 = __shfl_xor_sync(0xffffffffu, i1, mask),
+              j2 = __shfl_xor_sync(0xffffffffu, i2, mask), j3 = __shfl_xor_sync(0xffffffffu, i3, mask);
+    if (j0 >= 0) insert(t0, j0);
+    if (j1 >= 0) insert(t1, j1);
+    if (j2 >= 0) insert(t2, j2);
+    if (j3 >= 0) insert(t3, j3);
+  }
+};
+
+// SiftGPU RowMatch / ColMatch bookkeeping of one query row (ProgramCU.cu:1708-1736, 1463-1478, 1771-1777): strict >, only
+// positive dots register, the runner-up VALUE counts duplicates of the maximum.  best = (dot << 17) | (0x1FFFF - tie priority),
+// -1 = no positive dot yet; next = the largest dot of every other column -- both independent of the visiting order.
+struct U8Best {
+  long long best = -1;
+  int next = 0;
+  __device__ __forceinline__ void add_key(long long key) {
+    if (key > best) {
+      if (best >= 0) next = max(next, (int)(best >> 17));
+      best = key;
+    } else {
+      next = max(next, (int)(key >> 17));
+    }
+  }
+  __device__ __forceinline__ void add(int dv, int col, int tie_rule) {
+    // common case first: a dot product below the current best only feeds the runner-up value
+    if (dv > 0 && dv >= (best >= 0 ? (int)(best >> 17) : 0)) {
+      const int prio = tie_rule ? col : (((col & 31) << 12) | (col >> 5));
+      add_key(((long long)dv << 17) | (long long)(0x1FFFF - prio));
+    } else {
+      next = max(next, dv);
+    }
+  }
+  __device__ __forceinline__ void merge_xor(int mask) {
+    const long long pb = __shfl_xor_sync(0xffffffffu, best, mask);
+    const int pn = __shfl_xor_sync(0xffffffffu, next, mask);
+    if (pb >= 0) add_key(pb);
+    next = max(next, pn);
+  }
+};
+
 template <int MODE>
 __global__ void __launch_bounds__(kTc256Threads, 1) tc_match256_kernel(const HamItem* __restrict__ items, int n_items) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sA = smem_u32(smem);
-  const uint32_t sB = sA + kASt * kA256;
-  const uint32_t bars = sA + kSmem256Bars;
+  const uint32_t sB = sA + kA256;
+  const uint32_t bars = sA + kTc256BarsOff;
   auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + kSmem256Bars + 192);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kBarAccEmpty; i++) mbar_init(bar(i), 1);
-    mbar_init(bar(kBarAccEmpty), 8);  // tmem_empty: one arrival per epilogue warp
-    mbar_init(bar(kBarAccEmpty + 1), 8);
+    mbar_init(bar(kBarAFull), 1);
+    mbar_init(bar(kBarAEmpty), kTc256ConsumerWarps);
+    for (int i = 0; i < kBSt; i++) {
+      mbar_init(bar(kBarBFull + i), 1);
+      mbar_init(bar(kBarBEmpty + i), kTc256ConsumerWarps);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32((const void*)tmem_ptr_smem))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-#ifdef RB200_PROFILE_TC
-  long long pf_a = 0, pf_b = 0, pf_acc = 0, pf_t0 = clock64();
-#define RB200_TIMED_WAIT(ACC, ...) { const long long c0_ = clock64(); mbar_wait(__VA_ARGS__); ACC += clock64() - c0_; }
-#else
-#define RB200_TIMED_WAIT(ACC, ...) mbar_wait(__VA_ARGS__);
-#endif
 
-  if (warp == 0) {
+  if (warp == kTc256ConsumerWarps) {
     if (lane == 0) {
-      uint32_t sa = 0, pa = 0, sb = 0, pb = 0;
+      uint32_t na = 0, nb_seq = 0;
       for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
         const HamItem item = items[it];
-#if RB200_TC_L2_PREFETCH
-        // Experiment (off by default): the operands of this CTA's NEXT item go to L2 now.  No gain -- a cold launch is only
-        // ~2 us slower than a warm one (59 vs 57 us), the 3-deep ring already covers the HBM latency.
-        if (it + (int)gridDim.x < n_items) {
-          const HamItem nx = items[it + gridDim.x];
-          bulk_prefetch_l2(nx.a, kA256);
-          for (int nb = 0; nb < nx.n_btiles; nb++) bulk_prefetch_l2(nx.b + (size_t)nb * kB128, kB128);
-        }
-#endif
-        RB200_TIMED_WAIT(pf_a, bar(kBarAEmpty + sa), pa ^ 1)
-        mbar_expect_tx(bar(kBarAFull + sa), kA256);
-        bulk_g2s(sA + sa * kA256, item.a, kA256, bar(kBarAFull + sa));
-        if (++sa == kASt) { sa = 0; pa ^= 1; }
-        for (int nb = 0; nb < item.n_btiles; nb++) {
-          RB200_TIMED_WAIT(pf_b, bar(kBarBEmpty + sb), pb ^ 1)
-          mbar_expect_tx(bar(kBarBFull + sb), kB128);
-          bulk_g2s(sB + sb * kB128, item.b + (size_t)nb * kB128, kB128, bar(kBarBFull + sb));
-          if (++sb == kBSt) { sb = 0; pb ^= 1; }
+        mbar_wait(bar(kBarAEmpty), (na & 1u) ^ 1u);
+        na++;
+        mbar_expect_tx(bar(kBarAFull), kA256);
+        bulk_g2s(sA, item.a, kA256, bar(kBarAFull));
+        for (int nb = 0; nb < item.n_btiles; nb++, nb_seq++) {
+          const uint32_t slot = nb_seq % kBSt;
+          mbar_wait(bar(kBarBEmpty + slot), ((nb_seq / kBSt) & 1u) ^ 1u);
+          mbar_expect_tx(bar(kBarBFull + slot), kB128);
+          bulk_g2s(sB + slot * kB128, item.b + (size_t)nb * kB128, kB128, bar(kBarBFull + slot));
         }
       }
     }
-  } else if (warp == 1) {
-    // The whole warp walks the pipeline and one elected lane issues the tcgen05 instructions (issuing from inside an
-    // `if (lane == 0)` region makes the compiler wrap every UTCIMMA in an ELECT / BRA.U.ANY retry loop: ~13 dependent
-    // instructions per MMA).  ONE issuer for both accumulator halves: the issuing thread runs only ~2 MMAs ahead of the tensor
-    // pipe (tc_hamming_expand_kernel uses one issuer per half for that reason); here the top-4 / runner-up epilogue, not the
-    // tensor pipe, bounds the kernel (10 % of the bf16 peak), so the simpler form stays.
-    uint32_t sa = 0, pa = 0, sb = 0, pb = 0, acc = 0, pacc = 0;
-    constexpr uint32_t kIdesc = MODE == 2 ? kIdescU8_N128 : kIdescBF16_N128;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const int n_btiles = items[it].n_btiles;
-      RB200_TIMED_WAIT(pf_a, bar(kBarAFull + sa), pa)
-      tc_fence_after();
-      for (int nb = 0; nb < n_btiles; nb++) {
-        RB200_TIMED_WAIT(pf_b, bar(kBarBFull + sb), pb)
-        RB200_TIMED_WAIT(pf_acc, bar(kBarAccEmpty + acc), pacc ^ 1)
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t da = make_desc(sA + sa * kA256), db = make_desc(sB + sb * kB128);  // start-address field += bytes >> 4
+    return;
+  }
+
+  const int wg = warp >> 2;                                   // warp group = 64-row block of the query tile
+  const int r0 = 16 * (warp & 3) + (lane >> 2);               // this thread's rows: r0 and r0 + 8 of the block
+  const int cq = 2 * (lane & 3);                              // and columns cq, cq + 1 of every 8-column block
+  const uint64_t da = make_desc(sA + wg * kWgRows, 128, kGroupStride);
+  using Acc = typename std::conditional<MODE == 2, uint32_t, float>::type;
+  Acc d[64];
+  uint32_t na = 0, nb_seq = 0;
+  for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+    const HamItem item = items[it];
+    Top4 t4[2];
+    U8Best u8[2];
+    mbar_wait(bar(kBarAFull), na & 1u);
+    na++;
+    for (int nb = 0; nb < item.n_btiles; nb++, nb_seq++) {
+      const uint32_t slot = nb_seq % kBSt;
+      mbar_wait(bar(kBarBFull + slot), (nb_seq / kBSt) & 1u);
+      const uint64_t db = make_desc(sB + slot * kB128, 128, kGroupStride);
+      wgmma_fence();
 #pragma unroll
-          for (int h = 0; h < 2; h++) {
-#pragma unroll
-            for (int k = 0; k < (MODE == 2 ? 4 : 8); k++) {  // u8 SIFT rows carry 128 B of data: 4 k-steps of 32 B
-              const uint32_t d = tmem_base + acc * 256 + h * 128;
-              const uint64_t dak = da + (uint64_t)((h * kTileA + k * 256) >> 4), dbk = db + (uint64_t)((k * 256) >> 4);
-              if (MODE == 1) tc_mma_bf16(d, dak, dbk, kIdesc, k > 0 ? 1u : 0u);
-              else tc_mma_i8(d, dak, dbk, kIdesc, k > 0 ? 1u : 0u);
-            }
-          }
-          tc_commit(bar(kBarBEmpty + sb));
-          tc_commit(bar(kBarAccFull + acc));
-        }
-        __syncwarp();
-        if (++sb == kBSt) { sb = 0; pb ^= 1; }
-        if (++acc == 2) { acc = 0; pacc ^= 1; }
-      }
-      if (elect_one()) tc_commit(bar(kBarAEmpty + sa));
+      for (int k = 0; k < (MODE == 2 ? 4 : 8); k++)  // u8 SIFT rows carry 128 B of data: 4 k-steps of 32 B
+        wgmma_acc(d, da + (uint64_t)((k * 256) >> 4), db + (uint64_t)((k * 256) >> 4), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait_all();
       __syncwarp();
-      if (++sa == kASt) { sa = 0; pa ^= 1; }
-    }
-  } else {
-    const int h = (warp - 2) >> 2;  // accumulator half drained by this warp group
-    const int wq = warp & 3;        // TMEM lane quadrant
-    const int row = h * 128 + wq * 32 + lane;
-    uint32_t acc = 0, pacc = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-      const HamItem item = items[it];
-      float s0 = -3.0e38f, s1 = -3.0e38f, s2 = -3.0e38f, s3 = -3.0e38f;
-      int i0 = -1, i1 = -1, i2 = -1, i3 = -1;
-      long long u8_best = -1;  // MODE 2: (dot << 17) | (0x1FFFF - tie priority); -1 = no positive dot yet
-      int u8_next = 0;
-      for (int nb = 0; nb < item.n_btiles; nb++) {
-        RB200_TIMED_WAIT(pf_acc, bar(kBarAccFull + acc), pacc)
-        tc_fence_after();
-        const uint32_t t0 = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * 256 + h * 128;
-#pragma unroll 1
-        for (int c = 0; c < 4; c++) {
-          uint32_t v[32];
-          tc_ld32(t0 + c * 32, v);
-          tc_wait_ld();
-          const int col0 = nb * 128 + c * 32;
-          if (MODE == 2) {
-            // SiftGPU RowMatch / ColMatch bookkeeping (ProgramCU.cu:1708-1736, 1463-1478, 1771-1777): strict >, only
-            // positive dots register, the runner-up VALUE counts duplicates of the maximum.
-            // common case first: a dot product below the current best only feeds the runner-up value (one IMNMX); the 64-bit
-            // (dot, tie priority) key is built only for candidates that reach the best dot product
-            const int nvalid = item.nsearch - col0;  // columns j < nvalid exist
-            int best_dot = u8_best >= 0 ? (int)(u8_best >> 17) : 0;
+      if (lane == 0) mbar_arrive(bar(kBarBEmpty + slot));
+      const int colb = nb * 128 + cq;
+      if (MODE == 2) {
+        const int nvalid = item.nsearch;  // columns col < nvalid exist; dot products are >= 0 and 0 never registers
 #pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const int dv = j < nvalid ? (int)v[j] : 0;  // dot products are >= 0 (unsigned operands); 0 never registers
-              if (dv >= best_dot && dv > 0) {
-                const int col = col0 + j;
-                const int prio = item.pad_ ? col : (((col & 31) << 12) | (col >> 5));
-                const long long key = ((long long)dv << 17) | (long long)(0x1FFFF - prio);
-                if (key > u8_best) {
-                  if (u8_best >= 0) u8_next = max(u8_next, (int)(u8_best >> 17));
-                  u8_best = key;
-                  best_dot = dv;
-                } else {
-                  u8_next = max(u8_next, dv);
-                }
-              } else {
-                u8_next = max(u8_next, dv);
-              }
-            }
-          } else {
-            // |b|^2 of the chunk's 32 train rows: eight 16-byte loads with a warp-uniform address (one transaction each, L1
-            // resident), issued before the comparisons.  (First version: one global load per element inside the branchy insertion,
-            // 20 x slower than the MMAs it drains; second: one load per lane + a shuffle per element -- the shuffle unit became
-            // the bottleneck, ncu: 50 % of the stall samples on the SHFL.)  Columns past the last train row get +inf = score -inf.
-            float bn[32];
-            {
-              const float4* np4 = reinterpret_cast<const float4*>(item.bnorm + col0);
-#pragma unroll
-              for (int i = 0; i < 8; i++) {
-                const float4 t = __ldg(np4 + i);
-                bn[4 * i] = t.x; bn[4 * i + 1] = t.y; bn[4 * i + 2] = t.z; bn[4 * i + 3] = t.w;
-              }
-            }
-            if (col0 + 32 > item.nsearch) {
-#pragma unroll
-              for (int j = 0; j < 32; j++)
-                if (col0 + j >= item.nsearch) bn[j] = __int_as_float(0x7f800000);
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j++) {
-              const float sc = fmaf(2.f, __uint_as_float(v[j]), -bn[j]);
-              if (sc > s3) {  // rare after the first tiles: insert (ties keep the earlier = lower index)
-                const int col = col0 + j;
-                if (sc > s2) {
-                  s3 = s2; i3 = i2;
-                  if (sc > s1) {
-                    s2 = s1; i2 = i1;
-                    if (sc > s0) { s1 = s0; i1 = i0; s0 = sc; i0 = col; }
-                    else { s1 = sc; i1 = col; }
-                  } else { s2 = sc; i2 = col; }
-                } else { s3 = sc; i3 = col; }
-              }
-            }
-          }
+        for (int j = 0; j < 64; j++) {
+          const int col = colb + 8 * (j >> 2) + (j & 1);
+          u8[(j >> 1) & 1].add(col < nvalid ? (int)d[j] : 0, col, item.pad_);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kBarAccEmpty + acc));
-        if (++acc == 2) { acc = 0; pacc ^= 1; }
+      } else {
+        // |b|^2 of this thread's two columns of every 8-column block; columns past the last train row get +inf = score -inf
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+          const int col = colb + 8 * i;
+          float2 bn = __ldg(reinterpret_cast<const float2*>(item.bnorm + col));
+          if (col >= item.nsearch) bn.x = __int_as_float(0x7f800000);
+          if (col + 1 >= item.nsearch) bn.y = __int_as_float(0x7f800000);
+          t4[0].insert(fmaf(2.f, (float)d[4 * i], -bn.x), col);
+          t4[0].insert(fmaf(2.f, (float)d[4 * i + 1], -bn.y), col + 1);
+          t4[1].insert(fmaf(2.f, (float)d[4 * i + 2], -bn.x), col);
+          t4[1].insert(fmaf(2.f, (float)d[4 * i + 3], -bn.y), col + 1);
+        }
       }
-      if (row < item.nq_valid) {
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar(kBarAEmpty));
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      if (MODE == 2) {
+        u8[h].merge_xor(1);
+        u8[h].merge_xor(2);
+      } else {
+        t4[h].merge_xor(1);
+        t4[h].merge_xor(2);
+      }
+      const int row = wg * 64 + r0 + 8 * h;
+      if ((lane & 3) == 0 && row < item.nq_valid) {
         if (MODE == 2) {
-          int4 o = make_int4(0, -1, u8_next, 0);
-          if (u8_best >= 0) {
-            const int prio = 0x1FFFF - (int)(u8_best & 0x1FFFF);
-            o.x = (int)(u8_best >> 17);
+          int4 o = make_int4(0, -1, u8[h].next, 0);
+          if (u8[h].best >= 0) {
+            const int prio = 0x1FFFF - (int)(u8[h].best & 0x1FFFF);
+            o.x = (int)(u8[h].best >> 17);
             o.y = item.pad_ ? prio : (((prio & 0xFFF) << 5) | (prio >> 12));
           }
           reinterpret_cast<int4*>(item.out)[row] = o;
         } else {
-          reinterpret_cast<int4*>(item.out)[row] = make_int4(i0, i1, i2, i3);
+          reinterpret_cast<int4*>(item.out)[row] = make_int4(t4[h].i0, t4[h].i1, t4[h].i2, t4[h].i3);
         }
       }
     }
-  }
-#ifdef RB200_PROFILE_TC
-  if (lane == 0 && MODE == 1) {
-    const int role = warp == 0 ? 0 : (warp == 1 ? 1 : 2);
-    atomicAdd(&g_tc_prof[role][0], (unsigned long long)pf_a);
-    atomicAdd(&g_tc_prof[role][1], (unsigned long long)pf_b);
-    atomicAdd(&g_tc_prof[role][2], (unsigned long long)pf_acc);
-    atomicAdd(&g_tc_prof[role][3], (unsigned long long)(clock64() - pf_t0));
-    atomicAdd(&g_tc_prof[role][4], 1ull);
-  }
-#endif
-#undef RB200_TIMED_WAIT
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -435,50 +327,26 @@ cudaError_t launch_siftgpu_tc256(const HamItem* d_items, int n_items, int sm_cou
 // ---------------------------------------------------------------------------------------------
 // Hamming match with IN-KERNEL operand expansion (the default ORB path, `set_hamming_path(1)`).
 //
-// The resident-tile kernel above reads a +-1 int8 expansion of every descriptor (256 B per 32-byte descriptor) that
-// the nodes keep in HBM: 7.6 x the algorithmic DRAM traffic of the stage and 8 x the node memory.  Here the producer warps read
-// the 32-byte descriptors themselves and expand them straight into the UMMA operand layout in shared memory.
-// Two more things ride on the expansion:
+// The threads read the 32-byte descriptors themselves and expand them straight into the operand layout in shared memory
+// (8 x the descriptor bytes: expanding in HBM would multiply the stage's DRAM traffic by that).  Two more things ride on it:
 //  * operands are +-64 instead of +-1, so the accumulator holds 4096 * dot;
 //  * a NINTH k-step multiplies two constant operand blocks, A_idx rows (64, 1, 0 ...) x B_idx row j (hi_j, lo_j, 0 ...) with
 //    64 hi_j + lo_j = 127 - j: the accumulator of column j of a train tile becomes  4096 * dot + (127 - j),  i.e. the
-//    (dot product, lowest-column-wins) key the arg-max needs is produced BY THE TENSOR CORE.  The epilogue no longer builds a
-//    key per element (IMAD + VIADDMNMX, two issue slots per element, half of the SM's issue bandwidth): it takes a plain
-//    three-input maximum (VIMNMX3: half a slot per element), adds the tile's column offset once per tile, and leaves the
-//    issue slots to the expansion.  One extra MMA in nine (+12.5 % tensor time) buys a 4 x cheaper epilogue.
+//    (dot product, lowest-column-wins) key the arg-max needs is produced BY THE TENSOR CORE, and the epilogue is a plain
+//    three-input maximum (VIMNMX3) per two elements.
 // Exactness: |4096 dot| <= 2^20, 127 - j in [0, 128), global key = acc + (3968 - 128 tile) = 4096 dot + (4095 - col) with
 // col <= 4095 -- all exact in int32; dot = key >> 12 (arithmetic), col = 4095 - (key & 4095).
 //
-// Work item = 256 queries of one pair (two 128-row halves) against all train rows, 128-row train tiles.
-//   warps 0-7  : producers, two groups of 128 threads filling alternate tiles, one thread per tile row (2 x LDG.128 -> 64 words of +-64 -> 16 x STS.128, layout
-//                tile[row_group 16][k_chunk 16][row 8][16 B]); writes are published to the async proxy (fence.proxy.async)
-//                before the arrival on the tile's mbarrier
-//   warps 8-9  : MMA issuers, one per query half (one elected lane each): per train tile (8 + 1) tcgen05.mma.kind::i8 M128 N128 K32
-//   warps 10-17: epilogue (TMEM lane quadrant = warp & 3, half = (warp - 10) >> 2)
-// Shared memory: A ring 3 x 32 KiB (one query half per slot: the next item's first half is expanded while the current item
-// runs), B ring 3 x 32 KiB, the two 4 KiB index blocks.  TMEM: 2 stages x 2 halves x 128 int32 columns.
-#ifndef RB200_X_EPI_PAIR
-#define RB200_X_EPI_PAIR 1
-#endif
-constexpr int kXProducerGroups = 2;                     // tiles are filled alternately by two groups of 128 threads
-constexpr int kXProducerWarps = 4 * kXProducerGroups, kXIssuerWarps = 2, kXEpiWarps = 8;
-constexpr int kXThreads = (kXProducerWarps + kXIssuerWarps + kXEpiWarps) * 32;  // 576
-constexpr int kXASlots = 3, kXBSlots = 3;
-constexpr uint32_t kXIdxOff = (kXASlots + kXBSlots) * kTileA;      // 192 KiB
-constexpr uint32_t kXBarsOff = kXIdxOff + 2 * 4096;
-constexpr uint32_t kXSmemBytes = kXBarsOff + 256;
+// 512 threads = four warp groups of 64 query rows.  Per item: all threads expand the 256 query rows (two threads per row) and
+// train tile 0; then per train tile n: every warp group issues its nine MMAs asynchronously, all threads expand tile n+1 into
+// the other half of the double-buffered B area (four threads per row), wait for the MMAs, and take the row maxima.
+// Shared memory: A 64 KiB + B 2 x 32 KiB + the two 4 KiB index blocks.
+constexpr int kXThreads = 512;
+constexpr uint32_t kXBOff = kA256;
+constexpr uint32_t kXIdxOff = kXBOff + 2 * kB128;
+constexpr uint32_t kXSmemBytes = kXIdxOff + 2 * 4096;
 static_assert(kXSmemBytes <= 232448, "tc_hamming_expand: shared memory over the 227 KiB per-CTA limit");
-constexpr int kXAFull = 0, kXAEmpty = kXASlots, kXBFull = 2 * kXASlots, kXBEmpty = 2 * kXASlots + kXBSlots,
-              kXAccFull = 2 * kXASlots + 2 * kXBSlots, kXAccEmpty = kXAccFull + 4, kXBarCount = kXAccEmpty + 4;  // [stage][half]
-static_assert(kXBarCount * 8 <= 192, "barrier area");
 
-__device__ __forceinline__ uint64_t make_desc_lbo_sbo(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46);
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
 // 4 descriptor bits (bits 0-3 of x, x < 16) -> 4 int8: bit set -> +64, clear -> -64
 // (x & 0x80808080) ^ 0xC0C0C0C0 in ONE LOP3 (immLut (a & b) ^ c = (0xF0 & 0xCC) ^ 0xAA = 0x6A): bit 7 of every byte of x selects
 // 0x40 (+64, bit set) or 0xC0 (-64, bit clear)
@@ -487,42 +355,37 @@ __device__ __forceinline__ uint32_t pm64_from_bit7(uint32_t x) {
   asm("lop3.b32 %0, %1, %2, %3, 0x6A;" : "=r"(r) : "r"(x), "r"(0x80808080u), "r"(0xC0C0C0C0u));
   return r;
 }
-// A 256-bit descriptor (8 words) becomes 256 int8 (+-64) at tile_row_addr + k_chunk * 128 (k_chunk = 16 operand bytes).
+// Descriptor word wi (0..7) of a row becomes 32 int8 (+-64) in k-chunks 2 wi and 2 wi + 1 of the row at row_addr.
 // The order of the 256 k positions inside a row is free as long as both operands use the same one (a dot product is a sum),
-// so no bit is ever moved to a "natural" place: output word s of input word w is the four bits 7-s, 15-s, 23-s, 31-s, brought
-// to bit 7 of their byte by one left shift (an IMAD on the FMA pipe) and turned into +-64 by one LOP3 -- one ALU-pipe
-// instruction per 4 operand bytes.
-// half a descriptor (4 words) -> 128 int8 in 8 consecutive k-chunks starting at addr (the caller adds 1024 B for the upper half)
-__device__ __forceinline__ void expand_half_row(uint32_t addr, const uint4 v) {
-  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+// so no bit is ever moved to a "natural" place: output word s of a chunk is the four bits 7-s, 15-s, 23-s, 31-s (shifted by
+// 4 for the second chunk), brought to bit 7 of their byte by one left shift and turned into +-64 by one LOP3.
+__device__ __forceinline__ void expand_word(uint32_t row_addr, int wi, uint32_t w) {
 #pragma unroll
-  for (int i = 0; i < 4; i++) {
-#pragma unroll
-    for (int hf = 0; hf < 2; hf++)
-      sts128(addr + (uint32_t)(2 * i + hf) * 128u, pm64_from_bit7(w[i] << (4 * hf)), pm64_from_bit7(w[i] << (4 * hf + 1)),
-             pm64_from_bit7(w[i] << (4 * hf + 2)), pm64_from_bit7(w[i] << (4 * hf + 3)));
-  }
+  for (int hf = 0; hf < 2; hf++)
+    sts128(row_addr + (uint32_t)(2 * wi + hf) * 128u, pm64_from_bit7(w << (4 * hf)), pm64_from_bit7(w << (4 * hf + 1)),
+           pm64_from_bit7(w << (4 * hf + 2)), pm64_from_bit7(w << (4 * hf + 3)));
 }
+__device__ __forceinline__ uint32_t row_offset(int r) { return (uint32_t)(r >> 3) * kGroupStride + (uint32_t)(r & 7) * 16u; }
+
+// train tile nb of the item -> the B buffer at dst (four threads per row, two descriptor words each; missing rows: zeros)
+__device__ __forceinline__ uint2 load_b_words(const HamItem& item, int nb) {
+  const int r = threadIdx.x >> 2, row = nb * 128 + r;
+  if (row < item.nsearch) return __ldg(reinterpret_cast<const uint2*>(item.b) + 4 * (size_t)row + (threadIdx.x & 3));
+  return make_uint2(0, 0);
+}
+__device__ __forceinline__ void store_b_words(uint32_t dst, uint2 v) {
+  const int r = threadIdx.x >> 2, w0 = 2 * (threadIdx.x & 3);
+  expand_word(dst + row_offset(r), w0, v.x);
+  expand_word(dst + row_offset(r), w0 + 1, v.y);
+}
+
 __global__ void __launch_bounds__(kXThreads, 1) tc_hamming_expand_kernel(const HamItem* __restrict__ items, int n_items) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sA = smem_u32(smem);
-  const uint32_t sB = sA + kXASlots * kTileA;
+  const uint32_t sB = sA + kXBOff;
   const uint32_t sIdxA = sA + kXIdxOff, sIdxB = sIdxA + 4096;
-  const uint32_t bars = sA + kXBarsOff;
-  auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem + kXBarsOff + 192);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#ifdef RB200_PROFILE_TC
-  unsigned long long gt_entry;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_entry));
-#endif
 
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kXASlots; i++) { mbar_init(bar(kXAFull + i), 128); mbar_init(bar(kXAEmpty + i), 1); }
-    for (int i = 0; i < kXBSlots; i++) { mbar_init(bar(kXBFull + i), 128); mbar_init(bar(kXBEmpty + i), kXIssuerWarps); }
-    for (int i = 0; i < 4; i++) { mbar_init(bar(kXAccFull + i), 1); mbar_init(bar(kXAccEmpty + i), kXEpiWarps / 2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
   if (threadIdx.x < 128) {
     // index blocks, K-major no-swizzle: [row_group 16][k_chunk 2][row 8][16 B]; only bytes 0 and 1 of a row are non-zero
     const int r = threadIdx.x;
@@ -532,253 +395,82 @@ __global__ void __launch_bounds__(kXThreads, 1) tc_hamming_expand_kernel(const H
     const uint32_t rem = 127u - (uint32_t)r;    // 64 * hi + lo
     sts128(sIdxB + off, (rem >> 6) | ((rem & 63u) << 8), 0, 0, 0);
     sts128(sIdxB + off + 128u, 0, 0, 0, 0);
-    fence_proxy_async_smem();
   }
-  if (warp == kXProducerWarps) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32((const void*)tmem_ptr_smem))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  const int my_items = blockIdx.x < n_items ? (n_items - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-#ifdef RB200_PROFILE_TC
-  // cycles this warp spends in each kind of wait (role 0 producers: [0] slot empty; role 1 issuer: [0] A full, [1] B full,
-  // [2] accumulator empty; role 2 epilogue: [2] accumulator full), [3] = lifetime, [4] = warps, [5] = cycles inside expand_row /
-  // the drain of a tile
-  long long pf_a = 0, pf_b = 0, pf_acc = 0, pf_work = 0;
-  const long long pf_t0 = clock64();
-  unsigned long long pf_gt_start;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(pf_gt_start));
-#define XWAIT(ACC, BAR, PAR, TAG, I, J) { const long long c0_ = clock64(); mbar_wait(BAR, PAR); ACC += clock64() - c0_; }
-#else
-#define XWAIT(ACC, BAR, PAR, TAG, I, J) RB200_WAIT(BAR, PAR, TAG, I, J)
-#endif
+  const int wg = warp >> 2;
+  const int r0 = 16 * (warp & 3) + (lane >> 2);  // this thread's accumulator rows: r0 and r0 + 8 of the warp group's 64
+  const int cq = 2 * (lane & 3);                 // and columns cq, cq + 1 of every 8-column block
+  const uint64_t da = make_desc(sA + wg * kWgRows, 128, kGroupStride);
+  const uint64_t dia = make_desc(sIdxA, 128, 256), dib = make_desc(sIdxB, 128, 256);
+  uint32_t d[64];
 
-  if (warp < kXProducerWarps) {
-    // ---------------- producers: two groups of 128 threads filling ALTERNATE tiles, thread t & 127 <-> row of the tile.
-    // (One fence.proxy.async per thread and tile costs a few hundred cycles in which the warp issues nothing: with all 256
-    // threads on every tile, two per row, the match kernel was 4 us slower than with the other group expanding meanwhile.)
-    // Order of production (the consumers need, per item: half 0 + tile 0, then half 1, then the other tiles):
-    //   A(0,0) B(0,0) A(0,1) | B(k,1) A(k+1,0) B(k,2) ... B(k,n-1) B(k+1,0) A(k+1,1) | ...
-    // A(k+1,0) goes into the ring slot item k-1 has released, A(k+1,1) into item k's first slot, i.e. after item k is done --
-    // by then the consumers already have half 0 and tile 0 of item k+1 to work on.  The schedule is written out as plain loops
-    // (an earlier resumable state machine cost the producer warps 2.8 x the cycles of the expansion itself -- ncu source
-    // view); one operation is kept in flight: produce() first issues the loads of the NEW operation, then waits for the ring
-    // slot of the PREVIOUS one and expands it, so the load latency hides behind the expansion.
-    const int prow = threadIdx.x & 127, group = threadIdx.x >> 7;
-    int op_index = 0;
-    const uint32_t row_off = (uint32_t)(prow >> 3) * 2048u + (uint32_t)(prow & 7) * 16u;
-    uint32_t a_seq = 0, b_seq = 0;  // A halves / B tiles scheduled so far (slot = seq % slots, phase = (seq / slots) & 1)
-    uint32_t p_dst = 0, p_full = 0, p_empty = 0, p_parity = 0;  // the operation in flight
-    uint4 p_lo = make_uint4(0, 0, 0, 0), p_hi = p_lo;
-    bool pending = false;
-    auto finish = [&]() {
-      if (!pending) return;
-      XWAIT(pf_a, p_empty, p_parity, 1, (int)a_seq, (int)b_seq);
-#ifdef RB200_PROFILE_TC
-      const long long w0_ = clock64();
-#endif
-      expand_half_row(p_dst, p_lo);
-      expand_half_row(p_dst + 1024u, p_hi);
-#ifdef RB200_PROFILE_TC
-      pf_work += clock64() - w0_;
-#endif
-#ifndef RB200_X_NO_PROXY_FENCE  // timing experiment only: without the fence the MMA may read stale operand bytes
-      fence_proxy_async_smem();
-#endif
-      mbar_arrive(p_full);
-      pending = false;
-    };
-    auto produce = [&](const int8_t* rows, int row, int n_rows, uint32_t tile, uint32_t full, uint32_t empty, uint32_t seq, uint32_t slots) {
-      if ((op_index++ & 1) != group) return;  // the other group's tile
-      uint4 lo = make_uint4(0, 0, 0, 0), hi = lo;
-      if (row < n_rows) {  // rows that do not exist: zeros
-        lo = __ldg(reinterpret_cast<const uint4*>(rows) + 2 * (size_t)row);
-        hi = __ldg(reinterpret_cast<const uint4*>(rows) + 2 * (size_t)row + 1);
-      }
-      finish();
-      p_lo = lo;
-      p_hi = hi;
-      p_dst = tile + row_off;
-      p_full = full;
-      p_empty = empty;
-      p_parity = ((seq / slots) & 1u) ^ 1u;
-      pending = true;
-    };
-    auto produce_a = [&](const HamItem& it, int h) {
-      const uint32_t slot = a_seq % kXASlots;
-      produce(it.a, h * 128 + prow, it.nq_valid, sA + slot * kTileA, bar(kXAFull + slot), bar(kXAEmpty + slot), a_seq, kXASlots);
-      a_seq++;
-    };
-    auto produce_b = [&](const HamItem& it, int nb) {
-      const uint32_t slot = b_seq % kXBSlots;
-      produce(it.b, nb * 128 + prow, it.nsearch, sB + slot * kTileA, bar(kXBFull + slot), bar(kXBEmpty + slot), b_seq, kXBSlots);
-      b_seq++;
-    };
-    if (my_items > 0) {
-      HamItem cur = items[blockIdx.x];
-      produce_a(cur, 0);
-      if (cur.n_btiles > 0) produce_b(cur, 0);
-      produce_a(cur, 1);
-      for (int k = 0; k < my_items; k++) {
-        const bool more = k + 1 < my_items;
-        HamItem nxt = cur;
-        if (more) nxt = items[blockIdx.x + (size_t)(k + 1) * gridDim.x];
-        for (int nb = 1; nb < cur.n_btiles; nb++) {
-          produce_b(cur, nb);
-          if (nb == 1 && more) produce_a(nxt, 0);
-        }
-        if (more) {
-          if (cur.n_btiles <= 1) produce_a(nxt, 0);
-          if (nxt.n_btiles > 0) produce_b(nxt, 0);
-          produce_a(nxt, 1);
-        }
-        cur = nxt;
-      }
-      finish();
+  for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+    const HamItem item = items[it];
+    __syncthreads();  // every MMA of the previous item has completed: A and both B buffers may be rewritten
+    {
+      const int r = threadIdx.x >> 1, hw = threadIdx.x & 1;  // two threads per query row, four descriptor words each
+      uint4 v = make_uint4(0, 0, 0, 0);
+      if (r < item.nq_valid) v = __ldg(reinterpret_cast<const uint4*>(item.a) + 2 * (size_t)r + hw);
+      const uint2 b0 = item.n_btiles > 0 ? load_b_words(item, 0) : make_uint2(0, 0);
+      const uint32_t ra = sA + row_offset(r);
+      expand_word(ra, 4 * hw, v.x);
+      expand_word(ra, 4 * hw + 1, v.y);
+      expand_word(ra, 4 * hw + 2, v.z);
+      expand_word(ra, 4 * hw + 3, v.w);
+      if (item.n_btiles > 0) store_b_words(sB, b0);
     }
-  } else if (warp < kXProducerWarps + kXIssuerWarps) {
-    // ---------------- MMA issuers: warp 8 owns query half 0, warp 9 half 1 (one elected lane each).
-    // Measured (tools/microbench/tc_ts_probe.cu, "issue_queue"): the issuing thread can run only ~2 MMAs (128 cycles) ahead of
-    // the tensor pipe, so every cycle beyond that which it spends between two bursts -- barrier checks, descriptor set-up,
-    // ~50 single-lane instructions per burst -- is a cycle the pipe idles (one issuer: tensor pipe 65 % busy).  With one issuer
-    // per accumulator half, one of them is setting up its next burst while the other one's nine MMAs execute.
-    const int h = warp - kXProducerWarps;
-    uint32_t a_seq = (uint32_t)h, b_seq = 0, acc = 0, pacc = 0;
-    const uint64_t dia = make_desc_lbo_sbo(sIdxA, 128, 256), dib = make_desc_lbo_sbo(sIdxB, 128, 256);
-    for (int k = 0; k < my_items; k++) {
-      const int n_btiles = items[blockIdx.x + (size_t)k * gridDim.x].n_btiles;
-      const uint32_t slot = a_seq % kXASlots, ph = (a_seq / kXASlots) & 1u;
-      a_seq += 2;
-      const uint64_t da = make_desc(sA + slot * kTileA);
-      for (int nb = 0; nb < n_btiles; nb++) {
-        const uint32_t sb = b_seq % kXBSlots, pb = (b_seq / kXBSlots) & 1u;
-        b_seq++;
-        const uint64_t db = make_desc(sB + sb * kTileA);
-        const uint32_t d = tmem_base + acc * 256 + h * 128;
-        XWAIT(pf_b, bar(kXBFull + sb), pb, 2, k, nb);
-        if (nb == 0) XWAIT(pf_a, bar(kXAFull + slot), ph, 3, k, nb);
-        XWAIT(pf_acc, bar(kXAccEmpty + 2 * acc + h), pacc ^ 1u, 4, k, nb);
-        tc_fence_after();
-        if (elect_one()) {
+    fence_proxy_async_smem();  // generic-proxy operand writes -> visible to the tensor core's (async proxy) reads
+    __syncthreads();
+    int best[2] = {kNoBest, kNoBest};
+    for (int nb = 0; nb < item.n_btiles; nb++) {
+      const uint64_t db = make_desc(sB + (uint32_t)(nb & 1) * kB128, 128, kGroupStride);
+      wgmma_fence();
 #pragma unroll
-          for (int ks = 0; ks < 8; ks++) tc_mma_i8(d, da + (uint64_t)((ks * 256) >> 4), db + (uint64_t)((ks * 256) >> 4), kIdescI8_N128, ks > 0 ? 1u : 0u);
-          tc_mma_i8(d, dia, dib, kIdescI8_N128, 1u);
-          tc_commit(bar(kXBEmpty + sb));            // the tile is free once BOTH issuers' MMAs on it have retired (count 2)
-          tc_commit(bar(kXAccFull + 2 * acc + h));
-        }
-        __syncwarp();
-        if (++acc == 2) { acc = 0; pacc ^= 1u; }
-      }
-      if (n_btiles == 0) {
-        // nothing to multiply (empty train set): the half is still produced and must be consumed before it is released --
-        // releasing a slot the producer has not filled yet flips the barrier phase under its feet (deadlock)
-        XWAIT(pf_a, bar(kXAFull + slot), ph, 7, k, 0);
-      }
-      if (elect_one()) tc_commit(bar(kXAEmpty + slot));  // free once every MMA this thread has issued so far has retired
-      __syncwarp();
-    }
-  } else {
-    // ---------------- epilogue
-    const int e = warp - (kXProducerWarps + kXIssuerWarps);
-    const int h = e >> 2;      // query half drained by this warp
-    const int wq = warp & 3;   // TMEM lane quadrant this warp may access
-    const int row = h * 128 + wq * 32 + lane;
-    uint32_t acc = 0, pacc = 0;
-    for (int k = 0; k < my_items; k++) {
-      const HamItem item = items[blockIdx.x + (size_t)k * gridDim.x];
-      int best = kNoBest;
-      for (int nb = 0; nb < item.n_btiles; nb++) {
-        XWAIT(pf_acc, bar(kXAccFull + 2 * acc + h), pacc, 6, k, nb);
-        tc_fence_after();
-#ifdef RB200_PROFILE_TC
-        const long long w0_ = clock64();
-#endif
-        const uint32_t t0 = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * 256 + h * 128;
-        const int nvalid = item.nsearch - nb * 128;  // train rows of this tile that exist (>= 128: all)
+      for (int ks = 0; ks < 8; ks++) wgmma_s8(d, da + (uint64_t)((ks * 256) >> 4), db + (uint64_t)((ks * 256) >> 4), ks > 0 ? 1u : 0u);
+      wgmma_s8(d, dia, dib, 1u);
+      wgmma_commit();
+      if (nb + 1 < item.n_btiles) store_b_words(sB + (uint32_t)((nb + 1) & 1) * kB128, load_b_words(item, nb + 1));
+      wgmma_wait_all();
+      const int nvalid = item.nsearch - nb * 128;  // train rows of this tile that exist (>= 128: all)
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
         int m = kNoBest;
-        // maximum of one 32-column chunk (columns at or beyond nvalid do not exist)
-        auto chunk_max = [&](const uint32_t (&v)[32], int c) {
-          if (c * 32 + 32 <= nvalid) {
-            int m0 = __vimax3_s32((int)v[0], (int)v[1], (int)v[2]), m1 = __vimax3_s32((int)v[3], (int)v[4], (int)v[5]);
+        if (nvalid >= 128) {
+          int m0 = __vimax3_s32((int)d[2 * h], (int)d[2 * h + 1], (int)d[4 + 2 * h]);
+          int m1 = __vimax3_s32((int)d[4 + 2 * h + 1], (int)d[8 + 2 * h], (int)d[8 + 2 * h + 1]);
 #pragma unroll
-            for (int j = 6; j < 30; j += 4) {
-              m0 = __vimax3_s32(m0, (int)v[j], (int)v[j + 1]);
-              m1 = __vimax3_s32(m1, (int)v[j + 2], (int)v[j + 3]);
-            }
-            m = __vimax3_s32(m, __vimax3_s32(m0, (int)v[30], (int)v[31]), m1);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; j++)
-              if (c * 32 + j < nvalid) m = max(m, (int)v[j]);
+          for (int i = 3; i < 15; i += 2) {
+            m0 = __vimax3_s32(m0, (int)d[4 * i + 2 * h], (int)d[4 * i + 2 * h + 1]);
+            m1 = __vimax3_s32(m1, (int)d[4 * i + 4 + 2 * h], (int)d[4 * i + 4 + 2 * h + 1]);
           }
-        };
-#if RB200_X_EPI_PAIR
-#pragma unroll 1
-        for (int c = 0; c < 4; c += 2) {  // two chunk loads in flight per wait: two TMEM round trips per tile instead of four
-          uint32_t v[32], u[32];
-          tc_ld32(t0 + c * 32, v);
-          tc_ld32(t0 + c * 32 + 32, u);
-          tc_wait_ld();
-          chunk_max(v, c);
-          chunk_max(u, c + 1);
+          m = __vimax3_s32(m0, m1, max((int)d[60 + 2 * h], (int)d[60 + 2 * h + 1]));
+        } else {
+#pragma unroll
+          for (int i = 0; i < 16; i++) {
+            if (8 * i + cq < nvalid) m = max(m, (int)d[4 * i + 2 * h]);
+            if (8 * i + cq + 1 < nvalid) m = max(m, (int)d[4 * i + 2 * h + 1]);
+          }
         }
-#else
-#pragma unroll 1
-        for (int c = 0; c < 4; c++) {
-          uint32_t v[32];
-          tc_ld32(t0 + c * 32, v);
-          tc_wait_ld();
-          chunk_max(v, c);
-        }
-#endif
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(kXAccEmpty + 2 * acc + h));
-#ifdef RB200_PROFILE_TC
-        pf_work += clock64() - w0_;
-#endif
-        if (++acc == 2) { acc = 0; pacc ^= 1u; }
-        if (m != kNoBest) best = max(best, m + (3968 - 128 * nb));  // 4096 dot + (4095 - col)
+        if (m != kNoBest) best[h] = max(best[h], m + (3968 - 128 * nb));  // 4096 dot + (4095 - col)
       }
-      if (row < item.nq_valid) {
+      fence_proxy_async_smem();
+      __syncthreads();  // tile nb+1 is complete, and every warp group is done with tile nb's buffer
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      int b = best[h];
+      b = max(b, __shfl_xor_sync(0xffffffffu, b, 1));
+      b = max(b, __shfl_xor_sync(0xffffffffu, b, 2));
+      const int row = wg * 64 + r0 + 8 * h;
+      if ((lane & 3) == 0 && row < item.nq_valid) {
         int2 o = make_int2(257, -1);  // features.cpp:172-173
-        if (best != kNoBest) {
-          const int dot = best >> 12;
+        if (b != kNoBest) {
+          const int dot = b >> 12;
           o.x = (256 - dot) >> 1;
-          o.y = 4095 - (best & 4095);
+          o.y = 4095 - (b & 4095);
         }
         item.out[row] = o;
       }
     }
-  }
-#ifdef RB200_PROFILE_TC
-  if (lane == 0) {
-    const int role = warp < kXProducerWarps ? 0 : (warp < kXProducerWarps + kXIssuerWarps ? 1 : 2);
-    atomicAdd(&g_tc_prof[role][0], (unsigned long long)pf_a);
-    atomicAdd(&g_tc_prof[role][1], (unsigned long long)pf_b);
-    atomicAdd(&g_tc_prof[role][2], (unsigned long long)pf_acc);
-    atomicAdd(&g_tc_prof[role][3], (unsigned long long)(clock64() - pf_t0));
-    atomicAdd(&g_tc_prof[role][4], 1ull);
-    atomicAdd(&g_tc_prof[role][5], (unsigned long long)pf_work);
-    // wall clock (ns): [0][6] = ~(earliest CTA entry), [0][7] = latest warp exit, [1][6] = longest entry -> pipeline start,
-    // [2][6] = ~(earliest pipeline start)
-    unsigned long long gt_now;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt_now));
-    atomicMax(&g_tc_prof[0][6], ~gt_entry);
-    atomicMax(&g_tc_prof[0][7], gt_now);
-    atomicMax(&g_tc_prof[1][6], pf_gt_start - gt_entry);
-    atomicMax(&g_tc_prof[2][6], ~pf_gt_start);
-  }
-#endif
-#undef XWAIT
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kXProducerWarps) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 

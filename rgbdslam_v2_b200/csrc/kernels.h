@@ -1,4 +1,4 @@
-// kernels.h -- host-side launchers of the sm_100a kernels (implemented in *.cu).
+// kernels.h -- host-side launchers of the sm_90a kernels (implemented in *.cu).
 #pragma once
 #include "common.cuh"
 

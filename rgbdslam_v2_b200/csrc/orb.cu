@@ -1,4 +1,4 @@
-// orb.cu -- ORB keypoint detection / description kernels for sm_100a (see orb.cuh for provenance).
+// orb.cu -- ORB keypoint detection / description kernels for sm_90a (see orb.cuh for provenance).
 //
 // Node constructor path (src/node.cpp:101-240), batched over frames:
 //   detector->detect(gray, kp, mask)      VideoGridAdaptedFeatureDetector (feature_adjuster.cpp:286-317) over

@@ -1,6 +1,6 @@
 // sift_l2.cu -- the SIFT-128 float-descriptor path (BASELINE config C3):
 //   k_sift_prepare      squareroot_descriptor_space (RootSIFT, node.cpp:1557-1571) + bf16 operand tiles + |b|^2
-//   tc_match_kernel<1>  (hamming_tc.cu) N x M score matrix 2 a.b - |b|^2 as a bf16 tcgen05 GEMM, 4 best per query
+//   tc_match_kernel<1>  (hamming_tc.cu) N x M score matrix 2 a.b - |b|^2 as a bf16 wgmma GEMM, 4 best per query
 //   k_l2_refine         exact fp32 squared L2 of the 4 candidates -> exact 2-NN among them
 //   k_select_sift       ratio test (nn_distance_ratio) + first-come uniqueness of trainIdx + keepStrongestMatches
 //                       (node.cpp:638-667, 674) -- replaces the approximate FLANN kd-tree 2-NN of node.cpp:493-514,610-636

@@ -91,7 +91,7 @@ struct State {
   Workspace& W() { return *cur; }
   DevBuf d_f32_a, d_f32_b, d_root_a, d_root_b, d_norm_a, d_norm_b;  // SIFT staging of the synchronous calls
   int sift_matcher = 0;  // float-descriptor nodes created from now on: 0 = exact 2-NN ratio matcher (FLANN branch), 1 = SiftGPU matcher
-  int hamming_path = 1;  // 1 = tcgen05 int8 GEMM, operands expanded inside the kernel (default); 0 = SIMT popcount (cross-check)
+  int hamming_path = 1;  // 1 = wgmma int8 GEMM, operands expanded inside the kernel (default); 0 = SIMT popcount (cross-check)
   void release_workspaces() {
     for (Workspace& w : ws) w.release();
     DevBuf* all[] = {&d_f32_a, &d_f32_b, &d_root_a, &d_root_b, &d_norm_a, &d_norm_b};

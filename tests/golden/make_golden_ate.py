@@ -1,14 +1,15 @@
 """Generates tests/golden/ate_align.npz by running the REFERENCE's own align()
-(/root/reference/rgbd_benchmark/evaluate_ate_module.pyx:35-55, extracted by line range and executed under Python 3 --
+(<reference tree>/rgbd_benchmark/evaluate_ate_module.pyx:35-55, extracted by line range and executed under Python 3 --
 the one substitution is numpy.linalg.linalg.svd -> numpy.linalg.svd, a module path numpy 2 no longer has) together with
 the RMSE expression of :197 (`numpy.sqrt(numpy.dot(trans_error,trans_error) / len(trans_error))`).
-Run here (container with /root/reference); the .npz is committed and travels to the GPU box."""
+Usage: python tests/golden/make_golden_ate.py <reference tree>; the .npz is committed, so the test needs no reference tree."""
+import sys
 from pathlib import Path
 
 import numpy
 import numpy as np
 
-REF = Path("/root/reference/rgbd_benchmark/evaluate_ate_module.pyx")
+REF = Path(sys.argv[1]) / "rgbd_benchmark" / "evaluate_ate_module.pyx"
 lines = REF.read_text().splitlines()
 start = next(i for i, l in enumerate(lines) if l.startswith("def align(model,data):"))
 end = next(i for i in range(start + 1, len(lines)) if lines[i].startswith("def "))

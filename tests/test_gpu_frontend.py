@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path through the C ABI vs the CPU oracle."""
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI vs the CPU oracle."""
 from pathlib import Path
 
 import numpy as np
@@ -66,7 +66,7 @@ def test_brute_force_vs_oracle_bit_exact(fe, oracle_mod, nq, nt):
 @pytest.mark.parametrize("nq,nt", [(1, 2), (5, 1), (128, 257), (129, 256), (1000, 1000), (1000, 1001), (1500, 700),
                                    (4096, 4096), (300, 4000)])
 def test_hamming_tensor_core_path_equals_simt_path(fe, oracle_mod, nq, nt):
-    """tcgen05 int8 GEMM formulation (hd = (256 - a.b)/2) is exact: identical to the popcount kernel."""
+    """wgmma int8 GEMM formulation (hd = (256 - a.b)/2) is exact: identical to the popcount kernel."""
     rng = np.random.default_rng(nq * 31 + nt)
     q = rng.integers(0, 256, (nq, 32), dtype=np.uint8)
     t = rng.integers(0, 256, (nt, 32), dtype=np.uint8)

@@ -7,7 +7,7 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from rgbdslam_v2_b200.build import CSRC, _nvcc, sources
 OUT = ROOT / "build_variants"; OBJ = OUT / "obj"; OBJ.mkdir(parents=True, exist_ok=True)
-FL = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-ccbin", shutil.which("g++")]
+FL = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-ccbin", shutil.which("g++")]
 TUNED = {"frontend_kernels.cu", "hamming_tc.cu", "posegraph.cu"}
 def cc(src, obj, extra=()):
     subprocess.run([_nvcc(), *FL, *extra, "-c", str(src), "-o", str(obj)], check=True)
@@ -24,5 +24,5 @@ for spec in sys.argv[1:]:
     for t in sorted(TUNED):
         o = OBJ / f"{Path(t).stem}.{name}.o"; cc(CSRC / t, o, extra); objs.append(o)
     lib = OUT / f"librgbdslam_b200.{name}.so"
-    subprocess.run([_nvcc(), "-shared", "-ldl", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(lib), *map(str, common + objs), "-ccbin", shutil.which("g++")], check=True)
+    subprocess.run([_nvcc(), "-shared", "-ldl", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(lib), *map(str, common + objs), "-ccbin", shutil.which("g++")], check=True)
     print("built", lib)

@@ -1,4 +1,4 @@
-"""A few synchronous passes of the C2 workload (256 pairs x 1000 ORB keypoints, resident nodes) -- the target of ncu captures."""
+"""A few synchronous passes of the C2 workload (256 pairs x 1000 ORB keypoints, resident nodes): per-launch Hamming kernel times."""
 import sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -20,20 +20,4 @@ for k in range(n):
     fe.match_node_pairs(newer, older, seed=1, out=(r, None, None))
     ham.append(fe.stage_times(0)["hamming"] * 1e3)
 print("hamming us per call:", " ".join(f"{x:.1f}" for x in ham), "| median %.1f min %.1f" % (float(np.median(ham[1:])), min(ham)))
-if hasattr(fe.lib, "rb200_debug_tc_profile"):
-    import ctypes as C
-    buf = (C.c_ulonglong * 24)()
-    fe.lib.rb200_debug_tc_profile(buf, 1)
-    fe.match_node_pairs(newer, older, seed=1, out=(r, None, None))
-    fe.lib.rb200_debug_tc_profile(buf, 0)
-    a = np.array(buf[:], dtype=np.float64).reshape(3, 8)
-    for role, name in enumerate(("loader", "mma", "epilogue")):
-        n = max(a[role, 4], 1)
-        print(f"  {name:9s} per participant: wait A {a[role,0]/n:9.0f}  wait B {a[role,1]/n:9.0f}  wait acc {a[role,2]/n:9.0f}  work {a[role,5]/n:9.0f}  total {a[role,3]/n:9.0f} cycles")
-    if a[0, 7] > 0:
-        M = 2 ** 64 - 1
-        ai = [[int(buf[8 * i + j]) for j in range(8)] for i in range(3)]
-        entry, exit_, pipe0 = M - ai[0][6], ai[0][7], M - ai[2][6]
-        print(f"  wall (globaltimer): first CTA entry -> last warp exit {(exit_ - entry) / 1e3:.1f} us; first pipeline start {(pipe0 - entry) / 1e3:.1f} us "
-              f"after entry; longest prologue {a[1, 6] / 1e3:.1f} us")
 print("valid", int((r["id1"] >= 0).sum()), "stages", fe.stage_times(0))

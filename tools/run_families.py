@@ -1,5 +1,5 @@
 """One pass over every kernel family that has a SURVEY section-8 row (ORB node constructor, SIFT matchers, pose graph,
-landmark bundle adjustment, EMM, pairwise refinement) -- the target of the ncu launch list / `--set full` captures under profiles/.
+landmark bundle adjustment, EMM, pairwise refinement) -- one run to time or profile them together.
 
   python tools/run_families.py [orb] [sift] [posegraph] [landmark] [emm] [refine]      (default: all)
 Prints CUDA-event / wall times per family as one JSON line (NOT a bench value when run under ncu)."""
