@@ -16,8 +16,9 @@
  *  - caller owns all host buffers.  Device memory is owned by the library
  *    (node handles, workspaces) unless a function name ends in _device, in
  *    which case the pointers are device pointers owned by the caller.
- *  - there is NO CPU fallback: without a CUDA device every compute call fails
- *    with RGBDSLAM_B200_ERR_CUDA.
+ *  - there is NO CPU fallback: without a CUDA device rgbdslam_b200_init fails
+ *    with RGBDSLAM_B200_ERR_CUDA, and every later call that needs the library
+ *    returns RGBDSLAM_B200_ERR_STATE.
  */
 #ifndef RGBDSLAM_B200_H
 #define RGBDSLAM_B200_H

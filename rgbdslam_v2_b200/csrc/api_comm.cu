@@ -43,6 +43,15 @@ int nccl_fail(ncclResult_t r, const char* what) {
   return RGBDSLAM_B200_ERR_NCCL;
 }
 
+Comm* get_comm(uint64_t h) {
+  Comm* c = (Comm*)(uintptr_t)h;
+  if (!c || c->magic != Comm::kMagic) {
+    set_error("invalid communicator handle");
+    return nullptr;
+  }
+  return c;
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -53,7 +62,10 @@ int rgbdslam_b200_comm_unique_id(uint8_t* id128) {
   std::lock_guard<std::mutex> lk(g_state.mu);
   int rc = load_nccl();
   if (rc) return rc;
-  if (!id128) return RGBDSLAM_B200_ERR_ARG;
+  if (!id128) {
+    set_error("comm_unique_id: null output");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
   ncclUniqueId id;
   ncclResult_t r = g_nccl.GetUniqueId(&id);
   if (r != 0) return nccl_fail(r, "ncclGetUniqueId");
@@ -62,10 +74,8 @@ int rgbdslam_b200_comm_unique_id(uint8_t* id128) {
 }
 
 int rgbdslam_b200_comm_init(int rank, int world, const uint8_t* id128, uint64_t* comm_handle) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
-  if ((rc = load_nccl())) return rc;
+  RB200_ENTER_INITED();
+  if (int rc = load_nccl()) return rc;
   if (!id128 || !comm_handle || world < 1 || rank < 0 || rank >= world) {
     set_error("comm_init: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
@@ -87,8 +97,8 @@ int rgbdslam_b200_comm_init(int rank, int world, const uint8_t* id128, uint64_t*
 
 int rgbdslam_b200_comm_destroy(uint64_t comm_handle) {
   std::lock_guard<std::mutex> lk(g_state.mu);
-  Comm* c = (Comm*)(uintptr_t)comm_handle;
-  if (!c || c->magic != Comm::kMagic) return RGBDSLAM_B200_ERR_ARG;
+  Comm* c = get_comm(comm_handle);
+  if (!c) return RGBDSLAM_B200_ERR_ARG;
   if (g_nccl.ok && c->comm) g_nccl.CommDestroy(c->comm);
   c->send.release();
   c->recv.release();
@@ -102,25 +112,23 @@ int rgbdslam_b200_comm_destroy(uint64_t comm_handle) {
 
 int rgbdslam_b200_allgather_edges(uint64_t comm_handle, const rgbdslam_b200_pair_result* local, int n_per_rank,
                                   rgbdslam_b200_pair_result* all) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
-  Comm* c = (Comm*)(uintptr_t)comm_handle;
-  if (!c || c->magic != Comm::kMagic || n_per_rank < 0 || (n_per_rank > 0 && (!local || !all))) {
+  RB200_ENTER_INITED();
+  Comm* c = get_comm(comm_handle);
+  if (!c) return RGBDSLAM_B200_ERR_ARG;
+  if (n_per_rank < 0 || (n_per_rank > 0 && (!local || !all))) {
     set_error("allgather_edges: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
   if (n_per_rank == 0) return 0;
   const size_t bytes = sizeof(rgbdslam_b200_pair_result) * (size_t)n_per_rank;
+  int rc;
   if ((rc = c->send.ensure(bytes)) || (rc = c->recv.ensure(bytes * c->world))) return rc;
   cudaStream_t st = g_state.stream;
-  cudaError_t e = cudaMemcpyAsync(c->send.ptr, local, bytes, cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) return cuda_fail(e, "allgather_edges upload");
+  RB200_CUDA(cudaMemcpyAsync(c->send.ptr, local, bytes, cudaMemcpyHostToDevice, st));
   ncclResult_t r = g_nccl.AllGather(c->send.ptr, c->recv.ptr, bytes, 0 /* ncclInt8 */, c->comm, st);
   if (r != 0) return nccl_fail(r, "ncclAllGather");
-  e = cudaMemcpyAsync(all, c->recv.ptr, bytes * c->world, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return cuda_fail(e, "allgather_edges download");
+  RB200_CUDA(cudaMemcpyAsync(all, c->recv.ptr, bytes * c->world, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -129,15 +137,15 @@ int rgbdslam_b200_allgather_edges(uint64_t comm_handle, const rgbdslam_b200_pair
 // rgbdslam_b200_match_pairs_wait(slot) also waits for this.  No host round trip, the next batch can be submitted meanwhile.
 // Every rank must issue these calls in the same slot order.
 int rgbdslam_b200_allgather_slot_edges(uint64_t comm_handle, int slot, int n_per_rank, rgbdslam_b200_pair_result* all) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
-  Comm* c = (Comm*)(uintptr_t)comm_handle;
-  if (!c || c->magic != Comm::kMagic || slot < 0 || slot >= kSlots || n_per_rank < 0 || (n_per_rank > 0 && !all)) {
+  RB200_ENTER_INITED();
+  Comm* c = get_comm(comm_handle);
+  Workspace* ws = c ? get_slot(slot) : nullptr;
+  if (!ws) return RGBDSLAM_B200_ERR_ARG;
+  if (n_per_rank < 0 || (n_per_rank > 0 && !all)) {
     set_error("allgather_slot_edges: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  Workspace& w = g_state.ws[slot];
+  Workspace& w = *ws;
   if (!w.pending || n_per_rank == 0) {
     set_error("allgather_slot_edges: the slot has no batch in flight (call it right after match_pairs*_submit)");
     return RGBDSLAM_B200_ERR_STATE;
@@ -147,19 +155,14 @@ int rgbdslam_b200_allgather_slot_edges(uint64_t comm_handle, int slot, int n_per
     set_error("allgather_slot_edges: n_per_rank exceeds the batch submitted on this slot");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  cudaError_t e = cudaSuccess;
-  if (!c->gstream) e = cudaStreamCreateWithFlags(&c->gstream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaStreamCreate(gather)");
-  if ((rc = c->slot_recv[slot].ensure(bytes * c->world))) return rc;
-  cudaStream_t st = slot == 0 ? g_state.stream : w.stream;
-  e = cudaEventRecord(w.ev[7], st);  // everything the slot has queued so far
-  if (e == cudaSuccess) e = cudaStreamWaitEvent(c->gstream, w.ev[7], 0);
-  if (e != cudaSuccess) return cuda_fail(e, "allgather_slot_edges dependency");
+  if (!c->gstream) RB200_CUDA(cudaStreamCreateWithFlags(&c->gstream, cudaStreamNonBlocking));
+  if (int rc = c->slot_recv[slot].ensure(bytes * c->world)) return rc;
+  RB200_CUDA(cudaEventRecord(w.ev[kEvGatherDep], w.stream));  // everything the slot has queued so far
+  RB200_CUDA(cudaStreamWaitEvent(c->gstream, w.ev[kEvGatherDep], 0));
   ncclResult_t r = g_nccl.AllGather(w.d_results.ptr, c->slot_recv[slot].ptr, bytes, 0 /* ncclInt8 */, c->comm, c->gstream);
   if (r != 0) return nccl_fail(r, "ncclAllGather");
-  e = cudaMemcpyAsync(all, c->slot_recv[slot].ptr, bytes * c->world, cudaMemcpyDeviceToHost, c->gstream);
-  if (e == cudaSuccess) e = cudaEventRecord(w.ev_gather, c->gstream);
-  if (e != cudaSuccess) return cuda_fail(e, "allgather_slot_edges download");
+  RB200_CUDA(cudaMemcpyAsync(all, c->slot_recv[slot].ptr, bytes * c->world, cudaMemcpyDeviceToHost, c->gstream));
+  RB200_CUDA(cudaEventRecord(w.ev_gather, c->gstream));
   w.gather_pending = true;
   return 0;
 }

@@ -77,7 +77,7 @@ static void build_table(int src_n, int dst_n, std::vector<int16_t>& ofs, std::ve
   }
 }
 
-static int orb_prepare(int W, int H, int nframes_hint) {
+static int orb_prepare(int W, int H) {
   State& s = g_state;
   OrbCtx& o = g_orb;
   const int grid = s.params.detector_grid_resolution > 1 ? s.params.detector_grid_resolution : 1;
@@ -202,7 +202,6 @@ static int orb_prepare(int W, int H, int nframes_hint) {
   }
   o.kp_stride = std::min(kOrbFrameCap, o.max_per_cell * g.ncells);
   o.W = W; o.H = H; o.grid = grid; o.max_kp = K;
-  (void)nframes_hint;
   int rc;
   if ((rc = o.d_ofs.ensure(o.h_ofs.size() * 2 + 16)) || (rc = o.d_w1.ensure(o.h_w1.size() * 2 + 16))) return rc;
   cudaStream_t st = s.stream;
@@ -312,6 +311,142 @@ static int orb_check_err_flag(int flag) {
   return 0;
 }
 
+static bool is_pinned(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return a.type == cudaMemoryTypeHost;
+}
+
+// Argument checks shared by nodes_create_ex and nodes_create_sharded.
+static int check_nodes_args(const char* what, const Detector* det, int nframes, const float* K4, const uint64_t* node_handles,
+                            int flags) {
+  if (!det || nframes < 0 || (nframes > 0 && (!K4 || !node_handles)) || (flags & ~RGBDSLAM_B200_MASK_FROM_DEPTH)) {
+    set_error(std::string(what) + ": bad arguments");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  return 0;
+}
+
+// The nodes of one nodes_create* call share one device allocation (no per-node cudaMalloc), every region 256-byte aligned:
+// [desc nodes x K x 32][xyz nodes x K x 16][n nodes x 4][kp kp_frames x K x 28]
+struct NodeBatch {
+  NodeSlab* slab = nullptr;
+  int K = 0;  // feature rows per node
+  uint8_t* desc = nullptr;
+  float4* xyz = nullptr;
+  int* n = nullptr;
+  size_t n_bytes = 0;
+  rgbdslam_b200_keypoint* kp = nullptr;
+  std::vector<NodeDev*> made;  // nodes that own device memory before they are published (depth clouds)
+};
+
+static int batch_alloc(NodeBatch& nb, int nodes, int kp_frames, int K) {
+  auto up = [](size_t v) { return (v + 255) / 256 * 256; };
+  const size_t b_desc = up((size_t)nodes * K * 32), b_xyz = up((size_t)nodes * K * 16), b_n = up((size_t)nodes * 4);
+  const size_t b_kp = up((size_t)kp_frames * K * sizeof(rgbdslam_b200_keypoint));
+  nb.slab = new NodeSlab();
+  cudaError_t e = cudaMalloc(&nb.slab->base, b_desc + b_xyz + b_n + b_kp);
+  if (e != cudaSuccess) {
+    delete nb.slab;
+    nb.slab = nullptr;
+    return cuda_fail(e, "cudaMalloc(node slab)");
+  }
+  nb.K = K;
+  nb.desc = (uint8_t*)nb.slab->base;
+  nb.xyz = (float4*)(nb.desc + b_desc);
+  nb.n = (int*)((uint8_t*)nb.xyz + b_xyz);
+  nb.n_bytes = b_n;
+  nb.kp = (rgbdslam_b200_keypoint*)((uint8_t*)nb.n + b_n);
+  return 0;
+}
+
+// Failure after batch_alloc: waits for the work already queued on both streams, frees what the batch owns, returns code.
+static int batch_fail(NodeBatch& nb, int code) {
+  cudaStreamSynchronize(g_orb.copy_stream);
+  cudaStreamSynchronize(g_state.stream);
+  for (NodeDev* x : nb.made) {
+    if (x->cloud_z) cudaFree(x->cloud_z);
+    delete x;
+  }
+  cudaFree(nb.slab->base);
+  delete nb.slab;
+  return code;
+}
+
+// Frame input of a nodes_create* call: the caller's buffers are copied from directly when they are pinned, else through the two
+// pinned staging buffers (chunk frames each).
+static int setup_staging(const uint8_t* gray, const float* depth, const uint8_t* mask, size_t px, int chunk, bool* pinned) {
+  OrbCtx& o = g_orb;
+  *pinned = is_pinned(gray) && is_pinned(depth) && (!mask || is_pinned(mask));
+  if (*pinned) return 0;
+  const size_t bytes = (px + px * 4 + (mask ? px : 0)) * chunk;
+  int rc;
+  if ((rc = o.stage[0].ensure(bytes)) || (rc = o.stage[1].ensure(bytes))) return rc;
+  return 0;
+}
+
+// Host -> device copy of the F frames of chunk ci (gray, depth, optional mask) into dg / dd / dm on the copy stream, through
+// staging buffer ci & 1 unless pinned.  The copy stream first waits for `after` (if given); the compute stream waits for the copy.
+static int upload_chunk(int ci, int F, int chunk, size_t px, bool pinned, const uint8_t* hg, const float* hd, const uint8_t* hm,
+                        uint8_t* dg, float* dd, uint8_t* dm, cudaEvent_t after) {
+  OrbCtx& o = g_orb;
+  const int b = ci & 1;
+  cudaStream_t cs = o.copy_stream;
+  if (!pinned) {  // the previous copy out of this staging buffer must have finished
+    if (ci >= 2) RB200_CUDA(cudaEventSynchronize(o.ev_copied[b]));
+    uint8_t* sp = (uint8_t*)o.stage[b].ptr;
+    memcpy(sp, hg, px * F);
+    memcpy(sp + px * chunk, hd, px * 4 * F);
+    if (hm) memcpy(sp + px * 5 * chunk, hm, px * F);
+    hg = sp;
+    hd = (const float*)(sp + px * chunk);
+    if (hm) hm = sp + px * 5 * chunk;
+  }
+  if (after) RB200_CUDA(cudaStreamWaitEvent(cs, after, 0));
+  RB200_CUDA(cudaMemcpyAsync(dg, hg, px * F, cudaMemcpyHostToDevice, cs));
+  RB200_CUDA(cudaMemcpyAsync(dd, hd, px * 4 * F, cudaMemcpyHostToDevice, cs));
+  if (hm) RB200_CUDA(cudaMemcpyAsync(dm, hm, px * F, cudaMemcpyHostToDevice, cs));
+  RB200_CUDA(cudaEventRecord(o.ev_ready[b], cs));
+  RB200_CUDA(cudaEventRecord(o.ev_copied[b], cs));
+  RB200_CUDA(cudaStreamWaitEvent(g_state.stream, o.ev_ready[b], 0));
+  return 0;
+}
+
+// End of a nodes_create* call: waits for it, checks the device error flag and hands out one node per frame -- features of
+// frame f at slab row f * K, 2-D keypoints only for frames [kp_first, kp_first + kp_frames).  Frees the batch on failure.
+static int batch_publish(NodeBatch& nb, int nframes, int kp_first, int kp_frames, const int32_t* ids, uint64_t* node_handles,
+                         int32_t* n_features, const char* what) {
+  OrbCtx& o = g_orb;
+  cudaStream_t st = g_state.stream;
+  std::vector<int> n(nframes);
+  int flag = 0;
+  cudaError_t e = cudaMemcpyAsync(n.data(), nb.n, 4 * (size_t)nframes, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&flag, o.err.ptr, 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(o.copy_stream);
+  if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, what));
+  if (int rc = orb_check_err_flag(flag)) return batch_fail(nb, rc);
+  const int K = nb.K, Kpad = ((K > 0 ? K : 1) + 255) / 256 * 256;
+  for (int f = 0; f < nframes; f++) {
+    NodeDev* nd = nb.made.empty() ? new NodeDev() : nb.made[f];
+    nd->magic = NodeDev::kMagic;
+    nd->id = ids ? ids[f] : f;
+    nd->n = n[f];
+    nd->n_pad = Kpad;
+    nd->desc = nb.desc + (size_t)f * K * 32;
+    nd->xyz = nb.xyz + (size_t)f * K;
+    nd->kp = (f >= kp_first && f < kp_first + kp_frames) ? nb.kp + (size_t)(f - kp_first) * K : nullptr;
+    nd->slab = nb.slab;
+    nb.slab->refs++;
+    node_handles[f] = (uint64_t)(uintptr_t)nd;
+    if (n_features) n_features[f] = n[f];
+  }
+  return 0;
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -319,7 +454,10 @@ using namespace rb200;
 extern "C" {
 
 int rgbdslam_b200_detector_create(uint64_t* detector) {
-  if (!detector) return RGBDSLAM_B200_ERR_ARG;
+  if (!detector) {
+    set_error("detector_create: null output");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
   *detector = (uint64_t)(uintptr_t) new Detector();
   return 0;
 }
@@ -339,7 +477,11 @@ int rgbdslam_b200_detector_destroy(uint64_t detector) {
 int rgbdslam_b200_detector_thresholds(uint64_t detector, double* thresholds16, int set) {
   std::lock_guard<std::mutex> lk(g_state.mu);
   Detector* d = get_detector(detector);
-  if (!d || !thresholds16) return RGBDSLAM_B200_ERR_ARG;
+  if (!d) return RGBDSLAM_B200_ERR_ARG;
+  if (!thresholds16) {
+    set_error("detector_thresholds: null thresholds");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
   if (!d->host_valid) {
     int rc = check_inited();
     if (rc) return rc;
@@ -357,15 +499,14 @@ int rgbdslam_b200_detector_thresholds(uint64_t detector, double* thresholds16, i
 
 int rgbdslam_b200_orb_detect(uint64_t detector, const uint8_t* gray, const uint8_t* mask, int w, int h,
                              rgbdslam_b200_keypoint* kp_out, int capacity, int* n_out) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   Detector* det = get_detector(detector);
   if (!det || !gray || !kp_out || !n_out || capacity < 0) {
     set_error("orb_detect: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if ((rc = orb_prepare(w, h, 1)) || (rc = orb_ensure_buffers(1, 1, true))) return rc;
+  int rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_buffers(1, 1, true))) return rc;
   OrbCtx& o = g_orb;
   cudaStream_t st = g_state.stream;
   const size_t px = (size_t)w * h;
@@ -403,14 +544,13 @@ int rgbdslam_b200_orb_detect(uint64_t detector, const uint8_t* gray, const uint8
 
 int rgbdslam_b200_orb_compute(const uint8_t* gray, int w, int h, const rgbdslam_b200_keypoint* kp_in, int n_in,
                               rgbdslam_b200_keypoint* kp_out, uint8_t* desc_out, int* n_out) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   if (!gray || n_in < 0 || (n_in > 0 && (!kp_in || !kp_out || !desc_out)) || !n_out) {
     set_error("orb_compute: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if ((rc = orb_prepare(w, h, 1)) || (rc = orb_ensure_buffers(1, 1, true))) return rc;
+  int rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_buffers(1, 1, true))) return rc;
   OrbCtx& o = g_orb;
   // cv::ORB::compute: runByImageBorder(31) on cvRound'ed coordinates, then group by octave (stable)
   std::vector<rgbdslam_b200_keypoint> kept;
@@ -449,15 +589,6 @@ int rgbdslam_b200_orb_compute(const uint8_t* gray, int w, int h, const rgbdslam_
   return 0;
 }
 
-static bool is_pinned(const void* p) {
-  cudaPointerAttributes a;
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return a.type == cudaMemoryTypeHost;
-}
-
 // Node::Node for nframes frames in order.  Pipeline per chunk of kOrbChunk frames:
 //   copy stream    : host -> device of the chunk's gray / depth / mask into one of two input buffers (straight from the caller's
 //                    buffers when they are pinned, else through pinned staging filled by this thread)
@@ -467,135 +598,65 @@ static bool is_pinned(const void* p) {
 int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                   int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
                                   int32_t* n_features) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   Detector* det = get_detector(detector);
-  if (!det || nframes < 0 || (nframes > 0 && (!gray || !depth || !K4 || !node_handles)) ||
-      (flags & ~RGBDSLAM_B200_MASK_FROM_DEPTH)) {
-    set_error("nodes_create: bad arguments");
+  int rc;
+  if ((rc = check_nodes_args("nodes_create", det, nframes, K4, node_handles, flags))) return rc;
+  if (nframes > 0 && (!gray || !depth)) {
+    set_error("nodes_create: null image buffers");
     return RGBDSLAM_B200_ERR_ARG;
   }
   if (nframes == 0) return 0;
   State& s = g_state;
   const bool mask_from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
   if (mask_from_depth) mask = nullptr;
-  if ((rc = orb_prepare(w, h, nframes)) || (rc = orb_ensure_streams())) return rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const int chunk = std::min(nframes, kOrbChunk);
   if ((rc = orb_ensure_buffers(chunk, 2, mask != nullptr))) return rc;
   const size_t px = (size_t)w * h;
-  cudaStream_t st = s.stream, cs = o.copy_stream;
+  cudaStream_t st = s.stream;
   const int K = std::min(o.kp_stride, s.params.max_keypoints);  // features per node (finalize mode 1 emits <= max_keypoints)
-  const int Kpad = ((K > 0 ? K : 1) + 255) / 256 * 256;
-  // slab: [desc F x K x 32][xyz F x K x 16][kp F x K x 28][n F x 4]
-  const size_t b_desc = ((size_t)nframes * K * 32 + 255) / 256 * 256, b_xyz = ((size_t)nframes * K * 16 + 255) / 256 * 256;
-  const size_t b_kp = ((size_t)nframes * K * sizeof(rgbdslam_b200_keypoint) + 255) / 256 * 256;
-  const size_t b_n = ((size_t)nframes * 4 + 255) / 256 * 256;
-  NodeSlab* slab = new NodeSlab();
-  cudaError_t e = cudaMalloc(&slab->base, b_desc + b_xyz + b_kp + b_n);
-  if (e != cudaSuccess) {
-    delete slab;
-    return cuda_fail(e, "cudaMalloc(node slab)");
-  }
-  uint8_t* sl_desc = (uint8_t*)slab->base;
-  float4* sl_xyz = (float4*)(sl_desc + b_desc);
-  rgbdslam_b200_keypoint* sl_kp = (rgbdslam_b200_keypoint*)((uint8_t*)sl_xyz + b_xyz);
-  int* sl_n = (int*)((uint8_t*)sl_kp + b_kp);
-  auto fail = [&](int code) {
-    cudaStreamSynchronize(cs);
-    cudaStreamSynchronize(st);
-    cudaFree(slab->base);
-    delete slab;
-    return code;
-  };
-  const bool pinned = is_pinned(gray) && is_pinned(depth) && (!mask || is_pinned(mask));
-  const size_t stage_bytes = (px + px * 4 + (mask ? px : 0)) * chunk;
-  if (!pinned && ((rc = o.stage[0].ensure(stage_bytes)) || (rc = o.stage[1].ensure(stage_bytes)))) return fail(rc);
+  NodeBatch nb;
+  if ((rc = batch_alloc(nb, nframes, nframes, K))) return rc;
+  bool pinned = false;
+  if ((rc = setup_staging(gray, depth, mask, px, chunk, &pinned))) return batch_fail(nb, rc);
   // projectTo3D intrinsics (node.cpp:913-916): fxinv, fyinv as float(1./fx)
   const float4 Kinv = make_float4((float)(1. / (double)K4[0]), (float)(1. / (double)K4[1]), K4[2], K4[3]);
-  e = cudaMemsetAsync(o.err.ptr, 0, 4, st);
-  if (e != cudaSuccess) return fail(cuda_fail(e, "nodes_create"));
+  cudaError_t e = cudaMemsetAsync(o.err.ptr, 0, 4, st);
   // the copy stream must not run ahead of work already queued on the compute stream that still reads the input buffers
-  e = cudaEventRecord(o.ev_free[0], st);
+  if (e == cudaSuccess) e = cudaEventRecord(o.ev_free[0], st);
   if (e == cudaSuccess) e = cudaEventRecord(o.ev_free[1], st);
-  if (e != cudaSuccess) return fail(cuda_fail(e, "nodes_create events"));
+  if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "nodes_create setup"));
   int launches = 0, ci = 0;
-  std::vector<NodeDev*> made;
   for (int f0 = 0; f0 < nframes; f0 += chunk, ci++) {
     const int F = std::min(chunk, nframes - f0), b = ci & 1;
-    const uint8_t* hg = gray + px * f0;
-    const float* hd = depth + px * f0;
-    const uint8_t* hm = mask ? mask + px * f0 : nullptr;
-    if (!pinned) {  // stage through pinned memory (the previous copy out of this staging buffer must have finished)
-      if (ci >= 2 && (e = cudaEventSynchronize(o.ev_copied[b])) != cudaSuccess) return fail(cuda_fail(e, "staging wait"));
-      uint8_t* sp = (uint8_t*)o.stage[b].ptr;
-      memcpy(sp, hg, px * F);
-      memcpy(sp + px * chunk, hd, px * 4 * F);
-      if (hm) memcpy(sp + px * 5 * chunk, hm, px * F);
-      hg = sp;
-      hd = (const float*)(sp + px * chunk);
-      if (hm) hm = sp + px * 5 * chunk;
-    }
-    e = cudaStreamWaitEvent(cs, o.ev_free[b], 0);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(o.in_gray[b].ptr, hg, px * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(o.in_depth[b].ptr, hd, px * 4 * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess && hm) e = cudaMemcpyAsync(o.in_mask[b].ptr, hm, px * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess) e = cudaEventRecord(o.ev_ready[b], cs);
-    if (e == cudaSuccess) e = cudaEventRecord(o.ev_copied[b], cs);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(st, o.ev_ready[b], 0);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "frame upload"));
-    const uint8_t* dg = (const uint8_t*)o.in_gray[b].ptr;
-    const float* dd = (const float*)o.in_depth[b].ptr;
+    uint8_t* dg = (uint8_t*)o.in_gray[b].ptr;
+    float* dd = (float*)o.in_depth[b].ptr;
+    uint8_t* dm = mask ? (uint8_t*)o.in_mask[b].ptr : nullptr;
+    if ((rc = upload_chunk(ci, F, chunk, px, pinned, gray + px * f0, depth + px * f0, mask ? mask + px * f0 : nullptr, dg, dd, dm,
+                           o.ev_free[b])))
+      return batch_fail(nb, rc);
     if (f0 == 0) o.last_gray = dg;
-    if ((rc = orb_detect_stage(det, F, dg, hm ? (const uint8_t*)o.in_mask[b].ptr : nullptr, mask_from_depth ? dd : nullptr, st,
-                               &launches)))
-      return fail(rc);
+    if ((rc = orb_detect_stage(det, F, dg, dm, mask_from_depth ? dd : nullptr, st, &launches))) return batch_fail(nb, rc);
     e = orb_run_select(o.g, F, 1, o.max_per_cell, s.params.max_keypoints, (const uint8_t*)o.cell_img.ptr,
                        (const OrbCand*)o.cand.ptr, (const int*)o.cand_count.ptr, (const int*)o.thr.ptr, (float*)o.resp.ptr,
                        (unsigned long long*)o.cell_out.ptr, (int*)o.cell_out_count.ptr, dd, (float)s.params.depth_scaling_factor, Kinv,
-                       o.scratch.ptr, sl_kp + (size_t)f0 * K, sl_xyz + (size_t)f0 * K, (float2*)o.trig.ptr, sl_n + f0, K, st, &launches);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "orb select kernels"));
-    e = orb_run_describe(o.g, o.tab, F, dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, sl_kp + (size_t)f0 * K, sl_n + f0, K, K,
-                         (const float2*)o.trig.ptr, sl_desc + (size_t)f0 * K * 32, st, &launches);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "orb describe kernels"));
+                       o.scratch.ptr, nb.kp + (size_t)f0 * K, nb.xyz + (size_t)f0 * K, (float2*)o.trig.ptr, nb.n + f0, K, st, &launches);
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb select kernels"));
+    e = orb_run_describe(o.g, o.tab, F, dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, nb.kp + (size_t)f0 * K, nb.n + f0, K, K,
+                         (const float2*)o.trig.ptr, nb.desc + (size_t)f0 * K * 32, st, &launches);
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb describe kernels"));
     if (s.params.observability_threshold > 0.0) {  // Node::pc_col for the environment measurement model
       for (int f = 0; f < F; f++) {
-        NodeDev* nd = new NodeDev();
-        made.push_back(nd);
-        if ((rc = node_build_cloud(nd, dd + (size_t)f * px, w, h, K4, st))) {
-          for (NodeDev* x : made) { if (x->cloud_z) cudaFree(x->cloud_z); delete x; }
-          return fail(rc);
-        }
+        nb.made.push_back(new NodeDev());
+        if ((rc = node_build_cloud(nb.made.back(), dd + (size_t)f * px, w, h, K4, st))) return batch_fail(nb, rc);
       }
     }
     e = cudaEventRecord(o.ev_free[b], st);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "nodes_create events"));
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "nodes_create events"));
   }
-  std::vector<int> n(nframes);
-  int flag = 0;
-  e = cudaMemcpyAsync(n.data(), sl_n, 4 * (size_t)nframes, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&flag, o.err.ptr, 4, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-  if (e != cudaSuccess || (rc = orb_check_err_flag(flag))) {
-    for (NodeDev* x : made) { if (x->cloud_z) cudaFree(x->cloud_z); delete x; }
-    return fail(e != cudaSuccess ? cuda_fail(e, "nodes_create finish") : rc);
-  }
-  for (int f = 0; f < nframes; f++) {
-    NodeDev* nd = made.empty() ? new NodeDev() : made[f];
-    nd->magic = NodeDev::kMagic;
-    nd->id = ids ? ids[f] : f;
-    nd->n = n[f];
-    nd->n_pad = Kpad;
-    nd->desc = sl_desc + (size_t)f * K * 32;
-    nd->xyz = sl_xyz + (size_t)f * K;
-    nd->kp = sl_kp + (size_t)f * K;
-    nd->slab = slab;
-    slab->refs++;
-    node_handles[f] = (uint64_t)(uintptr_t)nd;
-    if (n_features) n_features[f] = n[f];
-  }
+  if ((rc = batch_publish(nb, nframes, 0, nframes, ids, node_handles, n_features, "nodes_create finish"))) return rc;
   s.launches += launches;
   return 0;
 }
@@ -605,15 +666,12 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
 int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
                                        const float* depth, const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids,
                                        int flags, uint64_t* node_handles, int32_t* n_features) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
-  Detector* det = get_detector(detector);
+  RB200_ENTER_INITED();
   Comm* cm = get_comm(comm_handle);
-  if (!det || !cm || total_frames < 0 || (total_frames > 0 && (!K4 || !node_handles)) || (flags & ~RGBDSLAM_B200_MASK_FROM_DEPTH)) {
-    set_error("nodes_create_sharded: bad arguments");
-    return RGBDSLAM_B200_ERR_ARG;
-  }
+  if (!cm) return RGBDSLAM_B200_ERR_ARG;
+  Detector* det = get_detector(detector);
+  int rc;
+  if ((rc = check_nodes_args("nodes_create_sharded", det, total_frames, K4, node_handles, flags))) return rc;
   if (total_frames == 0) return 0;
   State& s = g_state;
   if (s.params.observability_threshold > 0.0) {
@@ -630,7 +688,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   }
   const bool mask_from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
   if (mask_from_depth) mask = nullptr;
-  if ((rc = orb_prepare(w, h, own)) || (rc = orb_ensure_streams())) return rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
   const int chunk = std::max(1, std::min(own, kOrbChunk));
@@ -644,78 +702,40 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     return rc;
   cudaStream_t st = s.stream, cs = o.copy_stream;
   const int K = std::min(o.kp_stride, s.params.max_keypoints);
-  const int Kpad = ((K > 0 ? K : 1) + 255) / 256 * 256;
-  // slab: [desc Wp x K x 32][xyz Wp x K x 16][n Wp x 4][kp own x K x 28]
-  auto up = [](size_t v) { return (v + 255) / 256 * 256; };
-  const size_t b_desc = up((size_t)Wp * K * 32), b_xyz = up((size_t)Wp * K * 16), b_n = up((size_t)Wp * 4);
-  const size_t b_kp = up(own_ * K * sizeof(rgbdslam_b200_keypoint));
-  NodeSlab* slab = new NodeSlab();
-  cudaError_t e = cudaMalloc(&slab->base, b_desc + b_xyz + b_n + b_kp);
-  if (e != cudaSuccess) {
-    delete slab;
-    return cuda_fail(e, "cudaMalloc(node slab)");
-  }
-  uint8_t* sl_desc = (uint8_t*)slab->base;
-  float4* sl_xyz = (float4*)(sl_desc + b_desc);
-  int* sl_n = (int*)((uint8_t*)sl_xyz + b_xyz);
-  rgbdslam_b200_keypoint* sl_kp = (rgbdslam_b200_keypoint*)((uint8_t*)sl_n + b_n);
-  auto fail = [&](int code) {
-    cudaStreamSynchronize(cs);
-    cudaStreamSynchronize(st);
-    cudaFree(slab->base);
-    delete slab;
-    return code;
-  };
-  const bool pinned = own == 0 || (is_pinned(gray) && is_pinned(depth) && (!mask || is_pinned(mask)));
-  const size_t stage_bytes = (px + px * 4 + (mask ? px : 0)) * chunk;
-  if (!pinned && ((rc = o.stage[0].ensure(stage_bytes)) || (rc = o.stage[1].ensure(stage_bytes)))) return fail(rc);
+  NodeBatch nb;  // descriptors, points and counts of all Wp frames; 2-D keypoints of the own frames
+  if ((rc = batch_alloc(nb, Wp, (int)own_, K))) return rc;
+  bool pinned = true;
+  if (own > 0 && (rc = setup_staging(gray, depth, mask, px, chunk, &pinned))) return batch_fail(nb, rc);
   const float4 Kinv = make_float4((float)(1. / (double)K4[0]), (float)(1. / (double)K4[1]), K4[2], K4[3]);
   int* hist_all = (int*)o.all_hist.ptr;
   int* cnt_all = (int*)o.all_cnt.ptr;
   int* many_all = (int*)o.all_many.ptr;
   int* thr_all = (int*)o.all_thr.ptr;
-  e = cudaMemsetAsync(o.err.ptr, 0, 4, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(sl_n, 0, b_n, st);
+  cudaError_t e = cudaMemsetAsync(o.err.ptr, 0, 4, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(nb.n, 0, nb.n_bytes, st);
   // frames of the padding (Wp > total_frames) and of ranks without frames must read as "no candidates"
   if (e == cudaSuccess) e = cudaMemsetAsync(hist_all, 0, (size_t)Wp * nc * 256 * 4, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(cnt_all, 0, (size_t)Wp * nc * 4, st);
   if (e == cudaSuccess) e = cudaMemsetAsync(many_all, 0, (size_t)Wp * nc * 4, st);
   if (e == cudaSuccess) e = cudaEventRecord(o.ev_free[0], st);  // uploads start after everything queued so far
   if (e == cudaSuccess) e = cudaStreamWaitEvent(cs, o.ev_free[0], 0);
-  if (e != cudaSuccess) return fail(cuda_fail(e, "nodes_create_sharded setup"));
+  if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "nodes_create_sharded setup"));
   int launches = 0, ci = 0;
   // ---- pass A: upload + pyramids + FAST / NMS candidates + score histograms of the own frames
   for (int c0 = 0; c0 < own; c0 += chunk, ci++) {
-    const int F = std::min(chunk, own - c0), b = ci & 1;
-    const uint8_t* hg = gray + px * c0;
-    const float* hd = depth + px * c0;
-    const uint8_t* hm = mask ? mask + px * c0 : nullptr;
-    if (!pinned) {
-      if (ci >= 2 && (e = cudaEventSynchronize(o.ev_copied[b])) != cudaSuccess) return fail(cuda_fail(e, "staging wait"));
-      uint8_t* sp = (uint8_t*)o.stage[b].ptr;
-      memcpy(sp, hg, px * F);
-      memcpy(sp + px * chunk, hd, px * 4 * F);
-      if (hm) memcpy(sp + px * 5 * chunk, hm, px * F);
-      hg = sp;
-      hd = (const float*)(sp + px * chunk);
-      if (hm) hm = sp + px * 5 * chunk;
-    }
+    const int F = std::min(chunk, own - c0);
     uint8_t* dg = (uint8_t*)o.sh_gray.ptr + px * c0;
     float* dd = (float*)o.sh_depth.ptr + px * c0;
-    uint8_t* dm = hm ? (uint8_t*)o.sh_mask.ptr + px * c0 : nullptr;
-    e = cudaMemcpyAsync(dg, hg, px * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dd, hd, px * 4 * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess && hm) e = cudaMemcpyAsync(dm, hm, px * F, cudaMemcpyHostToDevice, cs);
-    if (e == cudaSuccess) e = cudaEventRecord(o.ev_ready[b], cs);
-    if (e == cudaSuccess) e = cudaEventRecord(o.ev_copied[b], cs);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(st, o.ev_ready[b], 0);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "frame upload"));
+    uint8_t* dm = mask ? (uint8_t*)o.sh_mask.ptr + px * c0 : nullptr;
+    if ((rc = upload_chunk(ci, F, chunk, px, pinned, gray + px * c0, depth + px * c0, mask ? mask + px * c0 : nullptr, dg, dd, dm,
+                           nullptr)))
+      return batch_fail(nb, rc);
     if (c0 == 0) o.last_gray = dg;
     const size_t gf = (size_t)(f0 + c0);  // global index of the chunk's first frame
     e = orb_run_detect(g, o.tab, F, dg, dm, mask_from_depth ? dd : nullptr, (uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0,
                        (uint8_t*)o.cell_mask.ptr, (uint8_t*)o.score.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
                        cnt_all + gf * nc, hist_all + gf * nc * 256, many_all + gf * nc, st, &launches);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "orb detect kernels"));
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb detect kernels"));
   }
   // ---- the exchange that makes the frames independent: every rank gets every frame's score histograms, replays the
   //      threshold recurrence of the whole sequence (feature_adjuster.cpp:131-150, 185-224) and keeps its own frames' thresholds
@@ -723,12 +743,12 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     ncclResult_t r = g_nccl.AllGather(hist_all + (size_t)rank * per * nc * 256, hist_all, (size_t)per * nc * 256 * 4, 0, cm->comm, st);
     if (r == 0) r = g_nccl.AllGather(cnt_all + (size_t)rank * per * nc, cnt_all, (size_t)per * nc * 4, 0, cm->comm, st);
     if (r == 0) r = g_nccl.AllGather(many_all + (size_t)rank * per * nc, many_all, (size_t)per * nc * 4, 0, cm->comm, st);
-    if (r != 0) return fail(nccl_fail(r, "ncclAllGather(histograms)"));
+    if (r != 0) return batch_fail(nb, nccl_fail(r, "ncclAllGather(histograms)"));
   }
-  if ((rc = detector_to_device(det, st))) return fail(rc);
+  if ((rc = detector_to_device(det, st))) return batch_fail(nb, rc);
   e = orb_run_adapt(g, total_frames, hist_all, cnt_all, many_all, (double*)det->d_state.ptr, thr_all, o.min_cell, o.max_cell,
                     s.params.adjuster_max_iterations, (int*)o.err.ptr, st, &launches);
-  if (e != cudaSuccess) return fail(cuda_fail(e, "orb threshold kernel"));
+  if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb threshold kernel"));
   det->host_valid = false;
   // ---- pass B: Harris / keepStrongest / finalize / describe of the own frames, straight into the slab
   for (int c0 = 0; c0 < own; c0 += chunk) {
@@ -739,42 +759,21 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     const uint8_t* cimg = (const uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0;
     e = orb_run_select(g, F, 1, o.max_per_cell, s.params.max_keypoints, cimg, (const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
                        cnt_all + gf * nc, thr_all + gf * nc, (float*)o.resp.ptr, (unsigned long long*)o.cell_out.ptr,
-                       (int*)o.cell_out_count.ptr, dd, (float)s.params.depth_scaling_factor, Kinv, o.scratch.ptr, sl_kp + (size_t)c0 * K,
-                       sl_xyz + gf * K, (float2*)o.trig.ptr, sl_n + gf, K, st, &launches);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "orb select kernels"));
-    e = orb_run_describe(g, o.tab, F, dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, sl_kp + (size_t)c0 * K, sl_n + gf, K, K,
-                         (const float2*)o.trig.ptr, sl_desc + gf * K * 32, st, &launches);
-    if (e != cudaSuccess) return fail(cuda_fail(e, "orb describe kernels"));
+                       (int*)o.cell_out_count.ptr, dd, (float)s.params.depth_scaling_factor, Kinv, o.scratch.ptr, nb.kp + (size_t)c0 * K,
+                       nb.xyz + gf * K, (float2*)o.trig.ptr, nb.n + gf, K, st, &launches);
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb select kernels"));
+    e = orb_run_describe(g, o.tab, F, dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, nb.kp + (size_t)c0 * K, nb.n + gf, K, K,
+                         (const float2*)o.trig.ptr, nb.desc + gf * K * 32, st, &launches);
+    if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb describe kernels"));
   }
   // ---- every rank gets every node's features (48 KB per 1000-keypoint frame over NVLink)
   if (world > 1) {
-    ncclResult_t r = g_nccl.AllGather(sl_desc + (size_t)rank * per * K * 32, sl_desc, (size_t)per * K * 32, 0, cm->comm, st);
-    if (r == 0) r = g_nccl.AllGather((uint8_t*)(sl_xyz + (size_t)rank * per * K), sl_xyz, (size_t)per * K * 16, 0, cm->comm, st);
-    if (r == 0) r = g_nccl.AllGather((uint8_t*)(sl_n + (size_t)rank * per), sl_n, (size_t)per * 4, 0, cm->comm, st);
-    if (r != 0) return fail(nccl_fail(r, "ncclAllGather(features)"));
+    ncclResult_t r = g_nccl.AllGather(nb.desc + (size_t)rank * per * K * 32, nb.desc, (size_t)per * K * 32, 0, cm->comm, st);
+    if (r == 0) r = g_nccl.AllGather((uint8_t*)(nb.xyz + (size_t)rank * per * K), nb.xyz, (size_t)per * K * 16, 0, cm->comm, st);
+    if (r == 0) r = g_nccl.AllGather((uint8_t*)(nb.n + (size_t)rank * per), nb.n, (size_t)per * 4, 0, cm->comm, st);
+    if (r != 0) return batch_fail(nb, nccl_fail(r, "ncclAllGather(features)"));
   }
-  std::vector<int> n(total_frames);
-  int flag = 0;
-  e = cudaMemcpyAsync(n.data(), sl_n, 4 * (size_t)total_frames, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&flag, o.err.ptr, 4, cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(cs);
-  if (e != cudaSuccess) return fail(cuda_fail(e, "nodes_create_sharded finish"));
-  if ((rc = orb_check_err_flag(flag))) return fail(rc);
-  for (int f = 0; f < total_frames; f++) {
-    NodeDev* nd = new NodeDev();
-    nd->magic = NodeDev::kMagic;
-    nd->id = ids ? ids[f] : f;
-    nd->n = n[f];
-    nd->n_pad = Kpad;
-    nd->desc = sl_desc + (size_t)f * K * 32;
-    nd->xyz = sl_xyz + (size_t)f * K;
-    nd->kp = (f >= f0 && f < f1) ? sl_kp + (size_t)(f - f0) * K : nullptr;  // 2-D keypoints stay on the rank that built the node
-    nd->slab = slab;
-    slab->refs++;
-    node_handles[f] = (uint64_t)(uintptr_t)nd;
-    if (n_features) n_features[f] = n[f];
-  }
+  if ((rc = batch_publish(nb, total_frames, f0, own, ids, node_handles, n_features, "nodes_create_sharded finish"))) return rc;
   s.launches += launches;
   return 0;
 }
@@ -788,9 +787,7 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * frame 0 of the last detect / nodes_create call: 8-byte records {u16 x, u16 y, u8 level, u8 score, u16 0} and their
  * Harris responses (NaN = below the cell's final threshold). */
 int rgbdslam_b200_orb_debug_candidates(int cell, void* cand_out, float* resp_out, int capacity, int* n_out, int* thr_out) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   OrbCtx& o = g_orb;
   if (!o.ready || cell < 0 || cell >= o.g.ncells || !n_out) {
     set_error("orb_debug_candidates: no detection has run / bad cell");
@@ -819,15 +816,15 @@ int rgbdslam_b200_orb_debug_detect_path(int unfused) {
 }
 
 int rgbdslam_b200_orb_debug_plane(int which, int cell, int level, uint8_t* out, int capacity, int* w_out, int* h_out) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   OrbCtx& o = g_orb;
-  if (!o.ready || level < 0 || level >= kOrbLevels || !w_out || !h_out) return RGBDSLAM_B200_ERR_ARG;
+  if (!o.ready || level < 0 || level >= kOrbLevels || !w_out || !h_out || (which <= 2 && (cell < 0 || cell >= o.g.ncells))) {
+    set_error("orb_debug_plane: no detection has run / bad level or cell");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
   const OrbPlane* p;
   const uint8_t* base;
   if (which <= 2) {
-    if (cell < 0 || cell >= o.g.ncells) return RGBDSLAM_B200_ERR_ARG;
     p = &o.g.cell[cell][level];
     base = (const uint8_t*)(which == 0 ? o.cell_img.ptr : which == 1 ? o.cell_mask.ptr : o.score.ptr);
   } else {
@@ -845,12 +842,11 @@ int rgbdslam_b200_orb_debug_plane(int which, int cell, int level, uint8_t* out, 
 }
 
 int rgbdslam_b200_node_download_keypoints(uint64_t node_handle, rgbdslam_b200_keypoint* kp_out) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
-  NodeDev* nd = (NodeDev*)(uintptr_t)node_handle;
-  if (!nd || nd->magic != NodeDev::kMagic || !kp_out) {
-    set_error("node_download_keypoints: bad arguments");
+  RB200_ENTER_INITED();
+  NodeDev* nd = get_node(node_handle);
+  if (!nd) return RGBDSLAM_B200_ERR_ARG;
+  if (!kp_out) {
+    set_error("node_download_keypoints: null output");
     return RGBDSLAM_B200_ERR_ARG;
   }
   if (!nd->kp) {

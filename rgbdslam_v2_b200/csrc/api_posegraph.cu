@@ -13,9 +13,7 @@ extern "C" {
 int rgbdslam_b200_posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, const int32_t* ij,
                                      const double* meas, const double* info, double stop, double huber_delta,
                                      double* chi2, int* iters, int* cg_iters) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   if (nv <= 0 || ne < 0 || !poses || !fixed || (ne > 0 && (!ij || !meas || !info)) || !(stop > 0) || !(huber_delta > 0)) {
     set_error("posegraph_optimize: bad arguments (nv > 0, stop > 0, huber_delta > 0)");
     return RGBDSLAM_B200_ERR_ARG;
@@ -29,9 +27,7 @@ int rgbdslam_b200_posegraph_optimize(int nv, double* poses, const uint8_t* fixed
 }
 
 int rgbdslam_b200_posegraph_reserve(int nv, int ne) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   if (nv < 0 || ne < 0) {
     set_error("posegraph_reserve: negative size");
     return RGBDSLAM_B200_ERR_ARG;
@@ -41,9 +37,7 @@ int rgbdslam_b200_posegraph_reserve(int nv, int ne) {
 
 int rgbdslam_b200_posegraph_chi2(int nv, const double* poses, int ne, const int32_t* ij, const double* meas,
                                  const double* info, double huber_delta, double* chi2, double* per_edge_chi2) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   if (nv <= 0 || ne < 0 || !poses || (ne > 0 && (!ij || !meas || !info)) || !(huber_delta > 0)) {
     set_error("posegraph_chi2: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
@@ -58,9 +52,7 @@ int rgbdslam_b200_landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, 
                               const double* K4, int n_edges, const int32_t* ij, const double* meas7, const double* info36,
                               int iterations, double huber_delta, double* chi2_before, double* chi2_after, int* lm_iterations,
                               int* pcg_iterations) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  int rc = check_inited();
-  if (rc) return rc;
+  RB200_ENTER_INITED();
   if (n_cams <= 0 || n_points < 0 || n_obs < 0 || n_edges < 0 || iterations < 0 || !poses7 || !fixed || !K4 ||
       (n_points > 0 && !points3) || (n_obs > 0 && (!obs_cam || !obs_point || !obs_uvd || !obs_info3)) ||
       (n_edges > 0 && (!ij || !meas7 || !info36)) || !(huber_delta > 0)) {

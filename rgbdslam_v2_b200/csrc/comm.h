@@ -32,9 +32,6 @@ struct Comm {
 
 int load_nccl();
 int nccl_fail(ncclResult_t r, const char* what);
-inline Comm* get_comm(uint64_t h) {
-  Comm* c = (Comm*)(uintptr_t)h;
-  return (c && c->magic == Comm::kMagic) ? c : nullptr;
-}
+Comm* get_comm(uint64_t h);  // nullptr (and last_error set) unless h is a live communicator handle
 
 }  // namespace rb200

@@ -431,12 +431,6 @@ int landmark_ba_release() {
   return 0;
 }
 
-#define BA_CUDA(call)                                     \
-  do {                                                    \
-    cudaError_t e__ = (call);                             \
-    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
-  } while (0)
-
 struct BaProblem {
   int nc, np, no, ne;
   double K[4], delta;
@@ -453,17 +447,17 @@ static int ba_chi2(BaProblem& P, const double* poses, const double* pts, double*
     ba_chi2_obs_kernel<<<nb, 256, 0, P.st>>>(P.no, poses, pts, (const int*)d.obs_cam.ptr, (const int*)d.obs_pt.ptr,
                                              (const double*)d.uvd.ptr, (const double*)d.w3.ptr, P.K[0], P.K[1], P.K[2], P.K[3],
                                              (double*)d.chipart.ptr);
-    BA_CUDA(cudaGetLastError());
+    RB200_CUDA(cudaGetLastError());
     P.launches++;
   }
   if (P.ne > 0) {
-    BA_CUDA(pg_launch_chi2(P.ne, poses, (const int32_t*)d.ij.ptr, (const double*)d.meas.ptr, (const double*)d.info.ptr, P.delta,
+    RB200_CUDA(pg_launch_chi2(P.ne, poses, (const int32_t*)d.ij.ptr, (const double*)d.meas.ptr, (const double*)d.info.ptr, P.delta,
                            (double*)d.chipart.ptr + nb, P.st));
     P.launches++;
   }
   std::vector<double> part(nb + 2 * (size_t)neb);
-  BA_CUDA(cudaMemcpyAsync(part.data(), d.chipart.ptr, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, P.st));
-  BA_CUDA(cudaStreamSynchronize(P.st));
+  RB200_CUDA(cudaMemcpyAsync(part.data(), d.chipart.ptr, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, P.st));
+  RB200_CUDA(cudaStreamSynchronize(P.st));
   double s = 0;
   for (int i = 0; i < nb; i++) s += part[i];
   for (int i = 0; i < neb; i++) s += part[nb + 2 * i];  // robust chi2 of the pose edges (activeRobustChi2)
@@ -481,12 +475,12 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
     ba_linearize_kernel<<<(P.no + 127) / 128, 128, 0, P.st>>>(P.no, (const double*)d.poses.ptr, (const double*)d.pts.ptr, (const int*)d.obs_cam.ptr,
                                                             (const int*)d.obs_pt.ptr, (const double*)d.uvd.ptr, (const double*)d.w3.ptr, P.K[0],
                                                             P.K[1], P.K[2], P.K[3], (double*)d.blk.ptr);
-  if (cudaGetLastError() != cudaSuccess) return -RGBDSLAM_B200_ERR_CUDA;
+  if (cudaError_t e = cudaGetLastError()) return -cuda_fail(e, "ba_linearize_kernel");
   P.launches++;
   if (P.ne > 0) {
     if (pg_launch_linearize(P.ne, (const double*)d.poses.ptr, (const int32_t*)d.ij.ptr, (const double*)d.meas.ptr, (const double*)d.info.ptr,
                             P.delta, (double*)d.eblk.ptr, P.st) != cudaSuccess)
-      return -RGBDSLAM_B200_ERR_CUDA;
+      return -cuda_fail(cudaGetLastError(), "pg_launch_linearize");
     P.launches++;
   }
   auto assemble = [&](double lam) -> int {
@@ -499,7 +493,8 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
                                           (const double*)d.bp.ptr, (double*)d.Hcc.ptr, (double*)d.bc.ptr, (double*)d.g.ptr,
                                           (double*)d.Minv.ptr, (double*)d.maxd_c.ptr);
     P.launches += 2;
-    return cudaGetLastError() == cudaSuccess ? 0 : RGBDSLAM_B200_ERR_CUDA;
+    RB200_CUDA(cudaGetLastError());
+    return 0;
   };
   if (iteration == 0) {  // computeLambdaInit: tau * max diag(H)
     if ((rc = assemble(0.0))) return -rc;
@@ -507,7 +502,7 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
     if (cudaMemcpyAsync(mc.data(), d.maxd_c.ptr, 8 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
         cudaMemcpyAsync(mp.data(), d.maxd_p.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
         cudaStreamSynchronize(P.st) != cudaSuccess)
-      return -RGBDSLAM_B200_ERR_CUDA;
+      return -cuda_fail(cudaGetLastError(), "landmark_ba lambda init download");
     double m = 0;
     for (double v : mc) m = v > m ? v : m;
     for (double v : mp) m = v > m ? v : m;
@@ -544,7 +539,7 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
       it += burst;
       if (cudaMemcpyAsync(st4, d.state.ptr, sizeof(st4), cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
           cudaStreamSynchronize(P.st) != cudaSuccess)
-        return -RGBDSLAM_B200_ERR_CUDA;
+        return -cuda_fail(cudaGetLastError(), "landmark_ba PCG state download");
       if (st4[2] != 0.0) break;
     }
     P.pcg_iters += (int)st4[1];
@@ -557,14 +552,14 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
                                                (double*)d.scpart.ptr);
     if (pg_launch_update(P.nc, (const double*)d.poses.ptr, (const double*)d.x.ptr, (const uint8_t*)d.fixed.ptr, (double*)d.poses_trial.ptr,
                          P.st) != cudaSuccess)
-      return -RGBDSLAM_B200_ERR_CUDA;
+      return -cuda_fail(cudaGetLastError(), "pg_launch_update");
     P.launches += 2;
     std::vector<double> sp(npb), xc(6 * (size_t)P.nc), bcv(6 * (size_t)P.nc);
     if (cudaMemcpyAsync(sp.data(), d.scpart.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
         cudaMemcpyAsync(xc.data(), d.x.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
         cudaMemcpyAsync(bcv.data(), d.bc.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
         cudaStreamSynchronize(P.st) != cudaSuccess)
-      return -RGBDSLAM_B200_ERR_CUDA;
+      return -cuda_fail(cudaGetLastError(), "landmark_ba gain ratio download");
     double scale = 0;
     for (double v : sp) scale += v;
     for (size_t i = 0; i < xc.size(); i++) scale += xc[i] * (lambda * xc[i] + bcv[i]);
@@ -661,28 +656,28 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
       (rc = d.e_oth.ensure(8 * ne)) || (rc = d.scpart.ensure(8 * (size_t)(npb + 1))))
     return rc;
   cudaStream_t st = P.st;
-  BA_CUDA(cudaMemcpyAsync(d.poses.ptr, poses7, 56 * nc, cudaMemcpyHostToDevice, st));
-  BA_CUDA(cudaMemcpyAsync(d.pts.ptr, points3, 24 * np, cudaMemcpyHostToDevice, st));
-  BA_CUDA(cudaMemcpyAsync(d.fixed.ptr, fixed, nc, cudaMemcpyHostToDevice, st));
-  BA_CUDA(cudaMemcpyAsync(d.pt_off.ptr, pt_off.data(), 4 * (np + 1), cudaMemcpyHostToDevice, st));
-  BA_CUDA(cudaMemcpyAsync(d.cam_off.ptr, cam_off.data(), 4 * (nc + 1), cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.poses.ptr, poses7, 56 * nc, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.pts.ptr, points3, 24 * np, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.fixed.ptr, fixed, nc, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.pt_off.ptr, pt_off.data(), 4 * (np + 1), cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.cam_off.ptr, cam_off.data(), 4 * (nc + 1), cudaMemcpyHostToDevice, st));
   if (n_obs > 0) {
-    BA_CUDA(cudaMemcpyAsync(d.obs_cam.ptr, obs_cam, 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.obs_pt.ptr, obs_point, 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.uvd.ptr, obs_uvd, 24 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.w3.ptr, obs_info3, 24 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.pt_obs.ptr, pt_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.cam_obs.ptr, cam_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.obs_cam.ptr, obs_cam, 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.obs_pt.ptr, obs_point, 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.uvd.ptr, obs_uvd, 24 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.w3.ptr, obs_info3, 24 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.pt_obs.ptr, pt_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.cam_obs.ptr, cam_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
   }
   if (n_edges > 0) {
-    BA_CUDA(cudaMemcpyAsync(d.ij.ptr, ij, 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.meas.ptr, meas7, 56 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.info.ptr, info36, 288 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.e_off.ptr, e_off.data(), 4 * (nc + 1), cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.e_inc.ptr, e_inc.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    BA_CUDA(cudaMemcpyAsync(d.e_oth.ptr, e_oth.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.ij.ptr, ij, 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.meas.ptr, meas7, 56 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.info.ptr, info36, 288 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.e_off.ptr, e_off.data(), 4 * (nc + 1), cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.e_inc.ptr, e_inc.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.e_oth.ptr, e_oth.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
   }
-  BA_CUDA(cudaStreamSynchronize(st));
+  RB200_CUDA(cudaStreamSynchronize(st));
   double chi2 = 0;
   if ((rc = ba_chi2(P, (const double*)d.poses.ptr, (const double*)d.pts.ptr, &chi2))) return rc;
   if (chi2_before) *chi2_before = chi2;
@@ -694,9 +689,9 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
     done++;
     if (r == 0) break;
   }
-  BA_CUDA(cudaMemcpyAsync(poses7, d.poses.ptr, 56 * nc, cudaMemcpyDeviceToHost, st));
-  BA_CUDA(cudaMemcpyAsync(points3, d.pts.ptr, 24 * np, cudaMemcpyDeviceToHost, st));
-  BA_CUDA(cudaStreamSynchronize(st));
+  RB200_CUDA(cudaMemcpyAsync(poses7, d.poses.ptr, 56 * nc, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaMemcpyAsync(points3, d.pts.ptr, 24 * np, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
   if (chi2_after) *chi2_after = chi2;
   if (lm_iterations) *lm_iterations = done;
   if (pcg_iterations) *pcg_iterations = P.pcg_iters;

@@ -755,12 +755,6 @@ struct PgDevice {
   }
 };
 
-#define PG_CUDA(call)                                   \
-  do {                                                  \
-    cudaError_t e__ = (call);                           \
-    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
-  } while (0)
-
 // The solver's device buffers live for the lifetime of the library (grow-only): a cudaMalloc / cudaFree pair per buffer and call
 // costs far more than the solve itself once the process holds gigabytes of pinned memory (measured: ~200 ms of cudaFree per call
 // in the 2000-frame sequence run against 30 ms inside the PCG kernels).  Guarded by the state mutex like every entry point.
@@ -793,11 +787,11 @@ static int pg_errors(PgCtx& c, const double* dx_poses, double* robust, double* p
   }
   pg_chi2_kernel<<<nb, 256, 0, c.st>>>(c.ne, dx_poses, (const int2*)c.dev.ij.ptr, (const double*)c.dev.meas.ptr,
                                        (const double*)c.dev.info.ptr, c.delta, (double*)c.dev.chipart.ptr, per_edge);
-  PG_CUDA(cudaGetLastError());
+  RB200_CUDA(cudaGetLastError());
   c.launches++;
   std::vector<double> part(2 * (size_t)nb);
-  PG_CUDA(cudaMemcpyAsync(part.data(), c.dev.chipart.ptr, sizeof(double) * 2 * nb, cudaMemcpyDeviceToHost, c.st));
-  PG_CUDA(cudaStreamSynchronize(c.st));
+  RB200_CUDA(cudaMemcpyAsync(part.data(), c.dev.chipart.ptr, sizeof(double) * 2 * nb, cudaMemcpyDeviceToHost, c.st));
+  RB200_CUDA(cudaStreamSynchronize(c.st));
   double r = 0, p = 0;
   for (int i = 0; i < nb; i++) {
     r += part[2 * i];
@@ -813,26 +807,26 @@ static int pg_build(PgCtx& c, double* maxdiag) {
     pg_linearize_kernel<<<(c.ne + 127) / 128, 128, 0, c.st>>>(c.ne, (const double*)c.dev.x.ptr, (const int2*)c.dev.ij.ptr,
                                                                (const double*)c.dev.meas.ptr, (const double*)c.dev.info.ptr,
                                                                c.delta, (double*)c.dev.blk.ptr);
-    PG_CUDA(cudaGetLastError());
+    RB200_CUDA(cudaGetLastError());
     c.launches++;
   }
   const int nb = (c.nv + 2) / 3;
   pg_assemble_kernel<<<nb, 128, 0, c.st>>>(c.nv, (const int*)c.dev.off.ptr, (const int*)c.dev.inc.ptr,
                                            (const uint8_t*)c.dev.fixed.ptr, (const double*)c.dev.blk.ptr,
                                            (double*)c.dev.Hd.ptr, (double*)c.dev.b.ptr, (double*)c.dev.maxpart.ptr);
-  PG_CUDA(cudaGetLastError());
+  RB200_CUDA(cudaGetLastError());
   c.launches++;
   if (c.res_vpc > 0 && c.ne > 0) {
     pg_orient_kernel<<<(c.nv + 3) / 4, 128, 0, c.st>>>(c.nv, (const int*)c.dev.off.ptr, (const int*)c.dev.inc.ptr,
                                                        (const int*)c.dev.oth.ptr, (const double*)c.dev.blk.ptr,
                                                        (double*)c.dev.incblk.ptr);
-    PG_CUDA(cudaGetLastError());
+    RB200_CUDA(cudaGetLastError());
     c.launches++;
   }
   if (maxdiag) {
     std::vector<double> part(nb);
-    PG_CUDA(cudaMemcpyAsync(part.data(), c.dev.maxpart.ptr, sizeof(double) * nb, cudaMemcpyDeviceToHost, c.st));
-    PG_CUDA(cudaStreamSynchronize(c.st));
+    RB200_CUDA(cudaMemcpyAsync(part.data(), c.dev.maxpart.ptr, sizeof(double) * nb, cudaMemcpyDeviceToHost, c.st));
+    RB200_CUDA(cudaStreamSynchronize(c.st));
     double m = 0;
     for (double v : part) m = v > m ? v : m;
     *maxdiag = m;
@@ -866,21 +860,21 @@ static int pg_pcg(PgCtx& c, double lambda, double* scale, bool* ok) {
   void* args[] = {&a};
   const auto t0 = std::chrono::steady_clock::now();
   pg_precond_kernel<<<(c.nv + 127) / 128, 128, 0, c.st>>>(c.nv, a.Hd, a.fixed, lambda, a.Minv);
-  PG_CUDA(cudaGetLastError());
+  RB200_CUDA(cudaGetLastError());
   c.launches++;
   if (c.res_vpc > 0) {
-    PG_CUDA(cudaMemsetAsync(c.dev.part.ptr, 0xFF, 8 * (size_t)kPgBarrierDoubles, c.st));  // barrier slots: parity 1
+    RB200_CUDA(cudaMemsetAsync(c.dev.part.ptr, 0xFF, 8 * (size_t)kPgBarrierDoubles, c.st));  // barrier slots: parity 1
     const double* incblk = (const double*)c.dev.incblk.ptr;
     void* rargs[] = {&a, &incblk, &c.res_vpc, &c.res_cap};
-    PG_CUDA(cudaLaunchCooperativeKernel((void*)pg_pcg_resident_kernel, dim3(c.pcg_grid), dim3(kPgResWarps * 32), rargs,
+    RB200_CUDA(cudaLaunchCooperativeKernel((void*)pg_pcg_resident_kernel, dim3(c.pcg_grid), dim3(kPgResWarps * 32), rargs,
                                         (size_t)c.res_smem, c.st));
   } else {
-    PG_CUDA(cudaLaunchCooperativeKernel((void*)pg_pcg_kernel, dim3(c.pcg_grid), dim3(512), args, 0, c.st));
+    RB200_CUDA(cudaLaunchCooperativeKernel((void*)pg_pcg_kernel, dim3(c.pcg_grid), dim3(512), args, 0, c.st));
   }
   c.launches++;
   double res[10];
-  PG_CUDA(cudaMemcpyAsync(res, c.dev.result.ptr, sizeof(res), cudaMemcpyDeviceToHost, c.st));
-  PG_CUDA(cudaStreamSynchronize(c.st));
+  RB200_CUDA(cudaMemcpyAsync(res, c.dev.result.ptr, sizeof(res), cudaMemcpyDeviceToHost, c.st));
+  RB200_CUDA(cudaStreamSynchronize(c.st));
 #ifdef RB200_PG_PROFILE
   if (c.res_vpc > 0 && res[0] > 0)
     fprintf(stderr, "[pcg profile] %d iterations, cycles per iteration: spmv %.0f, block sums %.0f, fence+store %.0f, wait d.q %.0f, phase 1 %.0f, wait r.s %.0f\n",
@@ -912,7 +906,7 @@ static int pg_lm_solve(PgCtx& c, int iteration, double& lambda, double& ni) {
     if ((rc = pg_pcg(c, lambda, &scale, &ok2))) return -rc;
     pg_update_kernel<<<(c.nv + 127) / 128, 128, 0, c.st>>>(c.nv, (const double*)c.dev.x.ptr, (const double*)c.dev.dx.ptr,
                                                            (const uint8_t*)c.dev.fixed.ptr, (double*)c.dev.xtrial.ptr);
-    if (cudaGetLastError() != cudaSuccess) return -RGBDSLAM_B200_ERR_CUDA;
+    if (cudaError_t e = cudaGetLastError()) return -cuda_fail(e, "pg_update_kernel");
     c.launches++;
     double temp;
     if ((rc = pg_errors(c, (const double*)c.dev.xtrial.ptr, &temp, &plain, nullptr))) return -rc;
@@ -1008,7 +1002,7 @@ int posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, cons
   if ((rc = pg_ensure(d, nv, ne))) return rc;
   // cooperative grid: all co-resident blocks of the PCG kernel
   int per_sm = 0;
-  PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pg_pcg_kernel, 512, 0));
+  RB200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pg_pcg_kernel, 512, 0));
   if (per_sm < 1) {
     set_error("posegraph: PCG kernel cannot be made resident");
     return RGBDSLAM_B200_ERR_CUDA;
@@ -1031,28 +1025,28 @@ int posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, cons
       c.res_smem = (c.res_smem + 15) & ~15;
       static int attr_bytes = 0;
       if (c.res_smem > attr_bytes) {
-        PG_CUDA(cudaFuncSetAttribute(pg_pcg_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024 + 16));
+        RB200_CUDA(cudaFuncSetAttribute(pg_pcg_resident_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024 + 16));
         attr_bytes = 200 * 1024 + 16;
       }
       int per_sm_res = 0;
-      PG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_res, pg_pcg_resident_kernel, kPgResWarps * 32, (size_t)c.res_smem));
+      RB200_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_res, pg_pcg_resident_kernel, kPgResWarps * 32, (size_t)c.res_smem));
       if (per_sm_res >= 1) {
         c.res_vpc = vpc;
       }
     }
   }
   cudaStream_t st = c.st;
-  PG_CUDA(cudaMemcpyAsync(d.x.ptr, poses, 56 * (size_t)nv, cudaMemcpyHostToDevice, st));
-  PG_CUDA(cudaMemcpyAsync(d.fixed.ptr, fixed, (size_t)nv, cudaMemcpyHostToDevice, st));
-  PG_CUDA(cudaMemcpyAsync(d.off.ptr, off.data(), 4 * (size_t)(nv + 1), cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.x.ptr, poses, 56 * (size_t)nv, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.fixed.ptr, fixed, (size_t)nv, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(d.off.ptr, off.data(), 4 * (size_t)(nv + 1), cudaMemcpyHostToDevice, st));
   if (ne > 0) {
-    PG_CUDA(cudaMemcpyAsync(d.meas.ptr, meas, 56 * (size_t)ne, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d.info.ptr, info, 288 * (size_t)ne, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d.ij.ptr, ij, 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d.inc.ptr, inc.data(), 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
-    PG_CUDA(cudaMemcpyAsync(d.oth.ptr, oth.data(), 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.meas.ptr, meas, 56 * (size_t)ne, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.info.ptr, info, 288 * (size_t)ne, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.ij.ptr, ij, 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.inc.ptr, inc.data(), 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
+    RB200_CUDA(cudaMemcpyAsync(d.oth.ptr, oth.data(), 8 * (size_t)ne, cudaMemcpyHostToDevice, st));
   }
-  PG_CUDA(cudaStreamSynchronize(st));  // host vectors (off/inc) go out of scope safely
+  RB200_CUDA(cudaStreamSynchronize(st));  // host vectors (off/inc) go out of scope safely
 
   int it = 0;
   double chi2 = DBL_MAX, robust = 0;
@@ -1076,13 +1070,13 @@ int posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, cons
         if ((rc = pg_errors(c, (const double*)d.x.ptr, &robust, &chi2, per_edge_chi2 ? (double*)d.per_edge.ptr : nullptr))) return rc;
       } while (chi2 / prev < (1.0 - stop));
     }
-    PG_CUDA(cudaMemcpyAsync(poses, d.x.ptr, 56 * (size_t)nv, cudaMemcpyDeviceToHost, st));
+    RB200_CUDA(cudaMemcpyAsync(poses, d.x.ptr, 56 * (size_t)nv, cudaMemcpyDeviceToHost, st));
   } else {
     if ((rc = pg_errors(c, (const double*)d.x.ptr, &robust, &chi2, per_edge_chi2 ? (double*)d.per_edge.ptr : nullptr))) return rc;
   }
   if (per_edge_chi2 && ne > 0)
-    PG_CUDA(cudaMemcpyAsync(per_edge_chi2, d.per_edge.ptr, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st));
-  PG_CUDA(cudaStreamSynchronize(st));
+    RB200_CUDA(cudaMemcpyAsync(per_edge_chi2, d.per_edge.ptr, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
   if (getenv("RB200_PG_TIMING"))
     fprintf(stderr, "[posegraph] nv %d ne %d optimize %d: total %.3f ms, pcg launches %.3f ms (%d pcg iterations, grid %d), lm %d\n", nv, ne,
             (int)optimize, 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count(), 1e3 * c.pcg_seconds,

@@ -52,21 +52,34 @@ struct NodeDev {
 
 constexpr int kSlots = 8;  // independent in-flight match_pairs pipelines (stream + workspace each)
 
+// The timing events of a slot, in the order a match_pairs* call records them on the slot's stream.
+enum SlotEvent {
+  kEvSubmit,       // host-feature calls: before the feature uploads
+  kEvUploaded,     // host-feature calls: feature uploads queued
+  kEvTables,       // pair table and work items uploaded: the device part of the call starts
+  kEvMatchBegin,   // match kernel (Hamming / L2 / SiftGPU) start
+  kEvMatchEnd,     // match kernel end
+  kEvStagesEnd,    // match selection, RANSAC and the optional refinement / EMM done
+  kEvDownloaded,   // result downloads done
+  kEvGatherDep,    // rgbdslam_b200_allgather_slot_edges: everything the slot had queued
+  kSlotEvents
+};
+
 struct Workspace {
-  cudaStream_t stream = nullptr;  // slot 0: the library / user stream; slots 1..: own non-blocking streams
-  cudaEvent_t ev[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaStream_t stream = nullptr;  // slot 0: State::stream (set by init / set_stream); slots 1..: own non-blocking streams
+  cudaEvent_t ev[kSlotEvents] = {};
   bool timing_valid = false;
-  bool host_path = false;  // last call uploaded host features (ev[4], ev[5] valid)
+  bool host_path = false;  // last call uploaded host features (kEvSubmit, kEvUploaded valid)
   bool pending = false;
   cudaEvent_t ev_gather = nullptr;  // rgbdslam_b200_allgather_slot_edges: the slot's collective + download have finished
   bool gather_pending = false;
   DevBuf d_pairs, d_best, d_matches, d_inliers, d_mfrom, d_mto, d_nall, d_hyp, d_results;
   DevBuf d_feat_a, d_feat_b, d_xyz_a, d_xyz_b;
-  DevBuf d_i8_a, d_i8_b, d_jobs, d_items, d_top4, d_knn, d_cen, d_nextn;
+  DevBuf d_jobs, d_items, d_top4, d_knn, d_cen, d_nextn;
   PinBuf h_pairs, h_jobs, h_items;
   void release() {
     DevBuf* all[] = {&d_pairs, &d_best, &d_matches, &d_inliers, &d_mfrom, &d_mto, &d_nall, &d_hyp, &d_results, &d_feat_a,
-                     &d_feat_b, &d_xyz_a, &d_xyz_b, &d_i8_a, &d_i8_b, &d_jobs, &d_items, &d_top4, &d_knn, &d_cen, &d_nextn};
+                     &d_feat_b, &d_xyz_a, &d_xyz_b, &d_jobs, &d_items, &d_top4, &d_knn, &d_cen, &d_nextn};
     for (DevBuf* b : all) b->release();
     h_pairs.release();
     h_jobs.release();
@@ -87,14 +100,12 @@ struct State {
   int64_t launches = 0;
   int comm_count = 0;  // live NCCL communicators (rgbdslam_b200_comm_init)
   Workspace ws[kSlots];
-  Workspace* cur = &ws[0];
-  Workspace& W() { return *cur; }
-  DevBuf d_f32_a, d_f32_b, d_root_a, d_root_b, d_norm_a, d_norm_b;  // SIFT staging of the synchronous calls
+  DevBuf d_f32_a, d_f32_b, d_root_a, d_root_b, d_norm_a, d_norm_b, d_i8_a, d_i8_b;  // SIFT staging of the synchronous calls
   int sift_matcher = 0;  // float-descriptor nodes created from now on: 0 = exact 2-NN ratio matcher (FLANN branch), 1 = SiftGPU matcher
   int hamming_path = 1;  // 1 = wgmma int8 GEMM, operands expanded inside the kernel (default); 0 = SIMT popcount (cross-check)
   void release_workspaces() {
     for (Workspace& w : ws) w.release();
-    DevBuf* all[] = {&d_f32_a, &d_f32_b, &d_root_a, &d_root_b, &d_norm_a, &d_norm_b};
+    DevBuf* all[] = {&d_f32_a, &d_f32_b, &d_root_a, &d_root_b, &d_norm_a, &d_norm_b, &d_i8_a, &d_i8_b};
     for (DevBuf* b : all) b->release();
   }
 };
@@ -103,6 +114,21 @@ extern State g_state;
 void set_error(const std::string& s);
 int cuda_fail(cudaError_t e, const char* what);
 int check_inited();
+NodeDev* get_node(uint64_t h);  // nullptr (and last_error set) unless h is a live node handle
+Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot < kSlots
+
+// Return cuda_fail(...) from the enclosing function when a CUDA runtime call fails.
+#define RB200_CUDA(call)                                  \
+  do {                                                    \
+    cudaError_t e__ = (call);                             \
+    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
+  } while (0)
+
+// Preamble of every entry point that needs an initialised library: holds the library lock for the rest of the scope and
+// returns ERR_STATE (or ERR_CUDA) unless rgbdslam_b200_init has succeeded.
+#define RB200_ENTER_INITED()                                    \
+  std::lock_guard<std::mutex> entry_lock__(rb200::g_state.mu); \
+  if (int entry_rc__ = rb200::check_inited()) return entry_rc__
 int node_build_cloud(NodeDev* nd, const float* d_depth, int w, int h, const float K4[4], cudaStream_t st);
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
 

@@ -56,3 +56,43 @@ def test_missing_library_fails_loudly(tmp_path):
     from rgbdslam_v2_b200 import _capi
     with pytest.raises(_capi.LibraryMissingError):
         _capi.load_library(tmp_path / "nope.so")
+
+
+# Return code of every entry point called before rgbdslam_b200_init with zero / NULL arguments.  Entry points that need an
+# initialised library return ERR_STATE (3); the ones below work without init.  init itself: test_no_cpu_fallback.
+_NO_INIT_RC = {
+    "rgbdslam_b200_launch_count": 0, "rgbdslam_b200_depth_cov_z0": 0, "rgbdslam_b200_set_hamming_path": 0,
+    "rgbdslam_b200_set_sift_matcher": 0, "rgbdslam_b200_orb_debug_detect_path": 0, "rgbdslam_b200_shutdown": 0,
+    "rgbdslam_b200_comm_destroy": 1, "rgbdslam_b200_detector_create": 1, "rgbdslam_b200_detector_destroy": 1,
+    "rgbdslam_b200_detector_thresholds": 1, "rgbdslam_b200_get_params": 1, "rgbdslam_b200_graph_from_pairs": 1,
+    "rgbdslam_b200_node_destroy": 1, "rgbdslam_b200_node_num_features": 1,
+    "rgbdslam_b200_comm_unique_id": (1, 4),  # 4 = ERR_NCCL when libnccl.so.2 cannot be loaded
+}
+_NOT_CALLED = {"rgbdslam_b200_init", "rgbdslam_b200_default_params", "rgbdslam_b200_last_error"}
+
+
+def test_every_entry_point_before_init(built):
+    """Every declared entry point, called before init with zero / NULL arguments, returns its documented code, and every
+    non-zero return replaces last_error (no stale message from the previous call)."""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("GPU present: the library may already be initialised in this process")
+    from rgbdslam_v2_b200 import _capi
+    lib = _capi.load_library()
+    names = [n for n in _capi.declared_symbols() if n not in _NOT_CALLED]
+    assert len(names) == 50
+    for name in names:
+        fn = getattr(lib, name)
+        assert lib.rgbdslam_b200_set_hamming_path(7) == 1  # leaves a known message in last_error
+        sentinel = lib.rgbdslam_b200_last_error()
+        args = [None if t is C.c_void_p or issubclass(t, C._Pointer) else 0.0 if t is C.c_double else 0 for t in fn.argtypes]
+        rc = fn(*args)
+        want = _NO_INIT_RC.get(name, 3)
+        if name == "rgbdslam_b200_depth_cov_z0":
+            assert rc == 0.0, name
+            continue
+        assert rc in (want if isinstance(want, tuple) else (want,)), (name, rc)
+        if rc != 0:
+            msg = lib.rgbdslam_b200_last_error()
+            assert msg and msg != sentinel, (name, msg)
+    lib.rgbdslam_b200_set_hamming_path(1)  # the default

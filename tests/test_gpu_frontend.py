@@ -1,4 +1,5 @@
 """GPU parity tests (run with -m gpu on an H100): the CUDA path through the C ABI vs the CPU oracle."""
+import ctypes as C
 from pathlib import Path
 
 import numpy as np
@@ -355,5 +356,78 @@ def test_pipelined_submit_wait_equals_synchronous(fe, oracle_mod):
         fe.submit_node_pairs(1 + it % 2, newer, older, (outs[it % 2][0], None, None), seed=31, first_pair_index=0)
     fe.wait_slot(1); fe.wait_slot(2)
     assert outs[0][0].tobytes() == ref[0][0].tobytes() and outs[1][0].tobytes() == ref[0][0].tobytes()
+    for h in list(newer) + list(older):
+        fe.node_destroy(int(h))
+
+
+def _node_batch(fe, seed0):
+    from rgbdslam_v2_b200 import synth
+    b = synth.make_batch(4, 600, seed0=seed0)
+    newer = np.array([fe.node_from_features(int(b["id_newer"][i]), p["desc_newer"], p["xyz_newer"]) for i, p in enumerate(b["pairs"])],
+                     np.uint64)
+    older = np.array([fe.node_from_features(int(b["id_older"][i]), p["desc_older"], p["xyz_older"]) for i, p in enumerate(b["pairs"])],
+                     np.uint64)
+    return newer, older
+
+
+def _assert_same_results(a, b):
+    (r, m, i), (rr, rm, ri) = a, b
+    assert r.tobytes() == rr.tobytes() and m.tobytes() == rm.tobytes()
+    for k in range(len(r)):  # inlier rows past n_inliers are not written
+        assert np.array_equal(i[k, :r[k]["n_inliers"]], ri[k, :rr[k]["n_inliers"]])
+
+
+def test_argument_and_state_errors_leave_the_library_usable(fe):
+    """Bad slots, handles and states are rejected with their codes; a valid call afterwards gives the same bytes as before."""
+    from rgbdslam_v2_b200._capi import KEYPOINT_DTYPE, PAIR_RESULT_DTYPE, _ptr
+    _reinit(fe)
+    lib = fe.lib
+    newer, older = _node_batch(fe, 4100)
+    ref = fe.match_node_pairs(list(newer), list(older), seed=9)
+    res = np.zeros(len(newer), PAIR_RESULT_DTYPE)
+    assert lib.rgbdslam_b200_match_pairs_submit(8, _ptr(newer), _ptr(older), len(newer), 9, 0, _ptr(res), None, None) == 1
+    assert lib.rgbdslam_b200_match_pairs_wait(-1) == 1
+    t = np.zeros(7, np.float32)
+    assert lib.rgbdslam_b200_slot_stage_times(7, _ptr(t)) == 3  # slot 7 has never been submitted to
+    assert lib.rgbdslam_b200_last_timing_slot(7, None, None) == 3
+    bad = newer.copy()
+    bad[1] = 0
+    assert lib.rgbdslam_b200_match_pairs(_ptr(bad), _ptr(older), len(newer), 9, 0, _ptr(res), None, None) == 1
+    comm = fe.comm_init(0, 1, fe.comm_unique_id())
+    fe.wait_slot(5)
+    assert lib.rgbdslam_b200_allgather_slot_edges(C.c_uint64(comm), 5, 1, _ptr(res)) == 3
+    fe.comm_destroy(comm)
+    kp = np.zeros(fe.node_num_features(int(newer[0])), KEYPOINT_DTYPE)
+    assert lib.rgbdslam_b200_node_download_keypoints(int(newer[0]), _ptr(kp)) == 3
+    again = fe.match_node_pairs(list(newer), list(older), seed=9)
+    _assert_same_results(ref, again)
+    for h in list(newer) + list(older):
+        fe.node_destroy(int(h))
+
+
+def test_rejected_match_calls_launch_nothing(fe):
+    """Preconditions that the pair table decides (keypoints for the refinement, clouds for the measurement model, the z0 latch
+    of a synchronous first batch) are checked before anything is queued: a rejected call launches no kernel, and the next
+    submit on the same slot gives the synchronous results."""
+    from rgbdslam_v2_b200._capi import _ptr
+    lib = fe.lib
+    _reinit(fe)
+    newer, older = _node_batch(fe, 4200)
+    ref = fe.match_node_pairs(list(newer), list(older), seed=13, first_pair_index=4)
+    rejected = [(dict(g2o_transformation_refinement=3), 2, 4), (dict(observability_threshold=0.5), 3, 4),
+                (dict(depth_cov_z0=0.0), 0, 4)]
+    for kw, slot, first in rejected:
+        _reinit(fe, **kw)
+        out = fe._alloc_out(len(newer), True)
+        launches = fe.launch_count
+        rc = lib.rgbdslam_b200_match_pairs_submit(slot, _ptr(newer), _ptr(older), len(newer), 13, first, *(_ptr(a) for a in out))
+        assert rc == 3, kw
+        if slot == 0:
+            assert lib.rgbdslam_b200_match_pairs(_ptr(newer), _ptr(older), len(newer), 13, first, *(_ptr(a) for a in out)) == 3
+        assert fe.launch_count == launches, kw
+        _reinit(fe)
+        fe.submit_node_pairs(slot, newer, older, out, seed=13, first_pair_index=first)
+        fe.wait_slot(slot)
+        _assert_same_results(ref, out)
     for h in list(newer) + list(older):
         fe.node_destroy(int(h))
