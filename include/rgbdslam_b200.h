@@ -314,12 +314,10 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
 /* Inspection hook: FAST/NMS candidates {u16 x, u16 y, u8 level, u8 score, u16 0} and Harris responses (NaN = below
  * the cell's final threshold) of grid cell `cell` in frame 0 of the last detect / nodes_create call. */
 int rgbdslam_b200_orb_debug_candidates(int cell, void* cand_out, float* resp_out, int capacity, int* n_out, int* thr_out);
-/* Inspection hook: one plane of frame 0 of the last call.  which: 0 cell image, 1 cell mask, 2 FAST score map
- * (cell pyramids); 3 raw / 4 blurred extractor pyramid (cell ignored). */
+/* Inspection hook: one plane of frame 0 of the last call.  which: 0 cell image, 1 cell mask (cell pyramids); 3 raw /
+ * 4 blurred extractor pyramid (cell ignored).  2 (the FAST score map, which the detector never stores) and any other
+ * value return ERR_ARG. */
 int rgbdslam_b200_orb_debug_plane(int which, int cell, int level, uint8_t* out, int capacity, int* w_out, int* h_out);
-/* Inspection hook: 1 = detect with the unfused kernels (FAST score by threshold search into a global score map -- the one
- * orb_debug_plane(2, ...) returns --, separate NMS and resize passes), 0 = the default fused kernels.  Identical results. */
-int rgbdslam_b200_orb_debug_detect_path(int unfused);
 /* feature_locations_2d_ (node.h:167) of a node built by nodes_create. */
 int rgbdslam_b200_node_download_keypoints(uint64_t node_handle, rgbdslam_b200_keypoint* kp_out);
 

@@ -135,7 +135,6 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_nodes_create_ex.argtypes = [u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_nodes_create_sharded.argtypes = [u64, u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_node_download_keypoints.argtypes = [u64, vp]
-    lib.rgbdslam_b200_orb_debug_detect_path.argtypes = [C.c_int]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -452,9 +451,6 @@ class Frontend:
             _ptr(None if (mask_from_depth or not own) else mask), W, H, _ptr(K4), _ptr(ids), 1 if mask_from_depth else 0, _ptr(handles), _ptr(nf)))
         self._nodes += [int(h) for h in handles]
         return [int(h) for h in handles], nf
-
-    def orb_debug_detect_path(self, unfused: bool):
-        self._check(self.lib.rgbdslam_b200_orb_debug_detect_path(1 if unfused else 0))
 
     def orb_debug_plane(self, which: int, cell: int, level: int) -> np.ndarray:
         buf = np.zeros(1024 * 1024, np.uint8)

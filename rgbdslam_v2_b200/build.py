@@ -18,9 +18,8 @@ NVCC_FLAGS = [
 
 
 def library_path() -> Path:
-    """In-tree library; RGBDSLAM_B200_LIB points tools/ at an A/B variant built by tools/build_variants.py."""
-    override = os.environ.get("RGBDSLAM_B200_LIB")
-    return Path(override) if override else PKG_DIR / LIB_NAME
+    """The in-tree library."""
+    return PKG_DIR / LIB_NAME
 
 
 def _nvcc() -> str:

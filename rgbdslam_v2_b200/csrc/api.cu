@@ -408,7 +408,7 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
     if ((rc = launch_hamming(w, d_pairs, npairs, max_nq, stride, n_items))) return rc;
     e = launch_select_matches(d_pairs, npairs, (const int2*)w.d_best.ptr, stride, seed, first_pair,
                               (rgbdslam_b200_dmatch*)w.d_matches.ptr, (float4*)w.d_mfrom.ptr, (float4*)w.d_mto.ptr,
-                              (int32_t*)w.d_nall.ptr, max_nq, st);
+                              (int32_t*)w.d_nall.ptr, st);
     if (e != cudaSuccess) return cuda_fail(e, "select_matches kernel");
     s.launches += 1;
   }

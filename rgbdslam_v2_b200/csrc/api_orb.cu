@@ -41,7 +41,7 @@ struct OrbCtx {
   PinBuf stage[2];                             // pinned staging for callers that pass pageable memory
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
-  DevBuf cell_img, cell_mask, score, cand, cand_count, hist, mask_any, thr, resp, cell_out, cell_out_count, scratch, kp, xyz, n,
+  DevBuf cell_img, cell_mask, cand, cand_count, hist, mask_any, thr, resp, cell_out, cell_out_count, scratch, kp, xyz, n,
       pyr_raw, pyr_blur, desc, err, trig;
   // rgbdslam_b200_nodes_create_sharded: what must survive between the detection pass and the finishing pass of ALL own frames,
   // and the per-(frame, cell) tables every rank holds for ALL frames of the sequence
@@ -49,7 +49,7 @@ struct OrbCtx {
   const uint8_t* last_gray = nullptr;  // device pointers of frame 0 of the last call (debug hooks)
   void release() {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &cell_img,
-                     &cell_mask, &score, &cand, &cand_count, &hist, &mask_any, &thr, &resp, &cell_out, &cell_out_count, &scratch,
+                     &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp, &cell_out, &cell_out_count, &scratch,
                      &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand,
                      &all_hist, &all_cnt, &all_many, &all_thr};
     for (DevBuf* b : all) b->release();
@@ -241,7 +241,7 @@ static int orb_ensure_buffers(int F, int nbuf, bool want_mask) {
     if ((rc = o.in_gray[b].ensure(px * F)) || (want_mask && (rc = o.in_mask[b].ensure(px * F))) || (rc = o.in_depth[b].ensure(px * F * 4)))
       return rc;
   if ((rc = o.cell_img.ensure((size_t)g.cell_bytes * F)) || (rc = o.cell_mask.ensure((size_t)g.cell_bytes * F)) ||
-      (rc = o.score.ensure((size_t)g.cell_bytes * F)) || (rc = o.cand.ensure(z * kOrbCandCap * sizeof(OrbCand))) ||
+      (rc = o.cand.ensure(z * kOrbCandCap * sizeof(OrbCand))) ||
       (rc = o.cand_count.ensure(z * 4)) || (rc = o.hist.ensure(z * 256 * 4)) || (rc = o.mask_any.ensure(z * 4)) ||
       (rc = o.thr.ensure(z * 4)) || (rc = o.resp.ensure(z * kOrbCandCap * 4)) ||
       (rc = o.cell_out.ensure(z * (size_t)o.max_per_cell * 8)) || (rc = o.cell_out_count.ensure(z * 4)) ||
@@ -293,7 +293,7 @@ static int orb_detect_stage(Detector* det, int F, const uint8_t* d_gray, const u
   int rc;
   if ((rc = detector_to_device(det, st))) return rc;
   cudaError_t e = orb_run_detect(g, o.tab, F, d_gray, d_mask, d_depth_for_mask, (uint8_t*)o.cell_img.ptr, (uint8_t*)o.cell_mask.ptr,
-                                 (uint8_t*)o.score.ptr, (OrbCand*)o.cand.ptr, (int*)o.cand_count.ptr, (int*)o.hist.ptr,
+                                 (OrbCand*)o.cand.ptr, (int*)o.cand_count.ptr, (int*)o.hist.ptr,
                                  (int*)o.mask_any.ptr, st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb detect kernels");
   e = orb_run_adapt(g, F, (const int*)o.hist.ptr, (const int*)o.cand_count.ptr, (const int*)o.mask_any.ptr, (double*)det->d_state.ptr,
@@ -733,7 +733,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     if (c0 == 0) o.last_gray = dg;
     const size_t gf = (size_t)(f0 + c0);  // global index of the chunk's first frame
     e = orb_run_detect(g, o.tab, F, dg, dm, mask_from_depth ? dd : nullptr, (uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0,
-                       (uint8_t*)o.cell_mask.ptr, (uint8_t*)o.score.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
+                       (uint8_t*)o.cell_mask.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
                        cnt_all + gf * nc, hist_all + gf * nc * 256, many_all + gf * nc, st, &launches);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb detect kernels"));
   }
@@ -809,24 +809,22 @@ int rgbdslam_b200_orb_debug_candidates(int cell, void* cand_out, float* resp_out
   return 0;
 }
 
-int rgbdslam_b200_orb_debug_detect_path(int unfused) {
-  std::lock_guard<std::mutex> lk(g_state.mu);
-  orb_set_legacy_detect(unfused);
-  return 0;
-}
-
 int rgbdslam_b200_orb_debug_plane(int which, int cell, int level, uint8_t* out, int capacity, int* w_out, int* h_out) {
   RB200_ENTER_INITED();
   OrbCtx& o = g_orb;
-  if (!o.ready || level < 0 || level >= kOrbLevels || !w_out || !h_out || (which <= 2 && (cell < 0 || cell >= o.g.ncells))) {
+  if (which < 0 || which == 2 || which > 4) {
+    set_error("orb_debug_plane: which must be 0, 1, 3 or 4 (the FAST score map is never stored: scores stay in shared memory)");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  if (!o.ready || level < 0 || level >= kOrbLevels || !w_out || !h_out || (which <= 1 && (cell < 0 || cell >= o.g.ncells))) {
     set_error("orb_debug_plane: no detection has run / bad level or cell");
     return RGBDSLAM_B200_ERR_ARG;
   }
   const OrbPlane* p;
   const uint8_t* base;
-  if (which <= 2) {
+  if (which <= 1) {
     p = &o.g.cell[cell][level];
-    base = (const uint8_t*)(which == 0 ? o.cell_img.ptr : which == 1 ? o.cell_mask.ptr : o.score.ptr);
+    base = (const uint8_t*)(which == 0 ? o.cell_img.ptr : o.cell_mask.ptr);
   } else {
     p = &o.g.full[level];
     base = (const uint8_t*)(which == 3 ? o.pyr_raw.ptr : o.pyr_blur.ptr);

@@ -7,14 +7,11 @@
 
 namespace rb200 {
 
-// 1: detect with the unfused k_fast_score / k_nms_collect / k_resize kernels (keeps the FAST score map in global memory)
-void orb_set_legacy_detect(int on);
-
 cudaError_t orb_upload_constants(const OrbGeom& g, const int* umax, cudaStream_t st);
 
 // d_depth_for_mask != nullptr: detection mask = depthToCV8UC1(depth) != 0 (misc.cpp:414-418), d_mask ignored
 cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, const uint8_t* d_mask,
-                           const float* d_depth_for_mask, uint8_t* d_cell_img, uint8_t* d_cell_mask, uint8_t* d_score, OrbCand* d_cand,
+                           const float* d_depth_for_mask, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
                            int* d_cand_count, int* d_hist, int* d_mask_any, cudaStream_t st, int* launches);
 
 // the adaptive-threshold recurrence of the F frames of a chunk, on the device (no host round trip)

@@ -18,9 +18,7 @@
 
 #include <algorithm>
 #include <cfloat>
-#include <chrono>
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -399,7 +397,7 @@ __global__ void __launch_bounds__(512, 1) pg_pcg_kernel(PcgArgs a) {
 // sequential sum over its incidences in one lane -- no warp reduction, no atomics, fixed order.  Two grid barriers per
 // iteration as in pg_pcg_kernel, but a barrier that carries the dot product itself (pg_tree_barrier).
 // C5 (5000 V / 30 000 E, 7814 PCG iterations): 25.5 -> 10.9 us per iteration, 0.20 -> 0.085 s for the whole solve.  Where the
-// remaining time goes (clock64 profile, -DRB200_PG_PROFILE): the two barriers 2 x 3.4 us (three fences and two global
+// remaining time goes (clock64 profile): the two barriers 2 x 3.4 us (three fences and two global
 // store -> poll hops each), gather + SpMV 2.4 us, block sums 0.9 us.
 // Incidences beyond the shared-memory capacity of a CTA (hub vertices) are read from the global copy.
 constexpr int kPgResGroups = 5, kPgResWarps = 16, kPgResSlots = kPgResGroups * kPgResWarps;
@@ -549,12 +547,6 @@ __global__ void __launch_bounds__(kPgResWarps * 32, 1) pg_pcg_resident_kernel(Pc
   double beta = 0.0;
   int it = 0;
   bool breakdown = false;
-#ifdef RB200_PG_PROFILE
-  long long pf[6] = {0, 0, 0, 0, 0, 0}, pc0 = clock64(), pc1;
-#define PG_LAP(k) { pc1 = clock64(); pf[k] += pc1 - pc0; pc0 = pc1; }
-#else
-#define PG_LAP(k)
-#endif
   for (;;) {
     // ---- phase 2: q = A s + beta q ; d = s + beta d ; partial d.q
     // the s rows of all neighbours of this CTA's vertices, fetched by the whole CTA in ONE round trip (one double per thread
@@ -619,13 +611,10 @@ __global__ void __launch_bounds__(kPgResWarps * 32, 1) pg_pcg_resident_kernel(Pc
     }
     qq = qn;
     dd = dnw;
-    PG_LAP(0)
     {
       bsum = block_partial(act ? dnw * qn : 0.0, sm);
-      PG_LAP(1)
     }
     const double dq = pg_tree_barrier(bsum, slots_b, gslots_b, eb & 1u, sm);
-    PG_LAP(3)
     eb++;
     if (it >= a.maxit || dn <= a.tol) break;
     if (!(dq > 0)) { breakdown = true; break; }
@@ -640,13 +629,10 @@ __global__ void __launch_bounds__(kPgResWarps * 32, 1) pg_pcg_resident_kernel(Pc
       sv = t;
     }
     if (act) a.s[6 * (size_t)v + row] = sv;
-    PG_LAP(4)
     {
       bsum = block_partial(act ? rr * sv : 0.0, sm);
-      PG_LAP(1)
     }
     const double dn_new = pg_tree_barrier(bsum, slots_a, gslots_a, ea & 1u, sm);
-    PG_LAP(5)
     ea++;
     beta = dn_new / dn;
     dn = dn_new;
@@ -662,9 +648,6 @@ __global__ void __launch_bounds__(kPgResWarps * 32, 1) pg_pcg_resident_kernel(Pc
     a.result[1] = dn;
     a.result[2] = scale;
     a.result[3] = breakdown ? 1.0 : 0.0;
-#ifdef RB200_PG_PROFILE
-    for (int k = 0; k < 6; k++) a.result[4 + k] = (double)pf[k];  // cycles of thread 0: spmv, block sum, fence+store, wait d.q, phase 1, wait r.s
-#endif
   }
 }
 
@@ -774,7 +757,6 @@ struct PgCtx {
   int64_t launches = 0;
   int cg_iters = 0;
   double pcg_residual = -1.0;  // LinearSolverPCG::_residual
-  double pcg_seconds = 0.0;    // wall time inside the PCG launches (RB200_PG_TIMING=1 prints the split)
   // resident solver (pg_pcg_resident_kernel): vertices per CTA, shared-memory capacity in incidences, dynamic bytes; vpc == 0: off
   int res_vpc = 0, res_cap = 0, res_smem = 0;
 };
@@ -858,7 +840,6 @@ static int pg_pcg(PgCtx& c, double lambda, double* scale, bool* ok) {
   a.tol = (c.pcg_residual > 0.0 && c.pcg_residual > 1e-6) ? c.pcg_residual : 1e-6;
   a.maxit = 6 * c.nv;
   void* args[] = {&a};
-  const auto t0 = std::chrono::steady_clock::now();
   pg_precond_kernel<<<(c.nv + 127) / 128, 128, 0, c.st>>>(c.nv, a.Hd, a.fixed, lambda, a.Minv);
   RB200_CUDA(cudaGetLastError());
   c.launches++;
@@ -872,15 +853,9 @@ static int pg_pcg(PgCtx& c, double lambda, double* scale, bool* ok) {
     RB200_CUDA(cudaLaunchCooperativeKernel((void*)pg_pcg_kernel, dim3(c.pcg_grid), dim3(512), args, 0, c.st));
   }
   c.launches++;
-  double res[10];
+  double res[4];
   RB200_CUDA(cudaMemcpyAsync(res, c.dev.result.ptr, sizeof(res), cudaMemcpyDeviceToHost, c.st));
   RB200_CUDA(cudaStreamSynchronize(c.st));
-#ifdef RB200_PG_PROFILE
-  if (c.res_vpc > 0 && res[0] > 0)
-    fprintf(stderr, "[pcg profile] %d iterations, cycles per iteration: spmv %.0f, block sums %.0f, fence+store %.0f, wait d.q %.0f, phase 1 %.0f, wait r.s %.0f\n",
-            (int)res[0], res[4] / res[0], res[5] / res[0], res[6] / res[0], res[7] / res[0], res[8] / res[0], res[9] / res[0]);
-#endif
-  c.pcg_seconds += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
   c.cg_iters += (int)res[0];
   c.pcg_residual = 0.5 * res[1];
   *scale = res[2];
@@ -970,7 +945,6 @@ int posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, cons
                        const double* info, double stop, double huber_delta, double* chi2_out, int* iters_out,
                        int* cg_iters_out, double* per_edge_chi2, bool optimize) {
   State& s = g_state;
-  const auto t_begin = std::chrono::steady_clock::now();
   if (!g_pg_dev) g_pg_dev = new PgDevice();
   PgCtx c(*g_pg_dev);
   c.nv = nv;
@@ -1077,10 +1051,6 @@ int posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, cons
   if (per_edge_chi2 && ne > 0)
     RB200_CUDA(cudaMemcpyAsync(per_edge_chi2, d.per_edge.ptr, 8 * (size_t)ne, cudaMemcpyDeviceToHost, st));
   RB200_CUDA(cudaStreamSynchronize(st));
-  if (getenv("RB200_PG_TIMING"))
-    fprintf(stderr, "[posegraph] nv %d ne %d optimize %d: total %.3f ms, pcg launches %.3f ms (%d pcg iterations, grid %d), lm %d\n", nv, ne,
-            (int)optimize, 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count(), 1e3 * c.pcg_seconds,
-            c.cg_iters, c.pcg_grid, it);
   if (chi2_out) *chi2_out = chi2;
   if (iters_out) *iters_out = it;
   if (cg_iters_out) *cg_iters_out = c.cg_iters;

@@ -62,7 +62,7 @@ def test_missing_library_fails_loudly(tmp_path):
 # initialised library return ERR_STATE (3); the ones below work without init.  init itself: test_no_cpu_fallback.
 _NO_INIT_RC = {
     "rgbdslam_b200_launch_count": 0, "rgbdslam_b200_depth_cov_z0": 0, "rgbdslam_b200_set_hamming_path": 0,
-    "rgbdslam_b200_set_sift_matcher": 0, "rgbdslam_b200_orb_debug_detect_path": 0, "rgbdslam_b200_shutdown": 0,
+    "rgbdslam_b200_set_sift_matcher": 0, "rgbdslam_b200_shutdown": 0,
     "rgbdslam_b200_comm_destroy": 1, "rgbdslam_b200_detector_create": 1, "rgbdslam_b200_detector_destroy": 1,
     "rgbdslam_b200_detector_thresholds": 1, "rgbdslam_b200_get_params": 1, "rgbdslam_b200_graph_from_pairs": 1,
     "rgbdslam_b200_node_destroy": 1, "rgbdslam_b200_node_num_features": 1,
@@ -80,7 +80,7 @@ def test_every_entry_point_before_init(built):
     from rgbdslam_v2_b200 import _capi
     lib = _capi.load_library()
     names = [n for n in _capi.declared_symbols() if n not in _NOT_CALLED]
-    assert len(names) == 50
+    assert len(names) == 49
     for name in names:
         fn = getattr(lib, name)
         assert lib.rgbdslam_b200_set_hamming_path(7) == 1  # leaves a known message in last_error

@@ -54,14 +54,9 @@ for cell in (0, 4):
     y0, y1, x0, x1 = cells[cell]
     sub = np.ascontiguousarray(gray[y0:y1, x0:x1])
     for l in (0, 1):
-        gi = fe.orb_debug_plane(0, cell, l); gs = fe.orb_debug_plane(2, cell, l); gm = fe.orb_debug_plane(1, cell, l)
+        gi = fe.orb_debug_plane(0, cell, l); gm = fe.orb_debug_plane(1, cell, l)
         ref = sub if l == 0 else resize_exact(sub, gi.shape[1], gi.shape[0])
         print(f"cell {cell} level {l}: img shape {gi.shape} equal {np.array_equal(gi, ref)} ndiff {(gi != ref).sum() if gi.shape == ref.shape else -1}; mask all255 {(gm == 255).all()}")
-        Sref = score_map(ref)
-        print(f"   score equal {np.array_equal(gs, np.minimum(Sref,255))} ndiff {(gs != np.minimum(Sref,255)).sum()} gpu max {gs.max()} ref max {Sref.max()}")
-        bad = np.argwhere(gs != np.minimum(Sref, 255))[:5]
-        for (yy, xx) in bad:
-            print("    at", xx, yy, "gpu", gs[yy, xx], "ref", Sref[yy, xx], "img", gi[yy, xx])
     cand, resp, thr = fe.orb_debug_candidates(cell)
     y0, y1, x0, x1 = cells[cell]
     sub = np.ascontiguousarray(gray[y0:y1, x0:x1])
