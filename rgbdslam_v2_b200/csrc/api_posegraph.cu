@@ -1,7 +1,6 @@
 // api_posegraph.cu -- C ABI of the pose-graph solve (declared in include/rgbdslam_b200.h).
 #include <cmath>
 #include <mutex>
-#include <vector>
 
 #include "posegraph.h"
 #include "state.h"
@@ -23,7 +22,7 @@ int rgbdslam_b200_posegraph_optimize(int nv, double* poses, const uint8_t* fixed
       set_error("posegraph_optimize: non-finite entry in an information matrix");
       return RGBDSLAM_B200_ERR_ARG;
     }
-  return posegraph_optimize(nv, poses, fixed, ne, ij, meas, info, stop, huber_delta, chi2, iters, cg_iters, nullptr, true);
+  return posegraph_optimize(nv, poses, fixed, ne, ij, meas, info, stop, huber_delta, chi2, iters, cg_iters);
 }
 
 int rgbdslam_b200_posegraph_reserve(int nv, int ne) {
@@ -42,9 +41,7 @@ int rgbdslam_b200_posegraph_chi2(int nv, const double* poses, int ne, const int3
     set_error("posegraph_chi2: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  std::vector<uint8_t> fixed(nv, 0);
-  return posegraph_optimize(nv, const_cast<double*>(poses), fixed.data(), ne, ij, meas, info, 1.0, huber_delta, chi2,
-                            nullptr, nullptr, per_edge_chi2, false);
+  return posegraph_chi2(nv, poses, ne, ij, meas, info, huber_delta, chi2, per_edge_chi2);
 }
 
 int rgbdslam_b200_landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, double* points3, int n_obs,

@@ -12,12 +12,10 @@
 // -- the same normal equations, hence the same step and the same optimum.  S is never formed: the block-Jacobi PCG applies it
 // matrix-free (per point: u = Hpp^-1 sum Hpc d; per camera: q = Hcc d + sum pose-edge blocks - sum Hcp u), two gather kernels
 // and one single-CTA update kernel per iteration, all reductions in a fixed order (deterministic).
-// LM bookkeeping as in the pose-graph solver (g2o's OptimizationAlgorithmLevenberg: lambda0 = 1e-5 max diag H, <= 10 trials,
-// gain ratio with the + 1e-3 guard).  float64 throughout.  Oracle: oracle/landmark_oracle.py (dense solve of the FULL system).
+// The pose edges are the pose-graph solver's module (PoseEdges), the LM bookkeeping its driver (lm_optimize, posegraph.h).
+// float64 throughout.  Oracle: oracle/landmark_oracle.py (dense solve of the FULL system).
 #include <cuda_runtime.h>
 
-#include <cfloat>
-#include <cmath>
 #include <vector>
 
 #include "posegraph.h"
@@ -176,11 +174,11 @@ __global__ void __launch_bounds__(256) ba_cams_kernel(int n_cams, const int* __r
   if (e_off) {
     for (int q = e_off[c] + lane; q < e_off[c + 1]; q += 32) {
       const int code = e_inc[q];
-      const double* eb = eblk + (size_t)(code >> 1) * kPgEdgeBlk;
+      const double* eb = edge_blocks(eblk, code >> 1);
 #pragma unroll
-      for (int i = 0; i < 36; i++) H[i] += eb[(code & 1) * 36 + i];
+      for (int i = 0; i < 36; i++) H[i] += eb[edge_diag(code & 1) + i];
 #pragma unroll
-      for (int i = 0; i < 6; i++) b[i] -= eb[108 + (code & 1) * 6 + i];
+      for (int i = 0; i < 6; i++) b[i] -= eb[edge_grad(code & 1) + i];
     }
   }
 #pragma unroll
@@ -254,7 +252,7 @@ __global__ void __launch_bounds__(256) ba_cam_apply_kernel(int n_cams, const int
       for (int q = e_off[c] + lane; q < e_off[c + 1]; q += 32) {
         const int code = e_inc[q], other = e_oth[q];
         if (other == c) continue;
-        const double* C = eblk + (size_t)(code >> 1) * kPgEdgeBlk + 72;
+        const double* C = edge_blocks(eblk, code >> 1) + kEdgeC;
         const double* ov = d + 6 * (size_t)other;
         if ((code & 1) == 0) {
 #pragma unroll
@@ -415,12 +413,12 @@ __global__ void __launch_bounds__(128) ba_pt_update_kernel(int n_points, const i
 
 // ================================================================================================
 struct BaDevice {
+  PoseEdges edges;  // the camera-camera constraints
   DevBuf poses, poses_trial, pts, pts_trial, fixed, obs_cam, obs_pt, uvd, w3, pt_off, pt_obs, cam_off, cam_obs, blk, Hppinv, bp, Hcc, bc, g,
-      Minv, maxd_c, maxd_p, x, r, d, q, u, part, state, chipart, ij, meas, info, eblk, e_off, e_inc, e_oth, scpart;
+      Minv, maxd_c, maxd_p, x, r, d, q, u, part, state, chipart, scpart;
   ~BaDevice() {
     DevBuf* all[] = {&poses, &poses_trial, &pts, &pts_trial, &fixed, &obs_cam, &obs_pt, &uvd, &w3, &pt_off, &pt_obs, &cam_off, &cam_obs, &blk,
-                     &Hppinv, &bp, &Hcc, &bc, &g, &Minv, &maxd_c, &maxd_p, &x, &r, &d, &q, &u, &part, &state, &chipart, &ij, &meas, &info,
-                     &eblk, &e_off, &e_inc, &e_oth, &scpart};
+                     &Hppinv, &bp, &Hcc, &bc, &g, &Minv, &maxd_c, &maxd_p, &x, &r, &d, &q, &u, &part, &state, &chipart, &scpart};
     for (DevBuf* b : all) b->release();
   }
 };
@@ -432,8 +430,8 @@ int landmark_ba_release() {
 }
 
 struct BaProblem {
-  int nc, np, no, ne;
-  double K[4], delta;
+  int nc, np, no;
+  double K[4];
   cudaStream_t st;
   BaDevice* d;
   int64_t launches = 0;
@@ -442,7 +440,7 @@ struct BaProblem {
 
 static int ba_chi2(BaProblem& P, const double* poses, const double* pts, double* chi2) {
   BaDevice& d = *P.d;
-  const int nb = (P.no + 255) / 256, neb = P.ne > 0 ? (P.ne + 255) / 256 : 0;
+  const int nb = (P.no + 255) / 256, neb = d.edges.chi2_blocks();
   if (nb > 0) {
     ba_chi2_obs_kernel<<<nb, 256, 0, P.st>>>(P.no, poses, pts, (const int*)d.obs_cam.ptr, (const int*)d.obs_pt.ptr,
                                              (const double*)d.uvd.ptr, (const double*)d.w3.ptr, P.K[0], P.K[1], P.K[2], P.K[3],
@@ -450,11 +448,7 @@ static int ba_chi2(BaProblem& P, const double* poses, const double* pts, double*
     RB200_CUDA(cudaGetLastError());
     P.launches++;
   }
-  if (P.ne > 0) {
-    RB200_CUDA(pg_launch_chi2(P.ne, poses, (const int32_t*)d.ij.ptr, (const double*)d.meas.ptr, (const double*)d.info.ptr, P.delta,
-                           (double*)d.chipart.ptr + nb, P.st));
-    P.launches++;
-  }
+  if (int rc = d.edges.chi2(poses, (double*)d.chipart.ptr + nb, nullptr, P.st, P.launches)) return rc;
   std::vector<double> part(nb + 2 * (size_t)neb);
   RB200_CUDA(cudaMemcpyAsync(part.data(), d.chipart.ptr, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, P.st));
   RB200_CUDA(cudaStreamSynchronize(P.st));
@@ -465,54 +459,46 @@ static int ba_chi2(BaProblem& P, const double* poses, const double* pts, double*
   return 0;
 }
 
-// one LM iteration; returns 1 ok / 0 terminate / < 0 error
-static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& ni, double* chi2_io) {
+// SparseOptimizer::optimize(iterations); the chi2 of an iteration's start is the one of the trial last accepted
+static int ba_optimize(BaProblem& P, int iterations, double& chi2, int* done) {
   BaDevice& d = *P.d;
-  int rc;
-  double cur = *chi2_io;
   const int npb = (P.np + 127) / 128, ncb = (P.nc + 7) / 8;
-  if (P.no > 0)
-    ba_linearize_kernel<<<(P.no + 127) / 128, 128, 0, P.st>>>(P.no, (const double*)d.poses.ptr, (const double*)d.pts.ptr, (const int*)d.obs_cam.ptr,
-                                                            (const int*)d.obs_pt.ptr, (const double*)d.uvd.ptr, (const double*)d.w3.ptr, P.K[0],
-                                                            P.K[1], P.K[2], P.K[3], (double*)d.blk.ptr);
-  if (cudaError_t e = cudaGetLastError()) return -cuda_fail(e, "ba_linearize_kernel");
-  P.launches++;
-  if (P.ne > 0) {
-    if (pg_launch_linearize(P.ne, (const double*)d.poses.ptr, (const int32_t*)d.ij.ptr, (const double*)d.meas.ptr, (const double*)d.info.ptr,
-                            P.delta, (double*)d.eblk.ptr, P.st) != cudaSuccess)
-      return -cuda_fail(cudaGetLastError(), "pg_launch_linearize");
-    P.launches++;
-  }
+  const int* e_off = d.edges.ne > 0 ? (const int*)d.edges.off.ptr : nullptr;  // no pose-edge terms in ba_cams / ba_cam_apply
   auto assemble = [&](double lam) -> int {
     if (npb > 0)
       ba_points_kernel<<<npb, 128, 0, P.st>>>(P.np, (const int*)d.pt_off.ptr, (const int*)d.pt_obs.ptr, (const double*)d.blk.ptr, lam,
                                             (double*)d.Hppinv.ptr, (double*)d.bp.ptr, (double*)d.maxd_p.ptr);
     ba_cams_kernel<<<ncb, 256, 0, P.st>>>(P.nc, (const int*)d.cam_off.ptr, (const int*)d.cam_obs.ptr, (const int*)d.obs_pt.ptr,
-                                          (const double*)d.blk.ptr, P.ne > 0 ? (const int*)d.e_off.ptr : nullptr, (const int*)d.e_inc.ptr,
-                                          (const double*)d.eblk.ptr, (const uint8_t*)d.fixed.ptr, lam, (const double*)d.Hppinv.ptr,
-                                          (const double*)d.bp.ptr, (double*)d.Hcc.ptr, (double*)d.bc.ptr, (double*)d.g.ptr,
-                                          (double*)d.Minv.ptr, (double*)d.maxd_c.ptr);
+                                          (const double*)d.blk.ptr, e_off, (const int*)d.edges.inc.ptr, (const double*)d.edges.blk.ptr,
+                                          (const uint8_t*)d.fixed.ptr, lam, (const double*)d.Hppinv.ptr, (const double*)d.bp.ptr,
+                                          (double*)d.Hcc.ptr, (double*)d.bc.ptr, (double*)d.g.ptr, (double*)d.Minv.ptr,
+                                          (double*)d.maxd_c.ptr);
     P.launches += 2;
     RB200_CUDA(cudaGetLastError());
     return 0;
   };
-  if (iteration == 0) {  // computeLambdaInit: tau * max diag(H)
-    if ((rc = assemble(0.0))) return -rc;
+  auto linearize = [&](double&, double* maxdiag) -> int {
+    if (P.no > 0)
+      ba_linearize_kernel<<<(P.no + 127) / 128, 128, 0, P.st>>>(P.no, (const double*)d.poses.ptr, (const double*)d.pts.ptr,
+                                                              (const int*)d.obs_cam.ptr, (const int*)d.obs_pt.ptr, (const double*)d.uvd.ptr,
+                                                              (const double*)d.w3.ptr, P.K[0], P.K[1], P.K[2], P.K[3], (double*)d.blk.ptr);
+    RB200_CUDA(cudaGetLastError());
+    P.launches++;
+    if (int rc = d.edges.linearize((const double*)d.poses.ptr, P.st, P.launches)) return rc;
+    if (!maxdiag) return 0;
+    if (int rc = assemble(0.0)) return rc;
     std::vector<double> mc(P.nc), mp(npb);
-    if (cudaMemcpyAsync(mc.data(), d.maxd_c.ptr, 8 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-        cudaMemcpyAsync(mp.data(), d.maxd_p.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-        cudaStreamSynchronize(P.st) != cudaSuccess)
-      return -cuda_fail(cudaGetLastError(), "landmark_ba lambda init download");
+    RB200_CUDA(cudaMemcpyAsync(mc.data(), d.maxd_c.ptr, 8 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st));
+    RB200_CUDA(cudaMemcpyAsync(mp.data(), d.maxd_p.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st));
+    RB200_CUDA(cudaStreamSynchronize(P.st));
     double m = 0;
     for (double v : mc) m = v > m ? v : m;
     for (double v : mp) m = v > m ? v : m;
-    lambda = 1e-5 * m;
-    ni = 2;
-  }
-  double rho = 0;
-  int qmax = 0;
-  do {
-    if ((rc = assemble(lambda))) return -rc;
+    *maxdiag = m;
+    return 0;
+  };
+  auto trial = [&](double lambda, double& temp, double& scale, bool& ok) -> int {
+    if (int rc = assemble(lambda)) return rc;
     // ---- PCG on the reduced camera system
     ba_cg_step_kernel<<<1, 1024, 0, P.st>>>(0, P.nc, 0, nullptr, (const double*)d.g.ptr, (const double*)d.Minv.ptr, nullptr, (double*)d.x.ptr,
                                             (double*)d.r.ptr, (double*)d.d.ptr, (double*)d.state.ptr, 1e-18);
@@ -527,8 +513,8 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
                                                    (const double*)d.blk.ptr, (const double*)d.Hppinv.ptr, (const double*)d.d.ptr,
                                                    (double*)d.u.ptr);
         ba_cam_apply_kernel<<<ncb, 256, 0, P.st>>>(P.nc, (const int*)d.cam_off.ptr, (const int*)d.cam_obs.ptr, (const int*)d.obs_pt.ptr,
-                                                   (const double*)d.blk.ptr, P.ne > 0 ? (const int*)d.e_off.ptr : nullptr,
-                                                   (const int*)d.e_inc.ptr, (const int*)d.e_oth.ptr, (const double*)d.eblk.ptr,
+                                                   (const double*)d.blk.ptr, e_off, (const int*)d.edges.inc.ptr,
+                                                   (const int*)d.edges.oth.ptr, (const double*)d.edges.blk.ptr,
                                                    (const uint8_t*)d.fixed.ptr, (const double*)d.Hcc.ptr, (const double*)d.d.ptr,
                                                    (const double*)d.u.ptr, (double*)d.q.ptr, (double*)d.part.ptr);
         ba_cg_step_kernel<<<1, 1024, 0, P.st>>>(1, P.nc, ncb, (const double*)d.part.ptr, (const double*)d.g.ptr, (const double*)d.Minv.ptr,
@@ -537,56 +523,36 @@ static int ba_lm_iteration(BaProblem& P, int iteration, double& lambda, double& 
         P.launches += 3;
       }
       it += burst;
-      if (cudaMemcpyAsync(st4, d.state.ptr, sizeof(st4), cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-          cudaStreamSynchronize(P.st) != cudaSuccess)
-        return -cuda_fail(cudaGetLastError(), "landmark_ba PCG state download");
+      RB200_CUDA(cudaMemcpyAsync(st4, d.state.ptr, sizeof(st4), cudaMemcpyDeviceToHost, P.st));
+      RB200_CUDA(cudaStreamSynchronize(P.st));
       if (st4[2] != 0.0) break;
     }
     P.pcg_iters += (int)st4[1];
-    const bool ok = st4[2] != 2.0;
+    ok = st4[2] != 2.0;
     // ---- back-substitution, trial update, gain ratio
     if (npb > 0)
       ba_pt_update_kernel<<<npb, 128, 0, P.st>>>(P.np, (const int*)d.pt_off.ptr, (const int*)d.pt_obs.ptr, (const int*)d.obs_cam.ptr,
                                                (const double*)d.blk.ptr, (const double*)d.Hppinv.ptr, (const double*)d.bp.ptr,
                                                (const double*)d.x.ptr, lambda, (const double*)d.pts.ptr, (double*)d.pts_trial.ptr,
                                                (double*)d.scpart.ptr);
-    if (pg_launch_update(P.nc, (const double*)d.poses.ptr, (const double*)d.x.ptr, (const uint8_t*)d.fixed.ptr, (double*)d.poses_trial.ptr,
-                         P.st) != cudaSuccess)
-      return -cuda_fail(cudaGetLastError(), "pg_launch_update");
+    RB200_CUDA(pg_launch_update(P.nc, (const double*)d.poses.ptr, (const double*)d.x.ptr, (const uint8_t*)d.fixed.ptr,
+                                (double*)d.poses_trial.ptr, P.st));
     P.launches += 2;
     std::vector<double> sp(npb), xc(6 * (size_t)P.nc), bcv(6 * (size_t)P.nc);
-    if (cudaMemcpyAsync(sp.data(), d.scpart.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-        cudaMemcpyAsync(xc.data(), d.x.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-        cudaMemcpyAsync(bcv.data(), d.bc.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st) != cudaSuccess ||
-        cudaStreamSynchronize(P.st) != cudaSuccess)
-      return -cuda_fail(cudaGetLastError(), "landmark_ba gain ratio download");
-    double scale = 0;
+    RB200_CUDA(cudaMemcpyAsync(sp.data(), d.scpart.ptr, 8 * (size_t)npb, cudaMemcpyDeviceToHost, P.st));
+    RB200_CUDA(cudaMemcpyAsync(xc.data(), d.x.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st));
+    RB200_CUDA(cudaMemcpyAsync(bcv.data(), d.bc.ptr, 48 * (size_t)P.nc, cudaMemcpyDeviceToHost, P.st));
+    RB200_CUDA(cudaStreamSynchronize(P.st));
+    scale = 0;
     for (double v : sp) scale += v;
     for (size_t i = 0; i < xc.size(); i++) scale += xc[i] * (lambda * xc[i] + bcv[i]);
-    double temp;
-    if ((rc = ba_chi2(P, (const double*)d.poses_trial.ptr, (const double*)d.pts_trial.ptr, &temp))) return -rc;
-    if (!ok) temp = DBL_MAX;
-    rho = (cur - temp) / (scale + 1e-3);
-    if (rho > 0 && std::isfinite(temp)) {
-      double alpha = 1. - std::pow(2 * rho - 1, 3);
-      alpha = std::fmin(alpha, 2. / 3.);
-      lambda *= std::fmax(1. / 3., alpha);
-      ni = 2;
-      cur = temp;
-      std::swap(d.poses.ptr, d.poses_trial.ptr);
-      std::swap(d.poses.cap, d.poses_trial.cap);
-      std::swap(d.pts.ptr, d.pts_trial.ptr);
-      std::swap(d.pts.cap, d.pts_trial.cap);
-    } else {
-      lambda *= ni;
-      ni *= 2;
-      if (!std::isfinite(lambda)) break;
-    }
-    qmax++;
-  } while (rho < 0 && qmax < 10);
-  *chi2_io = cur;
-  if (qmax == 10 || rho == 0) return 0;
-  return 1;
+    return ba_chi2(P, (const double*)d.poses_trial.ptr, (const double*)d.pts_trial.ptr, &temp);
+  };
+  auto accept = [&] {
+    std::swap(d.poses, d.poses_trial);
+    std::swap(d.pts, d.pts_trial);
+  };
+  return lm_optimize(iterations, chi2, done, linearize, trial, accept);
 }
 
 int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, double* points3, int n_obs, const int32_t* obs_cam,
@@ -597,12 +563,11 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
   if (!g_ba) g_ba = new BaDevice();
   BaDevice& d = *g_ba;
   BaProblem P;
-  P.nc = n_cams; P.np = n_points; P.no = n_obs; P.ne = n_edges;
+  P.nc = n_cams; P.np = n_points; P.no = n_obs;
   for (int k = 0; k < 4; k++) P.K[k] = K4[k];
-  P.delta = huber_delta;
   P.st = s.stream;
   P.d = g_ba;
-  // CSR: observations by point and by camera (input order kept inside a row: deterministic sums); pose edges by camera
+  // CSR: observations by point and by camera (input order kept inside a row: deterministic sums)
   std::vector<int> pt_off(n_points + 1, 0), cam_off(n_cams + 1, 0), pt_obs(n_obs), cam_obs(n_obs);
   for (int o = 0; o < n_obs; o++) {
     if (obs_cam[o] < 0 || obs_cam[o] >= n_cams || obs_point[o] < 0 || obs_point[o] >= n_points) {
@@ -621,28 +586,11 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
       cam_obs[cc[obs_cam[o]]++] = o;
     }
   }
-  std::vector<int> e_off(n_cams + 1, 0), e_inc(2 * (size_t)(n_edges > 0 ? n_edges : 0)), e_oth(e_inc.size());
-  for (int k = 0; k < n_edges; k++) {
-    if (ij[2 * k] < 0 || ij[2 * k] >= n_cams || ij[2 * k + 1] < 0 || ij[2 * k + 1] >= n_cams) {
-      set_error("landmark_ba: edge vertex index out of range");
-      return RGBDSLAM_B200_ERR_ARG;
-    }
-    e_off[ij[2 * k] + 1]++;
-    e_off[ij[2 * k + 1] + 1]++;
-  }
-  for (int c = 0; c < n_cams; c++) e_off[c + 1] += e_off[c];
-  {
-    std::vector<int> cur(e_off.begin(), e_off.end() - 1);
-    for (int k = 0; k < n_edges; k++) {
-      e_oth[cur[ij[2 * k]]] = ij[2 * k + 1];
-      e_inc[cur[ij[2 * k]]++] = (k << 1) | 0;
-      e_oth[cur[ij[2 * k + 1]]] = ij[2 * k];
-      e_inc[cur[ij[2 * k + 1]]++] = (k << 1) | 1;
-    }
-  }
-  const size_t nc = (size_t)n_cams, np = (size_t)n_points, no = (size_t)(n_obs > 0 ? n_obs : 1), ne = (size_t)(n_edges > 0 ? n_edges : 1);
-  const int npb = (n_points + 127) / 128, ncb = (n_cams + 7) / 8, nchi = (n_obs + 255) / 256 + 2 * ((n_edges + 255) / 256) + 2;
+  cudaStream_t st = P.st;
   int rc;
+  if ((rc = d.edges.upload(n_cams, n_edges, ij, meas7, info36, huber_delta, true, st))) return rc;
+  const size_t nc = (size_t)n_cams, np = (size_t)n_points, no = (size_t)(n_obs > 0 ? n_obs : 1);
+  const int npb = (n_points + 127) / 128, ncb = (n_cams + 7) / 8, nchi = (n_obs + 255) / 256 + 2 * ((n_edges + 255) / 256) + 2;
   if ((rc = d.poses.ensure(56 * nc)) || (rc = d.poses_trial.ensure(56 * nc)) || (rc = d.pts.ensure(24 * np)) ||
       (rc = d.pts_trial.ensure(24 * np)) || (rc = d.fixed.ensure(nc)) || (rc = d.obs_cam.ensure(4 * no)) || (rc = d.obs_pt.ensure(4 * no)) ||
       (rc = d.uvd.ensure(24 * no)) || (rc = d.w3.ensure(24 * no)) || (rc = d.pt_off.ensure(4 * (np + 1))) || (rc = d.pt_obs.ensure(4 * no)) ||
@@ -651,11 +599,8 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
       (rc = d.g.ensure(48 * nc)) || (rc = d.Minv.ensure(288 * nc)) || (rc = d.maxd_c.ensure(8 * nc)) ||
       (rc = d.maxd_p.ensure(8 * (size_t)(npb + 1))) || (rc = d.x.ensure(48 * nc)) || (rc = d.r.ensure(48 * nc)) || (rc = d.d.ensure(48 * nc)) ||
       (rc = d.q.ensure(48 * nc)) || (rc = d.u.ensure(24 * np)) || (rc = d.part.ensure(8 * (size_t)(ncb + 1))) || (rc = d.state.ensure(64)) ||
-      (rc = d.chipart.ensure(8 * (size_t)nchi)) || (rc = d.ij.ensure(8 * ne)) || (rc = d.meas.ensure(56 * ne)) || (rc = d.info.ensure(288 * ne)) ||
-      (rc = d.eblk.ensure(8 * kPgEdgeBlk * ne)) || (rc = d.e_off.ensure(4 * (nc + 1))) || (rc = d.e_inc.ensure(8 * ne)) ||
-      (rc = d.e_oth.ensure(8 * ne)) || (rc = d.scpart.ensure(8 * (size_t)(npb + 1))))
+      (rc = d.chipart.ensure(8 * (size_t)nchi)) || (rc = d.scpart.ensure(8 * (size_t)(npb + 1))))
     return rc;
-  cudaStream_t st = P.st;
   RB200_CUDA(cudaMemcpyAsync(d.poses.ptr, poses7, 56 * nc, cudaMemcpyHostToDevice, st));
   RB200_CUDA(cudaMemcpyAsync(d.pts.ptr, points3, 24 * np, cudaMemcpyHostToDevice, st));
   RB200_CUDA(cudaMemcpyAsync(d.fixed.ptr, fixed, nc, cudaMemcpyHostToDevice, st));
@@ -669,26 +614,12 @@ int landmark_ba(int n_cams, double* poses7, const uint8_t* fixed, int n_points, 
     RB200_CUDA(cudaMemcpyAsync(d.pt_obs.ptr, pt_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
     RB200_CUDA(cudaMemcpyAsync(d.cam_obs.ptr, cam_obs.data(), 4 * (size_t)n_obs, cudaMemcpyHostToDevice, st));
   }
-  if (n_edges > 0) {
-    RB200_CUDA(cudaMemcpyAsync(d.ij.ptr, ij, 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    RB200_CUDA(cudaMemcpyAsync(d.meas.ptr, meas7, 56 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    RB200_CUDA(cudaMemcpyAsync(d.info.ptr, info36, 288 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    RB200_CUDA(cudaMemcpyAsync(d.e_off.ptr, e_off.data(), 4 * (nc + 1), cudaMemcpyHostToDevice, st));
-    RB200_CUDA(cudaMemcpyAsync(d.e_inc.ptr, e_inc.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-    RB200_CUDA(cudaMemcpyAsync(d.e_oth.ptr, e_oth.data(), 8 * (size_t)n_edges, cudaMemcpyHostToDevice, st));
-  }
   RB200_CUDA(cudaStreamSynchronize(st));
   double chi2 = 0;
   if ((rc = ba_chi2(P, (const double*)d.poses.ptr, (const double*)d.pts.ptr, &chi2))) return rc;
   if (chi2_before) *chi2_before = chi2;
-  double lambda = 0, ni = 2;
   int done = 0;
-  for (int it = 0; it < iterations; it++) {
-    const int r = ba_lm_iteration(P, it, lambda, ni, &chi2);
-    if (r < 0) return -r;
-    done++;
-    if (r == 0) break;
-  }
+  if ((rc = ba_optimize(P, iterations, chi2, &done))) return rc;
   RB200_CUDA(cudaMemcpyAsync(poses7, d.poses.ptr, 56 * nc, cudaMemcpyDeviceToHost, st));
   RB200_CUDA(cudaMemcpyAsync(points3, d.pts.ptr, 24 * np, cudaMemcpyDeviceToHost, st));
   RB200_CUDA(cudaStreamSynchronize(st));

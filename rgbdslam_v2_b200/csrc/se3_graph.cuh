@@ -1,9 +1,18 @@
 // se3_graph.cuh -- small device helpers shared by the pose-graph solver (posegraph.cu) and the landmark bundle adjustment
-// (landmark_ba.cu): quaternion / rotation conversions of the (t, q) pose vectors, a 6x6 inverse, a warp sum.
+// (landmark_ba.cu): quaternion / rotation conversions of the (t, q) pose vectors, a 6x6 inverse, a warp sum, the layout of
+// the per-edge normal-equation blocks of the pose edges.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace rb200 {
+
+// Per pose edge (written by pg_linearize_kernel), kEdgeBlk doubles: [A 36 | B 36 | C 36 | gi 6 | gj 6] with A = Ji'WJi,
+// B = Jj'WJj, C = Ji'WJj, g = J'We, all scaled by the Huber weight.  An incidence code is edge << 1 | role, role 0 for the
+// edge's vertex i, 1 for its vertex j.
+constexpr int kEdgeBlk = 120, kEdgeA = 0, kEdgeB = 36, kEdgeC = 72, kEdgeGi = 108, kEdgeGj = 114;
+__device__ __forceinline__ const double* edge_blocks(const double* blk, int edge) { return blk + (size_t)edge * kEdgeBlk; }
+__device__ __forceinline__ int edge_diag(int role) { return kEdgeA + role * 36; }  // offset of A (role 0) or B (role 1)
+__device__ __forceinline__ int edge_grad(int role) { return kEdgeGi + role * 6; }  // offset of gi (role 0) or gj (role 1)
 
 // SE(3) helpers, poses are (tx,ty,tz,qx,qy,qz,qw)
 __device__ __forceinline__ void quat_to_R(const double* q, double* R) {

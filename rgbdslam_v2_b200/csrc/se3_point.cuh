@@ -1,5 +1,5 @@
 // se3_point.cuh -- camera / 3-D point geometry shared by the pairwise g2o refinement (frontend_kernels.cu) and the landmark
-// bundle adjustment (posegraph.cu): g2o's EdgeSE3PointXYZDepth error with its Jacobians, VertexSE3::oplus, a 3x3 SPD inverse.
+// bundle adjustment (landmark_ba.cu): g2o's EdgeSE3PointXYZDepth error with its Jacobians, VertexSE3::oplus, a 3x3 SPD inverse.
 #pragma once
 #include <cuda_runtime.h>
 

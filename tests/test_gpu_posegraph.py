@@ -127,6 +127,39 @@ def test_resident_solver_matches_general_kernel_on_hub_graph(fe, monkeypatch):
     assert synth.ate_rmse(x1[:, :3], g["gt"][:, :3]) < 0.02
 
 
+def test_edge_vertex_index_out_of_range_is_rejected_before_any_launch(fe):
+    """an edge vertex index < 0 or >= the vertex count raises in optimize_graph, graph_chi2 and landmark_ba, launches nothing and
+    leaves nothing behind: the same valid calls give the same results before and after"""
+    from rgbdslam_v2_b200 import B200Error, synth
+    g = synth.make_pose_graph(60, 200, seed=8)
+    d = synth.make_ba_problem(n_cams=5, n_points=40, seed=3)
+
+    def valid():
+        x, chi2, it, cg = fe.optimize_graph(g["init"], g["fixed"], g["ij"], g["meas"], g["info"], stop=0.01)
+        c0, pe = fe.graph_chi2(g["init"], g["ij"], g["meas"], g["info"], per_edge=True)
+        ba = fe.landmark_ba(d["poses"], d["fixed"], d["points"], d["obs_cam"], d["obs_point"], d["obs_uvd"], d["obs_info3"], d["K4"],
+                            ij=d["ij"], meas=d["meas"], info=d["info"], iterations=4)
+        return (x, chi2, it, cg, c0, pe) + tuple(ba)
+
+    before = valid()
+    assert before[2] >= 1 and before[-2] >= 1
+    n0 = fe.launch_count
+    for k, bad in [(0, len(g["init"])), (1, -1), (1, 10**6)]:
+        ij = g["ij"].copy(); ij[len(ij) // 2, k] = bad
+        with pytest.raises(B200Error):
+            fe.optimize_graph(g["init"], g["fixed"], ij, g["meas"], g["info"], stop=0.01)
+        with pytest.raises(B200Error):
+            fe.graph_chi2(g["init"], ij, g["meas"], g["info"], per_edge=True)
+        bij = d["ij"].copy(); bij[-1, k] = len(d["poses"]) if bad >= 0 else bad
+        with pytest.raises(B200Error):
+            fe.landmark_ba(d["poses"], d["fixed"], d["points"], d["obs_cam"], d["obs_point"], d["obs_uvd"], d["obs_info3"], d["K4"],
+                           ij=bij, meas=d["meas"], info=d["info"], iterations=4)
+    assert fe.launch_count == n0
+    after = valid()
+    for a, b in zip(before, after):
+        assert np.array_equal(a, b)
+
+
 def test_reserve_then_solve(fe):
     from rgbdslam_v2_b200 import synth
     fe.posegraph_reserve(3000, 40000)
