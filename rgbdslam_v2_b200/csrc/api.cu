@@ -283,7 +283,13 @@ static int launch_hamming(Workspace& w, const PairDesc* d_pairs, int npairs, int
   if (s.hamming_path == 0) {
     e = launch_hamming_simt(d_pairs, npairs, max_nq, (int2*)w.d_best.ptr, stride, w.stream);
   } else if (n_items > 0) {
-    e = launch_hamming_tc_expand((const HamItem*)w.d_items.ptr, n_items, s.sm_count, w.stream);
+    if (!w.d_claim.ptr) {  // zeroed once; from then on every launch leaves the ticket where the next one expects it
+      if (int rc = w.d_claim.ensure(sizeof(unsigned long long))) return rc;
+      e = cudaMemsetAsync(w.d_claim.ptr, 0, sizeof(unsigned long long), w.stream);
+      if (e != cudaSuccess) return cuda_fail(e, "zero the match kernel's claim counter");
+      w.claim = ClaimCounter{(unsigned long long*)w.d_claim.ptr, 0};
+    }
+    e = launch_hamming_tc_expand((const HamItem*)w.d_items.ptr, n_items, s.sm_count, w.claim, w.stream);
   } else {
     cudaEventRecord(w.ev[kEvMatchEnd], w.stream);
     return 0;

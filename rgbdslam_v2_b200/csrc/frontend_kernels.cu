@@ -715,8 +715,9 @@ __global__ void __launch_bounds__(kRansacWarps * 32, kRansacMinBlocks)
                       const float4* __restrict__ mfrom, const float4* __restrict__ mto,
                       const int32_t* __restrict__ n_all, HypResult* __restrict__ hyp, float* __restrict__ cen,
                       int32_t* __restrict__ next_n) {
-  // NW * 32 rows each (20 KiB in total for the default max_matches = 300): small enough for one CTA of this kernel to share
-  // an SM with a CTA of the tensor-core match kernel of another batch in flight
+  // NW * 32 rows each (20 KiB in total for the default max_matches = 300).  This does not let a CTA share an SM with the
+  // tensor-core match kernel of another batch in flight: that kernel's CTA holds 61 440 of the SM's 65 536 registers and
+  // 216 KiB of its shared memory, so RANSAC CTAs run on the SMs it is not using.
   __shared__ float4 sfrom[NW * 32];
   __shared__ float4 sto[NW * 32];
   __shared__ float4 cfrom[NW * 32];  // centred copies for the fit (see fit_transform)

@@ -10,8 +10,9 @@
 //   tile[row_group][k_chunk 16][row_in_group 8][16 B]   (8 x 16 B core matrices, 2048 B per 8-row group)
 //
 // Two kernels:
-//  * tc_hamming_expand_kernel -- the ORB path: the threads expand the 32-byte descriptors to +-64 operands straight into shared
-//    memory, a ninth k-step carries the column index, and the expansion of train tile n+1 runs while the MMAs of tile n execute;
+//  * tc_hamming_expand_kernel -- the ORB path, warp-specialised: a producer warp group claims work items and expands the 32-byte
+//    descriptors to +-64 operands straight into shared memory (a ring of train-tile stages on mbarriers), four consumer warp
+//    groups issue the MMAs independently of each other, and a ninth k-step carries the column index;
 //  * tc_match256_kernel<1|2>  -- the float-descriptor matchers (bf16 RootSIFT scores / SiftGPU's u8 dot products): operand
 //    tiles resident in HBM in the layout above, each staged by ONE cp.async.bulk completing on an mbarrier, one producer warp
 //    and four consumer warp groups that run independently of each other (one group's epilogue overlaps another's MMAs).
@@ -327,25 +328,59 @@ cudaError_t launch_siftgpu_tc256(const HamItem* d_items, int n_items, int sm_cou
 // ---------------------------------------------------------------------------------------------
 // Hamming match with IN-KERNEL operand expansion (the default ORB path, `set_hamming_path(1)`).
 //
-// The threads read the 32-byte descriptors themselves and expand them straight into the operand layout in shared memory
-// (8 x the descriptor bytes: expanding in HBM would multiply the stage's DRAM traffic by that).  Two more things ride on it:
+// The 32-byte descriptors are expanded straight into the operand layout in shared memory (8 x the descriptor bytes: expanding
+// in HBM would multiply the stage's DRAM traffic by that).  Two more things ride on it:
 //  * operands are +-64 instead of +-1, so the accumulator holds 4096 * dot;
 //  * a NINTH k-step multiplies two constant operand blocks, A_idx rows (64, 1, 0 ...) x B_idx row j (hi_j, lo_j, 0 ...) with
 //    64 hi_j + lo_j = 127 - j: the accumulator of column j of a train tile becomes  4096 * dot + (127 - j),  i.e. the
 //    (dot product, lowest-column-wins) key the arg-max needs is produced BY THE TENSOR CORE, and the epilogue is a plain
-//    three-input maximum (VIMNMX3) per two elements.
+//    three-input maximum (VIMNMX3) per two elements.  Against adding the column term on the ALU (one IADD3 per element) in
+//    the same warp-specialised structure, the extra MMA is the faster of the two: 0.104-0.106 ms vs 0.108-0.109 ms per C2
+//    launch on an H100 80GB HBM3 at 700 W and 1980 MHz (DESIGN.md section 5).  The tensor pipe is not what binds this kernel.
 // Exactness: |4096 dot| <= 2^20, 127 - j in [0, 128), global key = acc + (3968 - 128 tile) = 4096 dot + (4095 - col) with
 // col <= 4095 -- all exact in int32; dot = key >> 12 (arithmetic), col = 4095 - (key & 4095).
 //
-// 512 threads = four warp groups of 64 query rows.  Per item: all threads expand the 256 query rows (two threads per row) and
-// train tile 0; then per train tile n: every warp group issues its nine MMAs asynchronously, all threads expand tile n+1 into
-// the other half of the double-buffered B area (four threads per row), wait for the MMAs, and take the row maxima.
-// Shared memory: A 64 KiB + B 2 x 32 KiB + the two 4 KiB index blocks.
-constexpr int kXThreads = 512;
+// Warp-specialised, 640 threads = five warp groups, one CTA per SM, persistent:
+//  * warp groups 0-3 (consumers, 64 query rows each): wait for an operand stage, issue the nine m64n128k32 MMAs of a train
+//    tile, release the stage after their wgmma.wait_group, take the row maxima.  No CTA-wide barrier inside the item loop:
+//    the groups drift apart, so one group's epilogue runs under the others' MMAs;
+//  * warp group 4 (producer): claims work items from the launch's ticket counter, fetches the next item's 256 query rows
+//    (8 KiB) with one cp.async.bulk while the current item runs, prefetches each train tile's rows (one row per thread) into
+//    registers one tile ahead, and expands them into a ring of kXStages B stages and into the A area (each consumer group's
+//    16 KiB slice is refilled as soon as that group has finished its last tile of the previous item).  Stages are published
+//    with fence.proxy.async + an mbarrier arrive.
+// The producer's order per item is B0, B1, A, B2, ...: the first two train tiles of the next item are expanded while the
+// consumers still run the previous one (a ring of >= 2 stages keeps that order deadlock-free: B tile j of an item only waits
+// for stages of earlier items, or, for j >= 2, of tiles whose A has been published).
+// Shared memory: A 64 KiB + kXStages x 32 KiB + the two 4 KiB index blocks + 2 x 8 KiB raw query staging + barriers.
+constexpr int kXConsumerGroups = 4;
+constexpr int kXThreads = (kXConsumerGroups + 1) * 128;
+constexpr int kXStages = 4;
+constexpr uint32_t kXRawA = 256 * 32;  // raw query rows of one item
 constexpr uint32_t kXBOff = kA256;
-constexpr uint32_t kXIdxOff = kXBOff + 2 * kB128;
-constexpr uint32_t kXSmemBytes = kXIdxOff + 2 * 4096;
+constexpr uint32_t kXIdxOff = kXBOff + kXStages * kB128;
+constexpr uint32_t kXRawOff = kXIdxOff + 2 * 4096;
+constexpr uint32_t kXBarsOff = kXRawOff + 2 * kXRawA;
+constexpr int kXBarAFull = 0, kXBarAEmpty = kXConsumerGroups, kXBarBFull = 2 * kXConsumerGroups,
+              kXBarBEmpty = kXBarBFull + kXStages, kXBarRaw = kXBarBEmpty + kXStages, kXNumBars = kXBarRaw + 2;
+constexpr uint32_t kXSmemBytes = kXBarsOff + 8 * kXNumBars + 4 * (kXConsumerGroups + 2);
 static_assert(kXSmemBytes <= 232448, "tc_hamming_expand: shared memory over the 227 KiB per-CTA limit");
+// Registers: 640 threads start with 65536 / 640 -> 96 each.  The producer gives registers back, the consumers take them:
+constexpr int kXLaunchRegs = 96, kXProducerRegs = 64, kXConsumerRegs = 104;
+static_assert(kXConsumerGroups * 128 * kXConsumerRegs + 128 * kXProducerRegs <= kXThreads * kXLaunchRegs,
+              "tc_hamming_expand: setmaxnreg budget over the registers the CTA is launched with");
+
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+// barrier 1 among the producer warp group's 128 threads (barrier 0 is __syncthreads)
+__device__ __forceinline__ void producer_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
 
 // 4 descriptor bits (bits 0-3 of x, x < 16) -> 4 int8: bit set -> +64, clear -> -64
 // (x & 0x80808080) ^ 0xC0C0C0C0 in ONE LOP3 (immLut (a & b) ^ c = (0xF0 & 0xCC) ^ 0xAA = 0x6A): bit 7 of every byte of x selects
@@ -367,25 +402,137 @@ __device__ __forceinline__ void expand_word(uint32_t row_addr, int wi, uint32_t 
 }
 __device__ __forceinline__ uint32_t row_offset(int r) { return (uint32_t)(r >> 3) * kGroupStride + (uint32_t)(r & 7) * 16u; }
 
-// train tile nb of the item -> the B buffer at dst (four threads per row, two descriptor words each; missing rows: zeros)
-__device__ __forceinline__ uint2 load_b_words(const HamItem& item, int nb) {
-  const int r = threadIdx.x >> 2, row = nb * 128 + r;
-  if (row < item.nsearch) return __ldg(reinterpret_cast<const uint2*>(item.b) + 4 * (size_t)row + (threadIdx.x & 3));
-  return make_uint2(0, 0);
-}
-__device__ __forceinline__ void store_b_words(uint32_t dst, uint2 v) {
-  const int r = threadIdx.x >> 2, w0 = 2 * (threadIdx.x & 3);
-  expand_word(dst + row_offset(r), w0, v.x);
-  expand_word(dst + row_offset(r), w0 + 1, v.y);
+// generic-proxy operand stores of this warp -> visible to the tensor core (async proxy) once `bar` completes
+__device__ __forceinline__ void publish(uint32_t bar) {
+  fence_proxy_async_smem();
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-__global__ void __launch_bounds__(kXThreads, 1) tc_hamming_expand_kernel(const HamItem* __restrict__ items, int n_items) {
+// The train rows of one item the producer needs (a whole HamItem would not fit its register budget).
+struct TrainRows {
+  const uint4* b;
+  int nsearch, n_btiles;
+};
+// row `r` of train tile nb (32 B; rows past the searched ones are zeros -- their columns are masked in the epilogue)
+__device__ __forceinline__ void load_train_row(const TrainRows& t, int nb, int r, uint4& v0, uint4& v1) {
+  const int row = nb * 128 + r;
+  v0 = v1 = make_uint4(0, 0, 0, 0);
+  if (row < t.nsearch) {
+    v0 = __ldg(t.b + 2 * (size_t)row);
+    v1 = __ldg(t.b + 2 * (size_t)row + 1);
+  }
+}
+
+__device__ __forceinline__ void hamming_producer(const HamItem* __restrict__ items, int n_items, unsigned long long* claim,
+                                                 unsigned long long claim_base, uint32_t sA, uint32_t sB, uint32_t sRaw,
+                                                 uint32_t bars, volatile int* s_item) {
+  setmaxnreg_dec<kXProducerRegs>();
+  const int pt = threadIdx.x - kXConsumerGroups * 128;  // 0..127
+  auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
+  // Claims the CTA's item number k (-1: none left) and starts the bulk copy of its query rows into raw buffer k & 1.  A CTA
+  // stops after its first -1, so a launch takes exactly n_items + gridDim.x tickets (the host advances claim_base by that).
+  auto claim_item = [&](uint32_t k) -> int {
+    if (pt == 0) {
+      const unsigned long long t = atomicAdd(claim, 1ull) - claim_base;
+      s_item[kXConsumerGroups + (k & 1)] = t < (unsigned long long)n_items ? (int)t : -1;
+    }
+    producer_bar_sync();  // publishes the claim; every thread is done expanding from raw buffer k & 1 (item k - 2)
+    const int it = s_item[kXConsumerGroups + (k & 1)];
+    if (pt == 0 && it >= 0) {
+      const uint32_t bytes = 32u * (uint32_t)items[it].nq_valid, rb = bar(kXBarRaw + (int)(k & 1));
+      mbar_expect_tx(rb, bytes);
+      bulk_g2s(sRaw + (k & 1) * kXRawA, items[it].a, bytes, rb);
+    }
+    return it;
+  };
+  auto train_rows = [&](int it) {
+    TrainRows t{nullptr, 0, 0};
+    if (it >= 0) t = TrainRows{reinterpret_cast<const uint4*>(items[it].b), items[it].nsearch, items[it].n_btiles};
+    return t;
+  };
+  // item k's query rows -> each consumer group's A slice as soon as that group has finished item k - 1 (it = -1: end marker)
+  auto produce_a = [&](uint32_t k, int it) {
+    if (it >= 0) mbar_wait(bar(kXBarRaw + (int)(k & 1)), (k >> 1) & 1u);
+    const int r = pt >> 1, hw = pt & 1;  // two threads per query row, four descriptor words each
+#pragma unroll 1
+    for (int g = 0; g < kXConsumerGroups; g++) {
+      mbar_wait(bar(kXBarAEmpty + g), (k & 1u) ^ 1u);
+      if (it >= 0) {
+        const uint4 v = lds128(sRaw + (k & 1) * kXRawA + (uint32_t)(g * 64 + r) * 32u + 16u * hw);
+        const uint32_t ra = sA + (uint32_t)g * kWgRows + row_offset(r);
+        expand_word(ra, 4 * hw, v.x);
+        expand_word(ra, 4 * hw + 1, v.y);
+        expand_word(ra, 4 * hw + 2, v.z);
+        expand_word(ra, 4 * hw + 3, v.w);
+      }
+      if (pt == 0) s_item[g] = it;
+      publish(bar(kXBarAFull + g));
+    }
+  };
+
+  uint32_t k = 0, s = 0;  // items claimed by this CTA, B stages produced
+  int cur = claim_item(0);
+  TrainRows ct = train_rows(cur);
+  uint4 p0, p1;  // this thread's row (pt) of the next train tile to expand
+  load_train_row(ct, 0, pt, p0, p1);
+  for (; cur >= 0; k++) {
+    const int nxt = claim_item(k + 1);
+    const TrainRows nt = train_rows(nxt);
+    if (ct.n_btiles == 0) {  // no train rows (nt <= 1): every query row gets "no match"; the next item's tile 0 comes now
+      produce_a(k, cur);
+      load_train_row(nt, 0, pt, p0, p1);
+    }
+#pragma unroll 1
+    for (int nb = 0; nb < ct.n_btiles; nb++, s++) {
+      const uint4 v0 = p0, v1 = p1;
+      if (nb + 1 < ct.n_btiles) load_train_row(ct, nb + 1, pt, p0, p1);
+      else load_train_row(nt, 0, pt, p0, p1);
+      const uint32_t slot = s % kXStages;
+      mbar_wait(bar(kXBarBEmpty + (int)slot), ((s / kXStages) & 1u) ^ 1u);
+      const uint32_t dst = sB + slot * kB128 + row_offset(pt);
+      expand_word(dst, 0, v0.x);
+      expand_word(dst, 1, v0.y);
+      expand_word(dst, 2, v0.z);
+      expand_word(dst, 3, v0.w);
+      expand_word(dst, 4, v1.x);
+      expand_word(dst, 5, v1.y);
+      expand_word(dst, 6, v1.z);
+      expand_word(dst, 7, v1.w);
+      publish(bar(kXBarBFull + (int)slot));
+      if (nb == min(1, ct.n_btiles - 1)) produce_a(k, cur);
+    }
+    cur = nxt;
+    ct = nt;
+  }
+  produce_a(k, -1);
+}
+
+__global__ void __launch_bounds__(kXThreads, 1)
+    tc_hamming_expand_kernel(const HamItem* __restrict__ items, int n_items, unsigned long long* __restrict__ claim,
+                             unsigned long long claim_base) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t sA = smem_u32(smem);
-  const uint32_t sB = sA + kXBOff;
+  const uint32_t sB = sA + kXBOff, sRaw = sA + kXRawOff, bars = sA + kXBarsOff;
   const uint32_t sIdxA = sA + kXIdxOff, sIdxB = sIdxA + 4096;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // [0, 4): the item in each consumer group's A slice (-1: no more); [4, 6): the producer's claims
+  volatile int* s_item = reinterpret_cast<volatile int*>(smem + kXBarsOff + 8 * kXNumBars);
+  auto bar = [&](int i) { return bars + 8u * (uint32_t)i; };
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
 
+  if (threadIdx.x == 0) {
+    for (int g = 0; g < kXConsumerGroups; g++) {
+      mbar_init(bar(kXBarAFull + g), 4);   // the producer's four warps
+      mbar_init(bar(kXBarAEmpty + g), 4);  // the group's four warps
+    }
+    for (int i = 0; i < kXStages; i++) {
+      mbar_init(bar(kXBarBFull + i), 4);
+      mbar_init(bar(kXBarBEmpty + i), 4 * kXConsumerGroups);
+    }
+    mbar_init(bar(kXBarRaw), 1);
+    mbar_init(bar(kXBarRaw + 1), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
   if (threadIdx.x < 128) {
     // index blocks, K-major no-swizzle: [row_group 16][k_chunk 2][row 8][16 B]; only bytes 0 and 1 of a row are non-zero
     const int r = threadIdx.x;
@@ -395,66 +542,68 @@ __global__ void __launch_bounds__(kXThreads, 1) tc_hamming_expand_kernel(const H
     const uint32_t rem = 127u - (uint32_t)r;    // 64 * hi + lo
     sts128(sIdxB + off, (rem >> 6) | ((rem & 63u) << 8), 0, 0, 0);
     sts128(sIdxB + off + 128u, 0, 0, 0, 0);
+    fence_proxy_async_smem();
   }
-  const int wg = warp >> 2;
-  const int r0 = 16 * (warp & 3) + (lane >> 2);  // this thread's accumulator rows: r0 and r0 + 8 of the warp group's 64
+  __syncthreads();
+
+  if (wg == kXConsumerGroups) {
+    hamming_producer(items, n_items, claim, claim_base, sA, sB, sRaw, bars, s_item);
+    return;
+  }
+
+  setmaxnreg_inc<kXConsumerRegs>();
+  const int r0 = 16 * (warp & 3) + (lane >> 2);  // this thread's accumulator rows: r0 and r0 + 8 of the group's 64
   const int cq = 2 * (lane & 3);                 // and columns cq, cq + 1 of every 8-column block
   const uint64_t da = make_desc(sA + wg * kWgRows, 128, kGroupStride);
   const uint64_t dia = make_desc(sIdxA, 128, 256), dib = make_desc(sIdxB, 128, 256);
   uint32_t d[64];
-
-  for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+  uint32_t s = 0;  // B stages consumed
+  for (uint32_t k = 0;; k++) {
+    mbar_wait(bar(kXBarAFull + wg), k & 1u);
+    const int it = s_item[wg];
+    if (it < 0) break;
     const HamItem item = items[it];
-    __syncthreads();  // every MMA of the previous item has completed: A and both B buffers may be rewritten
-    {
-      const int r = threadIdx.x >> 1, hw = threadIdx.x & 1;  // two threads per query row, four descriptor words each
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (r < item.nq_valid) v = __ldg(reinterpret_cast<const uint4*>(item.a) + 2 * (size_t)r + hw);
-      const uint2 b0 = item.n_btiles > 0 ? load_b_words(item, 0) : make_uint2(0, 0);
-      const uint32_t ra = sA + row_offset(r);
-      expand_word(ra, 4 * hw, v.x);
-      expand_word(ra, 4 * hw + 1, v.y);
-      expand_word(ra, 4 * hw + 2, v.z);
-      expand_word(ra, 4 * hw + 3, v.w);
-      if (item.n_btiles > 0) store_b_words(sB, b0);
-    }
-    fence_proxy_async_smem();  // generic-proxy operand writes -> visible to the tensor core's (async proxy) reads
-    __syncthreads();
     int best[2] = {kNoBest, kNoBest};
-    for (int nb = 0; nb < item.n_btiles; nb++) {
-      const uint64_t db = make_desc(sB + (uint32_t)(nb & 1) * kB128, 128, kGroupStride);
+#pragma unroll 1
+    for (int nb = 0; nb < item.n_btiles; nb++, s++) {
+      const uint32_t slot = s % kXStages;
+      mbar_wait(bar(kXBarBFull + (int)slot), (s / kXStages) & 1u);
+      const uint64_t db = make_desc(sB + slot * kB128, 128, kGroupStride);
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 8; ks++) wgmma_s8(d, da + (uint64_t)((ks * 256) >> 4), db + (uint64_t)((ks * 256) >> 4), ks > 0 ? 1u : 0u);
       wgmma_s8(d, dia, dib, 1u);
       wgmma_commit();
-      if (nb + 1 < item.n_btiles) store_b_words(sB + (uint32_t)((nb + 1) & 1) * kB128, load_b_words(item, nb + 1));
       wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar(kXBarBEmpty + (int)slot));
       const int nvalid = item.nsearch - nb * 128;  // train rows of this tile that exist (>= 128: all)
+      // key of column 8 i + cq + e of the tile, in this thread's row r0 + 8 h
+      auto key = [&](int i, int e, int h) { return (int)d[4 * i + 2 * h + e]; };
 #pragma unroll
       for (int h = 0; h < 2; h++) {
         int m = kNoBest;
         if (nvalid >= 128) {
-          int m0 = __vimax3_s32((int)d[2 * h], (int)d[2 * h + 1], (int)d[4 + 2 * h]);
-          int m1 = __vimax3_s32((int)d[4 + 2 * h + 1], (int)d[8 + 2 * h], (int)d[8 + 2 * h + 1]);
+          int m0 = __vimax3_s32(key(0, 0, h), key(0, 1, h), key(1, 0, h));
+          int m1 = __vimax3_s32(key(1, 1, h), key(2, 0, h), key(2, 1, h));
 #pragma unroll
           for (int i = 3; i < 15; i += 2) {
-            m0 = __vimax3_s32(m0, (int)d[4 * i + 2 * h], (int)d[4 * i + 2 * h + 1]);
-            m1 = __vimax3_s32(m1, (int)d[4 * i + 4 + 2 * h], (int)d[4 * i + 4 + 2 * h + 1]);
+            m0 = __vimax3_s32(m0, key(i, 0, h), key(i, 1, h));
+            m1 = __vimax3_s32(m1, key(i + 1, 0, h), key(i + 1, 1, h));
           }
-          m = __vimax3_s32(m0, m1, max((int)d[60 + 2 * h], (int)d[60 + 2 * h + 1]));
+          m = __vimax3_s32(m0, m1, max(key(15, 0, h), key(15, 1, h)));
         } else {
 #pragma unroll
           for (int i = 0; i < 16; i++) {
-            if (8 * i + cq < nvalid) m = max(m, (int)d[4 * i + 2 * h]);
-            if (8 * i + cq + 1 < nvalid) m = max(m, (int)d[4 * i + 2 * h + 1]);
+            if (8 * i + cq < nvalid) m = max(m, key(i, 0, h));
+            if (8 * i + cq + 1 < nvalid) m = max(m, key(i, 1, h));
           }
         }
         if (m != kNoBest) best[h] = max(best[h], m + (3968 - 128 * nb));  // 4096 dot + (4095 - col)
       }
-      fence_proxy_async_smem();
-      __syncthreads();  // tile nb+1 is complete, and every warp group is done with tile nb's buffer
     }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar(kXBarAEmpty + wg));  // every MMA of this item has completed: the A slice may be refilled
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       int b = best[h];
@@ -474,7 +623,7 @@ __global__ void __launch_bounds__(kXThreads, 1) tc_hamming_expand_kernel(const H
   }
 }
 
-cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm_count, cudaStream_t stream) {
+cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm_count, ClaimCounter& claim, cudaStream_t stream) {
   if (n_items <= 0) return cudaSuccess;
   static bool attr_set = false;
   if (!attr_set) {
@@ -483,8 +632,10 @@ cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm
     attr_set = true;
   }
   const int grid = n_items < sm_count ? n_items : sm_count;
-  tc_hamming_expand_kernel<<<grid, kXThreads, kXSmemBytes, stream>>>(d_items, n_items);
-  return cudaGetLastError();
+  tc_hamming_expand_kernel<<<grid, kXThreads, kXSmemBytes, stream>>>(d_items, n_items, claim.ticket, claim.base);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) claim.base += (unsigned long long)(n_items + grid);
+  return e;
 }
 
 }  // namespace rb200

@@ -11,9 +11,17 @@ cudaError_t set_dev_params(const DevParams& p, cudaStream_t stream);
 cudaError_t launch_hamming_simt(const PairDesc* pairs, int npairs, int max_nq, int2* best, int stride,
                                 cudaStream_t stream);
 
+// Work-item counter of a persistent kernel whose CTAs claim items dynamically: `ticket` (device) only grows, `base` is its
+// value when the next launch on the owner's stream starts.  One per slot, since slots run concurrently on their own streams.
+struct ClaimCounter {
+  unsigned long long* ticket = nullptr;
+  unsigned long long base = 0;
+};
+
 // Hamming brute force on the tensor cores, 32-byte descriptors expanded to int8 operands inside the kernel (HamItem::a / b =
-// descriptor rows); same output as launch_hamming_simt.
-cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm_count, cudaStream_t stream);
+// descriptor rows); same output as launch_hamming_simt.  Advances claim.base past the tickets the launch takes.
+cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm_count, ClaimCounter& claim,
+                                     cudaStream_t stream);
 cudaError_t launch_l2_tc256(const HamItem* d_items, int n_items, int sm_count, cudaStream_t stream);
 
 // SIFT-128 path (sift_l2.cu / hamming_tc.cu MODE 1)

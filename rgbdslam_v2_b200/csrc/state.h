@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "kernels.h"
 
 namespace rb200 {
 
@@ -77,9 +78,11 @@ struct Workspace {
   DevBuf d_feat_a, d_feat_b, d_xyz_a, d_xyz_b;
   DevBuf d_jobs, d_items, d_top4, d_knn, d_cen, d_nextn;
   PinBuf h_pairs, h_jobs, h_items;
+  DevBuf d_claim;      // ticket of claim (zeroed when allocated)
+  ClaimCounter claim;  // work-item counter of the ORB match kernel
   void release() {
     DevBuf* all[] = {&d_pairs, &d_best, &d_matches, &d_inliers, &d_mfrom, &d_mto, &d_nall, &d_hyp, &d_results, &d_feat_a,
-                     &d_feat_b, &d_xyz_a, &d_xyz_b, &d_jobs, &d_items, &d_top4, &d_knn, &d_cen, &d_nextn};
+                     &d_feat_b, &d_xyz_a, &d_xyz_b, &d_jobs, &d_items, &d_top4, &d_knn, &d_cen, &d_nextn, &d_claim};
     for (DevBuf* b : all) b->release();
     h_pairs.release();
     h_jobs.release();
