@@ -104,11 +104,12 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   // visual CV_8UC1, depth CV_32FC1 metres (NaN = invalid), detection_mask CV_8UC1 non-zero at potential keypoint locations
   // (node.h:61-63).  detector / extractor: createDetector / createDescriptorExtractor (features.hpp); the whole constructor
   // -- detect, removeDepthless, retainBest, compute, projectTo3D -- runs as one rgbdslam_b200_nodes_create call, the
-  // extractor argument only documents the pairing (ORB with ORB).  id_ stays -1 until GraphManager::addNode assigns it.
+  // extractor argument only documents the pairing (ORB or FAST keypoints, ORB descriptors).  id_ stays -1 until
+  // GraphManager::addNode assigns it.
   Node(const Mat& visual, const Mat& depth, const Mat& detection_mask, const CameraInfoConstPtr& cam_info, myHeader depth_header,
        Ptr<Feature2D> detector, Ptr<DescriptorExtractor> extractor)
       : stamp_(depth_header.stamp) {
-    if (!detector || !detector->handle()) throw std::invalid_argument("Node: detector must come from createDetector(\"ORB\")");
+    if (!detector || !detector->handle()) throw std::invalid_argument("Node: detector must come from createDetector(\"ORB\" or \"FAST\")");
     if (!extractor) throw std::invalid_argument("Node: null extractor");
     if (visual.type() != RB_8UC1 || depth.type() != RB_32FC1 || depth.rows != visual.rows || depth.cols != visual.cols)
       throw std::invalid_argument("Node: visual must be CV_8UC1 and depth CV_32FC1 of the same size");

@@ -598,6 +598,11 @@ int rgbdslam_b200_init(int device, const rgbdslam_b200_params* p) {
     set_error("use_feature_min_depth / allow_features_without_depth are not supported (reference defaults: false)");
     return RGBDSLAM_B200_ERR_ARG;
   }
+  if (prm.feature_detector_type != RGBDSLAM_B200_DETECTOR_ORB && prm.feature_detector_type != RGBDSLAM_B200_DETECTOR_FAST) {
+    // parameter_server.cpp:80; SIFT / SURF need OpenCV's non-free module and are not built
+    set_error("invalid parameters (feature_detector_type must be RGBDSLAM_B200_DETECTOR_ORB (0) or RGBDSLAM_B200_DETECTOR_FAST (1))");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess) return cuda_fail(e, "cudaGetDeviceCount (no CUDA device: this library has no CPU fallback)");

@@ -13,6 +13,12 @@
 //     k_frame_finalize                    one CTA per frame
 //   extractor->compute(gray, kp, desc)    cv::ORB::create() defaults (features.cpp:117-119)
 //     k_resize / k_blur / k_describe      full-image pyramid, 7-tap float Gaussian, steered BRIEF (one warp / keypoint)
+//
+// The FAST detector (feature_detector_type FAST: DetectorAdjuster("FAST", 20) -> cv::FastFeatureDetector::create(thresh),
+// feature_adjuster.cpp:88-91, under the same dynamic and grid wrappers) runs the same chain on level 0 only: k_cell_extract
+// (no k_resize_cells), k_fast9_nms (the k_fast_nms body with cv::FAST's 3 px frame, whose scores read as 0 in the NMS),
+// k_adapt_thresholds, k_fast_response (response = S) in place of k_harris, k_cell_select, k_frame_finalize,
+// k_frame_emit_fast (size 7, angle -1, no orientation) and level 0 of the extractor pyramid.
 #include "orb.cuh"
 
 #include <cuda_runtime.h>
@@ -30,13 +36,17 @@ constexpr int kFT_W = 56, kFT_H = 30;  // output pixels per CTA
 constexpr int kFS_W = 64, kFS_H = 32;  // scores computed per CTA: x in [-4, 60), y in [-1, 31) relative to the tile origin
 constexpr int kFI_W = 72, kFI_H = 38;  // image pixels staged: x in [-8, 64), y in [-4, 34)
 constexpr int kFastEdge = 15;          // ORB::create(..., edgeThreshold = 15, ...)  feature_adjuster.cpp:94
+constexpr int kFast9Edge = 3;          // cv::FAST scores rows / columns [3, n-4] only
 
 struct FastTiling {  // tiles of the fused kernel: per level the tile grid of the LARGEST cell, prefix sums over levels
   int32_t tiles_x[kOrbLevels], tiles_y[kOrbLevels], first[kOrbLevels + 1];
 };
-__constant__ FastTiling c_fast_tiling;
+__constant__ FastTiling c_fast_tiling;  // ORB detector (all levels)
 
-static int g_fast_tiles = 0;  // CTAs per (frame, cell) of the fused FAST + NMS kernel
+// CTAs per (frame, cell) of the fused FAST + NMS kernel, per detector type; the FAST detector tiles level 0 only, with its
+// own border, and takes its tile-grid width as a kernel argument
+static int g_fast_tiles[2] = {0, 0};
+static int g_fast9_tiles_x = 1;
 
 cudaError_t orb_upload_constants(const OrbGeom& g, const int* umax, cudaStream_t st) {
   cudaError_t e = cudaMemcpyToSymbolAsync(c_geom, &g, sizeof(OrbGeom), 0, cudaMemcpyHostToDevice, st);
@@ -62,7 +72,18 @@ cudaError_t orb_upload_constants(const OrbGeom& g, const int* umax, cudaStream_t
     ft.first[l + 1] = ft.first[l] + ft.tiles_x[l] * ft.tiles_y[l];
     if (ft.tiles_x[l] == 0) ft.tiles_x[l] = 1;  // never divided by for an empty level (no CTA maps to it)
   }
-  g_fast_tiles = ft.first[kOrbLevels];
+  g_fast_tiles[RGBDSLAM_B200_DETECTOR_ORB] = ft.first[kOrbLevels];
+  {
+    int lw = 0, lh = 0;
+    for (int c = 0; c < g.ncells; c++) {
+      lw = g.cell[c][0].w > lw ? g.cell[c][0].w : lw;
+      lh = g.cell[c][0].h > lh ? g.cell[c][0].h : lh;
+    }
+    const int iw = lw - 2 * kFast9Edge, ih = lh - 2 * kFast9Edge;
+    const int tx = iw > 0 ? (iw + kFT_W - 1) / kFT_W : 0, ty = ih > 0 ? (ih + kFT_H - 1) / kFT_H : 0;
+    g_fast_tiles[RGBDSLAM_B200_DETECTOR_FAST] = tx * ty;
+    g_fast9_tiles_x = tx > 0 ? tx : 1;
+  }
   return cudaMemcpyToSymbolAsync(c_fast_tiling, &ft, sizeof(ft), 0, cudaMemcpyHostToDevice, st);
 }
 
@@ -160,21 +181,34 @@ __device__ __forceinline__ uint32_t fast_score_pair(const uint16_t (*simg)[kFI_W
   return __vmaxs2(m, 0x01010101u) - 0x01010101u;  // (max(., 257) - 257) per half = max(A - 1, 0)
 }
 
-__global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
-                                                  OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist) {
+// kFast = false: the ORB detector -- every level, candidates at least 15 px inside the level, whose NMS sees the real scores
+// of the pixels around them.  kFast = true: the FAST detector -- level 0 only (tiles_x9 tiles per row); cv::FAST scores only
+// the pixels [3, n-4] of the cell and its NMS reads every other pixel as score 0, so the scores outside that band are zeroed
+// before the NMS.
+template <bool kFast>
+__device__ __forceinline__ void fast_nms_tile(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
+                                              OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist,
+                                              int tiles_x9) {
+  constexpr int kEdge = kFast ? kFast9Edge : kFastEdge;
   __shared__ __align__(16) uint16_t simg[kFI_H][kFI_W];
   __shared__ __align__(16) uint8_t ssc[kFS_H][kFS_W];
-  int level = 0;
+  int level = 0, tx, ty;
+  if constexpr (kFast) {
+    tx = blockIdx.x % tiles_x9;
+    ty = blockIdx.x / tiles_x9;
+  } else {
 #pragma unroll
-  for (int l = 1; l < kOrbLevels; l++)
-    if ((int)blockIdx.x >= c_fast_tiling.first[l]) level = l;
-  const int t = blockIdx.x - c_fast_tiling.first[level];
-  const int tx = t % c_fast_tiling.tiles_x[level], ty = t / c_fast_tiling.tiles_x[level];
+    for (int l = 1; l < kOrbLevels; l++)
+      if ((int)blockIdx.x >= c_fast_tiling.first[l]) level = l;
+    const int t = blockIdx.x - c_fast_tiling.first[level];
+    tx = t % c_fast_tiling.tiles_x[level];
+    ty = t / c_fast_tiling.tiles_x[level];
+  }
   const int fc = blockIdx.y;
   const int f = fc / c_geom.ncells, c = fc % c_geom.ncells;
   const int pw = c_geom.cell[c][level].w, ph = c_geom.cell[c][level].h;
-  const int ox0 = kFastEdge + tx * kFT_W, oy0 = kFastEdge + ty * kFT_H;
-  if (ox0 >= pw - kFastEdge || oy0 >= ph - kFastEdge) return;
+  const int ox0 = kEdge + tx * kFT_W, oy0 = kEdge + ty * kFT_H;
+  if (ox0 >= pw - kEdge || oy0 >= ph - kEdge) return;
   const size_t base = (size_t)f * c_geom.cell_bytes + c_geom.cell[c][level].off;
   const uint8_t* im = cell_img + base;
   for (int i = threadIdx.x; i < kFI_H * kFI_W; i += 256) {
@@ -187,7 +221,7 @@ __global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ ce
     const int q = threadIdx.x & 15, r0 = threadIdx.x >> 4;
     // rows below the last output row of this tile (+ 1 for the NMS) are never read: skipping them (a warp owns two
     // adjacent rows per pass) removes most of the waste of partially covered tiles
-    const int sy_last = min(kFT_H, ph - kFastEdge - oy0) + 1;
+    const int sy_last = min(kFT_H, ph - kEdge - oy0) + 1;
 #pragma unroll
     for (int pass = 0; pass < 2; pass++) {
       const int sy = r0 + 16 * pass;  // score row (relative y = sy - 1) -> image row sy + 3
@@ -195,15 +229,26 @@ __global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ ce
       const uint32_t s01 = fast_score_pair(simg, sy + 3, 4 * q + 4);
       const uint32_t s23 = fast_score_pair(simg, sy + 3, 4 * q + 6);
       // halves hold 0..254: pack the four scores into bytes
-      reinterpret_cast<uint32_t*>(ssc[sy])[q] = __byte_perm(s01, s23, 0x6420);
+      uint32_t s4 = __byte_perm(s01, s23, 0x6420);
+      if constexpr (kFast) {  // outside cv::FAST's scored band [3, n-4]: score 0
+        const int gy = oy0 + sy - 1, gx = ox0 + 4 * q - 4;
+        uint32_t keep = 0;
+        if (gy >= kEdge && gy < ph - kEdge) {
+#pragma unroll
+          for (int b = 0; b < 4; b++)
+            if (gx + b >= kEdge && gx + b < pw - kEdge) keep |= 0xFFu << (8 * b);
+        }
+        s4 &= keep;
+      }
+      reinterpret_cast<uint32_t*>(ssc[sy])[q] = s4;
     }
   }
   __syncthreads();
-  // strict 3x3 non-maximum suppression on S, runByPixelsMask, runByImageBorder(15) -> candidates + histogram
+  // strict 3x3 non-maximum suppression on S, runByPixelsMask, runByImageBorder(kEdge) -> candidates + histogram
   for (int i = threadIdx.x; i < kFT_W * kFT_H; i += 256) {
     const int oy = i / kFT_W, ox = i - oy * kFT_W;
     const int gx = ox0 + ox, gy = oy0 + oy;
-    if (gx >= pw - kFastEdge || gy >= ph - kFastEdge) continue;
+    if (gx >= pw - kEdge || gy >= ph - kEdge) continue;
     const int sx = ox + 4, sy = oy + 1;
     const int v = ssc[sy][sx];
     if (v < 2) continue;  // the adaptive threshold never drops below 2 (DetectorAdjuster min_thresh)
@@ -223,6 +268,17 @@ __global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ ce
       cand[(size_t)fc * kOrbCandCap + slot] = cd;
     }
   }
+}
+
+__global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
+                                                  OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist) {
+  fast_nms_tile<false>(cell_img, cell_mask, cand, cand_count, hist, 0);
+}
+
+__global__ void __launch_bounds__(256) k_fast9_nms(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
+                                                   OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist,
+                                                   int tiles_x) {
+  fast_nms_tile<true>(cell_img, cell_mask, cand, cand_count, hist, tiles_x);
 }
 
 // All cell planes of one level from the previous level, image and mask together (INTER_LINEAR_EXACT, 8.8 fixed-point taps;
@@ -393,6 +449,17 @@ __global__ void __launch_bounds__(256) k_harris(const uint8_t* __restrict__ cell
     r = harris_response(cell_img + (size_t)f * c_geom.cell_bytes + p.off, p.w, cd.x, cd.y);
   }
   resp[(size_t)fc * kOrbCandCap + i] = r;
+}
+
+// FAST detector: a keypoint's response is its corner score S (cv::FAST); NaN below the cell's final threshold (excluded).
+__global__ void __launch_bounds__(256) k_fast_response(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                       const int* __restrict__ thr, float* __restrict__ resp) {
+  const int fc = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int n = min(cand_count[fc], kOrbCandCap);
+  if (i >= n) return;
+  const int s = cand[(size_t)fc * kOrbCandCap + i].score;
+  resp[(size_t)fc * kOrbCandCap + i] = s >= thr[fc] ? (float)s : __int_as_float(0x7fc00000);
 }
 
 __device__ __forceinline__ uint32_t f32_ordered(float f) {  // ascending unsigned order == ascending float order
@@ -594,10 +661,12 @@ __global__ void __launch_bounds__(1024)
 
 // One warp per output keypoint: intensity-centroid orientation on the detector's (cell) pyramid, the cv::KeyPoint record,
 // in mode 1 projectTo3D (node.cpp:900-965) + backProject (misc2.h:49-65) and the rotation (cos, sin) compute() will use.
-__global__ void __launch_bounds__(256)
-    k_frame_emit(int mode, const FrameKp* __restrict__ scratch, const uint8_t* __restrict__ cell_img, const float* __restrict__ depth,
-                 float depth_scaling, float4 Kinv, rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out,
-                 float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
+// kFast: cv::FAST's KeyPoint(x, y, 7.f, -1, score) -- no orientation; compute() steers the pattern by the angle as given, -1.
+template <bool kFast>
+__device__ __forceinline__ void frame_emit_warp(int mode, const FrameKp* __restrict__ scratch, const uint8_t* __restrict__ cell_img,
+                                                const float* __restrict__ depth, float depth_scaling, float4 Kinv,
+                                                rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out,
+                                                float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
   const int f = blockIdx.y;
   const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (t >= n_out[f]) return;
@@ -605,12 +674,13 @@ __global__ void __launch_bounds__(256)
   const FrameKp* ka = scratch + (size_t)f * 2 * kFrameCap;
   const FrameKp q = (ka + kFrameCap)[reinterpret_cast<const uint16_t*>(ka)[t]];
   const OrbPlane& p = c_geom.cell[q.cell][q.level];
-  const float ang = ic_angle_warp(cell_img + (size_t)f * c_geom.cell_bytes + p.off, p.w, q.lx, q.ly, lane);
+  float ang = -1.f;
+  if constexpr (!kFast) ang = ic_angle_warp(cell_img + (size_t)f * c_geom.cell_bytes + p.off, p.w, q.lx, q.ly, lane);
   if (lane == 0) {
     rgbdslam_b200_keypoint o;
     o.x = q.x;
     o.y = q.y;
-    o.size = __fmul_rn(31.f, p.scale);
+    o.size = kFast ? 7.f : __fmul_rn(31.f, p.scale);
     o.angle = ang;
     o.response = q.resp;
     o.octave = q.level;
@@ -631,6 +701,20 @@ __global__ void __launch_bounds__(256)
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+    k_frame_emit(int mode, const FrameKp* __restrict__ scratch, const uint8_t* __restrict__ cell_img, const float* __restrict__ depth,
+                 float depth_scaling, float4 Kinv, rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out,
+                 float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
+  frame_emit_warp<false>(mode, scratch, cell_img, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
+}
+
+__global__ void __launch_bounds__(256)
+    k_frame_emit_fast(int mode, const FrameKp* __restrict__ scratch, const float* __restrict__ depth, float depth_scaling, float4 Kinv,
+                      rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out, float2* __restrict__ trig_out,
+                      const int* __restrict__ n_out, int kp_stride) {
+  frame_emit_warp<true>(mode, scratch, nullptr, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -727,8 +811,9 @@ __global__ void __launch_bounds__(256) k_describe(const uint8_t* __restrict__ py
 static inline dim3 plane_grid(int w, int h, int z) { return dim3((w + 31) / 32, (h + 7) / 8, z); }
 
 cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, const uint8_t* d_mask,
-                           const float* d_depth_for_mask, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
+                           const float* d_depth_for_mask, int detector, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
                            int* d_cand_count, int* d_hist, int* d_mask_any, cudaStream_t st, int* launches) {
+  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST;
   int maxw = 0, maxh = 0;
   for (int c = 0; c < g.ncells; c++) {
     maxw = g.cell[c][0].w > maxw ? g.cell[c][0].w : maxw;
@@ -741,7 +826,7 @@ cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, 
   k_cell_extract<<<plane_grid(maxw, maxh, z), 256, 0, st>>>(d_gray, d_mask, d_depth_for_mask, d_cell_img, d_cell_mask, d_mask_any);
   (*launches)++;
   const bool all_valid = d_mask == nullptr && d_depth_for_mask == nullptr;  // mask pyramid would stay 255 everywhere
-  for (int l = 1; l < kOrbLevels; l++) {
+  for (int l = 1; l < (fast ? 1 : kOrbLevels); l++) {  // the FAST detector works on level 0 only
     int lw = 0, lh = 0;
     for (int c = 0; c < g.ncells; c++) {
       lw = g.cell[c][l].w > lw ? g.cell[c][l].w : lw;
@@ -750,8 +835,13 @@ cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, 
     k_resize_cells<<<plane_grid(lw, lh, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, l, tab);
     (*launches)++;
   }
-  if (g_fast_tiles > 0) {
-    k_fast_nms<<<dim3(g_fast_tiles, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, d_cand, d_cand_count, d_hist);
+  const int tiles = g_fast_tiles[fast ? RGBDSLAM_B200_DETECTOR_FAST : RGBDSLAM_B200_DETECTOR_ORB];
+  if (tiles > 0) {
+    if (fast)
+      k_fast9_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, d_cand, d_cand_count, d_hist,
+                                                  g_fast9_tiles_x);
+    else
+      k_fast_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, d_cand, d_cand_count, d_hist);
     (*launches)++;
   }
   return cudaGetLastError();
@@ -766,13 +856,17 @@ cudaError_t orb_run_adapt(const OrbGeom& g, int nframes, const int* d_hist, cons
   return cudaGetLastError();
 }
 
-cudaError_t orb_run_select(const OrbGeom& g, int nframes, int mode, int max_per_cell, int max_keypoints,
+cudaError_t orb_run_select(const OrbGeom& g, int nframes, int mode, int detector, int max_per_cell, int max_keypoints,
                            const uint8_t* d_cell_img, const OrbCand* d_cand, const int* d_cand_count, const int* d_thr,
                            float* d_resp, unsigned long long* d_cell_out, int* d_cell_out_count, const float* d_depth,
                            float depth_scaling, float4 Kinv, void* d_scratch, rgbdslam_b200_keypoint* d_kp, float4* d_xyz,
                            float2* d_trig, int* d_n, int kp_stride, cudaStream_t st, int* launches) {
+  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST;
   const int z = nframes * g.ncells;
-  k_harris<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(d_cell_img, d_cand, d_cand_count, d_thr, d_resp);
+  if (fast)
+    k_fast_response<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(d_cand, d_cand_count, d_thr, d_resp);
+  else
+    k_harris<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(d_cell_img, d_cand, d_cand_count, d_thr, d_resp);
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(k_cell_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
@@ -783,24 +877,28 @@ cudaError_t orb_run_select(const OrbGeom& g, int nframes, int mode, int max_per_
   k_frame_finalize<<<nframes, 1024, 0, st>>>(mode, max_keypoints, d_cell_out, d_cell_out_count, max_per_cell, d_cell_img, d_depth,
                                              depth_scaling, Kinv, (FrameKp*)d_scratch, d_kp, d_xyz, d_n, kp_stride);
   const int max_out = mode == 1 ? (max_keypoints < kp_stride ? max_keypoints : kp_stride) : kp_stride;
-  k_frame_emit<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>(mode, (const FrameKp*)d_scratch, d_cell_img, d_depth, depth_scaling,
-                                                                 Kinv, d_kp, d_xyz, d_trig, d_n, kp_stride);
+  if (fast)
+    k_frame_emit_fast<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>(mode, (const FrameKp*)d_scratch, d_depth, depth_scaling, Kinv,
+                                                                         d_kp, d_xyz, d_trig, d_n, kp_stride);
+  else
+    k_frame_emit<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>(mode, (const FrameKp*)d_scratch, d_cell_img, d_depth,
+                                                                   depth_scaling, Kinv, d_kp, d_xyz, d_trig, d_n, kp_stride);
   (*launches) += 4;
   return cudaGetLastError();
 }
 
-cudaError_t orb_run_describe(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, uint8_t* d_pyr_raw,
-                             uint8_t* d_pyr_blur, const rgbdslam_b200_keypoint* d_kp, const int* d_n, int kp_stride, int max_kp,
-                             const float2* d_trig, uint8_t* d_desc, cudaStream_t st, int* launches) {
+cudaError_t orb_run_describe(const OrbGeom& g, const OrbTables& tab, int nframes, int levels, const uint8_t* d_gray,
+                             uint8_t* d_pyr_raw, uint8_t* d_pyr_blur, const rgbdslam_b200_keypoint* d_kp, const int* d_n,
+                             int kp_stride, int max_kp, const float2* d_trig, uint8_t* d_desc, cudaStream_t st, int* launches) {
   // level 0 = the image itself
   cudaError_t e = cudaMemcpy2DAsync(d_pyr_raw, g.full_bytes, d_gray, (size_t)g.W * g.H, (size_t)g.W * g.H, nframes,
                                     cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return e;
-  for (int l = 1; l < kOrbLevels; l++) {
+  for (int l = 1; l < levels; l++) {
     k_resize<<<plane_grid(g.full[l].w, g.full[l].h, nframes), 256, 0, st>>>(d_pyr_raw, g.full_bytes, l, tab);
     (*launches)++;
   }
-  for (int l = 0; l < kOrbLevels; l++) {
+  for (int l = 0; l < levels; l++) {
     k_blur<<<dim3((g.full[l].w + 31) / 32, (g.full[l].h + 15) / 16, nframes), 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
     (*launches)++;
   }
