@@ -44,7 +44,7 @@ class Params(C.Structure):
         ("max_translation_meter", C.c_double), ("max_rotation_degree", C.c_double),
         ("nn_distance_ratio", C.c_double), ("use_root_sift", C.c_int32), ("g2o_transformation_refinement", C.c_int32), ("observability_threshold", C.c_double), ("emm_skip_step", C.c_int32),
         ("cloud_creation_skip_step", C.c_int32), ("minimum_depth", C.c_float),
-        ("use_feature_min_depth_", C.c_uint8), ("allow_features_without_depth_", C.c_uint8),
+        ("use_feature_min_depth", C.c_uint8), ("allow_features_without_depth_", C.c_uint8),
         ("feature_detector_type", C.c_uint8), ("reserved_", C.c_uint8),
     ]
 

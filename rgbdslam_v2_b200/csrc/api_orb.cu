@@ -45,7 +45,7 @@ struct OrbCtx {
   PinBuf stage[2];                             // pinned staging for callers that pass pageable memory
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
-  DevBuf cell_img, cell_mask, cand, cand_count, hist, mask_any, thr, resp, cell_out, cell_out_count, scratch, kp, xyz, n,
+  DevBuf cell_img, cell_mask, cand, cand_count, hist, mask_any, thr, resp, cell_out, cell_out_count, cand_z, scratch, kp, xyz, n,
       pyr_raw, pyr_blur, desc, err, trig;
   // rgbdslam_b200_nodes_create_sharded: what must survive between the detection pass and the finishing pass of ALL own frames,
   // and the per-(frame, cell) tables every rank holds for ALL frames of the sequence
@@ -53,7 +53,7 @@ struct OrbCtx {
   const uint8_t* last_gray = nullptr;  // device pointers of frame 0 of the last call (debug hooks)
   void release() {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &cell_img,
-                     &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp, &cell_out, &cell_out_count, &scratch,
+                     &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp, &cell_out, &cell_out_count, &cand_z, &scratch,
                      &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand,
                      &all_hist, &all_cnt, &all_many, &all_thr};
     for (DevBuf* b : all) b->release();
@@ -249,7 +249,7 @@ static int orb_ensure_buffers(int F, int nbuf, bool want_mask) {
       (rc = o.cand_count.ensure(z * 4)) || (rc = o.hist.ensure(z * 256 * 4)) || (rc = o.mask_any.ensure(z * 4)) ||
       (rc = o.thr.ensure(z * 4)) || (rc = o.resp.ensure(z * kOrbCandCap * 4)) ||
       (rc = o.cell_out.ensure(z * (size_t)o.max_per_cell * 8)) || (rc = o.cell_out_count.ensure(z * 4)) ||
-      (rc = o.scratch.ensure((size_t)F * 2 * kOrbFrameCap * 24)) ||
+      (rc = o.cand_z.ensure(z * (size_t)o.max_per_cell * 4)) || (rc = o.scratch.ensure((size_t)F * 2 * kOrbFrameCap * kOrbFrameKpBytes)) ||
       (rc = o.kp.ensure((size_t)F * o.kp_stride * sizeof(rgbdslam_b200_keypoint))) ||
       (rc = o.xyz.ensure((size_t)F * o.kp_stride * 16)) || (rc = o.n.ensure((size_t)F * 4)) ||
       (rc = o.pyr_raw.ensure((size_t)g.full_bytes * F)) || (rc = o.pyr_blur.ensure((size_t)g.full_bytes * F)) ||
@@ -532,8 +532,8 @@ int rgbdslam_b200_orb_detect(uint64_t detector, const uint8_t* gray, const uint8
   e = orb_run_select(o.g, 1, 0, det->type, o.max_per_cell, g_state.params.max_keypoints, (const uint8_t*)o.cell_img.ptr,
                      (const OrbCand*)o.cand.ptr, (const int*)o.cand_count.ptr, (const int*)o.thr.ptr, (float*)o.resp.ptr,
                      (unsigned long long*)o.cell_out.ptr, (int*)o.cell_out_count.ptr, nullptr, 1.f, make_float4(0, 0, 0, 0),
-                     o.scratch.ptr, (rgbdslam_b200_keypoint*)o.kp.ptr, (float4*)o.xyz.ptr, nullptr, (int*)o.n.ptr, o.kp_stride, st,
-                     &launches);
+                     o.scratch.ptr, (rgbdslam_b200_keypoint*)o.kp.ptr, (float4*)o.xyz.ptr, nullptr, (int*)o.n.ptr, o.kp_stride, false,
+                     nullptr, st, &launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb select kernels");
   int n = 0, flag = 0;
   e = cudaMemcpyAsync(&n, o.n.ptr, 4, cudaMemcpyDeviceToHost, st);
@@ -620,6 +620,7 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   State& s = g_state;
   const bool mask_from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
   if (mask_from_depth) mask = nullptr;
+  const bool min_depth = s.params.use_feature_min_depth != 0;  // getMinDepthInNeighborhood (node.cpp:82-83, 940-941)
   if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const int chunk = std::min(nframes, kOrbChunk);
@@ -652,7 +653,8 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     e = orb_run_select(o.g, F, 1, det->type, o.max_per_cell, s.params.max_keypoints, (const uint8_t*)o.cell_img.ptr,
                        (const OrbCand*)o.cand.ptr, (const int*)o.cand_count.ptr, (const int*)o.thr.ptr, (float*)o.resp.ptr,
                        (unsigned long long*)o.cell_out.ptr, (int*)o.cell_out_count.ptr, dd, (float)s.params.depth_scaling_factor, Kinv,
-                       o.scratch.ptr, nb.kp + (size_t)f0 * K, nb.xyz + (size_t)f0 * K, (float2*)o.trig.ptr, nb.n + f0, K, st, &launches);
+                       o.scratch.ptr, nb.kp + (size_t)f0 * K, nb.xyz + (size_t)f0 * K, (float2*)o.trig.ptr, nb.n + f0, K, min_depth,
+                       (float*)o.cand_z.ptr, st, &launches);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb select kernels"));
     e = orb_run_describe(o.g, o.tab, F, det->describe_levels(), dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, nb.kp + (size_t)f0 * K, nb.n + f0, K, K,
                          (const float2*)o.trig.ptr, nb.desc + (size_t)f0 * K * 32, st, &launches);
@@ -698,6 +700,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   }
   const bool mask_from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
   if (mask_from_depth) mask = nullptr;
+  const bool min_depth = s.params.use_feature_min_depth != 0;  // getMinDepthInNeighborhood (node.cpp:82-83, 940-941)
   if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
@@ -770,7 +773,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     e = orb_run_select(g, F, 1, det->type, o.max_per_cell, s.params.max_keypoints, cimg, (const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
                        cnt_all + gf * nc, thr_all + gf * nc, (float*)o.resp.ptr, (unsigned long long*)o.cell_out.ptr,
                        (int*)o.cell_out_count.ptr, dd, (float)s.params.depth_scaling_factor, Kinv, o.scratch.ptr, nb.kp + (size_t)c0 * K,
-                       nb.xyz + gf * K, (float2*)o.trig.ptr, nb.n + gf, K, st, &launches);
+                       nb.xyz + gf * K, (float2*)o.trig.ptr, nb.n + gf, K, min_depth, (float*)o.cand_z.ptr, st, &launches);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb select kernels"));
     e = orb_run_describe(g, o.tab, F, det->describe_levels(), dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, nb.kp + (size_t)c0 * K, nb.n + gf, K, K,
                          (const float2*)o.trig.ptr, nb.desc + gf * K * 32, st, &launches);

@@ -19,9 +19,14 @@
 // (no k_resize_cells), k_fast9_nms (the k_fast_nms body with cv::FAST's 3 px frame, whose scores read as 0 in the NMS),
 // k_adapt_thresholds, k_fast_response (response = S) in place of k_harris, k_cell_select, k_frame_finalize,
 // k_frame_emit_fast (size 7, angle -1, no orientation) and level 0 of the extractor pyramid.
+//
+// use_feature_min_depth (parameter_server.cpp:90) adds k_min_depth after k_cell_select: the minimum depth in each keypoint's
+// neighbourhood (misc.cpp:774-791), which k_frame_finalize_md / k_frame_emit[_fast]_md use for removeDepthless and projectTo3D.
 #include "orb.cuh"
 
 #include <cuda_runtime.h>
+
+#include <type_traits>
 
 #include "orb_tables_generated.h"
 #include "orb_host.h"
@@ -532,25 +537,65 @@ struct FrameKp {
   uint8_t level, cell;
   uint16_t flag;
 };
+struct FrameKpZ : FrameKp {  // use_feature_min_depth: the keypoint carries its neighbourhood depth (k_min_depth)
+  float z;
+};
 constexpr int kFrameCap = 4096;  // >= ncells * max_per_cell
+static_assert(kFrameCap == kOrbFrameCap && sizeof(FrameKpZ) == kOrbFrameKpBytes && sizeof(FrameKp) <= sizeof(FrameKpZ),
+              "orb_host.h sizes the finalize scratch");
+
+// -------------------------------------------------------------------------------------------------
+// use_feature_min_depth (parameter_server.cpp:90): Z = getMinDepthInNeighborhood(depth, kp.pt, kp.size) (misc.cpp:774-791) for
+// every keepStrongest survivor of every frame, in place of depth(round(y), round(x)) -- removeDepthless (node.cpp:82-83) and
+// projectTo3D (:940-941) both read it.  The keypoint is the one k_frame_finalize / k_frame_emit will build: image coordinates
+// from the cell pyramid, size 31 * scale (ORB) or 7 (FAST).  radius = int((size - 1) / 2); the window is the half-open
+// [int(y - r), int(y + r)) x [int(x - r), int(x + r)) of the raw depth image (float arithmetic, truncation toward zero),
+// clamped to the image -- 2r x 2r, not centred.  Z = the minimum over the window, NaN pixels ignored (fminf), NaN when the
+// window holds no number or its minimum is 0 (the reference's FIXME branch; -0 == 0).  One warp per candidate, lanes stride
+// the columns of each window row.  cand_z[fc * out_stride + i] pairs with cell_out[fc * out_stride + i].
+__global__ void __launch_bounds__(256) k_min_depth(const unsigned long long* __restrict__ cell_out, const int* __restrict__ cell_out_count,
+                                                   int out_stride, const float* __restrict__ depth, int fast, float* __restrict__ cand_z) {
+  const int fc = blockIdx.y;
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= cell_out_count[fc]) return;
+  const int W = c_geom.W, H = c_geom.H;
+  const int f = fc / c_geom.ncells, c = fc % c_geom.ncells;
+  const uint32_t pos = (uint32_t)((cell_out[(size_t)fc * out_stride + i] >> 9) & 0x7FFFFFu);
+  const int level = pos >> 20, ly = (pos >> 10) & 1023, lx = pos & 1023;
+  const float sc = c_geom.cell[c][level].scale;
+  const float x = __fadd_rn(__fmul_rn((float)lx, sc), (float)c_geom.cell_x0[c]);  // as k_frame_finalize
+  const float y = __fadd_rn(__fmul_rn((float)ly, sc), (float)c_geom.cell_y0[c]);
+  const float size = fast ? 7.f : __fmul_rn(31.f, sc);  // as k_frame_emit / k_frame_emit_fast
+  const float r = (float)__float2int_rz(__fdiv_rn(__fsub_rn(size, 1.f), 2.f));
+  const int top = max(__float2int_rz(__fsub_rn(y, r)), 0), left = max(__float2int_rz(__fsub_rn(x, r)), 0);
+  const int bot = min(__float2int_rz(__fadd_rn(y, r)), H), right = min(__float2int_rz(__fadd_rn(x, r)), W);
+  const float* d = depth + (size_t)f * W * H;
+  float m = __int_as_float(0x7fc00000);
+  for (int yy = top; yy < bot; yy++)
+    for (int xx = left + lane; xx < right; xx += 32) m = fminf(m, d[(size_t)yy * W + xx]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) cand_z[(size_t)fc * out_stride + i] = m == 0.f ? __int_as_float(0x7fc00000) : m;
+}
 
 // mode 0: detector output, cell-major, inside a cell |response| descending (canonical stand-in for the unspecified
 //         nth_element order), ties by (level, y, x).
 // mode 1: Node constructor: removeDepthless -> retainBest(K) by signed response (ties canonical, cut at K) ->
 //         extractor border filter (31 px on cvRound'ed coordinates) -> stable sort by octave -> orientation ->
 //         projectTo3D.  Final order = (octave, response descending, cell, level, y, x).
-__global__ void __launch_bounds__(1024)
-    k_frame_finalize(int mode, int max_keypoints, const unsigned long long* __restrict__ cell_out,
-                     const int* __restrict__ cell_out_count, int out_stride, const uint8_t* __restrict__ cell_img,
-                     const float* __restrict__ depth, float depth_scaling, float4 Kinv /* 1/fx, 1/fy, cx, cy */,
-                     FrameKp* __restrict__ scratch /* nframes x 2 x kFrameCap */, rgbdslam_b200_keypoint* __restrict__ kp_out,
-                     float4* __restrict__ xyz_out, int* __restrict__ n_out, int kp_stride) {
+// kMinDepth (use_feature_min_depth, mode 1 only): removeDepthless tests k_min_depth's Z of the keypoint (cand_z, aligned with
+// cell_out) instead of the depth pixel, and the record carries Z on to k_frame_emit's projectTo3D.
+template <bool kMinDepth>
+__device__ __forceinline__ void frame_finalize(int mode, int max_keypoints, const unsigned long long* __restrict__ cell_out,
+                                               const int* __restrict__ cell_out_count, int out_stride, const float* __restrict__ depth,
+                                               const float* __restrict__ cand_z, void* __restrict__ scratch, int* __restrict__ n_out) {
+  using Kp = std::conditional_t<kMinDepth, FrameKpZ, FrameKp>;
   __shared__ unsigned long long keys[kFrameCap];
   __shared__ int s_n, s_m;
   const int f = blockIdx.x;
   const int W = c_geom.W, H = c_geom.H;
-  FrameKp* ka = scratch + (size_t)f * 2 * kFrameCap;  // gather order
-  FrameKp* kc = ka + kFrameCap;                       // canonical order
+  Kp* ka = reinterpret_cast<Kp*>(scratch) + (size_t)f * 2 * kFrameCap;  // gather order
+  Kp* kc = ka + kFrameCap;                                                // canonical order
   if (threadIdx.x == 0) { s_n = 0; s_m = 0; }
   __syncthreads();
   // A. gather, shift to image coordinates (pt *= scale; pt += cell origin: feature_adjuster.cpp:259-282), depth check
@@ -565,7 +610,7 @@ __global__ void __launch_bounds__(1024)
       float r = __uint_as_float(ord & 0x7FFFFFFFu);  // |resp| (ordered() of a non-negative float only sets bit 31)
       if (k & 1ull) r = -r;
       const float sc = c_geom.cell[c][level].scale;
-      FrameKp q;
+      Kp q;
       q.x = __fadd_rn(__fmul_rn((float)lx, sc), (float)c_geom.cell_x0[c]);
       q.y = __fadd_rn(__fmul_rn((float)ly, sc), (float)c_geom.cell_y0[c]);
       q.resp = r;
@@ -577,7 +622,10 @@ __global__ void __launch_bounds__(1024)
       bool ok = true;
       if (mode == 1) {  // removeDepthless (node.cpp:67-97)
         ok = !(q.x >= W || q.x < 0 || q.y >= H || q.y < 0);
-        if (ok) {
+        if constexpr (kMinDepth) {
+          q.z = cand_z[(size_t)fc * out_stride + i];  // getMinDepthInNeighborhood (node.cpp:82-83)
+          ok = ok && !(q.z != q.z);
+        } else if (ok) {
           const int rx = (int)floorf(q.x + 0.5f), ry = (int)floorf(q.y + 0.5f);  // round(): half away from zero
           const size_t idx = (size_t)ry * W + rx;
           const float Z = idx < (size_t)W * H ? depth[(size_t)f * W * H + idx] : __int_as_float(0x7fc00000);
@@ -598,7 +646,7 @@ __global__ void __launch_bounds__(1024)
   for (int i = threadIdx.x; i < N; i += blockDim.x) {
     unsigned long long k = ~0ull;
     if (i < cnt) {
-      const FrameKp q = ka[i];
+      const Kp q = ka[i];
       const unsigned long long canon = ((unsigned long long)q.cell << 27) | ((unsigned long long)q.level << 24) |
                                        ((unsigned long long)q.ly << 12) | q.lx;
       k = (canon << 16) | (unsigned)i;
@@ -625,7 +673,7 @@ __global__ void __launch_bounds__(1024)
       unsigned long long k2 = ~0ull;
       if (j < keepK) {
         const int r = (int)(keys[j] & 0xFFFFu);
-        const FrameKp q = kc[r];
+        const Kp q = kc[r];
         const int rx = __float2int_rn(q.x), ry = __float2int_rn(q.y);
         if (rx >= 31 && rx < W - 31 && ry >= 31 && ry < H - 31) {
           k2 = ((unsigned long long)q.level << 40) | ((unsigned long long)j << 16) | (unsigned)r;
@@ -644,7 +692,7 @@ __global__ void __launch_bounds__(1024)
     for (int r = threadIdx.x; r < N; r += blockDim.x) {
       unsigned long long k = ~0ull;
       if (r < cnt) {
-        const FrameKp q = kc[r];
+        const Kp q = kc[r];
         k = ((unsigned long long)q.cell << 56) | ((unsigned long long)(~f32_ordered(fabsf(q.resp))) << 16) | (unsigned)r;
       }
       keys[r] = k;
@@ -659,20 +707,39 @@ __global__ void __launch_bounds__(1024)
   if (threadIdx.x == 0) n_out[f] = n_final;
 }
 
+__global__ void __launch_bounds__(1024)
+    k_frame_finalize(int mode, int max_keypoints, const unsigned long long* __restrict__ cell_out,
+                     const int* __restrict__ cell_out_count, int out_stride, const uint8_t* __restrict__ cell_img,
+                     const float* __restrict__ depth, float depth_scaling, float4 Kinv /* 1/fx, 1/fy, cx, cy */,
+                     FrameKp* __restrict__ scratch /* nframes x 2 x kFrameCap */, rgbdslam_b200_keypoint* __restrict__ kp_out,
+                     float4* __restrict__ xyz_out, int* __restrict__ n_out, int kp_stride) {
+  frame_finalize<false>(mode, max_keypoints, cell_out, cell_out_count, out_stride, depth, nullptr, scratch, n_out);
+}
+
+__global__ void __launch_bounds__(1024)
+    k_frame_finalize_md(int max_keypoints, const unsigned long long* __restrict__ cell_out, const int* __restrict__ cell_out_count,
+                        int out_stride, const float* __restrict__ cand_z, FrameKpZ* __restrict__ scratch /* nframes x 2 x kFrameCap */,
+                        int* __restrict__ n_out) {
+  frame_finalize<true>(1, max_keypoints, cell_out, cell_out_count, out_stride, nullptr, cand_z, scratch, n_out);
+}
+
 // One warp per output keypoint: intensity-centroid orientation on the detector's (cell) pyramid, the cv::KeyPoint record,
 // in mode 1 projectTo3D (node.cpp:900-965) + backProject (misc2.h:49-65) and the rotation (cos, sin) compute() will use.
 // kFast: cv::FAST's KeyPoint(x, y, 7.f, -1, score) -- no orientation; compute() steers the pattern by the angle as given, -1.
-template <bool kFast>
-__device__ __forceinline__ void frame_emit_warp(int mode, const FrameKp* __restrict__ scratch, const uint8_t* __restrict__ cell_img,
+// kMinDepth (use_feature_min_depth, mode 1): projectTo3D takes the keypoint's neighbourhood depth that k_frame_finalize_md
+// carried over from k_min_depth (node.cpp:940-941) instead of the depth pixel.
+template <bool kFast, bool kMinDepth>
+__device__ __forceinline__ void frame_emit_warp(int mode, const void* __restrict__ scratch, const uint8_t* __restrict__ cell_img,
                                                 const float* __restrict__ depth, float depth_scaling, float4 Kinv,
                                                 rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out,
                                                 float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
+  using Kp = std::conditional_t<kMinDepth, FrameKpZ, FrameKp>;
   const int f = blockIdx.y;
   const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (t >= n_out[f]) return;
   const int W = c_geom.W, H = c_geom.H;
-  const FrameKp* ka = scratch + (size_t)f * 2 * kFrameCap;
-  const FrameKp q = (ka + kFrameCap)[reinterpret_cast<const uint16_t*>(ka)[t]];
+  const Kp* ka = reinterpret_cast<const Kp*>(scratch) + (size_t)f * 2 * kFrameCap;
+  const Kp q = (ka + kFrameCap)[reinterpret_cast<const uint16_t*>(ka)[t]];
   const OrbPlane& p = c_geom.cell[q.cell][q.level];
   float ang = -1.f;
   if constexpr (!kFast) ang = ic_angle_warp(cell_img + (size_t)f * c_geom.cell_bytes + p.off, p.w, q.lx, q.ly, lane);
@@ -687,8 +754,14 @@ __device__ __forceinline__ void frame_emit_warp(int mode, const FrameKp* __restr
     o.class_id = -1;
     kp_out[(size_t)f * kp_stride + t] = o;
     if (mode == 1) {
-      const int rx = (int)floorf(q.x + 0.5f), ry = (int)floorf(q.y + 0.5f);
-      const float Z = (float)((double)depth[(size_t)f * W * H + (size_t)ry * W + rx] * (double)depth_scaling);
+      float d;
+      if constexpr (kMinDepth) {
+        d = q.z;
+      } else {
+        const int rx = (int)floorf(q.x + 0.5f), ry = (int)floorf(q.y + 0.5f);
+        d = depth[(size_t)f * W * H + (size_t)ry * W + rx];
+      }
+      const float Z = (float)((double)d * (double)depth_scaling);
       float4 v;
       v.x = __fmul_rn(__fmul_rn(__fsub_rn(q.x, Kinv.z), Z), Kinv.x);
       v.y = __fmul_rn(__fmul_rn(__fsub_rn(q.y, Kinv.w), Z), Kinv.y);
@@ -707,14 +780,27 @@ __global__ void __launch_bounds__(256)
     k_frame_emit(int mode, const FrameKp* __restrict__ scratch, const uint8_t* __restrict__ cell_img, const float* __restrict__ depth,
                  float depth_scaling, float4 Kinv, rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out,
                  float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
-  frame_emit_warp<false>(mode, scratch, cell_img, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
+  frame_emit_warp<false, false>(mode, scratch, cell_img, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
 }
 
 __global__ void __launch_bounds__(256)
     k_frame_emit_fast(int mode, const FrameKp* __restrict__ scratch, const float* __restrict__ depth, float depth_scaling, float4 Kinv,
                       rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out, float2* __restrict__ trig_out,
                       const int* __restrict__ n_out, int kp_stride) {
-  frame_emit_warp<true>(mode, scratch, nullptr, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
+  frame_emit_warp<true, false>(mode, scratch, nullptr, depth, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
+}
+
+__global__ void __launch_bounds__(256)
+    k_frame_emit_md(const FrameKpZ* __restrict__ scratch, const uint8_t* __restrict__ cell_img, float depth_scaling, float4 Kinv,
+                    rgbdslam_b200_keypoint* __restrict__ kp_out, float4* __restrict__ xyz_out, float2* __restrict__ trig_out,
+                    const int* __restrict__ n_out, int kp_stride) {
+  frame_emit_warp<false, true>(1, scratch, cell_img, nullptr, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
+}
+
+__global__ void __launch_bounds__(256)
+    k_frame_emit_fast_md(const FrameKpZ* __restrict__ scratch, float depth_scaling, float4 Kinv, rgbdslam_b200_keypoint* __restrict__ kp_out,
+                         float4* __restrict__ xyz_out, float2* __restrict__ trig_out, const int* __restrict__ n_out, int kp_stride) {
+  frame_emit_warp<true, true>(1, scratch, nullptr, nullptr, depth_scaling, Kinv, kp_out, xyz_out, trig_out, n_out, kp_stride);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -860,9 +946,11 @@ cudaError_t orb_run_select(const OrbGeom& g, int nframes, int mode, int detector
                            const uint8_t* d_cell_img, const OrbCand* d_cand, const int* d_cand_count, const int* d_thr,
                            float* d_resp, unsigned long long* d_cell_out, int* d_cell_out_count, const float* d_depth,
                            float depth_scaling, float4 Kinv, void* d_scratch, rgbdslam_b200_keypoint* d_kp, float4* d_xyz,
-                           float2* d_trig, int* d_n, int kp_stride, cudaStream_t st, int* launches) {
+                           float2* d_trig, int* d_n, int kp_stride, bool min_depth, float* d_cand_z, cudaStream_t st,
+                           int* launches) {
   const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST;
   const int z = nframes * g.ncells;
+  min_depth = min_depth && mode == 1;
   if (fast)
     k_fast_response<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(d_cand, d_cand_count, d_thr, d_resp);
   else
@@ -874,9 +962,22 @@ cudaError_t orb_run_select(const OrbGeom& g, int nframes, int mode, int detector
     attr = true;
   }
   k_cell_select<<<z, 1024, 16384 * 8, st>>>(d_cand, d_cand_count, d_resp, max_per_cell, d_cell_out, d_cell_out_count, max_per_cell);
+  const int max_out = mode == 1 ? (max_keypoints < kp_stride ? max_keypoints : kp_stride) : kp_stride;
+  if (min_depth) {
+    k_min_depth<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(d_cell_out, d_cell_out_count, max_per_cell, d_depth, fast, d_cand_z);
+    k_frame_finalize_md<<<nframes, 1024, 0, st>>>(max_keypoints, d_cell_out, d_cell_out_count, max_per_cell, d_cand_z,
+                                                  (FrameKpZ*)d_scratch, d_n);
+    if (fast)
+      k_frame_emit_fast_md<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>((const FrameKpZ*)d_scratch, depth_scaling, Kinv, d_kp,
+                                                                            d_xyz, d_trig, d_n, kp_stride);
+    else
+      k_frame_emit_md<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>((const FrameKpZ*)d_scratch, d_cell_img, depth_scaling, Kinv,
+                                                                       d_kp, d_xyz, d_trig, d_n, kp_stride);
+    (*launches) += 5;
+    return cudaGetLastError();
+  }
   k_frame_finalize<<<nframes, 1024, 0, st>>>(mode, max_keypoints, d_cell_out, d_cell_out_count, max_per_cell, d_cell_img, d_depth,
                                              depth_scaling, Kinv, (FrameKp*)d_scratch, d_kp, d_xyz, d_n, kp_stride);
-  const int max_out = mode == 1 ? (max_keypoints < kp_stride ? max_keypoints : kp_stride) : kp_stride;
   if (fast)
     k_frame_emit_fast<<<dim3((max_out + 7) / 8, nframes), 256, 0, st>>>(mode, (const FrameKp*)d_scratch, d_depth, depth_scaling, Kinv,
                                                                          d_kp, d_xyz, d_trig, d_n, kp_stride);

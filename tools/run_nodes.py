@@ -5,7 +5,10 @@
 2. The C4 sequence (bench.py: --frames frames, 3 sequential + 4 window + 4 random candidate pairs per frame) with nodes of
    each detector type through matching, graph construction, the pose-graph solve and ATE against the rendering ground truth.
 
-Prints one JSON object, with the card name and power limit read in the same run.  Usage: python tools/run_nodes.py
+--min-depth: every detector type also with params.use_feature_min_depth (keypoint depth = the nearest point of its
+neighbourhood), alternated with the pointwise rule in step 1 and run through step 2 as well ("ORB+min_depth", ...).
+
+Prints one JSON object, with the card name and power limit read in the same run.  Usage: python tools/run_nodes.py [--min-depth]
 """
 import argparse
 import ctypes as C
@@ -32,6 +35,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--frames", type=int, default=2000, help="C4 sequence length")
     ap.add_argument("--keypoints", type=int, default=1000)
+    ap.add_argument("--min-depth", action="store_true", help="also with use_feature_min_depth, alternated with the pointwise rule")
     args = ap.parse_args()
 
     import torch
@@ -42,16 +46,19 @@ def main():
     dev = torch.device("cuda", 0)
     K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
     seed = 11
-    names = {DETECTOR_ORB: "ORB", DETECTOR_FAST: "FAST"}
+    types = {DETECTOR_ORB: "ORB", DETECTOR_FAST: "FAST"}
+    configs = [(t, m) for t in types for m in ((0, 1) if args.min_depth else (0,))]  # (detector type, use_feature_min_depth)
+    names = {(t, m): types[t] + ("+min_depth" if m else "") for t, m in configs}
 
-    def params(t):
-        p = default_params(); p.depth_cov_z0 = 2.0; p.max_keypoints = args.keypoints; p.feature_detector_type = t
+    def params(cfg):
+        p = default_params(); p.depth_cov_z0 = 2.0; p.max_keypoints = args.keypoints
+        p.feature_detector_type, p.use_feature_min_depth = cfg
         return p
 
-    fe = Frontend(0, params(DETECTOR_ORB))
+    fe = Frontend(0, params(configs[0]))
 
-    def use(t):
-        p = params(t)
+    def use(cfg):
+        p = params(cfg)
         fe.params = p
         fe._check(fe.lib.rgbdslam_b200_init(0, C.byref(p)))
 
@@ -64,12 +71,12 @@ def main():
     torch.cuda.synchronize()
     out = {"card": card(), "image": "640x480", "max_keypoints": args.keypoints}
 
-    # ---- 1. the Node constructor alone, detector types alternated
+    # ---- 1. the Node constructor alone, configurations alternated
     nt = args.timing_frames
-    timing = {names[t]: [] for t in names}
+    timing = {names[c]: [] for c in configs}
     feats = {}
-    for r in range(args.rounds + 1):  # round 0 warms up both types (allocations, first launches)
-        for t in (DETECTOR_ORB, DETECTOR_FAST):
+    for r in range(args.rounds + 1):  # round 0 warms up every configuration (allocations, first launches)
+        for t in configs:
             use(t)
             det = fe.detector_create()
             torch.cuda.synchronize()
@@ -114,7 +121,7 @@ def main():
         return nfeat, res, graph, traj, chi2, lm, (t0, t1, t2, t3)
 
     c4 = {}
-    for t in (DETECTOR_FAST, DETECTOR_ORB):
+    for t in configs[::-1]:
         sequence(t, min(nf_, 96))  # warm-up of every stage (allocations, first launches), as bench.py does
         nfeat, res, graph, traj, chi2, lm, (t0, t1, t2, t3) = sequence(t, nf_)
         c4[names[t]] = {"frames": nf_, "pairs": int(len(pairs)), "valid_edges": int(graph["n_valid_edges"]),
