@@ -311,8 +311,40 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * builds from the depth image -- depthToCV8UC1 (misc.cpp:414-418: depth.convertTo(mono8, CV_8UC1, 100, 0), NaN -> 0; handed
  * over as `depth_mono8_img`, openni_listener.cpp:779) -- computed on the device, `mask` is ignored (saves 1/6 of the upload).
  * Host buffers may be pinned (copied straight from, asynchronously) or pageable (staged through pinned memory); the upload
- * of a chunk of frames overlaps the kernels of the previous chunk; all nodes of a call share one device allocation. */
+ * of a chunk of frames overlaps the kernels of the previous chunk; all nodes of a call share one device allocation.
+ *
+ * RGBDSLAM_B200_VISUAL_RGB: `gray` holds nframes*w*h*3 bytes of colour (CV_8UC3), converted on the device as both reference
+ * constructors do, cvtColor(visual, gray, CV_RGB2GRAY) (node.cpp:139-144, 275-277): channel 0 is weighted as R whatever the
+ * real channel order (a bgr8 image is converted with R and B swapped, as in the reference), with OpenCV 4's arithmetic
+ * (R * 9798 + G * 19235 + B * 3735 + 2^14) >> 15.  For depth-image and cloud input alike.
+ *
+ * RGBDSLAM_B200_CLOUD_XYZRGB / RGBDSLAM_B200_CLOUD_XYZ: the point-cloud constructor, Node(visual, detector, extractor,
+ * point_cloud, detection_mask) (node.cpp:252-369; openni_listener.cpp:754 for registered Kinect clouds, stereo cameras and PCD
+ * replay).  `depth` points to nframes organised w x h clouds of pcl::PointXYZRGB (32 bytes per point, the default point_type)
+ * or pcl::PointXYZ (16 bytes, RGB_IS_4TH_DIM) (parameter_server.h:33-42): x, y, z at byte offsets 0, 4, 8.  Per frame: detect
+ * (the same detector and per-cell threshold state), then projectTo3D (:855-898) on the detector output in its order
+ * (cell-major, |response| descending inside a cell, ties by (octave, y, x)) with NO removeDepthless and NO retainBest: a
+ * keypoint is kept when the cloud point at ((int)x, (int)y) -- truncated, not rounded -- has no NaN coordinate, and the point
+ * is (x, y, z, 1) as stored (no intrinsics, no depth_scaling_factor); the first max_keypoints kept keypoints are the node's.
+ * Then compute(): the 31 px border filter and the stable octave sort.  Feature order inside a node: (octave, cell, |response|
+ * descending, y, x).  Unlike the reference, each 3-D point moves with its keypoint through compute() (the reference pairs
+ * descriptor i with another keypoint's point once compute() drops or re-orders keypoints, and its asserts at node.cpp:317-318
+ * fail).  maximum_depth (parameter_server.cpp:38) is fixed at its default, +inf: no point is too far and a +inf z is kept.
+ * K4 may be NULL; use_feature_min_depth and depth_scaling_factor are not read.  params.observability_threshold > 0 (the
+ * environment measurement model, which needs a cloud per node) returns ERR_STATE for cloud input.
+ *
+ * RGBDSLAM_B200_MASK_FROM_CLOUD: the detection mask is calculateDepthMask of the cloud (openni_listener.cpp:520-534, the
+ * stereo and PCD callers), computed on the device and `mask` ignored: static_cast<uchar>(z * 50.0) as x86-64 compilers emit
+ * it (truncation to int32, 0x80000000 when out of range, low byte), 0 for NaN -- so the mask is 0 below ~0.02 m, in a band at
+ * every multiple of 5.12 m and for +-inf.
+ *
+ * Rejected with ERR_ARG before any device work: unknown bits, CLOUD_XYZRGB with CLOUD_XYZ, MASK_FROM_CLOUD without a cloud
+ * bit, MASK_FROM_DEPTH with a cloud bit. */
 #define RGBDSLAM_B200_MASK_FROM_DEPTH 1
+#define RGBDSLAM_B200_VISUAL_RGB 2
+#define RGBDSLAM_B200_CLOUD_XYZRGB 4
+#define RGBDSLAM_B200_CLOUD_XYZ 8
+#define RGBDSLAM_B200_MASK_FROM_CLOUD 16
 int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                   int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
                                   int32_t* n_features);

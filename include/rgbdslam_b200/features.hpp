@@ -27,7 +27,10 @@ namespace rgbdslam_b200 {
 
 typedef rgbdslam_b200_keypoint KeyPoint;  // == cv::KeyPoint (7 x 4 B)
 
-enum { RB_8UC1 = 0, RB_32FC1 = 5 };  // == CV_8UC1, CV_32FC1
+enum { RB_8UC1 = 0, RB_32FC1 = 5, RB_8UC3 = 16 };  // == CV_8UC1, CV_32FC1, CV_8UC3
+
+inline int channels_of(int t) { return t == RB_8UC3 ? 3 : 1; }
+inline size_t pixel_bytes(int t) { return t == RB_32FC1 ? 4 : (size_t)channels_of(t); }
 
 struct Mat {  // non-owning view with cv::Mat's field names
   unsigned char* data = nullptr;
@@ -36,10 +39,11 @@ struct Mat {  // non-owning view with cv::Mat's field names
   int type_ = RB_8UC1;
   Mat() {}
   Mat(void* d, int r, int c, size_t s, int t) : data((unsigned char*)d), rows(r), cols(c), step(s), type_(t) {}
-  Mat(int r, int c, int t, void* d) : data((unsigned char*)d), rows(r), cols(c), step((size_t)c * (t == RB_32FC1 ? 4 : 1)), type_(t) {}
+  Mat(int r, int c, int t, void* d) : data((unsigned char*)d), rows(r), cols(c), step((size_t)c * pixel_bytes(t)), type_(t) {}
   int type() const { return type_; }
+  int channels() const { return channels_of(type_); }
   bool empty() const { return data == nullptr || rows == 0 || cols == 0; }
-  bool isContinuous() const { return step == (size_t)cols * (type_ == RB_32FC1 ? 4 : 1); }
+  bool isContinuous() const { return step == (size_t)cols * pixel_bytes(type_); }
 };
 
 namespace detail {
@@ -50,10 +54,11 @@ inline void check_rc(int rc, const char* what) {
 template <class T>
 inline const T* packed(const Mat& m, std::vector<T>& tmp) {
   if (m.isContinuous()) return reinterpret_cast<const T*>(m.data);
-  tmp.resize((size_t)m.rows * m.cols);
+  const size_t row = (size_t)m.cols * m.channels();
+  tmp.resize((size_t)m.rows * row);
   for (int r = 0; r < m.rows; r++)
-    std::copy(reinterpret_cast<const T*>(m.data + r * m.step), reinterpret_cast<const T*>(m.data + r * m.step) + m.cols,
-              tmp.begin() + (size_t)r * m.cols);
+    std::copy(reinterpret_cast<const T*>(m.data + r * m.step), reinterpret_cast<const T*>(m.data + r * m.step) + row,
+              tmp.begin() + (size_t)r * row);
   return tmp.data();
 }
 }  // namespace detail

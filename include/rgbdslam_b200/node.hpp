@@ -4,6 +4,7 @@
 //   LoadedEdge3D                 src/edge.h:24-32
 //   MatchingResult               src/matching_result.h:24-46
 //   Node (feature members, matchNodePair, featureMatching-free ctor from features)   src/node.h:64-178
+//   the two image constructors (depth image node.cpp:101-240, point cloud :252-369) and pcl::PointCloud / PointXYZ[RGB]
 //   bruteForceSearchORB          src/features.h:13, src/features.cpp:168-182
 // The reference types Eigen::Matrix4f / Eigen::Isometry3d / cv::DMatch / cv::KeyPoint are replaced by
 // layout-compatible PODs (column-major float[16] etc.) so this header has no third-party dependency; a
@@ -11,7 +12,9 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
+#include <type_traits>
 #include <string>
 #include <vector>
 
@@ -38,6 +41,31 @@ struct Matrix6d {
 struct Vector4f {
   float x, y, z, w;
 };
+
+// pcl::PointXYZ / pcl::PointXYZRGB as an organised cloud stores them (x, y, z at byte offsets 0, 4, 8; PointXYZRGB's colour
+// packed b, g, r, a at offset 16) and pcl::PointCloud<PointT> as far as the point-cloud Node constructor reads it.  The
+// reference's point_type is PointXYZRGB, or PointXYZ with RGB_IS_4TH_DIM (parameter_server.h:33-42).
+struct alignas(16) PointXYZ {
+  float x, y, z, data_w;
+};
+struct alignas(16) PointXYZRGB {
+  float x, y, z, data_w;
+  uint8_t b, g, r, a;
+  float data_c[3];
+};
+static_assert(sizeof(PointXYZ) == 16 && sizeof(PointXYZRGB) == 32, "layout of pcl::PointXYZ / pcl::PointXYZRGB");
+template <class PointT>
+struct PointCloud {
+  typedef std::shared_ptr<PointCloud<PointT>> Ptr;
+  typedef std::shared_ptr<const PointCloud<PointT>> ConstPtr;
+  myHeader header;
+  std::vector<PointT> points;  // row-major, width x height
+  uint32_t width = 0, height = 0;
+  bool is_dense = false;
+  bool isOrganized() const { return height > 1; }
+};
+typedef PointXYZRGB point_type;  // the reference's default point_type
+typedef PointCloud<point_type> pointcloud_type;
 typedef rgbdslam_b200_dmatch DMatch;  // == cv::DMatch  (KeyPoint: features.hpp)
 
 struct LoadedEdge3D {  // src/edge.h:24-32
@@ -101,7 +129,8 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   Node() {}
   // The reference's constructor, argument for argument (node.h:64-70, call site openni_listener.cpp:779):
   //   Node(visual, depth, detection_mask, cam_info, depth_header, detector, extractor)
-  // visual CV_8UC1, depth CV_32FC1 metres (NaN = invalid), detection_mask CV_8UC1 non-zero at potential keypoint locations
+  // visual CV_8UC1 or CV_8UC3 (converted as cvtColor(CV_RGB2GRAY): channel 0 weighted as R), depth CV_32FC1 metres (NaN =
+  // invalid), detection_mask CV_8UC1 non-zero at potential keypoint locations
   // (node.h:61-63).  detector / extractor: createDetector / createDescriptorExtractor (features.hpp); the whole constructor
   // -- detect, removeDepthless, retainBest, compute, projectTo3D -- runs as one rgbdslam_b200_nodes_create call, the
   // extractor argument only documents the pairing (ORB or FAST keypoints, ORB descriptors).  id_ stays -1 until
@@ -111,8 +140,9 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
       : stamp_(depth_header.stamp) {
     if (!detector || !detector->handle()) throw std::invalid_argument("Node: detector must come from createDetector(\"ORB\" or \"FAST\")");
     if (!extractor) throw std::invalid_argument("Node: null extractor");
-    if (visual.type() != RB_8UC1 || depth.type() != RB_32FC1 || depth.rows != visual.rows || depth.cols != visual.cols)
-      throw std::invalid_argument("Node: visual must be CV_8UC1 and depth CV_32FC1 of the same size");
+    if ((visual.type() != RB_8UC1 && visual.type() != RB_8UC3) || depth.type() != RB_32FC1 || depth.rows != visual.rows ||
+        depth.cols != visual.cols)
+      throw std::invalid_argument("Node: visual must be CV_8UC1 or CV_8UC3 and depth CV_32FC1 of the same size");
     seq_id_ = (int)depth_header.seq;
     std::vector<uint8_t> tg, tm;
     std::vector<float> td;
@@ -121,7 +151,36 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     const uint8_t* m = detection_mask.empty() ? nullptr : detail::packed<uint8_t>(detection_mask, tm);
     const CameraInfo ci = cam_info ? *cam_info : CameraInfo();
     const float K4[4] = {(float)ci.K[0], (float)ci.K[4], (float)ci.K[2], (float)ci.K[5]};  // node.cpp:913-916
-    construct(g, d, m, visual.cols, visual.rows, K4, detector->handle());
+    construct(g, d, m, visual.cols, visual.rows, K4, detector->handle(), visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0);
+  }
+  // The reference's point-cloud constructor, argument for argument (node.h:74-78, call site openni_listener.cpp:754):
+  //   Node(visual, detector, extractor, point_cloud, detection_mask)
+  // visual CV_8UC1 or CV_8UC3 (converted as cvtColor(CV_RGB2GRAY): channel 0 weighted as R), point_cloud an organised cloud of
+  // the same size as visual, detection_mask empty or of the same size.  detect, projectTo3D (the first max_keypoints keypoints
+  // whose cloud point at the truncated position has no NaN coordinate, the point as stored) and compute run as one
+  // rgbdslam_b200_nodes_create_ex call; each 3-D point stays with its keypoint through compute() (see rgbdslam_b200.h).
+  template <class PointT>
+  Node(const Mat& visual, Ptr<Feature2D> detector, Ptr<DescriptorExtractor> extractor, std::shared_ptr<PointCloud<PointT>> point_cloud,
+       const Mat& detection_mask = Mat()) {
+    static_assert(std::is_same<PointT, PointXYZRGB>::value || std::is_same<PointT, PointXYZ>::value,
+                  "Node: the point cloud must hold PointXYZRGB or PointXYZ");
+    if (!detector || !detector->handle()) throw std::invalid_argument("Node: detector must come from createDetector(\"ORB\" or \"FAST\")");
+    if (!extractor) throw std::invalid_argument("Node: null extractor");
+    if (!point_cloud || !point_cloud->isOrganized() || point_cloud->points.size() != (size_t)point_cloud->width * point_cloud->height)
+      throw std::invalid_argument("Node: the point cloud must be organised (height > 1, width x height points)");
+    if (visual.type() != RB_8UC1 && visual.type() != RB_8UC3) throw std::invalid_argument("Node: visual must be CV_8UC1 or CV_8UC3");
+    if ((int)point_cloud->width != visual.cols || (int)point_cloud->height != visual.rows ||
+        (!detection_mask.empty() && (detection_mask.type() != RB_8UC1 || detection_mask.rows != visual.rows ||
+                                     detection_mask.cols != visual.cols)))
+      throw std::invalid_argument("Node: visual, point cloud and detection_mask (CV_8UC1) must have the same size");
+    stamp_ = point_cloud->header.stamp;  // timestamp_(point_cloud->header.stamp)
+    std::vector<uint8_t> tg, tm;
+    const uint8_t* g = detail::packed<uint8_t>(visual, tg);
+    const uint8_t* m = detection_mask.empty() ? nullptr : detail::packed<uint8_t>(detection_mask, tm);
+    const int flags = (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) |
+                      (std::is_same<PointT, PointXYZRGB>::value ? RGBDSLAM_B200_CLOUD_XYZRGB : RGBDSLAM_B200_CLOUD_XYZ);
+    construct(g, reinterpret_cast<const float*>(point_cloud->points.data()), m, visual.cols, visual.rows, nullptr,
+              detector->handle(), flags);
   }
   // Node(visual, depth, detection_mask, cam_info, depth_header, detector, extractor) (node.cpp:101-240): detect, filter,
   // describe, back-project on the device; the public feature members are filled from the result.  `detector` is the handle of
@@ -144,10 +203,12 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   Node(const Node&) = delete;
   Node& operator=(const Node&) = delete;
 
+  // flags: rgbdslam_b200_nodes_create_ex's (colour visual, point cloud in place of the depth image)
   void construct(const uint8_t* gray, const float* depth_m, const uint8_t* detection_mask, int w, int h, const float K4[4],
-                 uint64_t detector) {
+                 uint64_t detector, int flags = 0) {
     int32_t n = 0, id32 = id_ < 0 ? 0 : id_;
-    check(rgbdslam_b200_nodes_create(detector, 1, gray, depth_m, detection_mask, w, h, K4, &id32, &handle_, &n), "nodes_create");
+    check(rgbdslam_b200_nodes_create_ex(detector, 1, gray, depth_m, detection_mask, w, h, K4, &id32, flags, &handle_, &n),
+          "nodes_create");
     feature_locations_2d_.resize(n);
     feature_locations_3d_.resize(n);
     feature_descriptors_.resize((size_t)n * 32);

@@ -50,6 +50,25 @@ class Params(C.Structure):
 
 
 DETECTOR_ORB, DETECTOR_FAST = 0, 1  # Params.feature_detector_type (RGBDSLAM_B200_DETECTOR_*)
+# flags of rgbdslam_b200_nodes_create_ex / _sharded (RGBDSLAM_B200_*)
+MASK_FROM_DEPTH, VISUAL_RGB, CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD = 1, 2, 4, 8, 16
+
+
+def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False) -> int:
+    """The nodes_create flags the array shapes select: gray (F,H,W) or (F,H,W,3) colour; depth (F,H,W) depth image, or an
+    organised cloud (F,H,W,8) of PointXYZRGB / (F,H,W,4) of PointXYZ as float32."""
+    flags = (MASK_FROM_DEPTH if mask_from_depth else 0) | (MASK_FROM_CLOUD if mask_from_cloud else 0)
+    if len(gray_shape) == 4:
+        if gray_shape[3] != 3:
+            raise ValueError(f"gray must be (F,H,W) or (F,H,W,3), got {tuple(gray_shape)}")
+        flags |= VISUAL_RGB
+    if len(depth_shape) == 4:
+        if depth_shape[3] not in (4, 8):
+            raise ValueError(f"depth must be (F,H,W), (F,H,W,4) or (F,H,W,8), got {tuple(depth_shape)}")
+        flags |= CLOUD_XYZRGB if depth_shape[3] == 8 else CLOUD_XYZ
+    if tuple(gray_shape[:3]) != tuple(depth_shape[:3]):
+        raise ValueError(f"gray {tuple(gray_shape)} and depth {tuple(depth_shape)} differ in frames or image size")
+    return flags
 
 
 class PairResult(C.Structure):
@@ -419,40 +438,47 @@ class Frontend:
                                                        _ptr(desc), C.byref(n)))
         return out[:n.value], desc[:n.value]
 
-    def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False):
-        """gray [F,H,W] u8, depth [F,H,W] f32, mask [F,H,W] u8 or None -> (handles, n_features).  numpy arrays or pinned torch
-        tensors (copied from asynchronously).  mask_from_depth: derive the detection mask on the device (depthToCV8UC1)."""
+    def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, mask_from_cloud: bool = False):
+        """gray [F,H,W] u8 or [F,H,W,3] colour (channel 0 = R), depth [F,H,W] f32, or an organised cloud [F,H,W,8] (PointXYZRGB)
+        / [F,H,W,4] (PointXYZ) f32 for the point-cloud constructor, mask [F,H,W] u8 or None -> (handles, n_features).  numpy
+        arrays or pinned torch tensors (copied from asynchronously).  mask_from_depth / mask_from_cloud: derive the detection
+        mask on the device (depthToCV8UC1 / calculateDepthMask).  K4 may be None for cloud input."""
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
             depth = np.ascontiguousarray(depth, np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        F, H, W = gray.shape
-        K4 = np.ascontiguousarray(K4, np.float32)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud)
+        F, H, W = gray.shape[:3]
+        K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
         handles = np.zeros(F, np.uint64)
         nf = np.zeros(F, np.int32)
-        self._check(self.lib.rgbdslam_b200_nodes_create_ex(det, F, _ptr(gray), _ptr(depth), _ptr(None if mask_from_depth else mask), W, H,
-                                                           _ptr(K4), _ptr(ids), 1 if mask_from_depth else 0, _ptr(handles), _ptr(nf)))
+        no_mask = mask_from_depth or mask_from_cloud
+        self._check(self.lib.rgbdslam_b200_nodes_create_ex(det, F, _ptr(gray), _ptr(depth), _ptr(None if no_mask else mask), W, H,
+                                                           _ptr(K4), _ptr(ids), flags, _ptr(handles), _ptr(nf)))
         self._nodes += [int(h) for h in handles]
         return [int(h) for h in handles], nf
 
     def nodes_create_sharded(self, det: int, comm: int, total_frames: int, gray, depth, mask, K4, ids=None,
-                             mask_from_depth: bool = False):
+                             mask_from_depth: bool = False, mask_from_cloud: bool = False):
         """Frame-sharded nodes_create: gray / depth / mask hold THIS rank's frames (sharding.frame_shard); returns handles and
-        feature counts of ALL total_frames nodes (every rank ends up holding every node)."""
+        feature counts of ALL total_frames nodes (every rank ends up holding every node).  Shapes select the input as in
+        nodes_create."""
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
             depth = np.ascontiguousarray(depth, np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        _, H, W = gray.shape
-        K4 = np.ascontiguousarray(K4, np.float32)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud)
+        H, W = gray.shape[1:3]
+        K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
         handles = np.zeros(total_frames, np.uint64)
         nf = np.zeros(total_frames, np.int32)
         own = gray.shape[0] > 0
         self._check(self.lib.rgbdslam_b200_nodes_create_sharded(
             det, C.c_uint64(comm), total_frames, _ptr(gray) if own else None, _ptr(depth) if own else None,
-            _ptr(None if (mask_from_depth or not own) else mask), W, H, _ptr(K4), _ptr(ids), 1 if mask_from_depth else 0, _ptr(handles), _ptr(nf)))
+            _ptr(None if (mask_from_depth or mask_from_cloud or not own) else mask), W, H, _ptr(K4), _ptr(ids), flags, _ptr(handles),
+            _ptr(nf)))
         self._nodes += [int(h) for h in handles]
         return [int(h) for h in handles], nf
 

@@ -8,11 +8,20 @@
 --min-depth: every detector type also with params.use_feature_min_depth (keypoint depth = the nearest point of its
 neighbourhood), alternated with the pointwise rule in step 1 and run through step 2 as well ("ORB+min_depth", ...).
 
-Prints one JSON object, with the card name and power limit read in the same run.  Usage: python tools/run_nodes.py [--min-depth]
+--cloud: instead, the ORB detector with other inputs, alternated --rounds times in step 1: the depth-image constructor with
+grey and with colour visuals (MASK_FROM_DEPTH, pinned), the point-cloud constructor with organised PointXYZRGB clouds
+(MASK_FROM_CLOUD) from pinned and from pageable memory (--cloud-frames frames per call: a 640x480 XYZRGB cloud is 9.8 MB);
+the host-to-device bytes per frame of each; the new kernels' device times from torch.profiler in a separate pass; and step 2
+with cloud nodes against depth-image nodes (cloud nodes built --cloud-chunk frames per call, one detector: the same nodes as
+one call).
+
+Prints one JSON object, with the card name and power limit read in the same run.
+Usage: python tools/run_nodes.py [--min-depth | --cloud]
 """
 import argparse
 import ctypes as C
 import json
+import re
 import subprocess
 import sys
 import time
@@ -36,7 +45,12 @@ def main():
     ap.add_argument("--frames", type=int, default=2000, help="C4 sequence length")
     ap.add_argument("--keypoints", type=int, default=1000)
     ap.add_argument("--min-depth", action="store_true", help="also with use_feature_min_depth, alternated with the pointwise rule")
+    ap.add_argument("--cloud", action="store_true", help="colour and point-cloud input (ORB detector) instead of the detector types")
+    ap.add_argument("--cloud-frames", type=int, default=256)
+    ap.add_argument("--cloud-chunk", type=int, default=128)
     args = ap.parse_args()
+    if args.cloud:
+        return main_cloud(args)
 
     import torch
     from rgbdslam_v2_b200 import Frontend, pipeline, synth
@@ -128,6 +142,149 @@ def main():
                         "mean_features": float(np.mean(nfeat)), "mean_inliers_valid": float(res["n_inliers"][res["id1"] >= 0].mean()),
                         "lm_iterations": lm, "chi2": chi2, "ate_vs_gt_m": synth.ate_rmse(traj[:, :3], gt[:, :3]),
                         "seconds": {"nodes": t1 - t0, "match": t2 - t1, "graph_and_solve": t3 - t2, "total": t3 - t0}}
+    out["c4"] = c4
+    fe.close()
+    print(json.dumps(out))
+
+
+def main_cloud(args):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    from rgbdslam_v2_b200 import Frontend, pipeline, synth
+    from rgbdslam_v2_b200._capi import DETECTOR_ORB, PAIR_RESULT_DTYPE, default_params, graph_from_pairs
+    if not torch.cuda.is_available():
+        raise SystemExit("run_nodes.py measures on the GPU; no CUDA device found")
+    dev = torch.device("cuda", 0)
+    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
+    seed = 11
+    p = default_params(); p.depth_cov_z0 = 2.0; p.max_keypoints = args.keypoints; p.feature_detector_type = DETECTOR_ORB
+    fe = Frontend(0, p)
+
+    n = max(args.frames, args.timing_frames, args.cloud_frames)
+    poses = synth.trajectory(n)
+    g_d, d_d = synth.render_frames_torch(poses, dev)
+    H, W = g_d.shape[1:]
+    v, u = torch.meshgrid(torch.arange(H, device=dev, dtype=torch.float32), torch.arange(W, device=dev, dtype=torch.float32),
+                          indexing="ij")
+
+    def cloud_of(d):  # organised PointXYZRGB clouds [n, H, W, 8] of depth frames (a registered depth camera's output)
+        c = torch.zeros(d.shape + (8,), dtype=torch.float32, device=dev)
+        c[..., 0] = (u - K4[2]) * d / K4[0]
+        c[..., 1] = (v - K4[3]) * d / K4[1]
+        c[..., 2] = d
+        return c
+
+    def pinned(t):
+        h = torch.empty(t.shape, dtype=t.dtype).pin_memory()
+        h.copy_(t)
+        return h
+
+    gray = pinned(g_d)
+    depth = pinned(d_d)
+    nt, nc = args.timing_frames, args.cloud_frames
+    rgb = pinned(torch.stack([g_d[:nt], g_d[:nt].roll(3, -1), g_d[:nt].roll(5, -2)], -1))
+    cloud_pin = pinned(cloud_of(d_d[:nc]))
+    cloud_pag = cloud_pin.numpy().copy()
+    del g_d
+    torch.cuda.synchronize()
+    px = H * W
+    out = {"card": card(), "image": f"{W}x{H}", "max_keypoints": args.keypoints, "detector": "ORB"}
+    # name: (visual, depth or cloud, frames, keyword, host->device bytes per frame)
+    configs = {
+        "depth_gray_pinned": (gray, depth, nt, {"mask_from_depth": True}, px + 4 * px),
+        "depth_rgb_pinned": (rgb, depth, nt, {"mask_from_depth": True}, 3 * px + 4 * px),
+        "cloud_xyzrgb_pinned": (gray, cloud_pin, nc, {"mask_from_cloud": True}, px + 32 * px),
+        "cloud_xyzrgb_pageable": (gray.numpy(), cloud_pag, nc, {"mask_from_cloud": True}, px + 32 * px),
+    }
+
+    def call(cfg, frames=None):
+        vis, dep, m, kw, _ = configs[cfg]
+        m = frames or m
+        det = fe.detector_create()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        hs, nf = fe.nodes_create(det, vis[:m], dep[:m], None, None if "mask_from_cloud" in kw else K4, **kw)
+        dt = time.perf_counter() - t0
+        fe.detector_destroy(det)
+        for h in hs:
+            fe.node_destroy(h)
+        return m / dt, float(np.mean(nf))
+
+    # ---- 1. the constructor alone, inputs alternated
+    timing = {c: [] for c in configs}
+    feats = {}
+    for r in range(args.rounds + 1):  # round 0 warms up every configuration
+        for c in configs:
+            fps, feats[c] = call(c)
+            if r:
+                timing[c].append(fps)
+    out["nodes_create_frames_per_s"] = {k: {"frames": configs[k][2], "runs": [round(x, 1) for x in vs], "min": round(min(vs), 1),
+                                            "max": round(max(vs), 1)} for k, vs in timing.items()}
+    out["nodes_create_mean_features"] = feats
+    out["h2d_bytes_per_frame"] = {k: c[4] for k, c in configs.items()}
+
+    # ---- the kernels' device time per frame (torch.profiler, separate pass: tracing slows the host)
+    kernels = ("k_rgb_to_gray", "k_cloud_mask", "k_frame_finalize_cloud", "k_frame_emit_cloud", "k_frame_finalize", "k_frame_emit")
+    prof_frames = min(64, nt, nc)
+    ktimes = {}
+    for c in ("depth_rgb_pinned", "cloud_xyzrgb_pinned"):
+        call(c, prof_frames)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call(c, prof_frames)
+        tot = {}
+        for e in prof.events():
+            if e.device_type.name != "CUDA":
+                continue
+            m = re.search(r"rb200::(k_\w+)", e.name)
+            if m and m.group(1) in kernels:
+                tot[m.group(1)] = tot.get(m.group(1), 0.0) + e.device_time
+        allk = sum(e.device_time for e in prof.events() if e.device_type.name == "CUDA" and "rb200::k_" in e.name)
+        ktimes[c] = {k: round(t / prof_frames, 2) for k, t in sorted(tot.items())}
+        ktimes[c]["all_library_kernels"] = round(allk / prof_frames, 2)
+    out["kernel_us_per_frame"] = ktimes
+
+    # ---- 2. the C4 sequence with cloud nodes against depth-image nodes
+    nf_ = args.frames
+    pairs = np.array(pipeline.candidate_pairs(nf_, seed=seed), np.int64)
+    gt = np.stack([pipeline.mat_to_pose7(np.linalg.inv(poses[0]) @ P) for P in poses[:nf_]])
+    fe.posegraph_reserve(nf_, 12 * nf_)
+    stage = torch.empty((args.cloud_chunk, H, W, 8), dtype=torch.float32).pin_memory()
+
+    def sequence(kind, nf):
+        pp = pairs[pairs[:, 0] < nf]
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        det = fe.detector_create()
+        if kind == "depth":
+            hs, nfeat = fe.nodes_create(det, gray[:nf], depth[:nf], None, K4, ids=np.arange(nf, dtype=np.int32), mask_from_depth=True)
+        else:
+            hs, nfeat = [], []
+            for a in range(0, nf, args.cloud_chunk):
+                b = min(a + args.cloud_chunk, nf)
+                stage[:b - a].copy_(cloud_of(d_d[a:b]))
+                h, f = fe.nodes_create(det, gray[a:b], stage[:b - a], None, None, ids=np.arange(a, b, dtype=np.int32),
+                                       mask_from_cloud=True)
+                hs += h
+                nfeat += list(f)
+        t1 = time.perf_counter()
+        res = np.zeros(len(pp), PAIR_RESULT_DTYPE); res["id1"] = -1; res["id2"] = -1
+        pipeline.match_pairs_pipelined(fe, hs, pp, seed=seed, first_pair_index=0, out=res)
+        graph = graph_from_pairs(pp, res, nf)
+        traj, chi2, lm, cg = fe.optimize_graph(graph["init"], graph["fixed"], graph["ij"], graph["meas"], graph["info"], stop=0.01)
+        t2 = time.perf_counter()
+        fe.detector_destroy(det)
+        for h in hs:
+            fe.node_destroy(h)
+        return nfeat, res, graph, traj, chi2, lm, t2 - t0
+
+    c4 = {}
+    for kind in ("cloud", "depth"):
+        sequence(kind, min(nf_, 96))
+        nfeat, res, graph, traj, chi2, lm, secs = sequence(kind, nf_)
+        c4[kind] = {"frames": nf_, "pairs": int(len(pairs)), "valid_edges": int(graph["n_valid_edges"]),
+                    "mean_features": float(np.mean(nfeat)), "mean_inliers_valid": float(res["n_inliers"][res["id1"] >= 0].mean()),
+                    "lm_iterations": lm, "chi2": chi2, "ate_vs_gt_m": synth.ate_rmse(traj[:, :3], gt[:, :3]), "seconds": secs}
     out["c4"] = c4
     fe.close()
     print(json.dumps(out))
