@@ -2,55 +2,25 @@
 bit for bit against tests/cloud_oracle.py (on top of the cv2-based ORB and FAST detection oracles), with the detector
 thresholds compared after every frame."""
 import copy
-import ctypes as C
 
 import cv2
 import numpy as np
 import pytest
 
+import node_helpers as nh
+from node_helpers import MAXK
+
 pytestmark = pytest.mark.gpu
 
 SCENARIOS = ["mask", "no_mask", "mask_from_cloud", "planted", "trunc"]
-MAXK = 600
-
-
-def _params(detector, **kw):
-    from rgbdslam_v2_b200._capi import default_params
-    p = default_params()
-    p.depth_cov_z0 = 2.0
-    p.max_keypoints = MAXK
-    p.feature_detector_type = detector
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
-
-
-def _reinit(fe, detector, **kw):
-    p = _params(detector, **kw)
-    fe.params = p
-    fe._check(fe.lib.rgbdslam_b200_init(0, C.byref(p)))
-
-
-def _make_detector(fe, detector, **kw):
-    _reinit(fe, detector, **kw)
-    return fe.detector_create()
-
-
-def _name(detector):
-    return "FAST" if detector == 1 else "ORB"
 
 
 @pytest.fixture(scope="module")
 def fe(built):
     from rgbdslam_v2_b200 import Frontend
-    f = Frontend(0, _params(0))
+    f = Frontend(0, nh.params(0))
     yield f
     f.close()
-
-
-def _K4():
-    from rgbdslam_v2_b200 import synth
-    return (synth.FX, synth.FY, synth.CX, synth.CY)
 
 
 def _colour(gray):
@@ -58,11 +28,8 @@ def _colour(gray):
     return np.ascontiguousarray(np.stack([gray, np.roll(gray, 3, axis=-1), np.roll(gray, 5, axis=-2)], -1))
 
 
-def _render(n, step=1):
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(240)
-    fr = [synth.render_frame(poses[k * step], seed=k) for k in range(n)]
-    return np.stack([f[0] for f in fr]), np.stack([f[1] for f in fr])
+def _render(n):
+    return nh.stack(nh.render(range(n)))
 
 
 @pytest.fixture(scope="module")
@@ -74,22 +41,6 @@ def frames():
 def seq24():
     """24 frames: several chunks of the constructor's pipeline with cloud input"""
     return _render(24)
-
-
-def _node_dump(fe, handles):
-    return [(fe.node_keypoints(h), *fe.node_download(h)) for h in handles]
-
-
-def _same_nodes(a, b):
-    for (ka, da, xa), (kb, db, xb) in zip(a, b):
-        if not (np.array_equal(ka, kb) and np.array_equal(da, db) and np.array_equal(xa.view(np.uint32), xb.view(np.uint32))):
-            return False
-    return len(a) == len(b)
-
-
-def _destroy(fe, handles):
-    for h in handles:
-        fe.node_destroy(h)
 
 
 def _plant_values(cloud, seed):
@@ -137,7 +88,7 @@ def test_cloud_nodes_vs_oracle(fe, frames, scenario, detector):
     import cloud_oracle as co
     from oracle import orb_oracle as oo
     gray, depth = frames
-    det = _make_detector(fe, detector)
+    det = nh.make_detector(fe, detector)
     st = oo.DetectorState()
     ptype = "XYZ" if scenario in ("no_mask", "planted") else "XYZRGB"
     handles, kept_inf, kept_nan_round = [], 0, 0
@@ -146,7 +97,7 @@ def test_cloud_nodes_vs_oracle(fe, frames, scenario, detector):
         if scenario == "mask_from_cloud":  # depths below 0.02 m and in the 5.12 m band read as "no mask"
             d[40:200, 60:300] = np.float32(0.015)
             d[250:420, 340:600] = np.float32(5.125)
-        cloud = co.cloud_from_depth(d, _K4(), ptype, _colour(gray[k]))
+        cloud = co.cloud_from_depth(d, nh.K4(), ptype, _colour(gray[k]))
         mask = None
         if scenario in ("mask", "trunc"):
             mask = oo.depth_to_mask(depth[k])  # kinectCallback's depthToCV8UC1
@@ -157,12 +108,12 @@ def test_cloud_nodes_vs_oracle(fe, frames, scenario, detector):
         if scenario == "planted":
             cloud = _plant_values(cloud, k)
         elif scenario == "trunc":
-            rec = co.detect(gray[k], mask, copy.deepcopy(st), MAXK, detector=_name(detector))
+            rec = co.detect(gray[k], mask, copy.deepcopy(st), MAXK, detector=nh.name(detector))
             cloud, at_round = _plant_trunc(cloud, rec)
         hs, nf = fe.nodes_create(det, gray[k:k + 1], cloud[None], None if scenario == "mask_from_cloud" else (None if mask is None else mask[None]),
                                  None, ids=[k], mask_from_cloud=scenario == "mask_from_cloud")
         handles += hs
-        okp, odesc, oxyz = co.node_construct(gray[k], cloud, mask, st, MAXK, detector=_name(detector))
+        okp, odesc, oxyz = co.node_construct(gray[k], cloud, mask, st, MAXK, detector=nh.name(detector))
         gkp = fe.node_keypoints(hs[0])
         gdesc, gxyz = fe.node_download(hs[0])
         assert nf[0] == len(okp) and 300 < len(okp) <= MAXK
@@ -183,7 +134,7 @@ def test_cloud_nodes_vs_oracle(fe, frames, scenario, detector):
         assert (res["id1"] == np.arange(len(handles) - 1)).all() and (res["id2"] == np.arange(1, len(handles))).all()
         assert (res["n_inliers"] > 50).all()
     fe.detector_destroy(det)
-    _destroy(fe, handles)
+    nh.destroy(fe, handles)
 
 
 @pytest.mark.parametrize("detector", [0, 1], ids=["ORB", "FAST"])
@@ -196,18 +147,18 @@ def test_colour_input_equals_cvtcolor(fe, frames, detector):
     rgb = np.stack([_colour(g) for g in gray])
     conv = np.stack([cv2.cvtColor(c, cv2.COLOR_RGB2GRAY) for c in rgb])
     mask = np.stack([oo.depth_to_mask(d) for d in depth])
-    clouds = np.stack([co.cloud_from_depth(d, _K4(), "XYZRGB", c) for d, c in zip(depth, rgb)])
+    clouds = np.stack([co.cloud_from_depth(d, nh.K4(), "XYZRGB", c) for d, c in zip(depth, rgb)])
     for dep, m, kw in ((depth, mask, {}), (depth, None, {"mask_from_depth": True}), (clouds, mask, {}),
                        (clouds, None, {"mask_from_cloud": True})):
         out = {}
         for name, vis in (("rgb", rgb), ("gray", conv)):
-            det = _make_detector(fe, detector)
+            det = nh.make_detector(fe, detector)
             l0 = fe.lib.rgbdslam_b200_launch_count()
-            hs = fe.nodes_create(det, vis, dep, m, _K4(), **kw)[0]
-            out[name] = (_node_dump(fe, hs), fe.detector_thresholds(det).copy(), fe.lib.rgbdslam_b200_launch_count() - l0)
+            hs = fe.nodes_create(det, vis, dep, m, nh.K4(), **kw)[0]
+            out[name] = (nh.node_dump(fe, hs), fe.detector_thresholds(det).copy(), fe.lib.rgbdslam_b200_launch_count() - l0)
             fe.detector_destroy(det)
-            _destroy(fe, hs)
-        assert _same_nodes(out["rgb"][0], out["gray"][0]) and min(len(x[0]) for x in out["rgb"][0]) > 300
+            nh.destroy(fe, hs)
+        assert nh.same_nodes(out["rgb"][0], out["gray"][0]) and min(len(x[0]) for x in out["rgb"][0]) > 300
         assert np.array_equal(out["rgb"][1], out["gray"][1])
         assert out["rgb"][2] == out["gray"][2] + 1  # k_rgb_to_gray, one chunk
 
@@ -227,17 +178,17 @@ def test_cloud_pipeline_variants_identical(fe, seq24, config, detector):
     gray, depth = seq24
     n = len(gray)
     vis = np.stack([_colour(g) for g in gray]) if vis_kind == "rgb" else gray
-    clouds = np.stack([co.cloud_from_depth(d, _K4(), ptype) for d in depth])
+    clouds = np.stack([co.cloud_from_depth(d, nh.K4(), ptype) for d in depth])
     mask = np.stack([oo.depth_to_mask(d) for d in depth]) if mask_kind == "caller" else None
     mfc = mask_kind == "cloud"
 
     def run(fn):
-        det = _make_detector(fe, detector)
+        det = nh.make_detector(fe, detector)
         out = fn(det)
         thr = fe.detector_thresholds(det).copy()
         fe.detector_destroy(det)
-        dump = _node_dump(fe, out)
-        _destroy(fe, out)
+        dump = nh.node_dump(fe, out)
+        nh.destroy(fe, out)
         return dump, thr
 
     ref, thr_ref = run(lambda det: fe.nodes_create(det, vis, clouds, mask, None, mask_from_cloud=mfc)[0])
@@ -250,15 +201,15 @@ def test_cloud_pipeline_variants_identical(fe, seq24, config, detector):
                                   mask_from_cloud=mfc)[0]
         return hs
     a, thr_a = run(one_by_one)
-    assert _same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
+    assert nh.same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
     pv, pc = torch.from_numpy(vis).pin_memory(), torch.from_numpy(clouds).pin_memory()
     pm = None if mask is None else torch.from_numpy(mask).pin_memory()
     b, thr_b = run(lambda det: fe.nodes_create(det, pv, pc, pm, None, mask_from_cloud=mfc)[0])
-    assert _same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
+    assert nh.same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
     comm = fe.comm_init(0, 1, fe.comm_unique_id())
     c, thr_c = run(lambda det: fe.nodes_create_sharded(det, comm, n, vis, clouds, mask, None, mask_from_cloud=mfc)[0])
     fe.comm_destroy(comm)
-    assert _same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
+    assert nh.same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
 
 
 @pytest.mark.parametrize("detector", [0, 1], ids=["ORB", "FAST"])
@@ -269,8 +220,8 @@ def test_cloud_and_depth_calls_interleaved(fe, seq24, detector):
     import fast_oracle
     from oracle import orb_oracle as oo
     gray, depth = seq24
-    K4 = _K4()
-    det = _make_detector(fe, detector)
+    K4 = nh.K4()
+    det = nh.make_detector(fe, detector)
     st = oo.DetectorState()
     depth_node = fast_oracle.node_construct if detector == 1 else oo.node_construct
     for i, a in enumerate(range(0, 8, 2)):
@@ -279,15 +230,15 @@ def test_cloud_and_depth_calls_interleaved(fe, seq24, detector):
         if i % 2 == 0:
             clouds = np.stack([co.cloud_from_depth(d, K4, "XYZRGB") for d in depth[a:b]])
             hs = fe.nodes_create(det, gray[a:b], clouds, mask, None)[0]
-            want = [co.node_construct(gray[k], clouds[k - a], mask[k - a], st, MAXK, detector=_name(detector)) for k in range(a, b)]
+            want = [co.node_construct(gray[k], clouds[k - a], mask[k - a], st, MAXK, detector=nh.name(detector)) for k in range(a, b)]
         else:
             hs = fe.nodes_create(det, gray[a:b], depth[a:b], mask, K4)[0]
             want = [depth_node(gray[k], depth[k], mask[k - a], K4, st, max_keypoints=MAXK) for k in range(a, b)]
-        got = _node_dump(fe, hs)
+        got = nh.node_dump(fe, hs)
         for (gk, gd, gx), (ok, od, ox) in zip(got, want):
             assert gk.tobytes() == ok.tobytes() and np.array_equal(gd, od) and np.array_equal(gx.view(np.uint32), ox.view(np.uint32))
         assert np.array_equal(fe.detector_thresholds(det)[:9], np.array(st.thresh[:9]))
-        _destroy(fe, hs)
+        nh.destroy(fe, hs)
     fe.detector_destroy(det)
 
 
@@ -296,26 +247,26 @@ def test_depth_parameters_do_not_touch_cloud_nodes(fe, frames, detector):
     """use_feature_min_depth and depth_scaling_factor are not read by the point-cloud constructor."""
     import cloud_oracle as co
     gray, depth = frames
-    clouds = np.stack([co.cloud_from_depth(d, _K4(), "XYZRGB") for d in depth])
+    clouds = np.stack([co.cloud_from_depth(d, nh.K4(), "XYZRGB") for d in depth])
     out = []
     for kw in ({}, {"use_feature_min_depth": 1}, {"depth_scaling_factor": 1.25}):
-        det = _make_detector(fe, detector, **kw)
+        det = nh.make_detector(fe, detector, **kw)
         hs = fe.nodes_create(det, gray, clouds, None, None, mask_from_cloud=True)[0]
-        out.append((_node_dump(fe, hs), fe.detector_thresholds(det).copy()))
+        out.append((nh.node_dump(fe, hs), fe.detector_thresholds(det).copy()))
         fe.detector_destroy(det)
-        _destroy(fe, hs)
+        nh.destroy(fe, hs)
     for dump, thr in out[1:]:
-        assert _same_nodes(out[0][0], dump) and np.array_equal(out[0][1], thr)
+        assert nh.same_nodes(out[0][0], dump) and np.array_equal(out[0][1], thr)
 
 
 def test_rejected_combinations_launch_nothing(fe, frames):
     from rgbdslam_v2_b200._capi import CLOUD_XYZ, CLOUD_XYZRGB, MASK_FROM_CLOUD, MASK_FROM_DEPTH, VISUAL_RGB, _ptr
     import cloud_oracle as co
     gray, depth = frames
-    det = _make_detector(fe, 0)
-    cloud = np.ascontiguousarray(co.cloud_from_depth(depth[0], _K4(), "XYZRGB")[None])
+    det = nh.make_detector(fe, 0)
+    cloud = np.ascontiguousarray(co.cloud_from_depth(depth[0], nh.K4(), "XYZRGB")[None])
     rgb = np.ascontiguousarray(_colour(gray[0])[None])
-    K4 = np.array(_K4(), np.float32)
+    K4 = np.array(nh.K4(), np.float32)
     handles = np.zeros(1, np.uint64)
     nf = np.zeros(1, np.int32)
     H, W = gray.shape[1:]
@@ -332,10 +283,10 @@ def test_rejected_combinations_launch_nothing(fe, frames):
         rc, msg = call(rgb if flags & VISUAL_RGB else gray[:1], cloud, flags)
         assert rc == 1 and word in msg, (flags, msg)
     # the environment measurement model is not built for cloud nodes
-    _reinit(fe, 0, observability_threshold=0.5)
+    nh.reinit(fe, 0, observability_threshold=0.5)
     rc, msg = call(gray[:1], cloud, CLOUD_XYZRGB, None)
     assert rc == 3 and b"measurement model" in msg
-    _reinit(fe, 0)
+    nh.reinit(fe, 0)
     # K4 may be NULL for cloud input, but not for a depth image
     rc, _ = call(gray[:1], np.ascontiguousarray(depth[:1]), 0, None)
     assert rc == 1
@@ -367,26 +318,26 @@ def test_colour_input_at_sizes_not_a_multiple_of_4(fe, seq20, size):
     assert (W * H) % 4 != 0
     rgb = np.stack([_colour(g) for g in gray])
     conv = np.stack([cv2.cvtColor(c, cv2.COLOR_RGB2GRAY) for c in rgb])
-    clouds = np.stack([co.cloud_from_depth(d, _K4(), "XYZRGB") for d in depth])
+    clouds = np.stack([co.cloud_from_depth(d, nh.K4(), "XYZRGB") for d in depth])
     n = len(gray)
 
     def run(fn):
-        det = _make_detector(fe, 0)
+        det = nh.make_detector(fe, 0)
         hs = fn(det)
-        out = (_node_dump(fe, hs), fe.detector_thresholds(det).copy())
+        out = (nh.node_dump(fe, hs), fe.detector_thresholds(det).copy())
         fe.detector_destroy(det)
-        _destroy(fe, hs)
+        nh.destroy(fe, hs)
         return out
 
     # _ex, depth image: 3 frames in one chunk, the last (W * H * 3) % 4 pixels take the tail path
-    a = run(lambda det: fe.nodes_create(det, rgb[:3], depth[:3], None, _K4(), mask_from_depth=True)[0])
-    b = run(lambda det: fe.nodes_create(det, conv[:3], depth[:3], None, _K4(), mask_from_depth=True)[0])
-    assert _same_nodes(a[0], b[0]) and np.array_equal(a[1], b[1]) and min(len(k) for k, _, _ in a[0]) > 300
+    a = run(lambda det: fe.nodes_create(det, rgb[:3], depth[:3], None, nh.K4(), mask_from_depth=True)[0])
+    b = run(lambda det: fe.nodes_create(det, conv[:3], depth[:3], None, nh.K4(), mask_from_depth=True)[0])
+    assert nh.same_nodes(a[0], b[0]) and np.array_equal(a[1], b[1]) and min(len(k) for k, _, _ in a[0]) > 300
     # _sharded (1 rank), XYZRGB clouds: 3 chunks at frames 0, 9, 18 of the rank's device buffers
     comm = fe.comm_init(0, 1, fe.comm_unique_id())
     c = run(lambda det: fe.nodes_create_sharded(det, comm, n, rgb, clouds, None, None, mask_from_cloud=True)[0])
     d = run(lambda det: fe.nodes_create_sharded(det, comm, n, conv, clouds, None, None, mask_from_cloud=True)[0])
     fe.comm_destroy(comm)
     e = run(lambda det: fe.nodes_create(det, rgb, clouds, None, None, mask_from_cloud=True)[0])
-    assert _same_nodes(c[0], d[0]) and np.array_equal(c[1], d[1]) and min(len(k) for k, _, _ in c[0]) > 300
-    assert _same_nodes(c[0], e[0]) and np.array_equal(c[1], e[1])
+    assert nh.same_nodes(c[0], d[0]) and np.array_equal(c[1], d[1]) and min(len(k) for k, _, _ in c[0]) > 300
+    assert nh.same_nodes(c[0], e[0]) and np.array_equal(c[1], e[1])

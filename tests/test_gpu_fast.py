@@ -5,78 +5,28 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import node_helpers as nh
+
 pytestmark = pytest.mark.gpu
-
-
-def _params(detector, **kw):
-    from rgbdslam_v2_b200._capi import default_params
-    p = default_params()
-    p.depth_cov_z0 = 2.0
-    p.max_keypoints = 600
-    p.feature_detector_type = detector
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
-
-
-def _reinit(fe, detector, **kw):
-    p = _params(detector, **kw)
-    fe.params = p
-    fe._check(fe.lib.rgbdslam_b200_init(0, C.byref(p)))
-
-
-def _make_detector(fe, detector, **kw):
-    """detector_create takes the type of the current parameters; the handle keeps it."""
-    _reinit(fe, detector, **kw)
-    return fe.detector_create()
 
 
 @pytest.fixture(scope="module")
 def fe(built):
     from rgbdslam_v2_b200 import Frontend
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    f = Frontend(0, _params(DETECTOR_FAST))
+    f = Frontend(0, nh.params(DETECTOR_FAST))
     yield f
     f.close()
 
 
 @pytest.fixture(scope="module")
 def frames():
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(40)
-    return [synth.render_frame(poses[k], seed=k) for k in (0, 1, 2, 9)]
+    return nh.render((0, 1, 2, 9), 40)
 
 
 @pytest.fixture(scope="module")
 def seq40():
-    from oracle import orb_oracle
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(240)[:40]
-    fr = [synth.render_frame(poses[k], seed=k) for k in range(40)]
-    gray = np.stack([f[0] for f in fr]); depth = np.stack([f[1] for f in fr])
-    mask = np.stack([orb_oracle.depth_to_mask(d) for d in depth])
-    return gray, depth, mask
-
-
-def _K4():
-    from rgbdslam_v2_b200 import synth
-    return (synth.FX, synth.FY, synth.CX, synth.CY)
-
-
-def _node_dump(fe, handles):
-    return [(fe.node_keypoints(h), *fe.node_download(h)) for h in handles]
-
-
-def _same_nodes(a, b):
-    for (ka, da, xa), (kb, db, xb) in zip(a, b):
-        if not (np.array_equal(ka, kb) and np.array_equal(da, db) and np.array_equal(xa.view(np.uint32), xb.view(np.uint32))):
-            return False
-    return len(a) == len(b)
-
-
-def _destroy(fe, handles):
-    for h in handles:
-        fe.node_destroy(h)
+    return nh.seq(40)
 
 
 def test_fast_detect_vs_cv2_over_a_sequence(fe, frames):
@@ -85,7 +35,7 @@ def test_fast_detect_vs_cv2_over_a_sequence(fe, frames):
     import fast_oracle
     from oracle import orb_oracle
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    det = _make_detector(fe, DETECTOR_FAST)
+    det = nh.make_detector(fe, DETECTOR_FAST)
     st = orb_oracle.DetectorState()
     for gray, depth in frames:
         mask = orb_oracle.depth_to_mask(depth)
@@ -108,7 +58,7 @@ def test_fast_textureless_frame_and_no_mask(fe, frames):
     import fast_oracle
     from oracle import orb_oracle
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    det = _make_detector(fe, DETECTOR_FAST, max_keypoints=1000)
+    det = nh.make_detector(fe, DETECTOR_FAST, max_keypoints=1000)
     st = orb_oracle.DetectorState()
     gray = frames[3][0]
     orec = fast_oracle.grid_detect(gray, None, st, max_keypoints=1000)
@@ -128,11 +78,11 @@ def test_fast_nodes_create_vs_oracle(fe, frames, oracle_mod):
     import fast_oracle
     from oracle import orb_oracle
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    det = _make_detector(fe, DETECTOR_FAST)
+    det = nh.make_detector(fe, DETECTOR_FAST)
     st = orb_oracle.DetectorState()
     gray = np.stack([f[0] for f in frames]); depth = np.stack([f[1] for f in frames])
     mask = np.stack([orb_oracle.depth_to_mask(f[1]) for f in frames])
-    K4 = _K4()
+    K4 = nh.K4()
     handles, nf = fe.nodes_create(det, gray, depth, mask, K4, ids=[10, 11, 12, 13])
     for i, h in enumerate(handles):
         okp, odesc, oxyz = fast_oracle.node_construct(frames[i][0], frames[i][1], mask[i], K4, st, max_keypoints=600)
@@ -147,7 +97,7 @@ def test_fast_nodes_create_vs_oracle(fe, frames, oracle_mod):
     res, _, _ = fe.match_node_pairs([handles[1]], [handles[0]], seed=3)
     assert res[0]["id1"] == 10 and res[0]["id2"] == 11 and res[0]["n_inliers"] > 50
     fe.detector_destroy(det)
-    _destroy(fe, handles)
+    nh.destroy(fe, handles)
 
 
 def test_fast_nodes_create_pipeline_variants_identical(fe, seq40):
@@ -155,15 +105,15 @@ def test_fast_nodes_create_pipeline_variants_identical(fe, seq40):
     import torch
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
     gray, depth, mask = seq40
-    K4 = _K4()
+    K4 = nh.K4()
 
     def run(fn):
-        det = _make_detector(fe, DETECTOR_FAST)
+        det = nh.make_detector(fe, DETECTOR_FAST)
         out = fn(det)
         thr = fe.detector_thresholds(det).copy()
         fe.detector_destroy(det)
-        dump = _node_dump(fe, out)
-        _destroy(fe, out)
+        dump = nh.node_dump(fe, out)
+        nh.destroy(fe, out)
         return dump, thr
 
     ref, thr_ref = run(lambda det: fe.nodes_create(det, gray, depth, mask, K4)[0])
@@ -175,19 +125,19 @@ def test_fast_nodes_create_pipeline_variants_identical(fe, seq40):
             hs += fe.nodes_create(det, gray[k:k + 1], depth[k:k + 1], mask[k:k + 1], K4, ids=[k])[0]
         return hs
     a, thr_a = run(one_by_one)
-    assert _same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
+    assert nh.same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
     pg, pd, pm = (torch.from_numpy(x).pin_memory() for x in (gray, depth, mask))
     b, thr_b = run(lambda det: fe.nodes_create(det, pg, pd, pm, K4)[0])
-    assert _same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
+    assert nh.same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
     c, thr_c = run(lambda det: fe.nodes_create(det, gray, depth, None, K4, mask_from_depth=True)[0])
-    assert _same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
+    assert nh.same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
 
 
 def test_fast_nodes_create_sharded_single_rank_equals_plain(fe, seq40):
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
     gray, depth, mask = seq40
-    K4 = _K4()
-    det = _make_detector(fe, DETECTOR_FAST)
+    K4 = nh.K4()
+    det = nh.make_detector(fe, DETECTOR_FAST)
     h1, n1 = fe.nodes_create(det, gray, depth, mask, K4)
     thr1 = fe.detector_thresholds(det).copy()
     fe.detector_destroy(det)
@@ -197,27 +147,27 @@ def test_fast_nodes_create_sharded_single_rank_equals_plain(fe, seq40):
     thr2 = fe.detector_thresholds(det).copy()
     fe.detector_destroy(det)
     assert np.array_equal(n1, n2) and np.array_equal(thr1, thr2)
-    assert _same_nodes(_node_dump(fe, h1), _node_dump(fe, h2))
+    assert nh.same_nodes(nh.node_dump(fe, h1), nh.node_dump(fe, h2))
     fe.comm_destroy(comm)
-    _destroy(fe, h1 + h2)
+    nh.destroy(fe, h1 + h2)
 
 
 def test_orb_and_fast_detectors_interleaved(fe, seq40):
     """An ORB and a FAST detector used alternately in one process give what each gives alone: the handle decides."""
     from rgbdslam_v2_b200._capi import DETECTOR_FAST, DETECTOR_ORB
     gray, depth, mask = seq40
-    K4 = _K4()
+    K4 = nh.K4()
     alone = {}
     for t in (DETECTOR_ORB, DETECTOR_FAST):
-        det = _make_detector(fe, t)
+        det = nh.make_detector(fe, t)
         hs = []
         for k in range(0, 12, 4):
             hs += fe.nodes_create(det, gray[k:k + 4], depth[k:k + 4], mask[k:k + 4], K4)[0]
-        alone[t] = (_node_dump(fe, hs), fe.detector_thresholds(det).copy(), fe.orb_detect(det, gray[20], mask[20]))
+        alone[t] = (nh.node_dump(fe, hs), fe.detector_thresholds(det).copy(), fe.orb_detect(det, gray[20], mask[20]))
         fe.detector_destroy(det)
-        _destroy(fe, hs)
-    d_orb = _make_detector(fe, DETECTOR_ORB)
-    d_fast = _make_detector(fe, DETECTOR_FAST)  # the parameters now say FAST; the ORB handle stays ORB
+        nh.destroy(fe, hs)
+    d_orb = nh.make_detector(fe, DETECTOR_ORB)
+    d_fast = nh.make_detector(fe, DETECTOR_FAST)  # the parameters now say FAST; the ORB handle stays ORB
     hs = {DETECTOR_ORB: [], DETECTOR_FAST: []}
     for k in range(0, 12, 4):
         for t, det in ((DETECTOR_FAST, d_fast), (DETECTOR_ORB, d_orb)):
@@ -225,18 +175,18 @@ def test_orb_and_fast_detectors_interleaved(fe, seq40):
     thr = {t: fe.detector_thresholds(det).copy() for t, det in ((DETECTOR_ORB, d_orb), (DETECTOR_FAST, d_fast))}
     kp = {DETECTOR_ORB: fe.orb_detect(d_orb, gray[20], mask[20]), DETECTOR_FAST: fe.orb_detect(d_fast, gray[20], mask[20])}
     for t, det in ((DETECTOR_ORB, d_orb), (DETECTOR_FAST, d_fast)):
-        assert _same_nodes(alone[t][0], _node_dump(fe, hs[t]))
+        assert nh.same_nodes(alone[t][0], nh.node_dump(fe, hs[t]))
         assert np.array_equal(alone[t][1], thr[t])  # thresholds after the node batches, before the detect call
         assert kp[t].tobytes() == alone[t][2].tobytes()
         fe.detector_destroy(det)
-        _destroy(fe, hs[t])
-    assert not _same_nodes(alone[DETECTOR_ORB][0], alone[DETECTOR_FAST][0])
+        nh.destroy(fe, hs[t])
+    assert not nh.same_nodes(alone[DETECTOR_ORB][0], alone[DETECTOR_FAST][0])
 
 
 def test_invalid_detector_type_rejected_by_init(fe):
     from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    _reinit(fe, DETECTOR_FAST)
-    p = _params(7)
+    nh.reinit(fe, DETECTOR_FAST)
+    p = nh.params(7)
     assert fe.lib.rgbdslam_b200_init(0, C.byref(p)) == 1
     assert b"feature_detector_type" in fe.lib.rgbdslam_b200_last_error()
     assert fe.lib.rgbdslam_b200_get_params(C.byref(p)) == 0 and p.feature_detector_type == DETECTOR_FAST  # unchanged

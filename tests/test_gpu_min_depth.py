@@ -6,55 +6,20 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import node_helpers as nh
+
 pytestmark = pytest.mark.gpu
 
 SCENARIOS = ["mask", "no_mask", "mask_from_depth", "depth_scaling", "blobs"]
-
-
-def _params(detector, **kw):
-    from rgbdslam_v2_b200._capi import default_params
-    p = default_params()
-    p.depth_cov_z0 = 2.0
-    p.max_keypoints = 600
-    p.feature_detector_type = detector
-    for k, v in kw.items():
-        setattr(p, k, v)
-    return p
-
-
-def _reinit(fe, detector, **kw):
-    p = _params(detector, **kw)
-    fe.params = p
-    fe._check(fe.lib.rgbdslam_b200_init(0, C.byref(p)))
-
-
-def _make_detector(fe, detector, **kw):
-    _reinit(fe, detector, **kw)
-    return fe.detector_create()
-
-
-def _name(detector):
-    from rgbdslam_v2_b200._capi import DETECTOR_FAST
-    return "FAST" if detector == DETECTOR_FAST else "ORB"
-
-
-def _detectors():
-    from rgbdslam_v2_b200._capi import DETECTOR_FAST, DETECTOR_ORB
-    return [DETECTOR_ORB, DETECTOR_FAST]
 
 
 @pytest.fixture(scope="module")
 def fe(built):
     from rgbdslam_v2_b200 import Frontend
     from rgbdslam_v2_b200._capi import DETECTOR_ORB
-    f = Frontend(0, _params(DETECTOR_ORB, use_feature_min_depth=1))
+    f = Frontend(0, nh.params(DETECTOR_ORB, use_feature_min_depth=1))
     yield f
     f.close()
-
-
-def _K4():
-    from rgbdslam_v2_b200 import synth
-    return (synth.FX, synth.FY, synth.CX, synth.CY)
 
 
 def _plant_blobs(depth, seed):
@@ -76,10 +41,7 @@ def _plant_blobs(depth, seed):
 
 @pytest.fixture(scope="module")
 def frames():
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(40)
-    fr = [synth.render_frame(poses[k], seed=k) for k in (0, 1, 2, 3)]
-    gray = np.stack([f[0] for f in fr]); depth = np.stack([f[1] for f in fr])
+    gray, depth = nh.stack(nh.render((0, 1, 2, 3), 40))
     blobs = np.stack([_plant_blobs(d, k) for k, d in enumerate(depth)])
     return gray, depth, blobs
 
@@ -87,29 +49,7 @@ def frames():
 @pytest.fixture(scope="module")
 def seq70():
     """70 frames: two chunks of the constructor's pipeline"""
-    from oracle import orb_oracle
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(240)[:70]
-    fr = [synth.render_frame(poses[k], seed=k) for k in range(70)]
-    gray = np.stack([f[0] for f in fr]); depth = np.stack([f[1] for f in fr])
-    mask = np.stack([orb_oracle.depth_to_mask(d) for d in depth])
-    return gray, depth, mask
-
-
-def _node_dump(fe, handles):
-    return [(fe.node_keypoints(h), *fe.node_download(h)) for h in handles]
-
-
-def _same_nodes(a, b):
-    for (ka, da, xa), (kb, db, xb) in zip(a, b):
-        if not (np.array_equal(ka, kb) and np.array_equal(da, db) and np.array_equal(xa.view(np.uint32), xb.view(np.uint32))):
-            return False
-    return len(a) == len(b)
-
-
-def _destroy(fe, handles):
-    for h in handles:
-        fe.node_destroy(h)
+    return nh.seq(70)
 
 
 def _pointwise_z(depth, kp, scaling=1.0):
@@ -130,9 +70,9 @@ def test_min_depth_nodes_vs_oracle(fe, frames, scenario, detector):
     if scenario == "blobs":
         depth = blobs
     scaling = 1.25 if scenario == "depth_scaling" else 1.0
-    det = _make_detector(fe, detector, use_feature_min_depth=1, depth_scaling_factor=scaling)
+    det = nh.make_detector(fe, detector, use_feature_min_depth=1, depth_scaling_factor=scaling)
     st = orb_oracle.DetectorState()
-    K4 = _K4()
+    K4 = nh.K4()
     handles, on_nan, below = [], 0, 0
     for k in range(len(gray)):
         mask = None if scenario in ("no_mask", "blobs") else orb_oracle.depth_to_mask(depth[k])
@@ -141,7 +81,7 @@ def test_min_depth_nodes_vs_oracle(fe, frames, scenario, detector):
                                  mask_from_depth=scenario == "mask_from_depth")
         handles += hs
         okp, odesc, oxyz = md.node_construct(gray[k], depth[k], mask, K4, st, max_keypoints=600, depth_scaling=scaling,
-                                             detector=_name(detector))
+                                             detector=nh.name(detector))
         gkp = fe.node_keypoints(hs[0])
         gdesc, gxyz = fe.node_download(hs[0])
         assert nf[0] == len(okp) and 300 < len(okp) <= 600
@@ -163,7 +103,7 @@ def test_min_depth_nodes_vs_oracle(fe, frames, scenario, detector):
     assert (res["id1"] == np.arange(len(handles) - 1)).all() and (res["id2"] == np.arange(1, len(handles))).all()
     assert (res["n_inliers"] > 50).all()
     fe.detector_destroy(det)
-    _destroy(fe, handles)
+    nh.destroy(fe, handles)
 
 
 @pytest.mark.parametrize("detector", [0, 1], ids=["ORB", "FAST"])
@@ -171,16 +111,16 @@ def test_min_depth_pipeline_variants_identical(fe, seq70, detector):
     """70 frames (2 chunks) == frame by frame == from pinned memory == mask from depth == 1-rank sharded."""
     import torch
     gray, depth, mask = seq70
-    K4 = _K4()
+    K4 = nh.K4()
     n = len(gray)
 
     def run(fn):
-        det = _make_detector(fe, detector, use_feature_min_depth=1)
+        det = nh.make_detector(fe, detector, use_feature_min_depth=1)
         out = fn(det)
         thr = fe.detector_thresholds(det).copy()
         fe.detector_destroy(det)
-        dump = _node_dump(fe, out)
-        _destroy(fe, out)
+        dump = nh.node_dump(fe, out)
+        nh.destroy(fe, out)
         return dump, thr
 
     ref, thr_ref = run(lambda det: fe.nodes_create(det, gray, depth, mask, K4)[0])
@@ -192,16 +132,16 @@ def test_min_depth_pipeline_variants_identical(fe, seq70, detector):
             hs += fe.nodes_create(det, gray[k:k + 1], depth[k:k + 1], mask[k:k + 1], K4, ids=[k])[0]
         return hs
     a, thr_a = run(one_by_one)
-    assert _same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
+    assert nh.same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
     pg, pd, pm = (torch.from_numpy(x).pin_memory() for x in (gray, depth, mask))
     b, thr_b = run(lambda det: fe.nodes_create(det, pg, pd, pm, K4)[0])
-    assert _same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
+    assert nh.same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
     c, thr_c = run(lambda det: fe.nodes_create(det, gray, depth, None, K4, mask_from_depth=True)[0])
-    assert _same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
+    assert nh.same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
     comm = fe.comm_init(0, 1, fe.comm_unique_id())
     d, thr_d = run(lambda det: fe.nodes_create_sharded(det, comm, n, gray, depth, mask, K4)[0])
     fe.comm_destroy(comm)
-    assert _same_nodes(ref, d) and np.array_equal(thr_ref, thr_d)
+    assert nh.same_nodes(ref, d) and np.array_equal(thr_ref, thr_d)
 
 
 @pytest.mark.parametrize("detector", [0, 1], ids=["ORB", "FAST"])
@@ -209,51 +149,51 @@ def test_flag_switches_between_calls(fe, seq70, detector):
     """The parameters current at each nodes_create call decide the rule: re-initialising with the flag off gives the
     pointwise nodes again, and alternating the flag between calls on one detector gives each rule's result."""
     gray, depth, mask = seq70
-    K4 = _K4()
+    K4 = nh.K4()
     chunks = [(k, k + 4) for k in range(0, 16, 4)]
     alone = {}
     for flag in (0, 1):
-        det = _make_detector(fe, detector, use_feature_min_depth=flag)
+        det = nh.make_detector(fe, detector, use_feature_min_depth=flag)
         hs = []
         for a, b in chunks:
             hs += fe.nodes_create(det, gray[a:b], depth[a:b], mask[a:b], K4)[0]
-        alone[flag] = _node_dump(fe, hs)
+        alone[flag] = nh.node_dump(fe, hs)
         fe.detector_destroy(det)
-        _destroy(fe, hs)
-    assert not _same_nodes(alone[0], alone[1])
+        nh.destroy(fe, hs)
+    assert not nh.same_nodes(alone[0], alone[1])
     # the thresholds depend only on the detection, so one detector serves both rules
-    det = _make_detector(fe, detector, use_feature_min_depth=0)
+    det = nh.make_detector(fe, detector, use_feature_min_depth=0)
     got = []
     for i, (a, b) in enumerate(chunks):
         flag = i % 2
-        _reinit(fe, detector, use_feature_min_depth=flag)
+        nh.reinit(fe, detector, use_feature_min_depth=flag)
         hs = fe.nodes_create(det, gray[a:b], depth[a:b], mask[a:b], K4)[0]
-        got += _node_dump(fe, hs)
-        _destroy(fe, hs)
-        assert _same_nodes(got[a:b], alone[flag][a:b])
+        got += nh.node_dump(fe, hs)
+        nh.destroy(fe, hs)
+        assert nh.same_nodes(got[a:b], alone[flag][a:b])
     fe.detector_destroy(det)
     # flag off again: the pointwise nodes, and the launch count of the pointwise path
-    det = _make_detector(fe, detector, use_feature_min_depth=0)
+    det = nh.make_detector(fe, detector, use_feature_min_depth=0)
     l0 = fe.lib.rgbdslam_b200_launch_count()
     hs = fe.nodes_create(det, gray[:4], depth[:4], mask[:4], K4)[0]
     l_off = fe.lib.rgbdslam_b200_launch_count() - l0
-    assert _same_nodes(_node_dump(fe, hs), alone[0][:4])
-    _destroy(fe, hs)
+    assert nh.same_nodes(nh.node_dump(fe, hs), alone[0][:4])
+    nh.destroy(fe, hs)
     fe.detector_destroy(det)
-    det = _make_detector(fe, detector, use_feature_min_depth=1)
+    det = nh.make_detector(fe, detector, use_feature_min_depth=1)
     l0 = fe.lib.rgbdslam_b200_launch_count()
     hs = fe.nodes_create(det, gray[:4], depth[:4], mask[:4], K4)[0]
     assert fe.lib.rgbdslam_b200_launch_count() - l0 == l_off + 1  # k_min_depth
-    _destroy(fe, hs)
+    nh.destroy(fe, hs)
     fe.detector_destroy(det)
 
 
 def test_init_rejects_other_values(fe):
     from rgbdslam_v2_b200._capi import DETECTOR_ORB
-    _reinit(fe, DETECTOR_ORB, use_feature_min_depth=1)
-    p = _params(DETECTOR_ORB, use_feature_min_depth=2)
+    nh.reinit(fe, DETECTOR_ORB, use_feature_min_depth=1)
+    p = nh.params(DETECTOR_ORB, use_feature_min_depth=2)
     assert fe.lib.rgbdslam_b200_init(0, C.byref(p)) == 1
     assert b"use_feature_min_depth" in fe.lib.rgbdslam_b200_last_error()
-    p = _params(DETECTOR_ORB, use_feature_min_depth=1, allow_features_without_depth_=1)
+    p = nh.params(DETECTOR_ORB, use_feature_min_depth=1, allow_features_without_depth_=1)
     assert fe.lib.rgbdslam_b200_init(0, C.byref(p)) == 1
     assert fe.lib.rgbdslam_b200_get_params(C.byref(p)) == 0 and p.use_feature_min_depth == 1  # unchanged

@@ -3,6 +3,8 @@
 import numpy as np
 import pytest
 
+import node_helpers as nh
+
 pytestmark = pytest.mark.gpu
 
 
@@ -20,24 +22,7 @@ def fe(built):
 
 @pytest.fixture(scope="module")
 def frames():
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(40)
-    out = []
-    for k in (0, 1, 2, 9):
-        g, d = synth.render_frame(poses[k], seed=k)
-        out.append((g, d))
-    return out
-
-
-def _reinit(fe, **kw):
-    import ctypes as C
-    from rgbdslam_v2_b200._capi import default_params
-    p = default_params()
-    p.depth_cov_z0 = 2.0
-    for k, v in kw.items():
-        setattr(p, k, v)
-    fe.params = p
-    fe._check(fe.lib.rgbdslam_b200_init(0, C.byref(p)))
+    return nh.render((0, 1, 2, 9), 40)
 
 
 def _canon(kp):
@@ -84,7 +69,7 @@ def test_grid_detect_vs_cv2_over_a_sequence(fe, frames):
     """detector->detect() incl. the per-cell adaptive thresholds carried across frames."""
     from oracle import orb_oracle
     from rgbdslam_v2_b200._capi import B200Error
-    _reinit(fe, max_keypoints=600)
+    nh.reinit(fe, max_keypoints=600)
     det = fe.detector_create()
     st = orb_oracle.DetectorState()
     for gray, depth in frames:
@@ -104,13 +89,12 @@ def test_grid_detect_vs_cv2_over_a_sequence(fe, frames):
 def test_nodes_create_vs_oracle(fe, frames, oracle_mod):
     """Full Node constructor (node.cpp:101-240) for a batch of frames processed in order."""
     from oracle import orb_oracle
-    from rgbdslam_v2_b200 import synth
-    _reinit(fe, max_keypoints=600)
+    nh.reinit(fe, max_keypoints=600)
     det = fe.detector_create()
     st = orb_oracle.DetectorState()
     gray = np.stack([f[0] for f in frames]); depth = np.stack([f[1] for f in frames])
     mask = np.stack([orb_oracle.depth_to_mask(f[1]) for f in frames])
-    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
+    K4 = nh.K4()
     handles, nf = fe.nodes_create(det, gray, depth, mask, K4, ids=[10, 11, 12, 13])
     for i, h in enumerate(handles):
         okp, odesc, oxyz = orb_oracle.node_construct(frames[i][0], frames[i][1], mask[i], K4, st, max_keypoints=600)
@@ -129,7 +113,7 @@ def test_nodes_create_vs_oracle(fe, frames, oracle_mod):
 
 def test_no_mask_and_other_parameters(fe, frames):
     from oracle import orb_oracle
-    _reinit(fe, max_keypoints=1000)
+    nh.reinit(fe, max_keypoints=1000)
     det = fe.detector_create()
     st = orb_oracle.DetectorState()
     gray = frames[3][0]
@@ -143,46 +127,28 @@ def test_no_mask_and_other_parameters(fe, frames):
     assert len(gkp) == len(orec) == 0
     assert np.array_equal(fe.detector_thresholds(det)[:9], np.array(st.thresh[:9]))
     fe.detector_destroy(det)
-    _reinit(fe, max_keypoints=600)
-
-
-def _node_dump(fe, handles):
-    return [(fe.node_keypoints(h), *fe.node_download(h)) for h in handles]
-
-
-def _same_nodes(a, b):
-    for (ka, da, xa), (kb, db, xb) in zip(a, b):
-        if not (np.array_equal(ka, kb) and np.array_equal(da, db) and np.array_equal(xa.view(np.uint32), xb.view(np.uint32))):
-            return False
-    return len(a) == len(b)
+    nh.reinit(fe, max_keypoints=600)
 
 
 @pytest.fixture(scope="module")
 def seq40():
-    from oracle import orb_oracle
-    from rgbdslam_v2_b200 import synth
-    poses = synth.trajectory(240)[:40]
-    fr = [synth.render_frame(poses[k], seed=k) for k in range(40)]
-    gray = np.stack([f[0] for f in fr]); depth = np.stack([f[1] for f in fr])
-    mask = np.stack([orb_oracle.depth_to_mask(d) for d in depth])
-    return gray, depth, mask
+    return nh.seq(40)
 
 
 def test_nodes_create_pipeline_variants_identical(fe, seq40):
     """The chunked, double-buffered constructor (40 frames = 2 chunks) gives bit-identical nodes and detector thresholds
     (a) frame by frame, (b) from pinned host memory, (c) with the mask derived from depth on the device."""
     import torch
-    from rgbdslam_v2_b200 import synth
     gray, depth, mask = seq40
-    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
-    _reinit(fe, max_keypoints=600)
+    K4 = nh.K4()
+    nh.reinit(fe, max_keypoints=600)
 
     def run(fn):
         det = fe.detector_create()
         out = fn(det)
         thr = fe.detector_thresholds(det).copy()
         fe.detector_destroy(det)
-        dump = _node_dump(fe, out)
+        dump = nh.node_dump(fe, out)
         for h in out:
             fe.node_destroy(h)
         return dump, thr
@@ -196,30 +162,29 @@ def test_nodes_create_pipeline_variants_identical(fe, seq40):
             hs += fe.nodes_create(det, gray[k:k + 1], depth[k:k + 1], mask[k:k + 1], K4, ids=[k])[0]
         return hs
     a, thr_a = run(one_by_one)
-    assert _same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
+    assert nh.same_nodes(ref, a) and np.array_equal(thr_ref, thr_a)
 
     pg, pd, pm = (torch.from_numpy(x).pin_memory() for x in (gray, depth, mask))
     b, thr_b = run(lambda det: fe.nodes_create(det, pg, pd, pm, K4)[0])
-    assert _same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
+    assert nh.same_nodes(ref, b) and np.array_equal(thr_ref, thr_b)
 
     c, thr_c = run(lambda det: fe.nodes_create(det, gray, depth, None, K4, mask_from_depth=True)[0])
-    assert _same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
+    assert nh.same_nodes(ref, c) and np.array_equal(thr_ref, thr_c)
 
 
 def test_nodes_create_without_mask_and_small_batches(fe, seq40):
     """mask = NULL (no mask pyramid at all) equals an all-255 mask; nodes of one call share a slab and survive the others"""
-    from rgbdslam_v2_b200 import synth
     gray, depth, _ = seq40
-    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
-    _reinit(fe, max_keypoints=600)
+    K4 = nh.K4()
+    nh.reinit(fe, max_keypoints=600)
     det = fe.detector_create()
     h1, _ = fe.nodes_create(det, gray[:3], depth[:3], None, K4)
     fe.detector_destroy(det)
     det = fe.detector_create()
     h2, _ = fe.nodes_create(det, gray[:3], depth[:3], np.full_like(gray[:3], 255), K4)
     fe.detector_destroy(det)
-    a, b = _node_dump(fe, h1), _node_dump(fe, h2)
-    assert _same_nodes(a, b)
+    a, b = nh.node_dump(fe, h1), nh.node_dump(fe, h2)
+    assert nh.same_nodes(a, b)
     fe.node_destroy(h1[0]); fe.node_destroy(h1[2])  # the slab stays alive for the remaining node
     k, d, x = fe.node_keypoints(h1[1]), *fe.node_download(h1[1])
     assert np.array_equal(k, b[1][0]) and np.array_equal(d, b[1][1])
@@ -230,10 +195,9 @@ def test_nodes_create_without_mask_and_small_batches(fe, seq40):
 def test_nodes_create_sharded_single_rank_equals_plain(fe, seq40):
     """The two-pass frame-sharded constructor (histogram exchange, threshold replay over the whole sequence, feature
     all-gather) on a 1-rank NCCL communicator == the plain constructor: nodes and final detector thresholds."""
-    from rgbdslam_v2_b200 import synth
     gray, depth, mask = seq40
-    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
-    _reinit(fe, max_keypoints=600)
+    K4 = nh.K4()
+    nh.reinit(fe, max_keypoints=600)
     det = fe.detector_create()
     h1, n1 = fe.nodes_create(det, gray, depth, mask, K4)
     thr1 = fe.detector_thresholds(det).copy()
@@ -244,7 +208,7 @@ def test_nodes_create_sharded_single_rank_equals_plain(fe, seq40):
     thr2 = fe.detector_thresholds(det).copy()
     fe.detector_destroy(det)
     assert np.array_equal(n1, n2) and np.array_equal(thr1, thr2)
-    assert _same_nodes(_node_dump(fe, h1), _node_dump(fe, h2))
+    assert nh.same_nodes(nh.node_dump(fe, h1), nh.node_dump(fe, h2))
     # matching works on the gathered nodes
     res, _, _ = fe.match_node_pairs(h2[1:6], h2[0:5], seed=3, want_matches=False)
     ref, _, _ = fe.match_node_pairs(h1[1:6], h1[0:5], seed=3, want_matches=False)

@@ -225,7 +225,7 @@ def main_cloud(args):
     out["h2d_bytes_per_frame"] = {k: c[4] for k, c in configs.items()}
 
     # ---- the kernels' device time per frame (torch.profiler, separate pass: tracing slows the host)
-    kernels = ("k_rgb_to_gray", "k_cloud_mask", "k_frame_finalize_cloud", "k_frame_emit_cloud", "k_frame_finalize", "k_frame_emit")
+    kernels = ("k_rgb_to_gray", "k_cloud_mask", "k_frame_finalize", "k_frame_emit")
     prof_frames = min(64, nt, nc)
     ktimes = {}
     for c in ("depth_rgb_pinned", "cloud_xyzrgb_pinned"):
@@ -236,8 +236,9 @@ def main_cloud(args):
         for e in prof.events():
             if e.device_type.name != "CUDA":
                 continue
-            m = re.search(r"rb200::(k_\w+)", e.name)
-            if m and m.group(1) in kernels:
+            # keyed on the template-id: one row per instantiation (point source, detector)
+            m = re.search(r"rb200::((k_\w+)(<[^>]*>)?)", e.name)
+            if m and m.group(2) in kernels:
                 tot[m.group(1)] = tot.get(m.group(1), 0.0) + e.device_time
         allk = sum(e.device_time for e in prof.events() if e.device_type.name == "CUDA" and "rb200::k_" in e.name)
         ktimes[c] = {k: round(t / prof_frames, 2) for k, t in sorted(tot.items())}
