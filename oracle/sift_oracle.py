@@ -41,7 +41,9 @@ def feature_matching(q_root, t_root, nn_ratio=0.95, max_matches=300):
     seen = set()
     for i in range(len(q_root)):
         ratio = np.float32(np.float32(d[i, 0]) / np.float32(d[i, 1]))
-        if nn_ratio > ratio:
+        # `double max_dist_ratio_fac > float dist_ratio_fac` compares in double; NumPy would compare a Python float
+        # with a float32 in float32 and reject fl32(0.95) = 0.949999988 against 0.95
+        if float(nn_ratio) > float(ratio):
             t = int(idx[i, 0])
             if t in seen:
                 continue
@@ -136,8 +138,8 @@ def siftgpu_match(desc1: np.ndarray, desc2: np.ndarray, distmax=0.9, ratiomax=0.
     d1, d2 = np.asarray(desc1, np.float32), np.asarray(desc2, np.float32)
     if len(d1) == 0 or len(d2) == 0:
         return np.zeros(0, co.DMATCH_DTYPE)
-    q1, q2 = siftgpu_quantise(d1).astype(np.int64), siftgpu_quantise(d2).astype(np.int64)
-    dot = q1 @ q2.T
+    q1, q2 = siftgpu_quantise(d1).astype(np.float64), siftgpu_quantise(d2).astype(np.float64)
+    dot = (q1 @ q2.T).astype(np.int64)  # every dot and partial sum is an integer below 128 * 255^2 < 2^53: exact
     rows, colsm = siftgpu_row_match(dot, distmax, ratiomax), siftgpu_col_match(dot, distmax, ratiomax)
     pairs = [(i, int(rows[i])) for i in range(len(d1)) if rows[i] >= 0 and colsm[rows[i]] == i]
     out = []

@@ -405,7 +405,7 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
     s.launches += 1;
   } else if (any_sift) {
     if ((rc = launch_sift_knn(w, d_pairs, npairs, max_nq, stride, n_items))) return rc;
-    e = launch_select_sift(d_pairs, npairs, (const float4*)w.d_knn.ptr, stride, (float)s.params.nn_distance_ratio, maxM,
+    e = launch_select_sift(d_pairs, npairs, (const float4*)w.d_knn.ptr, stride, s.params.nn_distance_ratio, maxM,
                            (rgbdslam_b200_dmatch*)w.d_matches.ptr, (float4*)w.d_mfrom.ptr, (float4*)w.d_mto.ptr,
                            (int32_t*)w.d_nall.ptr, st);
     if (e != cudaSuccess) return cuda_fail(e, "select_sift kernel");

@@ -42,7 +42,7 @@ cudaError_t launch_select_siftgpu(const PairDesc* pairs, int npairs, const int4*
                                   rgbdslam_b200_dmatch* matches, float4* mfrom, float4* mto, int32_t* n_all, cudaStream_t stream);
 cudaError_t launch_l2_refine(const PairDesc* pairs, int npairs, int max_nq, const int4* top4, int stride, float4* knn,
                              cudaStream_t stream);
-cudaError_t launch_select_sift(const PairDesc* pairs, int npairs, const float4* knn, int stride, float nn_ratio, int maxM,
+cudaError_t launch_select_sift(const PairDesc* pairs, int npairs, const float4* knn, int stride, double nn_ratio, int maxM,
                                rgbdslam_b200_dmatch* matches, float4* mfrom, float4* mto, int32_t* n_all, cudaStream_t stream);
 
 // hd<128 filter + jitter distance + sort + keep max_matches (node.cpp:572-573,674,1127).

@@ -20,12 +20,13 @@ __global__ void __launch_bounds__(256) k_sift_prepare(const SiftJob* __restrict_
     v = reinterpret_cast<const float4*>(job.in + (size_t)row * 128)[lane];
     if (root_sift) {
       v.x = fabsf(v.x); v.y = fabsf(v.y); v.z = fabsf(v.z); v.w = fabsf(v.w);  // descriptors = cv::abs(descriptors)
-      float s = (v.x + v.y) + (v.z + v.w);
+      // every rounding is spelled out (tests/sift_exact.py restates this arithmetic bit for bit)
+      float s = __fadd_rn(__fadd_rn(v.x, v.y), __fadd_rn(v.z, v.w));
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
       if (s != 0.f) {  // node.cpp:1565 (zero rows are left alone)
-        v.x = sqrtf(__fdiv_rn(v.x, s)); v.y = sqrtf(__fdiv_rn(v.y, s));
-        v.z = sqrtf(__fdiv_rn(v.z, s)); v.w = sqrtf(__fdiv_rn(v.w, s));
+        v.x = __fsqrt_rn(__fdiv_rn(v.x, s)); v.y = __fsqrt_rn(__fdiv_rn(v.y, s));
+        v.z = __fsqrt_rn(__fdiv_rn(v.z, s)); v.w = __fsqrt_rn(__fdiv_rn(v.w, s));
       }
     }
     reinterpret_cast<float4*>(job.root + (size_t)row * 128)[lane] = v;
@@ -50,9 +51,9 @@ __global__ void __launch_bounds__(256) k_sift_prepare(const SiftJob* __restrict_
   const __nv_bfloat16 b0 = __float2bfloat16_rn(v.x), b1 = __float2bfloat16_rn(v.y), b2 = __float2bfloat16_rn(v.z),
                       b3 = __float2bfloat16_rn(v.w);
   const float f0 = __bfloat162float(b0), f1 = __bfloat162float(b1), f2 = __bfloat162float(b2), f3 = __bfloat162float(b3);
-  float nrm = (f0 * f0 + f1 * f1) + (f2 * f2 + f3 * f3);
+  float nrm = __fadd_rn(__fmaf_rn(f0, f0, __fmul_rn(f1, f1)), __fmaf_rn(f2, f2, __fmul_rn(f3, f3)));
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) nrm += __shfl_xor_sync(0xffffffffu, nrm, o);
+  for (int o = 16; o > 0; o >>= 1) nrm = __fadd_rn(nrm, __shfl_xor_sync(0xffffffffu, nrm, o));
   if (lane == 0) job.norms[row] = nrm;
   // tile layout [row_group 16][k_chunk 16][row_in_group 8][16 B]; lane's 4 elements = 8 B of chunk lane/2
   const int kc = lane >> 1, half = lane & 1;
@@ -84,10 +85,12 @@ __global__ void __launch_bounds__(256) k_l2_refine(const PairDesc* __restrict__ 
     float s = 3.0e38f;
     if (cand[k] >= 0) {
       const float4 b = reinterpret_cast<const float4*>(pd.t_f32 + (size_t)cand[k] * 128)[lane];
-      const float dx = a.x - b.x, dy = a.y - b.y, dz = a.z - b.z, dw = a.w - b.w;
-      s = (dx * dx + dy * dy) + (dz * dz + dw * dw);
+      // fma(dx, dx, dy * dy) + fma(dz, dz, dw * dw) with every rounding spelled out, so no compiler can re-contract it
+      // (tests/sift_exact.py restates this arithmetic bit for bit)
+      const float dx = __fsub_rn(a.x, b.x), dy = __fsub_rn(a.y, b.y), dz = __fsub_rn(a.z, b.z), dw = __fsub_rn(a.w, b.w);
+      s = __fadd_rn(__fmaf_rn(dx, dx, __fmul_rn(dy, dy)), __fmaf_rn(dz, dz, __fmul_rn(dw, dw)));
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
     }
     d[k] = s;
   }
@@ -116,9 +119,10 @@ cudaError_t launch_l2_refine(const PairDesc* pairs, int npairs, int max_nq, cons
 
 // node.cpp:638-667 + 674 + 1127: ratio = d1/d2 (squared distances, as cv::flann returns them); accept if
 // nn_distance_ratio > ratio and the train index was not taken by an earlier query; distance = ratio; keep the
-// max_matches strongest, sorted.  One CTA per pair.
+// max_matches strongest, sorted.  One CTA per pair.  The threshold stays a double and the float ratio is widened, as
+// in the reference's `double max_dist_ratio_fac > float dist_ratio_fac`: fl32(19/20) = 0.949999988 passes 0.95.
 __global__ void __launch_bounds__(512) k_select_sift(const PairDesc* __restrict__ pairs, const float4* __restrict__ knn, int stride,
-                                                     float nn_ratio, int maxM, rgbdslam_b200_dmatch* __restrict__ matches,
+                                                     double nn_ratio, int maxM, rgbdslam_b200_dmatch* __restrict__ matches,
                                                      float4* __restrict__ mfrom, float4* __restrict__ mto, int32_t* __restrict__ n_all) {
   extern __shared__ unsigned long long sift_smem[];  // keys[kMaxFeatures] then owner[kMaxFeatures]
   unsigned long long* keys = sift_smem;
@@ -138,7 +142,7 @@ __global__ void __launch_bounds__(512) k_select_sift(const PairDesc* __restrict_
     const int t1 = __float_as_int(k.x), t2 = __float_as_int(k.y);
     if (t1 >= 0 && t2 >= 0) {
       const float ratio = __fdiv_rn(k.z, k.w);
-      if (nn_ratio > ratio) atomicMin(&owner[t1], i);  // first query (lowest index) keeps the train feature
+      if (nn_ratio > (double)ratio) atomicMin(&owner[t1], i);  // first query (lowest index) keeps the train feature
     }
   }
   __syncthreads();
@@ -149,7 +153,7 @@ __global__ void __launch_bounds__(512) k_select_sift(const PairDesc* __restrict_
       const int t1 = __float_as_int(k.x), t2 = __float_as_int(k.y);
       if (t1 >= 0 && t2 >= 0) {
         const float ratio = __fdiv_rn(k.z, k.w);
-        if (nn_ratio > ratio && owner[t1] == i) key = ((unsigned long long)__float_as_uint(ratio) << 32) | (unsigned)i;
+        if (nn_ratio > (double)ratio && owner[t1] == i) key = ((unsigned long long)__float_as_uint(ratio) << 32) | (unsigned)i;
       }
     }
     keys[i] = key;
@@ -190,7 +194,7 @@ __global__ void __launch_bounds__(512) k_select_sift(const PairDesc* __restrict_
   if (threadIdx.x == 0) n_all[p] = M;
 }
 
-cudaError_t launch_select_sift(const PairDesc* pairs, int npairs, const float4* knn, int stride, float nn_ratio, int maxM,
+cudaError_t launch_select_sift(const PairDesc* pairs, int npairs, const float4* knn, int stride, double nn_ratio, int maxM,
                                rgbdslam_b200_dmatch* matches, float4* mfrom, float4* mto, int32_t* n_all, cudaStream_t stream) {
   if (npairs <= 0) return cudaSuccess;
   const int smem = kMaxFeatures * 12;
