@@ -430,8 +430,8 @@ __device__ __forceinline__ void make_screen_ctx(const Rt& T, ScreenCtx& c) {
 //   m >= 0 : certainly an inlier, value = d^2 (float)          -1 : certainly rejected (shortcut of misc.cpp:726-735,
 //   d^2 > thr, NaN depth)                                      NaN: too close to call in float32 -> the caller
 //                                                                   evaluates the float64 reference formula
-// Margins: 1e-3 relative on both tests, orders of magnitude above the float32 evaluation error (~1e-5 relative for
-// the 3x3 SPD solve with condition number < 1e2).
+// Margins: 1e-3 relative on both tests.  The float32 evaluation error stays below 1e-4 relative for condition numbers of S
+// from ~1e2 to above 1e4 (latched far z0, per-point covariance at 4-30 m; tests/test_ransac_exact_cpu.py, DESIGN 4.4).
 template <bool kConstCov>
 __device__ __forceinline__ float mahal_screen(const float4 x1, const float4 x2, const Rt& T, const ScreenCtx& c) {
   const float d0 = fmaf(T.R[0], x1.x, fmaf(T.R[1], x1.y, fmaf(T.R[2], x1.z, T.t[0] * x1.w))) - x2.x;
