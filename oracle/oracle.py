@@ -196,7 +196,7 @@ def get_transform_from_matches_g2o(params: OParams, xyz_newer, kp_newer, xyz_old
     k1 = np.ascontiguousarray(kp_newer, np.float32).reshape(-1, 2); k2 = np.ascontiguousarray(kp_older, np.float32).reshape(-1, 2)
     m = np.ascontiguousarray(matches, DMATCH_DTYPE)
     s = np.ascontiguousarray(sel, np.int32)
-    T = np.ascontiguousarray(np.asarray(T4x4, np.float32).T)  # column-major storage
+    T = np.array(np.asarray(T4x4, np.float32).T, order="C")  # column-major storage; a copy: the call writes the result into it
     lib().oracle_get_transform_from_matches_g2o(C.byref(params), _p(x1), _p(k1), _p(x2), _p(k2), _p(m), _p(s), C.c_int(len(s)), _p(T),
                                                 C.c_int(int(iterations)))
     return T.T.copy()
@@ -207,7 +207,7 @@ def refine_g2o(params: OParams, iterations, xyz_newer, kp_newer, xyz_older, kp_o
     x1 = np.ascontiguousarray(xyz_newer, np.float32); x2 = np.ascontiguousarray(xyz_older, np.float32)
     k1 = np.ascontiguousarray(kp_newer, np.float32).reshape(-1, 2); k2 = np.ascontiguousarray(kp_older, np.float32).reshape(-1, 2)
     m = np.ascontiguousarray(matches, DMATCH_DTYPE)
-    T = np.ascontiguousarray(np.asarray(T4x4, np.float32).T)
+    T = np.array(np.asarray(T4x4, np.float32).T, order="C")  # a copy: the call writes the result into it
     inl = np.ascontiguousarray(inl_mask, np.uint8).copy()
     r = C.c_float(float(rmse)); n = C.c_int(int(inl.sum())); vi = C.c_int(int(valid_iterations))
     lib().oracle_refine_g2o(C.byref(params), C.c_int(int(iterations)), _p(x1), _p(k1), _p(x2), _p(k2), _p(m), C.c_int(len(m)), _p(T),

@@ -41,6 +41,13 @@ __device__ __forceinline__ int round_like_ref(float d) { return (int)floor((doub
 
 // One direction of the model: the `src` cloud transformed by T (row-major R, t: src frame -> dst frame) and projected into
 // the `dst` depth raster.  Each thread takes samples; returns this thread's (good, bad, occluded, all).
+// The float chain (back-projection, R p + t, projection) and the double sigma sums are written with explicit _rn intrinsics
+// in the reference's operation order: nvcc would otherwise contract them into FMAs, which the reference (built without
+// -mfma) does not do, and a projection near a floor(x + 0.5) boundary could then pick a different neighbourhood.
+__device__ __forceinline__ float dot3_rn(float a0, float b0, float a1, float b1, float a2, float b2) {  // (a0 b0 + a1 b1) + a2 b2
+  return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
+}
+
 __device__ void emm_direction(const EmmView& src, const EmmView& dst, const float R[9], const float t[3], int cloud_step,
                               int skip_step, double cov_z_const, double sigma_depth, unsigned& good, unsigned& bad, unsigned& occl,
                               unsigned& all) {
@@ -54,23 +61,17 @@ __device__ void emm_direction(const EmmView& src, const EmmView& dst, const floa
     const float Z = src.z[(size_t)ry * src.cw + rx];
     // the source point: NaN depth keeps x / y of the 1 m ray (misc.cpp:525-529) -> the transformed z is NaN as well
     const float u = (float)(rx * cloud_step), v = (float)(ry * cloud_step);
-    float px, py, pz;
-    if (isnan(Z)) {
-      px = (u - src.cx) * 1.0f * sfxinv;
-      py = (v - src.cy) * 1.0f * sfyinv;
-      pz = Z;
-    } else {
-      px = (u - src.cx) * Z * sfxinv;
-      py = (v - src.cy) * Z * sfyinv;
-      pz = Z;
-    }
-    const float qx = R[0] * px + R[1] * py + R[2] * pz + t[0];
-    const float qy = R[3] * px + R[4] * py + R[5] * pz + t[1];
-    const float qz = R[6] * px + R[7] * py + R[8] * pz + t[2];
+    const float zs = isnan(Z) ? 1.0f : Z;
+    const float px = __fmul_rn(__fmul_rn(__fsub_rn(u, src.cx), zs), sfxinv);
+    const float py = __fmul_rn(__fmul_rn(__fsub_rn(v, src.cy), zs), sfyinv);
+    const float pz = Z;
+    const float qx = __fadd_rn(dot3_rn(R[0], px, R[1], py, R[2], pz), t[0]);  // pcl::transformPointCloud
+    const float qy = __fadd_rn(dot3_rn(R[3], px, R[4], py, R[5], pz), t[1]);
+    const float qz = __fadd_rn(dot3_rn(R[6], px, R[7], py, R[8], pz), t[2]);
     if (qz != qz) continue;   // NaN
     if (qz < 0) continue;     // behind the camera
-    const int ocx = round_like_ref((qx / qz) * fx + cx);
-    const int ocy = round_like_ref((qy / qz) * fy + cy);
+    const int ocx = round_like_ref(__fadd_rn(__fmul_rn(__fdiv_rn(qx, qz), fx), cx));
+    const int ocy = round_like_ref(__fadd_rn(__fmul_rn(__fdiv_rn(qy, qz), fy), cy));
     if (ocx >= dst.cw || ocx < 0 || ocy >= dst.ch || ocy < 0) continue;
     const int nbhd = 2;
     bool good_point = false, occluded_point = false, bad_point = false;
@@ -80,9 +81,10 @@ __device__ void emm_direction(const EmmView& src, const EmmView& dst, const floa
       for (int ox = startx; ox < endx; ox += 2) {
         const float oz = dst.z[(size_t)oy * dst.cw + ox];
         if (oz != oz) continue;
-        const double old_sigma = cloud_step * (cov_z_const >= 0.0 ? cov_z_const : (sigma_depth * (double)oz * (double)oz) * (sigma_depth * (double)oz * (double)oz));
-        const double new_sigma = cloud_step * (cov_z_const >= 0.0 ? cov_z_const : (sigma_depth * (double)qz * (double)qz) * (sigma_depth * (double)qz * (double)qz));
-        const double joint_sigma = old_sigma + new_sigma;
+        const double sd_old = sigma_depth * (double)oz * (double)oz, sd_new = sigma_depth * (double)qz * (double)qz;
+        const double old_sigma = __dmul_rn((double)cloud_step, cov_z_const >= 0.0 ? cov_z_const : sd_old * sd_old);
+        const double new_sigma = __dmul_rn((double)cloud_step, cov_z_const >= 0.0 ? cov_z_const : sd_new * sd_new);
+        const double joint_sigma = __dadd_rn(old_sigma, new_sigma);
         // cdf(old_p.z, p.z, sqrt(joint_sigma)) with the reference's truncated SQRT_2 (misc.cpp:801, 809-812)
         const double p_new_in_front = 0.5 * (1 + erf(((double)oz - (double)qz) / (sqrt(joint_sigma) * 1.41421)));
         if (p_new_in_front < 0.001) occluded_point = true;
@@ -121,15 +123,23 @@ __device__ void emm_pair(const EmmView& newer, const EmmView& older, const float
     for (int c = 0; c < 3; c++) R[3 * r + c] = T16[4 * c + r];
     t[r] = T16[12 + r];
   }
-  // mr.final_trafo.inverse(): cofactor inverse of the affine matrix in float
-  const float c00 = R[4] * R[8] - R[5] * R[7], c01 = R[5] * R[6] - R[3] * R[8], c02 = R[3] * R[7] - R[4] * R[6];
-  const float det = R[0] * c00 + R[1] * c01 + R[2] * c02;
-  const float id = 1.0f / det;
-  Ri[0] = c00 * id; Ri[1] = (R[2] * R[7] - R[1] * R[8]) * id; Ri[2] = (R[1] * R[5] - R[2] * R[4]) * id;
-  Ri[3] = c01 * id; Ri[4] = (R[0] * R[8] - R[2] * R[6]) * id; Ri[5] = (R[2] * R[3] - R[0] * R[5]) * id;
-  Ri[6] = c02 * id; Ri[7] = (R[1] * R[6] - R[0] * R[7]) * id; Ri[8] = (R[0] * R[4] - R[1] * R[3]) * id;
+  // mr.final_trafo.inverse(): cofactor inverse of the affine matrix in float, uncontracted like the reference
+  const float c00 = __fsub_rn(__fmul_rn(R[4], R[8]), __fmul_rn(R[5], R[7]));
+  const float c01 = __fsub_rn(__fmul_rn(R[5], R[6]), __fmul_rn(R[3], R[8]));
+  const float c02 = __fsub_rn(__fmul_rn(R[3], R[7]), __fmul_rn(R[4], R[6]));
+  const float det = dot3_rn(R[0], c00, R[1], c01, R[2], c02);
+  const float id = __fdiv_rn(1.0f, det);
+  Ri[0] = __fmul_rn(c00, id);
+  Ri[1] = __fmul_rn(__fsub_rn(__fmul_rn(R[2], R[7]), __fmul_rn(R[1], R[8])), id);
+  Ri[2] = __fmul_rn(__fsub_rn(__fmul_rn(R[1], R[5]), __fmul_rn(R[2], R[4])), id);
+  Ri[3] = __fmul_rn(c01, id);
+  Ri[4] = __fmul_rn(__fsub_rn(__fmul_rn(R[0], R[8]), __fmul_rn(R[2], R[6])), id);
+  Ri[5] = __fmul_rn(__fsub_rn(__fmul_rn(R[2], R[3]), __fmul_rn(R[0], R[5])), id);
+  Ri[6] = __fmul_rn(c02, id);
+  Ri[7] = __fmul_rn(__fsub_rn(__fmul_rn(R[1], R[6]), __fmul_rn(R[0], R[7])), id);
+  Ri[8] = __fmul_rn(__fsub_rn(__fmul_rn(R[0], R[4]), __fmul_rn(R[1], R[3])), id);
 #pragma unroll
-  for (int r = 0; r < 3; r++) ti[r] = -(Ri[3 * r] * t[0] + Ri[3 * r + 1] * t[1] + Ri[3 * r + 2] * t[2]);
+  for (int r = 0; r < 3; r++) ti[r] = -dot3_rn(Ri[3 * r], t[0], Ri[3 * r + 1], t[1], Ri[3 * r + 2], t[2]);
   unsigned g = 0, b = 0, o = 0, al = 0;
   emm_direction(newer, older, R, t, a.cloud_step, a.skip_step, a.cov_z_const, a.sigma_depth, g, b, o, al);   // node.cpp:1527-1535
   emm_direction(older, newer, Ri, ti, a.cloud_step, a.skip_step, a.cov_z_const, a.sigma_depth, g, b, o, al);  // :1538-1548
