@@ -88,7 +88,8 @@ typedef struct rgbdslam_b200_params {
                                           * transformation_estimation.cpp:126-170); needs nodes with 2-D keypoints */
   /* Environment measurement model (node.cpp:1340-1342, misc.cpp:814-969, 1136-1148): > 0 enables it; an accepted RANSAC
    * transformation is kept only if inliers / (inliers + outliers) > threshold and inliers / (inl + outl + occluded) > 0.25.
-   * Needs nodes with a depth cloud (rgbdslam_b200_nodes_create keeps one when this is > 0, or rgbdslam_b200_node_set_depth). */
+   * Needs nodes with a depth cloud (rgbdslam_b200_nodes_create keeps one when this is > 0, or rgbdslam_b200_node_set_depth), or
+   * point-cloud nodes built with RGBDSLAM_B200_KEEP_CLOUD; a pair must not mix the two kinds. */
   double observability_threshold; /* -0.6 :114 (off) */
   int32_t emm_skip_step;          /* 8    :112       */
   int32_t cloud_creation_skip_step; /* 2  :36        */
@@ -184,7 +185,9 @@ int rgbdslam_b200_node_download(uint64_t node_handle, uint8_t* desc, float* xyz1
  * (misc.cpp:467-556) at every params.cloud_creation_skip_step-th pixel is kept on the device. */
 int rgbdslam_b200_node_set_depth(uint64_t node_handle, const float* depth_m, int w, int h, const float K4[4]);
 /* == pairwiseObservationLikelihood(newer, older, mr) (node.cpp:1520-1554) for an explicit transformation T (Eigen::Matrix4f,
- * column-major, newer -> older frame): counts[4] = inlier, outlier, occluded, all points. */
+ * column-major, newer -> older frame): counts[4] = inlier, outlier, occluded, all points.  Both nodes have a depth cloud, or
+ * both keep their organised cloud (RGBDSLAM_B200_KEEP_CLOUD); a mixed pair returns ERR_STATE.  node_set_depth on a node
+ * that keeps its cloud returns ERR_STATE. */
 int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const float T[16], uint32_t counts[4]);
 /* Attach the 2-D keypoints (feature_locations_2d_, n entries) to a node created from features: only the pairwise g2o
  * refinement reads them (edgeToFeature, transformation_estimation.cpp:91-124).  Nodes built from images carry theirs. */
@@ -331,7 +334,20 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * descriptor i with another keypoint's point once compute() drops or re-orders keypoints, and its asserts at node.cpp:317-318
  * fail).  maximum_depth (parameter_server.cpp:38) is fixed at its default, +inf: no point is too far and a +inf z is kept.
  * K4 may be NULL; use_feature_min_depth and depth_scaling_factor are not read.  params.observability_threshold > 0 (the
- * environment measurement model, which needs a cloud per node) returns ERR_STATE for cloud input.
+ * environment measurement model, which needs a cloud per node) returns ERR_STATE for cloud input without KEEP_CLOUD.
+ *
+ * RGBDSLAM_B200_KEEP_CLOUD (with a cloud bit only): the node keeps its organised cloud, the reference's pc_col (node.cpp:261,
+ * kept when store_pointclouds or emm__skip_step is set, :344-350): x, y and z planes at full resolution on the device, 12 bytes
+ * per point (3.7 MB at 640 x 480), de-interleaved from the uploaded cloud.  The environment measurement model then runs on
+ * these clouds as observationLikelihood (misc.cpp:814-969) does when clouds are the input (topic_points set): every
+ * emm_skip_step-th point of the full-resolution cloud, x / y / z as stored, cloud_creation_skip_step not applied (no division
+ * of the intrinsics, no sigma scaling); a point with a non-finite coordinate is left untransformed, as
+ * pcl::transformPointCloud does on a cloud that is not dense (a +inf z stays +inf and is judged); round() as x86-64 evaluates
+ * it (NaN -> INT_MIN, outside the raster); a direction whose two clouds differ in width contributes nothing (:844-847).  K4
+ * is here the camera the model projects into, the reference's depth_camera_fx / fy / cx / cy (misc.cpp:56-63); NULL means
+ * (0, 0, 0, 0), what the reference uses when those parameters are unset (the cloud constructor never sets cam_info): every
+ * finite point then projects to pixel (0, 0).  The node's features, and the detector thresholds, are those of the same call
+ * without the flag.  Rejected with ERR_ARG by rgbdslam_b200_nodes_create_sharded (clouds are not exchanged).
  *
  * RGBDSLAM_B200_MASK_FROM_CLOUD: the detection mask is calculateDepthMask of the cloud (openni_listener.cpp:520-534, the
  * stereo and PCD callers), computed on the device and `mask` ignored: static_cast<uchar>(z * 50.0) as x86-64 compilers emit
@@ -339,12 +355,13 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * every multiple of 5.12 m and for +-inf.
  *
  * Rejected with ERR_ARG before any device work: unknown bits, CLOUD_XYZRGB with CLOUD_XYZ, MASK_FROM_CLOUD without a cloud
- * bit, MASK_FROM_DEPTH with a cloud bit. */
+ * bit, MASK_FROM_DEPTH with a cloud bit, KEEP_CLOUD without a cloud bit. */
 #define RGBDSLAM_B200_MASK_FROM_DEPTH 1
 #define RGBDSLAM_B200_VISUAL_RGB 2
 #define RGBDSLAM_B200_CLOUD_XYZRGB 4
 #define RGBDSLAM_B200_CLOUD_XYZ 8
 #define RGBDSLAM_B200_MASK_FROM_CLOUD 16
+#define RGBDSLAM_B200_KEEP_CLOUD 128
 int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                   int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
                                   int32_t* n_features);

@@ -159,6 +159,8 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   // the same size as visual, detection_mask empty or of the same size.  detect, projectTo3D (the first max_keypoints keypoints
   // whose cloud point at the truncated position has no NaN coordinate, the point as stored) and compute run as one
   // rgbdslam_b200_nodes_create_ex call; each 3-D point stays with its keypoint through compute() (see rgbdslam_b200.h).
+  // With the environment measurement model on (observability_threshold > 0) the node keeps its cloud (pc_col, node.cpp:261;
+  // RGBDSLAM_B200_KEEP_CLOUD), which the model projects into depth_camera_intrinsics(); matchNodePair then reports its counts.
   template <class PointT>
   Node(const Mat& visual, Ptr<Feature2D> detector, Ptr<DescriptorExtractor> extractor, std::shared_ptr<PointCloud<PointT>> point_cloud,
        const Mat& detection_mask = Mat()) {
@@ -177,10 +179,13 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     std::vector<uint8_t> tg, tm;
     const uint8_t* g = detail::packed<uint8_t>(visual, tg);
     const uint8_t* m = detection_mask.empty() ? nullptr : detail::packed<uint8_t>(detection_mask, tm);
+    rgbdslam_b200_params prm;
+    const bool emm = rgbdslam_b200_get_params(&prm) == 0 && prm.observability_threshold > 0.0;
     const int flags = (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) |
-                      (std::is_same<PointT, PointXYZRGB>::value ? RGBDSLAM_B200_CLOUD_XYZRGB : RGBDSLAM_B200_CLOUD_XYZ);
-    construct(g, reinterpret_cast<const float*>(point_cloud->points.data()), m, visual.cols, visual.rows, nullptr,
-              detector->handle(), flags);
+                      (std::is_same<PointT, PointXYZRGB>::value ? RGBDSLAM_B200_CLOUD_XYZRGB : RGBDSLAM_B200_CLOUD_XYZ) |
+                      (emm ? RGBDSLAM_B200_KEEP_CLOUD : 0);
+    construct(g, reinterpret_cast<const float*>(point_cloud->points.data()), m, visual.cols, visual.rows,
+              emm ? depth_camera_intrinsics() : nullptr, detector->handle(), flags);
   }
   // Node(visual, depth, detection_mask, cam_info, depth_header, detector, extractor) (node.cpp:101-240): detect, filter,
   // describe, back-project on the device; the public feature members are filled from the result.  `detector` is the handle of
@@ -271,6 +276,13 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
 
   static int& max_connections() {  // parameter max_connections (parameter_server.cpp:104), -1 = unlimited
     static int v = -1;
+    return v;
+  }
+  // parameters depth_camera_fx, depth_camera_fy, depth_camera_cx, depth_camera_cy (parameter_server.cpp:42-45), default 0:
+  // the camera the environment measurement model projects kept point clouds into (misc.cpp:56-63).  Read when a point-cloud
+  // Node is constructed.  All zero, as in the reference with the parameters unset, projects every finite point to pixel (0, 0).
+  static float* depth_camera_intrinsics() {
+    static float v[4] = {0.f, 0.f, 0.f, 0.f};
     return v;
   }
 

@@ -51,13 +51,15 @@ class Params(C.Structure):
 
 DETECTOR_ORB, DETECTOR_FAST = 0, 1  # Params.feature_detector_type (RGBDSLAM_B200_DETECTOR_*)
 # flags of rgbdslam_b200_nodes_create_ex / _sharded (RGBDSLAM_B200_*)
-MASK_FROM_DEPTH, VISUAL_RGB, CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD = 1, 2, 4, 8, 16
+MASK_FROM_DEPTH, VISUAL_RGB, CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD, KEEP_CLOUD = 1, 2, 4, 8, 16, 128
 
 
-def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False) -> int:
+def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False, keep_cloud=False) -> int:
     """The nodes_create flags the array shapes select: gray (F,H,W) or (F,H,W,3) colour; depth (F,H,W) depth image, or an
-    organised cloud (F,H,W,8) of PointXYZRGB / (F,H,W,4) of PointXYZ as float32."""
+    organised cloud (F,H,W,8) of PointXYZRGB / (F,H,W,4) of PointXYZ as float32.  keep_cloud: the nodes keep their cloud
+    for the environment measurement model (cloud input only)."""
     flags = (MASK_FROM_DEPTH if mask_from_depth else 0) | (MASK_FROM_CLOUD if mask_from_cloud else 0)
+    flags |= KEEP_CLOUD if keep_cloud else 0
     if len(gray_shape) == 4:
         if gray_shape[3] != 3:
             raise ValueError(f"gray must be (F,H,W) or (F,H,W,3), got {tuple(gray_shape)}")
@@ -438,16 +440,19 @@ class Frontend:
                                                        _ptr(desc), C.byref(n)))
         return out[:n.value], desc[:n.value]
 
-    def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, mask_from_cloud: bool = False):
+    def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, mask_from_cloud: bool = False,
+                     keep_cloud: bool = False):
         """gray [F,H,W] u8 or [F,H,W,3] colour (channel 0 = R), depth [F,H,W] f32, or an organised cloud [F,H,W,8] (PointXYZRGB)
         / [F,H,W,4] (PointXYZ) f32 for the point-cloud constructor, mask [F,H,W] u8 or None -> (handles, n_features).  numpy
         arrays or pinned torch tensors (copied from asynchronously).  mask_from_depth / mask_from_cloud: derive the detection
-        mask on the device (depthToCV8UC1 / calculateDepthMask).  K4 may be None for cloud input."""
+        mask on the device (depthToCV8UC1 / calculateDepthMask).  K4 may be None for cloud input.  keep_cloud (cloud input):
+        the nodes keep their cloud for the environment measurement model, which projects into K4 (the reference's
+        depth_camera_fx / fy / cx / cy; None = all zero)."""
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
             depth = np.ascontiguousarray(depth, np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, keep_cloud)
         F, H, W = gray.shape[:3]
         K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)

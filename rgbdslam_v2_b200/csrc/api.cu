@@ -179,6 +179,11 @@ static PairDesc make_pair(const NodeDev& a, const NodeDev& b) {
   pd.t_kp = b.kp;
   pd.q_cloud = a.cloud_z;
   pd.t_cloud = b.cloud_z;
+  pd.q_cloud_x = a.cloud_x;
+  pd.q_cloud_y = a.cloud_y;
+  pd.t_cloud_x = b.cloud_x;
+  pd.t_cloud_y = b.cloud_y;
+  pd.emm_cloud = a.cloud_x ? 1 : 0;
   pd.q_cw = a.cw;
   pd.q_ch = a.ch;
   pd.t_cw = b.cw;
@@ -345,6 +350,10 @@ static int check_pairs(const std::vector<PairDesc>& h_pairs, int64_t first_pair,
       if (!pd.q_cloud || !pd.t_cloud) {
         set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth)");
         return RGBDSLAM_B200_ERR_STATE;
+      } else if (!pd.q_cloud_x != !pd.t_cloud_x) {
+        // the reference never holds both kinds in one process (topic_points is global): there is no rule to restate
+        set_error("observability_threshold > 0: a pair mixes a node that keeps its point cloud (KEEP_CLOUD) with a depth-image node");
+        return RGBDSLAM_B200_ERR_STATE;
       }
   return 0;
 }
@@ -467,10 +476,14 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
     s.launches += 1;
   }
   if (s.params.observability_threshold > 0.0) {  // node.cpp:1340-1342
-    e = launch_emm_pairs(d_pairs, npairs, s.params.cloud_creation_skip_step, s.params.emm_skip_step, s.dp.cov_z_const,
-                         s.params.sigma_depth, s.params.observability_threshold, (rgbdslam_b200_pair_result*)w.d_results.ptr, st);
+    bool depth_pairs = false, cloud_pairs = false;
+    for (const PairDesc& pd : h_pairs) (pd.emm_cloud ? cloud_pairs : depth_pairs) = true;
+    int emm_launches = 0;
+    e = launch_emm_pairs(d_pairs, npairs, depth_pairs, cloud_pairs, s.params.cloud_creation_skip_step, s.params.emm_skip_step,
+                         s.dp.cov_z_const, s.params.sigma_depth, s.params.observability_threshold,
+                         (rgbdslam_b200_pair_result*)w.d_results.ptr, st, &emm_launches);
     if (e != cudaSuccess) return cuda_fail(e, "emm kernel");
-    s.launches += 1;
+    s.launches += emm_launches;
   }
   cudaEventRecord(w.ev[kEvStagesEnd], st);
 
@@ -513,10 +526,16 @@ void free_node(NodeDev* nd) {
     if (nd->desc_i8) cudaFree(nd->desc_i8);
     if (nd->kp) cudaFree(nd->kp);
   }
-  if (nd->cloud_z) cudaFree(nd->cloud_z);
+  free_node_cloud(nd);
   if (nd->desc_f32) cudaFree(nd->desc_f32);
   if (nd->norms) cudaFree(nd->norms);
   delete nd;
+}
+
+void free_node_cloud(NodeDev* nd) {
+  if (nd->cloud_x) cudaFree(nd->cloud_x);  // x | y | z planes of a kept cloud
+  else if (nd->cloud_z) cudaFree(nd->cloud_z);
+  nd->cloud_x = nd->cloud_y = nd->cloud_z = nullptr;
 }
 
 int node_build_cloud(NodeDev* nd, const float* d_depth, int w, int h, const float K4[4], cudaStream_t st) {
@@ -704,6 +723,10 @@ int rgbdslam_b200_node_set_depth(uint64_t node_handle, const float* depth_m, int
     set_error("node_set_depth: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
+  if (nd->cloud_x) {
+    set_error("node_set_depth: the node keeps the organised cloud it was built from (KEEP_CLOUD)");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
   State& s = g_state;
   int rc;
   if ((rc = s.d_f32_a.ensure(sizeof(float) * (size_t)w * h))) return rc;
@@ -726,6 +749,10 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
     set_error("observation_likelihood: both nodes need a depth cloud (nodes_create with observability_threshold > 0 or node_set_depth)");
     return RGBDSLAM_B200_ERR_STATE;
   }
+  if (!a->cloud_x != !b->cloud_x) {
+    set_error("observation_likelihood: a node that keeps its point cloud (KEEP_CLOUD) and a depth-image node cannot be compared");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
   State& s = g_state;
   if (s.params.depth_cov_z0 == 0.0 && s.z0 == 0.0) {
     // the reference latches depth_covariance's static on its first call (misc2.h:30-35); here that happens in the first
@@ -737,9 +764,10 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
   if ((rc = s.d_f32_b.ensure(128))) return rc;
   cudaError_t e = cudaMemcpyAsync(s.d_f32_b.ptr, T, 64, cudaMemcpyHostToDevice, s.stream);
   if (e == cudaSuccess)
-    e = launch_emm_single(a->cloud_z, a->cw, a->ch, a->K, b->cloud_z, b->cw, b->ch, b->K, (const float*)s.d_f32_b.ptr,
-                          s.params.cloud_creation_skip_step, s.params.emm_skip_step, s.dp.cov_z_const, s.params.sigma_depth,
-                          (unsigned*)((char*)s.d_f32_b.ptr + 64), s.stream);
+    e = launch_emm_single(EmmNode{a->cloud_z, a->cloud_x, a->cloud_y, a->cw, a->ch, a->K},
+                          EmmNode{b->cloud_z, b->cloud_x, b->cloud_y, b->cw, b->ch, b->K}, a->cloud_x != nullptr,
+                          (const float*)s.d_f32_b.ptr, s.params.cloud_creation_skip_step, s.params.emm_skip_step, s.dp.cov_z_const,
+                          s.params.sigma_depth, (unsigned*)((char*)s.d_f32_b.ptr + 64), s.stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(counts, (char*)s.d_f32_b.ptr + 64, 16, cudaMemcpyDeviceToHost, s.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
   if (e != cudaSuccess) return cuda_fail(e, "observation_likelihood");

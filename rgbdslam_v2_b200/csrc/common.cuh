@@ -28,10 +28,14 @@ struct PairDesc {
   const rgbdslam_b200_keypoint* t_kp;
   const float* q_cloud;  // depth-cloud z-planes (environment measurement model), nullptr if the node has none
   const float* t_cloud;
+  const float* q_cloud_x;  // kept organised clouds (RGBDSLAM_B200_KEEP_CLOUD): x / y planes, nullptr for depth-image nodes
+  const float* q_cloud_y;
+  const float* t_cloud_x;
+  const float* t_cloud_y;
   int32_t q_cw, q_ch, t_cw, t_ch;
-  float q_K[4], t_K[4];  // fx, fy, cx, cy of the full-resolution cameras
+  float q_K[4], t_K[4];  // fx, fy, cx, cy of the full-resolution cameras (kept clouds: the camera the model projects into)
   int32_t sift_kind;   // float-descriptor nodes: 0 = RootSIFT / exact 2-NN ratio matcher, 1 = SiftGPU matcher (u8 tiles, raw rows)
-  int32_t pad_;
+  int32_t emm_cloud;   // 1: the newer node keeps its organised cloud (match_pairs* only runs the model on pairs of one kind)
 };
 
 // One work item of the tensor-core match kernels = 256 queries of one pair against all train rows.

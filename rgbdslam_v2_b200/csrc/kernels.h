@@ -28,12 +28,19 @@ cudaError_t launch_l2_tc256(const HamItem* d_items, int n_items, int sm_count, c
 cudaError_t launch_sift_prepare(const SiftJob* d_jobs, int njobs, int max_n_pad, int root_sift, int siftgpu, cudaStream_t stream);
 cudaError_t launch_build_cloud(const float* d_depth, int w, int h, int step, float scaling, float min_depth, float* cloud_z, int cw,
                                int ch, cudaStream_t stream);
-cudaError_t launch_emm_pairs(const PairDesc* pairs, int npairs, int cloud_step, int skip_step, double cov_z_const,
-                             double sigma_depth, double observability_threshold, rgbdslam_b200_pair_result* results,
-                             cudaStream_t stream);
-cudaError_t launch_emm_single(const float* q_cloud, int q_cw, int q_ch, const float* qK, const float* t_cloud, int t_cw, int t_ch,
-                              const float* tK, const float* d_T16, int cloud_step, int skip_step, double cov_z_const,
-                              double sigma_depth, unsigned* d_counts, cudaStream_t stream);
+cudaError_t launch_split_cloud(const float* d_cloud, int stride, int n, float* x, float* y, float* z, cudaStream_t stream);
+// Environment measurement model.  launch_emm_pairs launches the depth-node instantiation when depth_pairs, the kept-cloud one
+// when cloud_pairs (each skips the other kind's pairs) and adds the launches to *n_launches.
+cudaError_t launch_emm_pairs(const PairDesc* pairs, int npairs, bool depth_pairs, bool cloud_pairs, int cloud_step, int skip_step,
+                             double cov_z_const, double sigma_depth, double observability_threshold,
+                             rgbdslam_b200_pair_result* results, cudaStream_t stream, int* n_launches);
+struct EmmNode {  // one node's cloud as the model reads it (x / y only for kept clouds)
+  const float *z, *x, *y;
+  int cw, ch;
+  const float* K;
+};
+cudaError_t launch_emm_single(const EmmNode& q, const EmmNode& t, bool cloud, const float* d_T16, int cloud_step, int skip_step,
+                              double cov_z_const, double sigma_depth, unsigned* d_counts, cudaStream_t stream);
 cudaError_t launch_refine_g2o(const PairDesc* pairs, int npairs, int max_matches, int iterations, const float4* mfrom,
                               const float4* mto, const int32_t* n_all, const rgbdslam_b200_dmatch* matches,
                               rgbdslam_b200_pair_result* results, rgbdslam_b200_dmatch* inlier_matches, cudaStream_t stream);

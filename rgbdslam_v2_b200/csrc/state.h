@@ -45,8 +45,12 @@ struct NodeDev {
   int8_t* desc_i8 = nullptr;  // float-descriptor nodes only: n_pad x 256 B operand tiles (bf16 RootSIFT rows / u8 SiftGPU rows)
   int32_t n_pad = 0;
   float* cloud_z = nullptr;   // depth cloud z-plane (cw x ch) for the environment measurement model
+  // Kept organised cloud of the point-cloud constructor (RGBDSLAM_B200_KEEP_CLOUD): x / y / z planes at full resolution
+  // (cw x ch = w x h) in one allocation that starts at cloud_x (cloud_z = its third plane); nullptr for depth-image nodes.
+  float* cloud_x = nullptr;
+  float* cloud_y = nullptr;
   int32_t cw = 0, ch = 0;
-  float K[4] = {0, 0, 0, 0};  // fx, fy, cx, cy of the full-resolution camera
+  float K[4] = {0, 0, 0, 0};  // fx, fy, cx, cy of the full-resolution camera (kept clouds: the camera the model projects into)
   int32_t sift_kind = 0;      // SIFT nodes: 0 = RootSIFT rows + bf16 tiles, 1 = raw rows + u8 tiles (SiftGPU matcher)
   NodeSlab* slab = nullptr;   // desc / xyz / kp live inside this shared allocation (cloud_z is always separate)
 };
@@ -134,5 +138,6 @@ Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot
   if (int entry_rc__ = rb200::check_inited()) return entry_rc__
 int node_build_cloud(NodeDev* nd, const float* d_depth, int w, int h, const float K4[4], cudaStream_t st);
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
+void free_node_cloud(NodeDev* nd);  // frees the node's depth cloud or kept cloud (api.cu)
 
 }  // namespace rb200
