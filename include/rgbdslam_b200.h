@@ -354,14 +354,33 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * it (truncation to int32, 0x80000000 when out of range, low byte), 0 for NaN -- so the mask is 0 below ~0.02 m, in a band at
  * every multiple of 5.12 m and for +-inf.
  *
+ * RGBDSLAM_B200_DEPTH_U16 (depth-image input only): `depth` points to nframes*w*h uint16_t millimetres, 0 = no depth (16UC1,
+ * the default topic_image_depth .../sw_registered/image_rect_raw), converted on the device as the listener does before it
+ * builds the Node (noCloudCallback, openni_listener.cpp:633-659): depth = convertTo(CV_32FC1, 0.001), (float)d * 0.001f -- a
+ * hole becomes 0 m, not NaN, so removeDepthless keeps a keypoint there, and with use_feature_min_depth a neighbourhood that
+ * touches a hole has minimum 0, which drops the keypoint.  depth_scaling_factor, use_feature_min_depth and projectTo3D then act
+ * on these metres, and so does the environment measurement model.  With MASK_FROM_DEPTH the mask is depthToCV8UC1 of the
+ * 16-bit image (misc.cpp:414-425): convertTo(CV_8UC1, 0.05, -25) = saturate_cast<uchar>(fmaf(d, 0.05f, -25.f)), non-zero iff
+ * d >= 510 -- nothing closer than 0.51 m is detected, unlike the float rule above, which accepts depths from ~5 mm.  Without it
+ * the caller's mask, or none, as for float depth.  The upload moves 2 bytes per depth pixel.
+ *
+ * RGBDSLAM_B200_VISUAL_BAYER_GR (depth-image input only): `gray` holds nframes*w*h raw bayer_grbg8 bytes (G B on even rows,
+ * R G on odd rows), converted as the listener and the Node do: cvtColor(COLOR_BayerGR2RGB) (openni_listener.cpp:638-641, cv2
+ * 4.13's bilinear rule, borders repeating the nearest interior row / column), rounded to u8, then CV_RGB2GRAY as for
+ * VISUAL_RGB.  Every frame of the call is converted (the listener hands its first Bayer frame over raw: pass that one without
+ * the flag to do the same).
+ *
  * Rejected with ERR_ARG before any device work: unknown bits, CLOUD_XYZRGB with CLOUD_XYZ, MASK_FROM_CLOUD without a cloud
- * bit, MASK_FROM_DEPTH with a cloud bit, KEEP_CLOUD without a cloud bit. */
+ * bit, MASK_FROM_DEPTH with a cloud bit, KEEP_CLOUD without a cloud bit, DEPTH_U16 or VISUAL_BAYER_GR with a cloud bit,
+ * VISUAL_BAYER_GR with VISUAL_RGB. */
 #define RGBDSLAM_B200_MASK_FROM_DEPTH 1
 #define RGBDSLAM_B200_VISUAL_RGB 2
 #define RGBDSLAM_B200_CLOUD_XYZRGB 4
 #define RGBDSLAM_B200_CLOUD_XYZ 8
 #define RGBDSLAM_B200_MASK_FROM_CLOUD 16
 #define RGBDSLAM_B200_KEEP_CLOUD 128
+#define RGBDSLAM_B200_DEPTH_U16 256
+#define RGBDSLAM_B200_VISUAL_BAYER_GR 512
 int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                   int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
                                   int32_t* n_features);

@@ -27,10 +27,10 @@ namespace rgbdslam_b200 {
 
 typedef rgbdslam_b200_keypoint KeyPoint;  // == cv::KeyPoint (7 x 4 B)
 
-enum { RB_8UC1 = 0, RB_32FC1 = 5, RB_8UC3 = 16 };  // == CV_8UC1, CV_32FC1, CV_8UC3
+enum { RB_8UC1 = 0, RB_16UC1 = 2, RB_32FC1 = 5, RB_8UC3 = 16 };  // == CV_8UC1, CV_16UC1, CV_32FC1, CV_8UC3
 
 inline int channels_of(int t) { return t == RB_8UC3 ? 3 : 1; }
-inline size_t pixel_bytes(int t) { return t == RB_32FC1 ? 4 : (size_t)channels_of(t); }
+inline size_t pixel_bytes(int t) { return t == RB_32FC1 ? 4 : t == RB_16UC1 ? 2 : (size_t)channels_of(t); }
 
 struct Mat {  // non-owning view with cv::Mat's field names
   unsigned char* data = nullptr;

@@ -52,14 +52,22 @@ class Params(C.Structure):
 DETECTOR_ORB, DETECTOR_FAST = 0, 1  # Params.feature_detector_type (RGBDSLAM_B200_DETECTOR_*)
 # flags of rgbdslam_b200_nodes_create_ex / _sharded (RGBDSLAM_B200_*)
 MASK_FROM_DEPTH, VISUAL_RGB, CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD, KEEP_CLOUD = 1, 2, 4, 8, 16, 128
+DEPTH_U16, VISUAL_BAYER_GR = 256, 512
 
 
-def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False, keep_cloud=False) -> int:
+def _is_u16(a) -> bool:
+    """a uint16 numpy array or torch tensor"""
+    return str(a.dtype) in ("uint16", "torch.uint16")
+
+
+def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False, keep_cloud=False,
+                     depth_u16=False, bayer=False) -> int:
     """The nodes_create flags the array shapes select: gray (F,H,W) or (F,H,W,3) colour; depth (F,H,W) depth image, or an
     organised cloud (F,H,W,8) of PointXYZRGB / (F,H,W,4) of PointXYZ as float32.  keep_cloud: the nodes keep their cloud
-    for the environment measurement model (cloud input only)."""
+    for the environment measurement model (cloud input only).  depth_u16: the depth image is uint16 millimetres; bayer: gray
+    (F,H,W) holds bayer_grbg8 mosaics."""
     flags = (MASK_FROM_DEPTH if mask_from_depth else 0) | (MASK_FROM_CLOUD if mask_from_cloud else 0)
-    flags |= KEEP_CLOUD if keep_cloud else 0
+    flags |= (KEEP_CLOUD if keep_cloud else 0) | (DEPTH_U16 if depth_u16 else 0) | (VISUAL_BAYER_GR if bayer else 0)
     if len(gray_shape) == 4:
         if gray_shape[3] != 3:
             raise ValueError(f"gray must be (F,H,W) or (F,H,W,3), got {tuple(gray_shape)}")
@@ -441,18 +449,20 @@ class Frontend:
         return out[:n.value], desc[:n.value]
 
     def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, mask_from_cloud: bool = False,
-                     keep_cloud: bool = False):
-        """gray [F,H,W] u8 or [F,H,W,3] colour (channel 0 = R), depth [F,H,W] f32, or an organised cloud [F,H,W,8] (PointXYZRGB)
-        / [F,H,W,4] (PointXYZ) f32 for the point-cloud constructor, mask [F,H,W] u8 or None -> (handles, n_features).  numpy
-        arrays or pinned torch tensors (copied from asynchronously).  mask_from_depth / mask_from_cloud: derive the detection
-        mask on the device (depthToCV8UC1 / calculateDepthMask).  K4 may be None for cloud input.  keep_cloud (cloud input):
-        the nodes keep their cloud for the environment measurement model, which projects into K4 (the reference's
-        depth_camera_fx / fy / cx / cy; None = all zero)."""
+                     keep_cloud: bool = False, bayer: bool = False):
+        """gray [F,H,W] u8 or [F,H,W,3] colour (channel 0 = R), depth [F,H,W] f32 metres or u16 millimetres, or an organised
+        cloud [F,H,W,8] (PointXYZRGB) / [F,H,W,4] (PointXYZ) f32 for the point-cloud constructor, mask [F,H,W] u8 or None ->
+        (handles, n_features).  numpy arrays or pinned torch tensors (copied from asynchronously).  mask_from_depth /
+        mask_from_cloud: derive the detection mask on the device (depthToCV8UC1 of the float or 16-bit depth /
+        calculateDepthMask).  K4 may be None for cloud input.  keep_cloud (cloud input): the nodes keep their cloud for the
+        environment measurement model, which projects into K4 (the reference's depth_camera_fx / fy / cx / cy; None = all
+        zero).  bayer: gray [F,H,W] holds bayer_grbg8 mosaics, debayered on the device."""
+        depth_u16 = _is_u16(depth)
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
-            depth = np.ascontiguousarray(depth, np.float32)
+            depth = np.ascontiguousarray(depth, np.uint16 if depth_u16 else np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, keep_cloud)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, keep_cloud, depth_u16, bayer)
         F, H, W = gray.shape[:3]
         K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
@@ -465,15 +475,16 @@ class Frontend:
         return [int(h) for h in handles], nf
 
     def nodes_create_sharded(self, det: int, comm: int, total_frames: int, gray, depth, mask, K4, ids=None,
-                             mask_from_depth: bool = False, mask_from_cloud: bool = False):
+                             mask_from_depth: bool = False, mask_from_cloud: bool = False, bayer: bool = False):
         """Frame-sharded nodes_create: gray / depth / mask hold THIS rank's frames (sharding.frame_shard); returns handles and
-        feature counts of ALL total_frames nodes (every rank ends up holding every node).  Shapes select the input as in
-        nodes_create."""
+        feature counts of ALL total_frames nodes (every rank ends up holding every node).  Shapes and the depth dtype select
+        the input as in nodes_create."""
+        depth_u16 = _is_u16(depth)
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
-            depth = np.ascontiguousarray(depth, np.float32)
+            depth = np.ascontiguousarray(depth, np.uint16 if depth_u16 else np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, depth_u16=depth_u16, bayer=bayer)
         H, W = gray.shape[1:3]
         K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)

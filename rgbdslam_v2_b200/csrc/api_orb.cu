@@ -6,7 +6,9 @@
 //   rgbdslam_b200_nodes_create == Node::Node(visual, depth, mask, cam_info, ...)      (node.cpp:101-240), batched; with the
 //                                 CLOUD_* flags of _ex / _sharded Node::Node(visual, detector, extractor, point_cloud, mask)
 //                                 (node.cpp:252-369), with VISUAL_RGB the cvtColor of a colour visual (:139-144, 275-277),
-//                                 with KEEP_CLOUD the node keeps its organised cloud (pc_col, :261) for the measurement model
+//                                 with KEEP_CLOUD the node keeps its organised cloud (pc_col, :261) for the measurement model,
+//                                 with DEPTH_U16 / VISUAL_BAYER_GR the listener's conversions of its raw 16UC1 depth and
+//                                 bayer_grbg8 images (openni_listener.cpp:633-659)
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -45,7 +47,8 @@ struct OrbCtx {
   OrbTables tab;
   int max_per_cell = 0, min_cell = 0, max_cell = 0, kp_stride = 0;
   DevBuf in_gray[2], in_mask[2], in_depth[2];  // double-buffered chunk inputs (upload of chunk k+1 under the kernels of chunk k)
-  DevBuf in_rgb[2];                            // colour input, converted into in_gray on the device
+  DevBuf in_rgb[2];                            // colour or Bayer input, converted into in_gray on the device
+  DevBuf in_raw[2];                            // 16-bit millimetre depth, converted into in_depth (and in_mask) on the device
   PinBuf stage[2];                             // pinned staging for callers that pass pageable memory
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -53,14 +56,14 @@ struct OrbCtx {
       pyr_raw, pyr_blur, desc, err, trig;
   // rgbdslam_b200_nodes_create_sharded: what must survive between the detection pass and the finishing pass of ALL own frames,
   // and the per-(frame, cell) tables every rank holds for ALL frames of the sequence
-  DevBuf sh_gray, sh_rgb, sh_depth, sh_mask, sh_cell_img, sh_cand, all_hist, all_cnt, all_many, all_thr;
+  DevBuf sh_gray, sh_rgb, sh_raw, sh_depth, sh_mask, sh_cell_img, sh_cand, all_hist, all_cnt, all_many, all_thr;
   const uint8_t* last_gray = nullptr;  // device pointers of frame 0 of the last call (debug hooks)
   OrbCandidates candidates() const { return {(const OrbCand*)cand.ptr, (const int*)cand_count.ptr, (const int*)thr.ptr, (float*)resp.ptr}; }
   void release() {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &in_rgb[0],
-                     &in_rgb[1], &cell_img, &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp, &cell_out,
-                     &cell_out_count, &cand_z, &scratch, &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray, &sh_rgb,
-                     &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr};
+                     &in_rgb[1], &in_raw[0], &in_raw[1], &cell_img, &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp,
+                     &cell_out, &cell_out_count, &cand_z, &scratch, &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray,
+                     &sh_rgb, &sh_raw, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr};
     for (DevBuf* b : all) b->release();
     stage[0].release();
     stage[1].release();
@@ -231,10 +234,12 @@ constexpr int kOrbChunk = 64;  // frames per pass of nodes_create for grey + dep
 // become nodes (from the parameters).  A default FrameInput is orb_detect's: the detector output of a grey image (mode 0).
 struct FrameInput {
   int mode = 0;                               // 0: detector output, 1: Node constructor
-  bool rgb = false, mask_from_depth = false, mask_from_cloud = false;
+  bool rgb = false, bayer = false, mask_from_depth = false, mask_from_cloud = false;
+  bool depth_u16 = false, mask_from_u16 = false;  // 16-bit millimetres; its mask is written into the mask buffer (k_depth_u16)
   bool caller_mask = false;                   // the caller's mask is uploaded (not replaced by one derived on the device)
   int cloud_stride = 0;                       // floats per cloud point (4: PointXYZ, 8: PointXYZRGB); 0 = depth image
-  size_t gray_bytes = 0, depth_bytes = 0;     // per frame: the visual image, the depth image or cloud
+  size_t gray_bytes = 0, depth_bytes = 0;     // per frame, as the caller passes them: the visual image, the depth image or cloud
+  size_t plane_bytes = 0;                     // per frame on the device: the float depth image or the cloud
   OrbPoints points = OrbPoints::kDepthPixel;
   float depth_scaling = 1.f;
   float4 Kinv = {0.f, 0.f, 0.f, 0.f};         // projectTo3D intrinsics (node.cpp:913-916): float(1./fx), float(1./fy), cx, cy
@@ -242,12 +247,17 @@ struct FrameInput {
   FrameInput(int flags, size_t px, const rgbdslam_b200_params& p, const float* K4, const uint8_t* mask) {
     mode = 1;
     rgb = (flags & RGBDSLAM_B200_VISUAL_RGB) != 0;
-    mask_from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
+    bayer = (flags & RGBDSLAM_B200_VISUAL_BAYER_GR) != 0;
+    depth_u16 = (flags & RGBDSLAM_B200_DEPTH_U16) != 0;
+    const bool from_depth = (flags & RGBDSLAM_B200_MASK_FROM_DEPTH) != 0;
+    mask_from_depth = from_depth && !depth_u16;  // the float rule, applied by k_cell_extract
+    mask_from_u16 = from_depth && depth_u16;
     mask_from_cloud = (flags & RGBDSLAM_B200_MASK_FROM_CLOUD) != 0;
-    caller_mask = mask && !mask_from_depth && !mask_from_cloud;
+    caller_mask = mask && !from_depth && !mask_from_cloud;
     cloud_stride = (flags & RGBDSLAM_B200_CLOUD_XYZRGB) ? 8 : (flags & RGBDSLAM_B200_CLOUD_XYZ) ? 4 : 0;
     gray_bytes = rgb ? 3 * px : px;
-    depth_bytes = cloud_stride ? px * cloud_stride * 4 : px * 4;
+    depth_bytes = cloud_stride ? px * cloud_stride * 4 : depth_u16 ? px * 2 : px * 4;
+    plane_bytes = cloud_stride ? depth_bytes : px * 4;
     // getMinDepthInNeighborhood (node.cpp:82-83, 940-941) is a depth-image rule: the point-cloud constructor does not read it
     points = cloud_stride ? OrbPoints::kCloud : p.use_feature_min_depth ? OrbPoints::kMinDepth : OrbPoints::kDepthPixel;
     if (!cloud_stride) {  // the point-cloud constructor takes its points from the cloud: no intrinsics
@@ -255,12 +265,14 @@ struct FrameInput {
       Kinv = make_float4((float)(1. / (double)K4[0]), (float)(1. / (double)K4[1]), K4[2], K4[3]);
     }
   }
-  bool mask_buffer() const { return caller_mask || mask_from_cloud; }  // a device mask per frame
+  bool mask_buffer() const { return caller_mask || mask_from_cloud || mask_from_u16; }  // a device mask per frame
+  bool raw_visual() const { return rgb || bayer; }  // the visual is uploaded into in_rgb / sh_rgb and converted into grey
   // frames per chunk: the input and staging buffers hold about as many bytes as kOrbChunk grey + depth-image frames (a
-  // 640x480 XYZRGB cloud is 9.8 MB, against 1.5 MB); the chunk size does not change any result
+  // 640x480 XYZRGB cloud is 9.8 MB, against 1.5 MB), and never more than kOrbChunk frames, which bounds the per-frame work
+  // buffers (16-bit depth would allow 106); the chunk size does not change any result
   int chunk(int nframes, size_t px) const {
     const size_t cap = std::max<size_t>(1, (size_t)kOrbChunk * 5 * px / (gray_bytes + depth_bytes));
-    return (int)std::min<size_t>((size_t)std::max(nframes, 1), cap);
+    return (int)std::min<size_t>((size_t)std::min(std::max(nframes, 1), kOrbChunk), cap);
   }
 };
 
@@ -278,8 +290,9 @@ static int orb_ensure_streams() {
 }
 
 // work buffers for F frames per pass; nbuf input buffers (1: synchronous single-frame entry points, 2: nodes_create)
-// depth_bytes: per frame (0 = a w*h float depth image); want_rgb: also the colour input buffers (3 bytes per pixel)
-static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_bytes = 0, bool want_rgb = false) {
+// depth_bytes: per frame (0 = a w*h float depth image); visual_bytes / raw_bytes: per frame of the colour or Bayer input
+// buffers / of the 16-bit depth input buffers (0 = none)
+static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_bytes = 0, size_t visual_bytes = 0, size_t raw_bytes = 0) {
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
   const size_t px = (size_t)g.W * g.H, z = (size_t)F * g.ncells;
@@ -287,7 +300,8 @@ static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_byte
   int rc;
   for (int b = 0; b < nbuf; b++)
     if ((rc = o.in_gray[b].ensure(px * F)) || (want_mask && (rc = o.in_mask[b].ensure(px * F))) ||
-        (rc = o.in_depth[b].ensure(depth_bytes * F)) || (want_rgb && (rc = o.in_rgb[b].ensure(3 * px * F))))
+        (rc = o.in_depth[b].ensure(depth_bytes * F)) || (visual_bytes && (rc = o.in_rgb[b].ensure(visual_bytes * F))) ||
+        (raw_bytes && (rc = o.in_raw[b].ensure(raw_bytes * F))))
       return rc;
   if ((rc = o.cell_img.ensure((size_t)g.cell_bytes * F)) || (rc = o.cell_mask.ensure((size_t)g.cell_bytes * F)) ||
       (rc = o.cand.ensure(z * kOrbCandCap * sizeof(OrbCand))) ||
@@ -374,7 +388,8 @@ static bool is_pinned(const void* p) {
 static int check_nodes_args(const char* what, const Detector* det, int nframes, const float* K4, const uint64_t* node_handles,
                             int flags) {
   constexpr int kAll = RGBDSLAM_B200_MASK_FROM_DEPTH | RGBDSLAM_B200_VISUAL_RGB | RGBDSLAM_B200_CLOUD_XYZRGB | RGBDSLAM_B200_CLOUD_XYZ |
-                       RGBDSLAM_B200_MASK_FROM_CLOUD | RGBDSLAM_B200_KEEP_CLOUD;
+                       RGBDSLAM_B200_MASK_FROM_CLOUD | RGBDSLAM_B200_KEEP_CLOUD | RGBDSLAM_B200_DEPTH_U16 |
+                       RGBDSLAM_B200_VISUAL_BAYER_GR;
   const bool cloud = (flags & (RGBDSLAM_B200_CLOUD_XYZRGB | RGBDSLAM_B200_CLOUD_XYZ)) != 0;
   const char* bad = nullptr;
   if (flags & ~kAll) bad = "unknown flag bits";
@@ -382,6 +397,10 @@ static int check_nodes_args(const char* what, const Detector* det, int nframes, 
   else if ((flags & RGBDSLAM_B200_MASK_FROM_CLOUD) && !cloud) bad = "MASK_FROM_CLOUD needs CLOUD_XYZRGB or CLOUD_XYZ";
   else if ((flags & RGBDSLAM_B200_MASK_FROM_DEPTH) && cloud) bad = "MASK_FROM_DEPTH needs a depth image, not a cloud (MASK_FROM_CLOUD)";
   else if ((flags & RGBDSLAM_B200_KEEP_CLOUD) && !cloud) bad = "KEEP_CLOUD needs CLOUD_XYZRGB or CLOUD_XYZ";
+  else if ((flags & RGBDSLAM_B200_DEPTH_U16) && cloud) bad = "DEPTH_U16 describes a depth image, not a cloud";
+  else if ((flags & RGBDSLAM_B200_VISUAL_BAYER_GR) && (flags & RGBDSLAM_B200_VISUAL_RGB))
+    bad = "VISUAL_BAYER_GR and VISUAL_RGB are exclusive";
+  else if ((flags & RGBDSLAM_B200_VISUAL_BAYER_GR) && cloud) bad = "VISUAL_BAYER_GR needs a depth image, not a cloud";
   if (bad) {
     set_error(std::string(what) + ": " + bad);
     return RGBDSLAM_B200_ERR_ARG;
@@ -457,7 +476,7 @@ static int setup_staging(const uint8_t* gray, const float* depth, const uint8_t*
 // copy stream, through staging buffer ci & 1 unless pinned.  The copy stream first waits for `after` (if given); the compute
 // stream waits for the copy.
 static int upload_chunk(int ci, int F, int chunk, size_t px, const FrameInput& in, bool pinned, const uint8_t* hg, const float* hd,
-                        const uint8_t* hm, uint8_t* dg, float* dd, uint8_t* dm, cudaEvent_t after) {
+                        const uint8_t* hm, uint8_t* dg, void* dd, uint8_t* dm, cudaEvent_t after) {
   OrbCtx& o = g_orb;
   const int b = ci & 1;
   const size_t gb = in.gray_bytes, db = in.depth_bytes;
@@ -482,12 +501,14 @@ static int upload_chunk(int ci, int F, int chunk, size_t px, const FrameInput& i
   return 0;
 }
 
-// The input kernels of a chunk of F frames: cvtColor of the colour visuals drgb into dg, calculateDepthMask of the clouds dd
-// into dm.
-static cudaError_t chunk_inputs(const FrameInput& in, int F, size_t px, const uint8_t* drgb, uint8_t* dg, const float* dd,
-                                uint8_t* dm, cudaStream_t st, int* launches) {
+// The input kernels of a chunk of F frames: cvtColor of the colour or Bayer visuals drgb into dg, the conversion of the 16-bit
+// depth images draw into dd (and their mask into dm), calculateDepthMask of the clouds dd into dm.
+static cudaError_t chunk_inputs(const FrameInput& in, int F, size_t px, const uint8_t* drgb, uint8_t* dg, const uint16_t* draw,
+                                float* dd, uint8_t* dm, cudaStream_t st, int* launches) {
   cudaError_t e = cudaSuccess;
   if (in.rgb) e = orb_run_rgb_to_gray(F, px, drgb, dg, st, launches);
+  if (in.bayer) e = orb_run_bayer_gr_to_gray(F, g_orb.g.W, g_orb.g.H, drgb, dg, st, launches);
+  if (e == cudaSuccess && in.depth_u16) e = orb_run_depth_u16(F, px, draw, dd, in.mask_from_u16 ? dm : nullptr, st, launches);
   if (e == cudaSuccess && in.mask_from_cloud) e = orb_run_cloud_mask(F, px, dd, in.cloud_stride, dm, st, launches);
   return e;
 }
@@ -742,7 +763,9 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const int chunk = in.chunk(nframes, px);
-  if ((rc = orb_ensure_buffers(chunk, 2, in.mask_buffer(), in.depth_bytes, in.rgb))) return rc;
+  if ((rc = orb_ensure_buffers(chunk, 2, in.mask_buffer(), in.plane_bytes, in.raw_visual() ? in.gray_bytes : 0,
+                               in.depth_u16 ? in.depth_bytes : 0)))
+    return rc;
   cudaStream_t st = s.stream;
   const int K = std::min(o.kp_stride, s.params.max_keypoints);  // features per node (finalize mode 1 emits <= max_keypoints)
   NodeBatch nb;
@@ -773,12 +796,14 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     uint8_t* dg = (uint8_t*)o.in_gray[b].ptr;
     float* dd = (float*)o.in_depth[b].ptr;
     uint8_t* drgb = (uint8_t*)o.in_rgb[b].ptr;
+    uint16_t* draw = (uint16_t*)o.in_raw[b].ptr;
     uint8_t* dm = in.mask_buffer() ? (uint8_t*)o.in_mask[b].ptr : nullptr;
     if ((rc = upload_chunk(ci, F, chunk, px, in, pinned, gray + in.gray_bytes * f0, (const float*)((const uint8_t*)depth + in.depth_bytes * f0),
-                           mask ? mask + px * f0 : nullptr, in.rgb ? drgb : dg, dd, mask ? dm : nullptr, o.ev_free[b])))
+                           mask ? mask + px * f0 : nullptr, in.raw_visual() ? drgb : dg, in.depth_u16 ? (void*)draw : dd,
+                           mask ? dm : nullptr, o.ev_free[b])))
       return batch_fail(nb, rc);
     if (f0 == 0) o.last_gray = dg;
-    if ((e = chunk_inputs(in, F, px, drgb, dg, dd, dm, st, &launches)) != cudaSuccess)
+    if ((e = chunk_inputs(in, F, px, drgb, dg, draw, dd, dm, st, &launches)) != cudaSuccess)
       return batch_fail(nb, cuda_fail(e, "nodes_create input kernels"));
     if ((rc = orb_detect_stage(det, F, dg, dm, in.mask_from_depth ? dd : nullptr, st, &launches))) return batch_fail(nb, rc);
     const FeatureRows rows = {nb.kp + (size_t)f0 * K, nb.xyz + (size_t)f0 * K, nb.n + f0, nb.desc + (size_t)f0 * K * 32, K};
@@ -787,7 +812,7 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     if (keep_cloud) {
       for (int f = 0; f < F; f++) {
         NodeDev* nd = nb.made[f0 + f];
-        e = launch_split_cloud((const float*)((const uint8_t*)dd + in.depth_bytes * f), in.cloud_stride, (int)px, nd->cloud_x,
+        e = launch_split_cloud((const float*)((const uint8_t*)dd + in.plane_bytes * f), in.cloud_stride, (int)px, nd->cloud_x,
                                nd->cloud_y, nd->cloud_z, st);
         if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "split_cloud kernel"));
       }
@@ -845,8 +870,9 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   if ((rc = orb_ensure_buffers(chunk, 0, false))) return rc;
   const size_t nc = (size_t)g.ncells;
   const size_t own_ = (size_t)std::max(own, 1);
-  if ((rc = o.sh_gray.ensure(px * own_)) || (rc = o.sh_depth.ensure(in.depth_bytes * own_)) ||
-      (in.mask_buffer() && (rc = o.sh_mask.ensure(px * own_))) || (in.rgb && (rc = o.sh_rgb.ensure(3 * px * own_))) ||
+  if ((rc = o.sh_gray.ensure(px * own_)) || (rc = o.sh_depth.ensure(in.plane_bytes * own_)) ||
+      (in.mask_buffer() && (rc = o.sh_mask.ensure(px * own_))) || (in.raw_visual() && (rc = o.sh_rgb.ensure(in.gray_bytes * own_))) ||
+      (in.depth_u16 && (rc = o.sh_raw.ensure(in.depth_bytes * own_))) ||
       (rc = o.sh_cell_img.ensure((size_t)g.cell_bytes * own_)) || (rc = o.sh_cand.ensure(own_ * nc * kOrbCandCap * sizeof(OrbCand))) ||
       (rc = o.all_hist.ensure((size_t)Wp * nc * 256 * 4)) || (rc = o.all_cnt.ensure((size_t)Wp * nc * 4)) ||
       (rc = o.all_many.ensure((size_t)Wp * nc * 4)) || (rc = o.all_thr.ensure((size_t)Wp * nc * 4)))
@@ -875,14 +901,16 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   for (int c0 = 0; c0 < own; c0 += chunk, ci++) {
     const int F = std::min(chunk, own - c0);
     uint8_t* dg = (uint8_t*)o.sh_gray.ptr + px * c0;
-    uint8_t* drgb = in.rgb ? (uint8_t*)o.sh_rgb.ptr + 3 * px * c0 : nullptr;
-    float* dd = (float*)((uint8_t*)o.sh_depth.ptr + in.depth_bytes * c0);
+    uint8_t* drgb = in.raw_visual() ? (uint8_t*)o.sh_rgb.ptr + in.gray_bytes * c0 : nullptr;
+    uint16_t* draw = in.depth_u16 ? (uint16_t*)o.sh_raw.ptr + px * c0 : nullptr;
+    float* dd = (float*)((uint8_t*)o.sh_depth.ptr + in.plane_bytes * c0);
     uint8_t* dm = in.mask_buffer() ? (uint8_t*)o.sh_mask.ptr + px * c0 : nullptr;
     if ((rc = upload_chunk(ci, F, chunk, px, in, pinned, gray + in.gray_bytes * c0, (const float*)((const uint8_t*)depth + in.depth_bytes * c0),
-                           mask ? mask + px * c0 : nullptr, in.rgb ? drgb : dg, dd, mask ? dm : nullptr, nullptr)))
+                           mask ? mask + px * c0 : nullptr, in.raw_visual() ? drgb : dg, in.depth_u16 ? (void*)draw : dd,
+                           mask ? dm : nullptr, nullptr)))
       return batch_fail(nb, rc);
     if (c0 == 0) o.last_gray = dg;
-    if ((e = chunk_inputs(in, F, px, drgb, dg, dd, dm, st, &launches)) != cudaSuccess)
+    if ((e = chunk_inputs(in, F, px, drgb, dg, draw, dd, dm, st, &launches)) != cudaSuccess)
       return batch_fail(nb, cuda_fail(e, "nodes_create_sharded input kernels"));
     const size_t gf = (size_t)(f0 + c0);  // global index of the chunk's first frame
     e = orb_run_detect(g, o.tab, F, dg, dm, in.mask_from_depth ? dd : nullptr, det->type,
@@ -908,7 +936,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     const int F = std::min(chunk, own - c0);
     const size_t gf = (size_t)(f0 + c0);
     const uint8_t* dg = (const uint8_t*)o.sh_gray.ptr + px * c0;
-    const float* dd = (const float*)((const uint8_t*)o.sh_depth.ptr + in.depth_bytes * c0);
+    const float* dd = (const float*)((const uint8_t*)o.sh_depth.ptr + in.plane_bytes * c0);
     const uint8_t* cimg = (const uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0;
     const OrbCandidates c = {(const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap, cnt_all + gf * nc, thr_all + gf * nc,
                              (float*)o.resp.ptr};

@@ -29,6 +29,9 @@
 // The point-cloud constructor (node.cpp:252-369) adds k_cloud_mask when the caller derives the mask from the cloud
 // (calculateDepthMask, openni_listener.cpp:520-534) and runs k_frame_finalize<kCloud> / k_frame_emit<D, kCloud> in place
 // of the depth-image finalize and emit: projectTo3D (node.cpp:855-898) on the detector's output, then compute().
+// The listener's raw inputs (openni_listener.cpp:633-659) add k_depth_u16 (16UC1 millimetres -> metres and, optionally, the
+// detection mask) and k_bayer_gr_to_gray (Bayer GRBG -> grey) in front of the chain; everything after them is the grey,
+// float-depth, caller-mask path.
 #include "orb.cuh"
 
 #include <cuda_runtime.h>
@@ -163,6 +166,45 @@ __global__ void __launch_bounds__(256) k_cloud_mask(const float* __restrict__ cl
   const double v = __dmul_rn((double)z, 50.0);
   const int iv = (v > -2147483649.0 && v < 2147483648.0) ? __double2int_rz(v) : (int)0x80000000;  // NaN fails the test
   mask[i] = z != z ? 0 : (uint8_t)(iv & 0xFF);
+}
+
+// The listener's conversions of a 16UC1 millimetre depth image (openni_listener.cpp:633-659) for n pixels:
+//   depth = convertTo(CV_32FC1, 0.001)                            = (float)d * 0.001f, so a hole (0) reads as 0 m, not NaN
+//   mask  = depthToCV8UC1: convertTo(CV_8UC1, 0.05, -25) (misc.cpp:414-425) = saturate_cast<uchar>(fmaf(d, 0.05f, -25.f)),
+//           non-zero iff d >= 510 (an unfused d * 0.05f - 25 gives 0.5 -> 0 at d = 510); written only when mask != nullptr.
+// Both equal cv2 4.13 on all 65536 values.
+__global__ void __launch_bounds__(256) k_depth_u16(const uint16_t* __restrict__ raw, float* __restrict__ depth,
+                                                   uint8_t* __restrict__ mask, size_t n) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float d = (float)raw[i];
+  depth[i] = __fmul_rn(d, 0.001f);
+  if (mask) mask[i] = (uint8_t)min(max(__float2int_rn(__fmaf_rn(d, 0.05f, -25.f)), 0), 255);
+}
+
+// cvtColor(raw, rgb, COLOR_BayerGR2RGB) (openni_listener.cpp:638-641) then cvtColor(CV_RGB2GRAY) (node.cpp:139-144) of one
+// w x h frame per blockIdx.z.  The mosaic has G B on even rows and R G on odd rows; cv2 4.13's bilinear rule at an interior
+// pixel keeps its own channel and averages the others over pairs, (a + b + 1) >> 1, or over the cross / diagonal quads,
+// (a + b + c + d + 2) >> 2; rows 0 and h-1 repeat rows 1 and h-2, columns 0 and w-1 columns 1 and w-2.  RGB is rounded to u8
+// before the grey rule, as the two calls do (cv2's fused BayerGR2GRAY rounds differently).
+__global__ void __launch_bounds__(256) k_bayer_gr_to_gray(const uint8_t* __restrict__ raw, uint8_t* __restrict__ gray, int w, int h) {
+  const int x = blockIdx.x * 32 + (threadIdx.x & 31), y = blockIdx.y * 8 + (threadIdx.x >> 5);
+  if (x >= w || y >= h) return;
+  const size_t frame = (size_t)blockIdx.z * w * h;
+  const int sx = min(max(x, 1), w - 2), sy = min(max(y, 1), h - 2);
+  const uint8_t* p = raw + frame + (size_t)sy * w + sx;
+  const uint32_t c = p[0], up = p[-w], dn = p[w], lf = p[-1], rt = p[1];
+  const uint32_t pair_v = (up + dn + 1) >> 1, pair_h = (lf + rt + 1) >> 1, cross = (up + dn + lf + rt + 2) >> 2;
+  const uint32_t diag = (p[-w - 1] + p[-w + 1] + p[w - 1] + p[w + 1] + 2u) >> 2;
+  uint32_t r, g, b;
+  if (!(sy & 1)) {
+    if (!(sx & 1)) { r = pair_v; g = c; b = pair_h; }  // G, B to the sides
+    else { r = diag; g = cross; b = c; }               // B
+  } else {
+    if (!(sx & 1)) { r = c; g = cross; b = diag; }     // R
+    else { r = pair_h; g = c; b = pair_v; }            // G, R to the sides
+  }
+  gray[frame + (size_t)y * w + x] = (uint8_t)rgb_to_gray_px(r, g, b);
 }
 
 // level of the full-image pyramid = INTER_LINEAR_EXACT resize of the previous level (8.8 fixed-point taps, round to nearest at
@@ -1014,6 +1056,20 @@ cudaError_t orb_run_cloud_mask(int nframes, size_t px, const float* d_cloud, int
                                int* launches) {
   const size_t n = px * nframes;
   k_cloud_mask<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_cloud, cloud_stride, d_mask, n);
+  (*launches)++;
+  return cudaGetLastError();
+}
+
+cudaError_t orb_run_depth_u16(int nframes, size_t px, const uint16_t* d_raw, float* d_depth, uint8_t* d_mask, cudaStream_t st,
+                              int* launches) {
+  const size_t n = px * nframes;
+  k_depth_u16<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_raw, d_depth, d_mask, n);
+  (*launches)++;
+  return cudaGetLastError();
+}
+
+cudaError_t orb_run_bayer_gr_to_gray(int nframes, int w, int h, const uint8_t* d_raw, uint8_t* d_gray, cudaStream_t st, int* launches) {
+  k_bayer_gr_to_gray<<<plane_grid(w, h, nframes), 256, 0, st>>>(d_raw, d_gray, w, h);
   (*launches)++;
   return cudaGetLastError();
 }

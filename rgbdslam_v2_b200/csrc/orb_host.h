@@ -25,6 +25,12 @@ cudaError_t orb_run_rgb_to_gray(int nframes, size_t px, const uint8_t* d_rgb, ui
 // calculateDepthMask (openni_listener.cpp:520-534) of nframes organised clouds, cloud_stride floats per point.
 cudaError_t orb_run_cloud_mask(int nframes, size_t px, const float* d_cloud, int cloud_stride, uint8_t* d_mask, cudaStream_t st,
                                int* launches);
+// the listener's conversions of nframes 16UC1 millimetre depth images (openni_listener.cpp:633-659): metres into d_depth, and
+// depthToCV8UC1's mask into d_mask unless it is NULL
+cudaError_t orb_run_depth_u16(int nframes, size_t px, const uint16_t* d_raw, float* d_depth, uint8_t* d_mask, cudaStream_t st,
+                              int* launches);
+// cvtColor(COLOR_BayerGR2RGB) then cvtColor(CV_RGB2GRAY) of nframes w x h Bayer mosaics (openni_listener.cpp:638-641).
+cudaError_t orb_run_bayer_gr_to_gray(int nframes, int w, int h, const uint8_t* d_raw, uint8_t* d_gray, cudaStream_t st, int* launches);
 
 // Where the Node constructor takes a keypoint's 3-D point from (removeDepthless and projectTo3D).
 enum class OrbPoints {

@@ -15,8 +15,15 @@ the host-to-device bytes per frame of each; the new kernels' device times from t
 with cloud nodes against depth-image nodes (cloud nodes built --cloud-chunk frames per call, one detector: the same nodes as
 one call).
 
+--raw: instead, the ORB detector on the listener's raw inputs against the converted ones, alternated --rounds times in
+step 1 from pinned and from pageable memory: grey + float metres, grey + 16-bit millimetres (DEPTH_U16), colour + float
+metres and Bayer + 16-bit millimetres (VISUAL_BAYER_GR | DEPTH_U16), all with MASK_FROM_DEPTH; the host-to-device bytes per
+frame of each; the device time of the conversion kernels from torch.profiler in a separate pass; the host time per frame of
+the conversions a caller no longer makes (cv2 / numpy, one thread); and step 2 with 16-bit nodes against float nodes
+(millimetre quantisation and the 0.51 m mask change the results).
+
 Prints one JSON object, with the card name and power limit read in the same run.
-Usage: python tools/run_nodes.py [--min-depth | --cloud]
+Usage: python tools/run_nodes.py [--min-depth | --cloud | --raw]
 """
 import argparse
 import ctypes as C
@@ -48,9 +55,12 @@ def main():
     ap.add_argument("--cloud", action="store_true", help="colour and point-cloud input (ORB detector) instead of the detector types")
     ap.add_argument("--cloud-frames", type=int, default=256)
     ap.add_argument("--cloud-chunk", type=int, default=128)
+    ap.add_argument("--raw", action="store_true", help="16-bit depth and Bayer input (ORB detector) instead of the detector types")
     args = ap.parse_args()
     if args.cloud:
         return main_cloud(args)
+    if args.raw:
+        return main_raw(args)
 
     import torch
     from rgbdslam_v2_b200 import Frontend, pipeline, synth
@@ -286,6 +296,157 @@ def main_cloud(args):
         c4[kind] = {"frames": nf_, "pairs": int(len(pairs)), "valid_edges": int(graph["n_valid_edges"]),
                     "mean_features": float(np.mean(nfeat)), "mean_inliers_valid": float(res["n_inliers"][res["id1"] >= 0].mean()),
                     "lm_iterations": lm, "chi2": chi2, "ate_vs_gt_m": synth.ate_rmse(traj[:, :3], gt[:, :3]), "seconds": secs}
+    out["c4"] = c4
+    fe.close()
+    print(json.dumps(out))
+
+
+def main_raw(args):
+    import cv2
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    from rgbdslam_v2_b200 import Frontend, pipeline, synth
+    from rgbdslam_v2_b200._capi import DETECTOR_ORB, PAIR_RESULT_DTYPE, default_params, graph_from_pairs
+    if not torch.cuda.is_available():
+        raise SystemExit("run_nodes.py measures on the GPU; no CUDA device found")
+    dev = torch.device("cuda", 0)
+    K4 = (synth.FX, synth.FY, synth.CX, synth.CY)
+    seed = 11
+    p = default_params(); p.depth_cov_z0 = 2.0; p.max_keypoints = args.keypoints; p.feature_detector_type = DETECTOR_ORB
+    fe = Frontend(0, p)
+
+    n = max(args.frames, args.timing_frames)
+    poses = synth.trajectory(n)
+    g_d, d_d = synth.render_frames_torch(poses, dev)
+    H, W = g_d.shape[1:]
+
+    def pinned(t):
+        h = torch.empty(t.shape, dtype=t.dtype).pin_memory()
+        h.copy_(t)
+        return h
+
+    # what a 16UC1 sensor sends: millimetres, 0 where there is no depth
+    mm = d_d * 1000.0
+    ok = torch.isfinite(mm) & (mm > 0) & (mm < 65535.5)
+    depth_mm = pinned(torch.where(ok, mm.nan_to_num(0.0).round(), torch.zeros_like(mm)).to(torch.int32).cpu().to(torch.uint16))
+    del mm, ok
+    nt = args.timing_frames
+    rgb_d = torch.stack([g_d[:nt], g_d[:nt].roll(3, -1), g_d[:nt].roll(5, -2)], -1)
+    yy, xx = torch.meshgrid(torch.arange(H, device=dev), torch.arange(W, device=dev), indexing="ij")
+    ch = torch.where(yy % 2 == 0, torch.where(xx % 2 == 0, 1, 2), torch.where(xx % 2 == 0, 0, 1))  # G B / R G
+    bayer = pinned(torch.gather(rgb_d, 3, ch.expand(nt, H, W).unsqueeze(-1)).squeeze(-1).contiguous())
+    rgb = pinned(rgb_d)
+    gray = pinned(g_d)
+    depth = pinned(d_d)
+    del g_d, rgb_d
+    torch.cuda.synchronize()
+    px = H * W
+    out = {"card": card(), "image": f"{W}x{H}", "max_keypoints": args.keypoints, "detector": "ORB", "mask": "MASK_FROM_DEPTH"}
+    # name: (visual, depth, keyword, host->device bytes per frame)
+    base = {"gray_float": (gray, depth, {}, px + 4 * px), "gray_u16": (gray, depth_mm, {}, px + 2 * px),
+            "rgb_float": (rgb, depth, {}, 3 * px + 4 * px), "bayer_u16": (bayer, depth_mm, {"bayer": True}, px + 2 * px)}
+    configs = {}
+    for k, (v, d, kw, b) in base.items():
+        configs[k + "_pinned"] = (v[:nt], d[:nt], kw, b)
+    for k, (v, d, kw, b) in base.items():
+        configs[k + "_pageable"] = (v[:nt].numpy().copy(), d[:nt].numpy().copy(), kw, b)
+
+    def call(cfg, frames=None):
+        vis, dep, kw, _ = configs[cfg]
+        m = frames or nt
+        det = fe.detector_create()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        hs, nf = fe.nodes_create(det, vis[:m], dep[:m], None, K4, mask_from_depth=True, **kw)
+        dt = time.perf_counter() - t0
+        fe.detector_destroy(det)
+        for h in hs:
+            fe.node_destroy(h)
+        return m / dt, float(np.mean(nf))
+
+    # ---- 1. the constructor alone, inputs alternated
+    timing = {c: [] for c in configs}
+    feats = {}
+    for r in range(args.rounds + 1):  # round 0 warms up every configuration
+        for c in configs:
+            fps, feats[c] = call(c)
+            if r:
+                timing[c].append(fps)
+    out["nodes_create_frames"] = nt
+    out["nodes_create_frames_per_s"] = {k: {"runs": [round(x, 1) for x in vs], "min": round(min(vs), 1), "max": round(max(vs), 1)}
+                                        for k, vs in timing.items()}
+    out["nodes_create_mean_features"] = feats
+    out["h2d_bytes_per_frame"] = {k: c[3] for k, c in base.items()}
+
+    # ---- the conversion kernels' device time per frame (torch.profiler, separate pass)
+    kernels = ("k_depth_u16", "k_bayer_gr_to_gray", "k_rgb_to_gray")
+    prof_frames = min(64, nt)
+    ktimes = {}
+    for c in ("bayer_u16_pinned", "rgb_float_pinned"):
+        call(c, prof_frames)
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call(c, prof_frames)
+        tot = {}
+        for e in prof.events():
+            m = re.search(r"rb200::(k_\w+)", e.name)
+            if e.device_type.name == "CUDA" and m and m.group(1) in kernels:
+                tot[m.group(1)] = tot.get(m.group(1), 0.0) + e.device_time
+        allk = sum(e.device_time for e in prof.events() if e.device_type.name == "CUDA" and "rb200::k_" in e.name)
+        ktimes[c] = {k: round(t / prof_frames, 3) for k, t in sorted(tot.items())}
+        ktimes[c]["all_library_kernels"] = round(allk / prof_frames, 2)
+    out["kernel_us_per_frame"] = ktimes
+
+    # ---- the host conversions a caller no longer makes, per frame (one thread)
+    cv2.setNumThreads(1)
+    hb, hd = bayer[:64].numpy(), depth_mm[:64].numpy()
+
+    def per_frame_us(fn):
+        for f in range(4):
+            fn(f)
+        t0 = time.perf_counter()
+        for f in range(len(hb)):
+            fn(f)
+        return round((time.perf_counter() - t0) / len(hb) * 1e6, 1)
+    out["host_us_per_frame"] = {
+        "cv2_cvtColor_BayerGR2RGB": per_frame_us(lambda f: cv2.cvtColor(hb[f], cv2.COLOR_BayerGR2RGB)),
+        "numpy_depth_u16_to_float": per_frame_us(lambda f: hd[f].astype(np.float32) * np.float32(0.001)),
+        "cv2_convertScaleAbs_u16_mask": per_frame_us(lambda f: cv2.convertScaleAbs(hd[f], alpha=0.05, beta=-25)),
+    }
+
+    # ---- 2. the C4 sequence with 16-bit nodes against float nodes
+    nf_ = args.frames
+    pairs = np.array(pipeline.candidate_pairs(nf_, seed=seed), np.int64)
+    gt = np.stack([pipeline.mat_to_pose7(np.linalg.inv(poses[0]) @ P) for P in poses[:nf_]])
+    fe.posegraph_reserve(nf_, 12 * nf_)
+
+    def sequence(dep, nf):
+        pp = pairs[pairs[:, 0] < nf]
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        det = fe.detector_create()
+        hs, nfeat = fe.nodes_create(det, gray[:nf], dep[:nf], None, K4, ids=np.arange(nf, dtype=np.int32), mask_from_depth=True)
+        res = np.zeros(len(pp), PAIR_RESULT_DTYPE); res["id1"] = -1; res["id2"] = -1
+        pipeline.match_pairs_pipelined(fe, hs, pp, seed=seed, first_pair_index=0, out=res)
+        graph = graph_from_pairs(pp, res, nf)
+        traj, chi2, lm, cg = fe.optimize_graph(graph["init"], graph["fixed"], graph["ij"], graph["meas"], graph["info"], stop=0.01)
+        t1 = time.perf_counter()
+        zeros = 0
+        for h in hs[:64]:
+            zeros += int((fe.node_download(h)[1][:, 2] == 0).sum())
+        fe.detector_destroy(det)
+        for h in hs:
+            fe.node_destroy(h)
+        return nfeat, res, graph, traj, chi2, lm, t1 - t0, zeros
+
+    c4 = {}
+    for kind, dep in (("u16", depth_mm), ("float", depth)):
+        sequence(dep, min(nf_, 96))
+        nfeat, res, graph, traj, chi2, lm, secs, zeros = sequence(dep, nf_)
+        c4[kind] = {"frames": nf_, "pairs": int(len(pairs)), "valid_edges": int(graph["n_valid_edges"]),
+                    "mean_features": float(np.mean(nfeat)), "mean_inliers_valid": float(res["n_inliers"][res["id1"] >= 0].mean()),
+                    "lm_iterations": lm, "chi2": chi2, "ate_vs_gt_m": synth.ate_rmse(traj[:, :3], gt[:, :3]), "seconds": secs,
+                    "z0_points_first_64_nodes": zeros}
     out["c4"] = c4
     fe.close()
     print(json.dumps(out))
