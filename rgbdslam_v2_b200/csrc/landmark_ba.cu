@@ -13,7 +13,8 @@
 // matrix-free (per point: u = Hpp^-1 sum Hpc d; per camera: q = Hcc d + sum pose-edge blocks - sum Hcp u), two gather kernels
 // and one single-CTA update kernel per iteration, all reductions in a fixed order (deterministic).
 // The pose edges are the pose-graph solver's module (PoseEdges), the LM bookkeeping its driver (lm_optimize, posegraph.h).
-// float64 throughout.  Oracle: oracle/landmark_oracle.py (dense solve of the FULL system).
+// float64 throughout.  Oracles: oracle/landmark_oracle.py (dense solve of the FULL system), tests/ba_exact.py (float64
+// restatement of every step at multi-CTA shapes).
 #include <cuda_runtime.h>
 
 #include <vector>
@@ -319,6 +320,9 @@ __global__ void __launch_bounds__(1024) ba_cg_step_kernel(int mode, int n_cams, 
     return s_val;
   };
   if (mode == 1 && state[2] != 0.0) return;  // finished: further launches of the fixed-length host loop are no-ops
+  // dn of the previous step, read once before any barrier: thread 0 overwrites state[0] at the end of this launch, and a warp
+  // still computing beta after that write would otherwise see the new value
+  const double dn_old = mode == 1 ? state[0] : 0.0;
   double alpha = 0;
   if (mode == 1) {
     double t = 0;
@@ -328,7 +332,7 @@ __global__ void __launch_bounds__(1024) ba_cg_step_kernel(int mode, int n_cams, 
       if (threadIdx.x == 0) state[2] = 2.0;
       return;
     }
-    alpha = state[0] / dq;
+    alpha = dn_old / dq;
   }
   double loc = 0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -352,7 +356,7 @@ __global__ void __launch_bounds__(1024) ba_cg_step_kernel(int mode, int n_cams, 
     loc += r[i] * s;
   }
   const double dn_new = block_sum(loc);
-  const double beta = mode == 0 ? 0.0 : dn_new / state[0];
+  const double beta = mode == 0 ? 0.0 : dn_new / dn_old;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int c = i / 6, rr = i % 6;
     double s = 0;
