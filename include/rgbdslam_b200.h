@@ -370,9 +370,23 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * VISUAL_RGB.  Every frame of the call is converted (the listener hands its first Bayer frame over raw: pass that one without
  * the flag to do the same).
  *
+ * RGBDSLAM_B200_STORE_CLOUD: every node keeps its colour point cloud, the reference's pc_col (store_pointclouds, node.cpp:126-131,
+ * 261), for rgbdslam_b200_node_download_cloud and rgbdslam_b200_render_cloud (rgbdslam_b200/map.h).  Depth-image input: createXYZRGBPointCloud(depth,
+ * visual, cam_info) (misc.cpp:467-556) at every params.cloud_creation_skip_step-th pixel -- z = (float)((double)depth *
+ * depth_scaling_factor), NaN where !(z >= minimum_depth); x / y are not stored, they follow from the pixel and K4 -- and the
+ * packed colour word of the visual the Node receives (the grey image, the three-channel image, or the debayered RGB image of
+ * VISUAL_BAYER_GR): channel 0 is blue (encoding_bgr, the reference default) or red (RGBDSLAM_B200_ENCODING_RGB), alpha 0, and
+ * point 0 keeps colour 0 (misc.cpp:537).  8 bytes per point (614 kB per 640 x 480 node at skip step 2).  The skip step must
+ * divide w and h.  Cloud input: the node keeps its organised cloud as KEEP_CLOUD does (also without that flag) plus the colour
+ * word of each point (the float at byte 16 of PointXYZRGB, data[3] of PointXYZ), 16 bytes per point.  The planes of all nodes of
+ * a call share one device allocation, made before any work is queued, and are written by one kernel launch per chunk from the
+ * buffers the chunk already holds.  Features, detector thresholds and measurement-model counts are those of the same call
+ * without the flag.
+ *
  * Rejected with ERR_ARG before any device work: unknown bits, CLOUD_XYZRGB with CLOUD_XYZ, MASK_FROM_CLOUD without a cloud
  * bit, MASK_FROM_DEPTH with a cloud bit, KEEP_CLOUD without a cloud bit, DEPTH_U16 or VISUAL_BAYER_GR with a cloud bit,
- * VISUAL_BAYER_GR with VISUAL_RGB. */
+ * VISUAL_BAYER_GR with VISUAL_RGB, ENCODING_RGB without STORE_CLOUD, STORE_CLOUD on depth-image input whose w or h the skip step
+ * does not divide. */
 #define RGBDSLAM_B200_MASK_FROM_DEPTH 1
 #define RGBDSLAM_B200_VISUAL_RGB 2
 #define RGBDSLAM_B200_CLOUD_XYZRGB 4
@@ -381,6 +395,9 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
 #define RGBDSLAM_B200_KEEP_CLOUD 128
 #define RGBDSLAM_B200_DEPTH_U16 256
 #define RGBDSLAM_B200_VISUAL_BAYER_GR 512
+/* bits 32, 64, 1024 and 2048 stay unassigned: they have always been rejected as unknown */
+#define RGBDSLAM_B200_STORE_CLOUD 4096
+#define RGBDSLAM_B200_ENCODING_RGB 8192
 int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                   int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
                                   int32_t* n_features);
@@ -393,7 +410,8 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
  * would have used; the finished features (descriptors, 3-D points, counts) are all-gathered so that every rank holds every
  * node.  node_handles / n_features / ids: total_frames entries.  Bit-identical to rgbdslam_b200_nodes_create_ex on one GPU
  * (2-D keypoints, which only the pairwise g2o refinement reads, stay on the rank that built the node).  Collective: every
- * rank of the communicator must call it with the same total_frames and parameters. */
+ * rank of the communicator must call it with the same total_frames and parameters.  KEEP_CLOUD and STORE_CLOUD are rejected
+ * with ERR_ARG (clouds are not exchanged). */
 int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
                                        const float* depth, const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids,
                                        int flags, uint64_t* node_handles, int32_t* n_features);

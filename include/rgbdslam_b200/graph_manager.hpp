@@ -6,11 +6,13 @@
 //   double optimizeGraph(double break_criterion = -1, bool nonthreaded)  :900-1066  -> rgbdslam_b200_posegraph_optimize
 //   unsigned pruneEdgesWithErrorAbove(float)                             :1106-1246 -> rgbdslam_b200_posegraph_chi2
 //   void   saveTrajectory(filename)                                      graph_mgr_io.cpp:615-677 / logTransform misc.cpp:90-93
+//   void   saveAllClouds(filename)  == saveAllCloudsToFile               graph_mgr_io.cpp:502-583 -> rgbdslam_b200_render_cloud
 // Host logic only; every compute step is a C-ABI call.  The reference draws from the global rand(); here every draw comes
 // from the library's counter-based generator keyed by (seed, node id).  g2o's HyperDijkstra (not under /root/reference) is
 // restated in geodesicBall().  The Python mirror rgbdslam_v2_b200/graph_manager.py is the tested twin of this file.
 #pragma once
 #include <algorithm>
+#include <cctype>
 #include <cmath>
 #include <cstdio>
 #include <map>
@@ -337,6 +339,90 @@ class GraphManager {
     return counter;
   }
 
+  // parameters maximum_depth (parameter_server.cpp, default +inf: no point is dropped for its range; < 0 also disables the
+  // filter) and preserve_raster_on_save (default false) of saveAllClouds
+  static double& maximum_depth() {
+    static double v = INFINITY;
+    return v;
+  }
+  static bool& preserve_raster_on_save() {
+    static bool v = false;
+    return v;
+  }
+
+  // world2cam = cam2rgb * eigenTransf2TF(estimate of node id) in double (graph_mgr_io.cpp:526-541), row-major 3 x 4: cam2rgb has
+  // rotation createQuaternionFromRPY(-1.57, 0, -1.57) (-1.57, not -pi/2) and origin (0, -0.04, 0); eigenTransf2TF takes the
+  // rotation through a quaternion (Eigen's matrix -> quaternion, here normalised) and tf's quaternion -> matrix.
+  void mapTransform(int id, double T[12]) const {
+    const Pose7& p = estimates_.at(id);
+    double R[9], q[4];
+    quatToRot(p.v + 3, R);  // the VertexSE3 estimate as an Isometry3d
+    rotToQuat(R, q);
+    double P[12], C[12];
+    tfMatrix(q, P);
+    P[3] = p.v[0], P[7] = p.v[1], P[11] = p.v[2];
+    const double hr = -1.57 * 0.5, hp = 0.0, hy = -1.57 * 0.5;  // tf::Quaternion::setRPY(roll, pitch, yaw)
+    const double cr = std::cos(hr), sr = std::sin(hr), cp = std::cos(hp), sp = std::sin(hp), cy = std::cos(hy), sy = std::sin(hy);
+    const double qc[4] = {sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy,
+                          cr * cp * cy + sr * sp * sy};
+    tfMatrix(qc, C);
+    C[3] = 0.0, C[7] = -0.04, C[11] = 0.0;
+    for (int r = 0; r < 3; r++) {  // tf::Transform * tf::Transform: (Rc Rp, Rc tp + tc), sums (a0 b0 + a1 b1) + a2 b2
+      for (int c = 0; c < 3; c++) T[4 * r + c] = (C[4 * r] * P[c] + C[4 * r + 1] * P[4 + c]) + C[4 * r + 2] * P[8 + c];
+      T[4 * r + 3] = ((C[4 * r] * P[3] + C[4 * r + 1] * P[7]) + C[4 * r + 2] * P[11]) + C[4 * r + 3];
+    }
+  }
+
+  // GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583): the stored clouds (Node::store_pointclouds()) of the nodes
+  // with valid_tf_estimate_, in id order, each put through mapTransform and transformAndAppendPointCloud on the device, written
+  // as a binary PCD v0.7 (x y z rgb, 16 bytes per point; width 1 x height n, or n x 1 with preserve_raster_on_save, as PCL
+  // leaves the aggregate).  ".pcd" is appended when the name lacks it; a ".ply" name throws std::invalid_argument (PLY
+  // output is not built).  Returns the number of points written.
+  size_t saveAllClouds(std::string filename) const {
+    auto ends_with = [&](const char* ext) {
+      const size_t n = std::strlen(ext);
+      if (filename.size() < n) return false;
+      for (size_t i = 0; i < n; i++)
+        if (std::tolower((unsigned char)filename[filename.size() - n + i]) != ext[i]) return false;
+      return true;
+    };
+    if (ends_with(".ply")) throw std::invalid_argument("saveAllClouds: PLY output is not built (save as .pcd)");
+    if (!ends_with(".pcd")) filename += ".pcd";
+    std::vector<uint64_t> handles;
+    std::vector<double> T;
+    for (auto& kv : graph_) {
+      const Node* n = kv.second;
+      if (!n->valid_tf_estimate_ || !estimates_.count(n->vertex_id_)) continue;
+      handles.push_back(n->handle());
+      T.resize(T.size() + 12);
+      mapTransform(n->vertex_id_, &T[T.size() - 12]);
+    }
+    const int preserve = preserve_raster_on_save() ? 1 : 0;
+    int64_t count = 0;
+    check(rgbdslam_b200_render_cloud((int)handles.size(), handles.data(), T.data(), maximum_depth(), preserve, 32, nullptr, 0, &count,
+                                     nullptr),
+          "render_cloud");
+    std::vector<PointXYZRGB> pts((size_t)count);
+    check(rgbdslam_b200_render_cloud((int)handles.size(), handles.data(), T.data(), maximum_depth(), preserve, 32, pts.data(), count,
+                                     &count, nullptr),
+          "render_cloud");
+    FILE* f = std::fopen(filename.c_str(), "wb");
+    if (!f) throw std::runtime_error("cannot open " + filename);
+    const unsigned long long n = (unsigned long long)count;
+    std::fprintf(f,
+                 "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z rgb\nSIZE 4 4 4 4\nTYPE F F F F\n"
+                 "COUNT 1 1 1 1\nWIDTH %llu\nHEIGHT %llu\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %llu\nDATA binary\n",
+                 preserve ? n : 1ull, preserve ? 1ull : n, n);
+    std::vector<float> rec(4 * (size_t)count);
+    for (size_t i = 0; i < pts.size(); i++) {
+      rec[4 * i] = pts[i].x, rec[4 * i + 1] = pts[i].y, rec[4 * i + 2] = pts[i].z;
+      std::memcpy(&rec[4 * i + 3], &pts[i].b, 4);
+    }
+    const bool ok = std::fwrite(rec.data(), 16, pts.size(), f) == pts.size();
+    if (std::fclose(f) != 0 || !ok) throw std::runtime_error("cannot write " + filename);
+    return pts.size();
+  }
+
   // TUM trajectory "timestamp tx ty tz qx qy qz qw" (logTransform, misc.cpp:90-93)
   void saveTrajectory(const std::string& filename) const {
     FILE* f = std::fopen(filename.c_str(), "w");
@@ -351,6 +437,16 @@ class GraphManager {
 
  private:
   std::map<int, std::set<int>> adj_;
+
+  static void tfMatrix(const double* q, double M[12]) {  // tf::Matrix3x3::setRotation, into the rotation part of a 3 x 4
+    const double x = q[0], y = q[1], z = q[2], w = q[3];
+    const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
+    const double xs = x * s, ys = y * s, zs = z * s, wx = w * xs, wy = w * ys, wz = w * zs;
+    const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
+    M[0] = 1.0 - (yy + zz), M[1] = xy - wz, M[2] = xz + wy;
+    M[4] = xy + wz, M[5] = 1.0 - (xx + zz), M[6] = yz - wx;
+    M[8] = xz - wy, M[9] = yz + wx, M[10] = 1.0 - (xx + yy);
+  }
 
   struct Rand {  // rand() stand-in: the library's splitmix64 counter generator, stream 0xC0
     uint64_t key;

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../rgbdslam_b200.h"
+#include "map.h"
 #include "features.hpp"
 
 namespace rgbdslam_b200 {
@@ -157,7 +158,8 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     const CameraInfo ci = cam_info ? *cam_info : CameraInfo();
     const float K4[4] = {(float)ci.K[0], (float)ci.K[4], (float)ci.K[2], (float)ci.K[5]};  // node.cpp:913-916
     const int flags = (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) | (u16 ? RGBDSLAM_B200_DEPTH_U16 : 0) |
-                      (u16 && !m ? RGBDSLAM_B200_MASK_FROM_DEPTH : 0);
+                      (u16 && !m ? RGBDSLAM_B200_MASK_FROM_DEPTH : 0) |
+                      (store_pointclouds() ? RGBDSLAM_B200_STORE_CLOUD | (encoding_bgr() ? 0 : RGBDSLAM_B200_ENCODING_RGB) : 0);
     construct(g, d, m, visual.cols, visual.rows, K4, detector->handle(), flags);
   }
   // The reference's point-cloud constructor, argument for argument (node.h:74-78, call site openni_listener.cpp:754):
@@ -190,7 +192,7 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     const bool emm = rgbdslam_b200_get_params(&prm) == 0 && prm.observability_threshold > 0.0;
     const int flags = (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) |
                       (std::is_same<PointT, PointXYZRGB>::value ? RGBDSLAM_B200_CLOUD_XYZRGB : RGBDSLAM_B200_CLOUD_XYZ) |
-                      (emm ? RGBDSLAM_B200_KEEP_CLOUD : 0);
+                      (emm ? RGBDSLAM_B200_KEEP_CLOUD : 0) | (store_pointclouds() ? RGBDSLAM_B200_STORE_CLOUD : 0);
     construct(g, reinterpret_cast<const float*>(point_cloud->points.data()), m, visual.cols, visual.rows,
               emm ? depth_camera_intrinsics() : nullptr, detector->handle(), flags);
   }
@@ -279,6 +281,33 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
       }
     }
     return out;
+  }
+
+  // parameters store_pointclouds / encoding_bgr (parameter_server.cpp), read when an image Node is constructed.  With
+  // store_pointclouds the node keeps pc_col (createXYZRGBPointCloud, node.cpp:126-131; the input cloud, :261) on the device
+  // for pointCloud() and GraphManager::saveAllClouds.  Unlike the reference, whose default is true, it defaults to false here,
+  // so that a node costs no cloud memory (614 kB per 640 x 480 frame) unless the map is wanted.  encoding_bgr (default true,
+  // as in the reference) reads channel 0 of a three-channel visual as blue.
+  static bool& store_pointclouds() {
+    static bool v = false;
+    return v;
+  }
+  static bool& encoding_bgr() {
+    static bool v = true;
+    return v;
+  }
+  // Node::pc_col: the node's organised colour cloud, downloaded from the device (rgbdslam_b200_node_download_cloud); the
+  // node must have been built with store_pointclouds().
+  pointcloud_type::Ptr pointCloud() const {
+    int w = 0, h = 0;
+    check(rgbdslam_b200_node_download_cloud(handle_, (int)sizeof(point_type), nullptr, &w, &h), "node_download_cloud");
+    pointcloud_type::Ptr pc = std::make_shared<pointcloud_type>();
+    pc->points.resize((size_t)w * h);
+    pc->width = (uint32_t)w;
+    pc->height = (uint32_t)h;
+    if (w > 0 && h > 0)
+      check(rgbdslam_b200_node_download_cloud(handle_, (int)sizeof(point_type), pc->points.data(), &w, &h), "node_download_cloud");
+    return pc;
   }
 
   static int& max_connections() {  // parameter max_connections (parameter_server.cpp:104), -1 = unlimited

@@ -53,6 +53,11 @@ DETECTOR_ORB, DETECTOR_FAST = 0, 1  # Params.feature_detector_type (RGBDSLAM_B20
 # flags of rgbdslam_b200_nodes_create_ex / _sharded (RGBDSLAM_B200_*)
 MASK_FROM_DEPTH, VISUAL_RGB, CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD, KEEP_CLOUD = 1, 2, 4, 8, 16, 128
 DEPTH_U16, VISUAL_BAYER_GR = 256, 512
+STORE_CLOUD, ENCODING_RGB = 4096, 8192
+# records of rgbdslam_b200_node_download_cloud / render_cloud: pcl::PointXYZRGB (32 bytes) and pcl::PointXYZ (16 bytes, colour
+# word in data[3]); the colour word holds b, g, r, a bytes
+POINT32_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("w", "<u4"), ("rgb", "<u4"), ("pad", "<u4", (3,))])
+POINT16_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("w", "<u4")])
 
 
 def _is_u16(a) -> bool:
@@ -61,12 +66,14 @@ def _is_u16(a) -> bool:
 
 
 def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_cloud=False, keep_cloud=False,
-                     depth_u16=False, bayer=False) -> int:
+                     depth_u16=False, bayer=False, store_cloud=False, encoding_rgb=False) -> int:
     """The nodes_create flags the array shapes select: gray (F,H,W) or (F,H,W,3) colour; depth (F,H,W) depth image, or an
     organised cloud (F,H,W,8) of PointXYZRGB / (F,H,W,4) of PointXYZ as float32.  keep_cloud: the nodes keep their cloud
     for the environment measurement model (cloud input only).  depth_u16: the depth image is uint16 millimetres; bayer: gray
-    (F,H,W) holds bayer_grbg8 mosaics."""
+    (F,H,W) holds bayer_grbg8 mosaics.  store_cloud: the nodes keep their colour cloud (pc_col) for the map; encoding_rgb: its
+    colour reads channel 0 as red (encoding_bgr = false)."""
     flags = (MASK_FROM_DEPTH if mask_from_depth else 0) | (MASK_FROM_CLOUD if mask_from_cloud else 0)
+    flags |= (STORE_CLOUD if store_cloud else 0) | (ENCODING_RGB if encoding_rgb else 0)
     flags |= (KEEP_CLOUD if keep_cloud else 0) | (DEPTH_U16 if depth_u16 else 0) | (VISUAL_BAYER_GR if bayer else 0)
     if len(gray_shape) == 4:
         if gray_shape[3] != 3:
@@ -168,6 +175,8 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_nodes_create_ex.argtypes = [u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_nodes_create_sharded.argtypes = [u64, u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_node_download_keypoints.argtypes = [u64, vp]
+    lib.rgbdslam_b200_node_download_cloud.argtypes = [u64, C.c_int, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -449,20 +458,23 @@ class Frontend:
         return out[:n.value], desc[:n.value]
 
     def nodes_create(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, mask_from_cloud: bool = False,
-                     keep_cloud: bool = False, bayer: bool = False):
+                     keep_cloud: bool = False, bayer: bool = False, store_cloud: bool = False, encoding_rgb: bool = False):
         """gray [F,H,W] u8 or [F,H,W,3] colour (channel 0 = R), depth [F,H,W] f32 metres or u16 millimetres, or an organised
         cloud [F,H,W,8] (PointXYZRGB) / [F,H,W,4] (PointXYZ) f32 for the point-cloud constructor, mask [F,H,W] u8 or None ->
         (handles, n_features).  numpy arrays or pinned torch tensors (copied from asynchronously).  mask_from_depth /
         mask_from_cloud: derive the detection mask on the device (depthToCV8UC1 of the float or 16-bit depth /
         calculateDepthMask).  K4 may be None for cloud input.  keep_cloud (cloud input): the nodes keep their cloud for the
         environment measurement model, which projects into K4 (the reference's depth_camera_fx / fy / cx / cy; None = all
-        zero).  bayer: gray [F,H,W] holds bayer_grbg8 mosaics, debayered on the device."""
+        zero).  bayer: gray [F,H,W] holds bayer_grbg8 mosaics, debayered on the device.  store_cloud: every node keeps its
+        colour cloud (node_cloud, render_cloud); encoding_rgb: channel 0 of the visual is red (the reference default reads it
+        as blue, encoding_bgr)."""
         depth_u16 = _is_u16(depth)
         if isinstance(gray, np.ndarray):
             gray = np.ascontiguousarray(gray, np.uint8)
             depth = np.ascontiguousarray(depth, np.uint16 if depth_u16 else np.float32)
             mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, keep_cloud, depth_u16, bayer)
+        flags = node_input_flags(gray.shape, depth.shape, mask_from_depth, mask_from_cloud, keep_cloud, depth_u16, bayer, store_cloud,
+                                 encoding_rgb)
         F, H, W = gray.shape[:3]
         K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
         ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
@@ -517,6 +529,38 @@ class Frontend:
         out = np.zeros(self.node_num_features(h), KEYPOINT_DTYPE)
         self._check(self.lib.rgbdslam_b200_node_download_keypoints(h, _ptr(out)))
         return out
+
+    # -- stored clouds and the registered map ---------------------------------------------
+    def node_cloud(self, h: int, point_bytes: int = 32) -> np.ndarray:
+        """Node::pc_col of a node built with store_cloud: (H, W) records of POINT32_DTYPE or POINT16_DTYPE"""
+        w, hh = C.c_int(), C.c_int()
+        self._check(self.lib.rgbdslam_b200_node_download_cloud(C.c_uint64(int(h)), point_bytes, None, C.byref(w), C.byref(hh)))
+        out = np.zeros((hh.value, w.value), POINT32_DTYPE if point_bytes == 32 else POINT16_DTYPE)
+        self._check(self.lib.rgbdslam_b200_node_download_cloud(C.c_uint64(int(h)), point_bytes, _ptr(out), C.byref(w), C.byref(hh)))
+        return out
+
+    def render_cloud(self, nodes, transforms12, maximum_depth: float = float("inf"), preserve_raster: bool = False,
+                     point_bytes: int = 32, out=None, count_only: bool = False):
+        """transformAndAppendPointCloud of the nodes in order (transforms12: (n, 3, 4) float64, node -> map).  Returns
+        (records, used16) -- used16 (n, 4, 4) the float matrices applied -- or the record count with count_only.  out: an
+        optional host array (numpy or pinned torch uint8) large enough for the records."""
+        hs = np.ascontiguousarray(np.asarray(nodes, np.uint64))
+        T = np.ascontiguousarray(np.asarray(transforms12, np.float64).reshape(len(hs), 12))
+        n = C.c_int64()
+        if count_only:
+            self._check(self.lib.rgbdslam_b200_render_cloud(len(hs), _ptr(hs), _ptr(T), maximum_depth, int(preserve_raster), point_bytes,
+                                                            None, 0, C.byref(n), None))
+            return n.value
+        used = np.zeros((len(hs), 16), np.float32)
+        if out is None:
+            self._check(self.lib.rgbdslam_b200_render_cloud(len(hs), _ptr(hs), _ptr(T), maximum_depth, int(preserve_raster), point_bytes,
+                                                            None, 0, C.byref(n), None))
+            out = np.zeros(n.value, POINT32_DTYPE if point_bytes == 32 else POINT16_DTYPE)
+        cap = (out.numel() * out.element_size() if hasattr(out, "numel") else out.nbytes) // point_bytes
+        self._check(self.lib.rgbdslam_b200_render_cloud(len(hs), _ptr(hs), _ptr(T), maximum_depth, int(preserve_raster), point_bytes,
+                                                        _ptr(out), cap, C.byref(n), _ptr(used)))
+        return (out[:n.value] if isinstance(out, np.ndarray) and out.dtype.itemsize == point_bytes else out), \
+            used.reshape(-1, 4, 4).transpose(0, 2, 1)
 
     # -- multi-GPU exchange -------------------------------------------------------------
     def comm_unique_id(self) -> np.ndarray:

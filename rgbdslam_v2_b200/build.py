@@ -34,7 +34,9 @@ def sources() -> list[Path]:
 
 
 def _up_to_date(out: Path) -> bool:
-    deps = sources() + sorted(CSRC.glob("*.h")) + sorted(CSRC.glob("*.cuh")) + [PKG_DIR.parent / "include" / "rgbdslam_b200.h"]
+    include = PKG_DIR.parent / "include"
+    deps = (sources() + sorted(CSRC.glob("*.h")) + sorted(CSRC.glob("*.cuh")) + [include / "rgbdslam_b200.h"] +
+            sorted((include / "rgbdslam_b200").glob("*.h")))
     return out.exists() and out.stat().st_mtime >= max(p.stat().st_mtime for p in deps)
 
 

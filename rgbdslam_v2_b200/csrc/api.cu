@@ -527,13 +527,19 @@ void free_node(NodeDev* nd) {
     if (nd->kp) cudaFree(nd->kp);
   }
   free_node_cloud(nd);
+  if (nd->pc_slab && --nd->pc_slab->refs == 0) {
+    cudaFree(nd->pc_slab->base);
+    delete nd->pc_slab;
+  }
   if (nd->desc_f32) cudaFree(nd->desc_f32);
   if (nd->norms) cudaFree(nd->norms);
   delete nd;
 }
 
 void free_node_cloud(NodeDev* nd) {
-  if (nd->cloud_x) cudaFree(nd->cloud_x);  // x | y | z planes of a kept cloud
+  if (nd->cloud_x) {
+    if (!nd->pc_slab) cudaFree(nd->cloud_x);  // x | y | z planes of a kept cloud (a stored cloud's live in pc_slab)
+  }
   else if (nd->cloud_z) cudaFree(nd->cloud_z);
   nd->cloud_x = nd->cloud_y = nd->cloud_z = nullptr;
 }

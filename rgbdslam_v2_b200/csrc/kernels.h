@@ -41,6 +41,34 @@ struct EmmNode {  // one node's cloud as the model reads it (x / y only for kept
 };
 cudaError_t launch_emm_single(const EmmNode& q, const EmmNode& t, bool cloud, const float* d_T16, int cloud_step, int skip_step,
                               double cov_z_const, double sigma_depth, unsigned* d_counts, cudaStream_t stream);
+// Stored colour clouds (map.cu).  Per node `node_words` 4-byte words: depth-image frames [z | colour] planes at the skip-step
+// raster (w / step x h / step), clouds [x | y | z | colour] planes of n points.  vis_kind: 0 grey, 1 three-channel, 2 Bayer GRBG.
+cudaError_t launch_store_depth_cloud(int nframes, const float* d_depth, const uint8_t* d_visual, int vis_kind, bool bgr, int w, int h,
+                                     int step, double scaling, float min_depth, float* out, size_t node_words, cudaStream_t st);
+cudaError_t launch_store_cloud_points(int nframes, const float* d_cloud, int stride, int n, float* out, size_t node_words,
+                                      cudaStream_t st);
+// One node of a rgbdslam_b200_render_cloud / node_download_cloud call.
+struct MapNode {
+  const float *x, *y, *z;  // depth-image nodes: z only
+  const uint32_t* rgb;     // colour words
+  int cw, ch;
+  int step;                // > 0: depth-image node (x / y from pixel (rx * step, ry * step)); 0: x / y planes stored
+  float fxinv, fyinv, cx, cy;
+  float m[12];             // row-major 3 x 4 float transform
+};
+struct MapArgs {
+  float maxd2;     // maximum_depth^2 in float
+  int filter;      // maximum_depth >= 0
+  int preserve;    // preserve_raster_on_save
+  int transform;   // 0: the points as stored (node_download_cloud)
+  int point_bytes; // 16 or 32
+};
+constexpr int kMapBlockPoints = 1024;  // points per block of the count / scatter kernels
+cudaError_t launch_map_count(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const MapArgs& a, int* d_counts,
+                             cudaStream_t st);
+cudaError_t launch_map_scan(const int* d_counts, int nblocks, long long* d_offs, cudaStream_t st);
+cudaError_t launch_map_scatter(const MapNode* d_nodes, const int2* d_blocks, const long long* d_offs, int b0, int b1, long long lo,
+                               long long hi, const MapArgs& a, void* d_out, cudaStream_t st);
 cudaError_t launch_refine_g2o(const PairDesc* pairs, int npairs, int max_matches, int iterations, const float4* mfrom,
                               const float4* mto, const int32_t* n_all, const rgbdslam_b200_dmatch* matches,
                               rgbdslam_b200_pair_result* results, rgbdslam_b200_dmatch* inlier_matches, cudaStream_t stream);

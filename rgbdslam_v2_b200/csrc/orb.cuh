@@ -49,4 +49,26 @@ struct OrbCand {   // a FAST corner that survived NMS, mask and the 15 px border
   uint16_t pad_;
 };
 
+// cvtColor(raw, rgb, COLOR_BayerGR2RGB) (openni_listener.cpp:638-641) at pixel (x, y) of the w x h mosaic at byte `frame` of
+// raw (G B on even rows, R G on odd rows), cv2 4.13's bilinear rule: an interior pixel keeps its own channel and averages the
+// others over pairs, (a + b + 1) >> 1, or over the cross / diagonal quads, (a + b + c + d + 2) >> 2; rows 0 and h-1 repeat rows
+// 1 and h-2, columns 0 and w-1 columns 1 and w-2.  Used by the grey conversion (orb.cu) and by the stored colour clouds (map.cu).
+#ifdef __CUDACC__
+__device__ __forceinline__ void bayer_gr_rgb(const uint8_t* __restrict__ raw, size_t frame, int w, int h, int x, int y, uint32_t& r,
+                                             uint32_t& g, uint32_t& b) {
+  const int sx = min(max(x, 1), w - 2), sy = min(max(y, 1), h - 2);
+  const uint8_t* p = raw + frame + (size_t)sy * w + sx;
+  const uint32_t c = p[0], up = p[-w], dn = p[w], lf = p[-1], rt = p[1];
+  const uint32_t pair_v = (up + dn + 1) >> 1, pair_h = (lf + rt + 1) >> 1, cross = (up + dn + lf + rt + 2) >> 2;
+  const uint32_t diag = (p[-w - 1] + p[-w + 1] + p[w - 1] + p[w + 1] + 2u) >> 2;
+  if (!(sy & 1)) {
+    if (!(sx & 1)) { r = pair_v; g = c; b = pair_h; }  // G, B to the sides
+    else { r = diag; g = cross; b = c; }               // B
+  } else {
+    if (!(sx & 1)) { r = c; g = cross; b = diag; }     // R
+    else { r = pair_h; g = c; b = pair_v; }            // G, R to the sides
+  }
+}
+#endif
+
 }  // namespace rb200

@@ -53,6 +53,15 @@ struct NodeDev {
   float K[4] = {0, 0, 0, 0};  // fx, fy, cx, cy of the full-resolution camera (kept clouds: the camera the model projects into)
   int32_t sift_kind = 0;      // SIFT nodes: 0 = RootSIFT rows + bf16 tiles, 1 = raw rows + u8 tiles (SiftGPU matcher)
   NodeSlab* slab = nullptr;   // desc / xyz / kp live inside this shared allocation (cloud_z is always separate)
+  // Stored colour cloud (RGBDSLAM_B200_STORE_CLOUD), the reference's Node::pc_col: colour words (b, g, r, a bytes) at pc_w x
+  // pc_h; depth-image nodes also keep pc_z, the z-plane of createXYZRGBPointCloud at every pc_step-th pixel (x / y follow from
+  // the pixel and pc_K = fx, fy, cx, cy); point-cloud nodes keep x / y / z in cloud_x / cloud_y / cloud_z, inside the same
+  // allocation.  All of it lives in pc_slab, shared by the nodes of one nodes_create_ex call.
+  float* pc_z = nullptr;
+  uint32_t* pc_rgb = nullptr;
+  int32_t pc_w = 0, pc_h = 0, pc_step = 0;
+  float pc_K[4] = {0, 0, 0, 0};
+  NodeSlab* pc_slab = nullptr;
 };
 
 constexpr int kSlots = 8;  // independent in-flight match_pairs pipelines (stream + workspace each)
