@@ -88,8 +88,9 @@ typedef struct rgbdslam_b200_params {
                                           * transformation_estimation.cpp:126-170); needs nodes with 2-D keypoints */
   /* Environment measurement model (node.cpp:1340-1342, misc.cpp:814-969, 1136-1148): > 0 enables it; an accepted RANSAC
    * transformation is kept only if inliers / (inliers + outliers) > threshold and inliers / (inl + outl + occluded) > 0.25.
-   * Needs nodes with a depth cloud (rgbdslam_b200_nodes_create keeps one when this is > 0, or rgbdslam_b200_node_set_depth), or
-   * point-cloud nodes built with RGBDSLAM_B200_KEEP_CLOUD; a pair must not mix the two kinds. */
+   * Needs nodes with a depth cloud (rgbdslam_b200_nodes_create keeps one when this is > 0 or with RGBDSLAM_B200_STORE_CLOUD, or
+   * rgbdslam_b200_node_set_depth), or point-cloud nodes built with RGBDSLAM_B200_KEEP_CLOUD or STORE_CLOUD; a pair must not mix
+   * the two kinds.  A depth cloud's z is (float)((double)depth * depth_scaling_factor), NaN where !(z >= minimum_depth). */
   double observability_threshold; /* -0.6 :114 (off) */
   int32_t emm_skip_step;          /* 8    :112       */
   int32_t cloud_creation_skip_step; /* 2  :36        */
@@ -182,12 +183,13 @@ int rgbdslam_b200_node_download(uint64_t node_handle, uint8_t* desc, float* xyz1
 /* == Node::~Node (node.cpp:371). */
 /* Give a node its point cloud (Node::pc_col) for the environment measurement model: the depth image in metres (row-major
  * w x h float, NaN = no measurement) and K4 = (fx, fy, cx, cy).  Only the z-plane of createXYZRGBPointCloud
- * (misc.cpp:467-556) at every params.cloud_creation_skip_step-th pixel is kept on the device. */
+ * (misc.cpp:467-556) at every params.cloud_creation_skip_step-th pixel is kept on the device; it replaces a z-plane the node
+ * had.  A node that keeps the cloud it was built from (RGBDSLAM_B200_KEEP_CLOUD or RGBDSLAM_B200_STORE_CLOUD) returns
+ * ERR_STATE before any device work. */
 int rgbdslam_b200_node_set_depth(uint64_t node_handle, const float* depth_m, int w, int h, const float K4[4]);
 /* == pairwiseObservationLikelihood(newer, older, mr) (node.cpp:1520-1554) for an explicit transformation T (Eigen::Matrix4f,
  * column-major, newer -> older frame): counts[4] = inlier, outlier, occluded, all points.  Both nodes have a depth cloud, or
- * both keep their organised cloud (RGBDSLAM_B200_KEEP_CLOUD); a mixed pair returns ERR_STATE.  node_set_depth on a node
- * that keeps its cloud returns ERR_STATE. */
+ * both keep their organised cloud (RGBDSLAM_B200_KEEP_CLOUD); a mixed pair returns ERR_STATE. */
 int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const float T[16], uint32_t counts[4]);
 /* Attach the 2-D keypoints (feature_locations_2d_, n entries) to a node created from features: only the pairwise g2o
  * refinement reads them (edgeToFeature, transformation_estimation.cpp:91-124).  Nodes built from images carry theirs. */
@@ -334,11 +336,11 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * descriptor i with another keypoint's point once compute() drops or re-orders keypoints, and its asserts at node.cpp:317-318
  * fail).  maximum_depth (parameter_server.cpp:38) is fixed at its default, +inf: no point is too far and a +inf z is kept.
  * K4 may be NULL; use_feature_min_depth and depth_scaling_factor are not read.  params.observability_threshold > 0 (the
- * environment measurement model, which needs a cloud per node) returns ERR_STATE for cloud input without KEEP_CLOUD.
+ * environment measurement model, which needs a cloud per node) returns ERR_STATE for cloud input without KEEP_CLOUD or STORE_CLOUD.
  *
  * RGBDSLAM_B200_KEEP_CLOUD (with a cloud bit only): the node keeps its organised cloud, the reference's pc_col (node.cpp:261,
  * kept when store_pointclouds or emm__skip_step is set, :344-350): x, y and z planes at full resolution on the device, 12 bytes
- * per point (3.7 MB at 640 x 480), de-interleaved from the uploaded cloud.  The environment measurement model then runs on
+ * per point (3.7 MB at 640 x 480), de-interleaved from the uploaded cloud by one kernel launch per chunk.  The environment measurement model then runs on
  * these clouds as observationLikelihood (misc.cpp:814-969) does when clouds are the input (topic_points set): every
  * emm_skip_step-th point of the full-resolution cloud, x / y / z as stored, cloud_creation_skip_step not applied (no division
  * of the intrinsics, no sigma scaling); a point with a non-finite coordinate is left untransformed, as
@@ -378,10 +380,11 @@ int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gr
  * VISUAL_BAYER_GR): channel 0 is blue (encoding_bgr, the reference default) or red (RGBDSLAM_B200_ENCODING_RGB), alpha 0, and
  * point 0 keeps colour 0 (misc.cpp:537).  8 bytes per point (614 kB per 640 x 480 node at skip step 2).  The skip step must
  * divide w and h.  Cloud input: the node keeps its organised cloud as KEEP_CLOUD does (also without that flag) plus the colour
- * word of each point (the float at byte 16 of PointXYZRGB, data[3] of PointXYZ), 16 bytes per point.  The planes of all nodes of
- * a call share one device allocation, made before any work is queued, and are written by one kernel launch per chunk from the
- * buffers the chunk already holds.  Features, detector thresholds and measurement-model counts are those of the same call
- * without the flag.
+ * word of each point (the float at byte 16 of PointXYZRGB, data[3] of PointXYZ), 16 bytes per point.  The stored cloud is the
+ * node's only cloud: the environment measurement model reads it, also when it is switched on after the node was built.  The
+ * planes of all nodes of a call share one device allocation, made before any work is queued, and are written by one kernel
+ * launch per chunk from the buffers the chunk already holds.  Features, detector thresholds and measurement-model counts are
+ * those of the same call without the flag.
  *
  * Rejected with ERR_ARG before any device work: unknown bits, CLOUD_XYZRGB with CLOUD_XYZ, MASK_FROM_CLOUD without a cloud
  * bit, MASK_FROM_DEPTH with a cloud bit, KEEP_CLOUD without a cloud bit, DEPTH_U16 or VISUAL_BAYER_GR with a cloud bit,

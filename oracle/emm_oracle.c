@@ -24,14 +24,14 @@ static double depth_cov(const oracle_params* p, double z) { /* misc2.h:20-35 inc
   return sd * sd;
 }
 
-void oracle_create_cloud_z(const float* depth, int w, int h, int step, float scaling, float min_depth, float* cloud_z) {
+void oracle_create_cloud_z(const float* depth, int w, int h, int step, double scaling, float min_depth, float* cloud_z) {
   int cw = (w + step - 1) / step, ch = (h + step - 1) / step;
   for (int ry = 0; ry < ch; ry++)
     for (int rx = 0; rx < cw; rx++) {
       int u = rx * step, v = ry * step;
       float z = NAN;
       if (u < w && v < h) {
-        float Z = depth[(size_t)v * w + u] * scaling;
+        float Z = (float)((double)depth[(size_t)v * w + u] * scaling); /* double depth_scaling (misc.cpp:502, 522) */
         if (Z >= min_depth) z = Z;
       }
       cloud_z[(size_t)ry * cw + rx] = z;

@@ -221,7 +221,7 @@ def create_cloud_z(depth, step=2, scaling=1.0, min_depth=0.1):
     d = np.ascontiguousarray(depth, np.float32)
     h, w = d.shape
     out = np.zeros(((h + step - 1) // step, (w + step - 1) // step), np.float32)
-    lib().oracle_create_cloud_z(_p(d), C.c_int(w), C.c_int(h), C.c_int(step), C.c_float(scaling), C.c_float(min_depth), _p(out))
+    lib().oracle_create_cloud_z(_p(d), C.c_int(w), C.c_int(h), C.c_int(step), C.c_double(scaling), C.c_float(min_depth), _p(out))
     return out
 
 

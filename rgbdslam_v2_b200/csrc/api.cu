@@ -177,21 +177,8 @@ static PairDesc make_pair(const NodeDev& a, const NodeDev& b) {
   pd.sift_kind = a.sift_kind;
   pd.q_kp = a.kp;
   pd.t_kp = b.kp;
-  pd.q_cloud = a.cloud_z;
-  pd.t_cloud = b.cloud_z;
-  pd.q_cloud_x = a.cloud_x;
-  pd.q_cloud_y = a.cloud_y;
-  pd.t_cloud_x = b.cloud_x;
-  pd.t_cloud_y = b.cloud_y;
-  pd.emm_cloud = a.cloud_x ? 1 : 0;
-  pd.q_cw = a.cw;
-  pd.q_ch = a.ch;
-  pd.t_cw = b.cw;
-  pd.t_ch = b.ch;
-  for (int k = 0; k < 4; k++) {
-    pd.q_K[k] = a.K[k];
-    pd.t_K[k] = b.K[k];
-  }
+  pd.q_cloud = a.pc.view();
+  pd.t_cloud = b.pc.view();
   return pd;
 }
 
@@ -347,10 +334,10 @@ static int check_pairs(const std::vector<PairDesc>& h_pairs, int64_t first_pair,
       }
   if (s.params.observability_threshold > 0.0)
     for (const PairDesc& pd : h_pairs)
-      if (!pd.q_cloud || !pd.t_cloud) {
+      if (!pd.q_cloud.z || !pd.t_cloud.z) {
         set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth)");
         return RGBDSLAM_B200_ERR_STATE;
-      } else if (!pd.q_cloud_x != !pd.t_cloud_x) {
+      } else if (!pd.q_cloud.x != !pd.t_cloud.x) {
         // the reference never holds both kinds in one process (topic_points is global): there is no rule to restate
         set_error("observability_threshold > 0: a pair mixes a node that keeps its point cloud (KEEP_CLOUD) with a depth-image node");
         return RGBDSLAM_B200_ERR_STATE;
@@ -477,7 +464,7 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
   }
   if (s.params.observability_threshold > 0.0) {  // node.cpp:1340-1342
     bool depth_pairs = false, cloud_pairs = false;
-    for (const PairDesc& pd : h_pairs) (pd.emm_cloud ? cloud_pairs : depth_pairs) = true;
+    for (const PairDesc& pd : h_pairs) (pd.q_cloud.x ? cloud_pairs : depth_pairs) = true;
     int emm_launches = 0;
     e = launch_emm_pairs(d_pairs, npairs, depth_pairs, cloud_pairs, s.params.cloud_creation_skip_step, s.params.emm_skip_step,
                          s.dp.cov_z_const, s.params.sigma_depth, s.params.observability_threshold,
@@ -512,56 +499,29 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
   return 0;
 }
 
+// drops one node's reference to a shared allocation
+static void release_slab(NodeSlab* slab) {
+  if (slab && --slab->refs == 0) {
+    cudaFree(slab->base);
+    delete slab;
+  }
+}
+
 // frees everything a (possibly half-built) node owns
 void free_node(NodeDev* nd) {
   nd->magic = 0;
   if (nd->slab) {
-    if (--nd->slab->refs == 0) {
-      cudaFree(nd->slab->base);
-      delete nd->slab;
-    }
+    release_slab(nd->slab);
   } else {
     if (nd->desc) cudaFree(nd->desc);
     if (nd->xyz) cudaFree(nd->xyz);
     if (nd->desc_i8) cudaFree(nd->desc_i8);
     if (nd->kp) cudaFree(nd->kp);
   }
-  free_node_cloud(nd);
-  if (nd->pc_slab && --nd->pc_slab->refs == 0) {
-    cudaFree(nd->pc_slab->base);
-    delete nd->pc_slab;
-  }
+  release_slab(nd->pc.slab);
   if (nd->desc_f32) cudaFree(nd->desc_f32);
   if (nd->norms) cudaFree(nd->norms);
   delete nd;
-}
-
-void free_node_cloud(NodeDev* nd) {
-  if (nd->cloud_x) {
-    if (!nd->pc_slab) cudaFree(nd->cloud_x);  // x | y | z planes of a kept cloud (a stored cloud's live in pc_slab)
-  }
-  else if (nd->cloud_z) cudaFree(nd->cloud_z);
-  nd->cloud_x = nd->cloud_y = nd->cloud_z = nullptr;
-}
-
-int node_build_cloud(NodeDev* nd, const float* d_depth, int w, int h, const float K4[4], cudaStream_t st) {
-  State& s = g_state;
-  const int step = s.params.cloud_creation_skip_step > 0 ? s.params.cloud_creation_skip_step : 1;
-  const int cw = (w + step - 1) / step, ch = (h + step - 1) / step;  // ceil(cols / skip), misc.cpp:482-483
-  if (nd->cloud_z && (nd->cw != cw || nd->ch != ch)) {
-    cudaFree(nd->cloud_z);
-    nd->cloud_z = nullptr;
-  }
-  cudaError_t e = cudaSuccess;
-  if (!nd->cloud_z) e = cudaMalloc(&nd->cloud_z, sizeof(float) * (size_t)cw * ch);
-  if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(cloud)");
-  nd->cw = cw;
-  nd->ch = ch;
-  for (int k = 0; k < 4; k++) nd->K[k] = K4[k];
-  e = launch_build_cloud(d_depth, w, h, step, (float)s.params.depth_scaling_factor, s.params.minimum_depth, nd->cloud_z, cw, ch, st);
-  if (e != cudaSuccess) return cuda_fail(e, "build_cloud kernel");
-  s.launches += 1;
-  return 0;
 }
 
 }  // namespace rb200
@@ -729,15 +689,40 @@ int rgbdslam_b200_node_set_depth(uint64_t node_handle, const float* depth_m, int
     set_error("node_set_depth: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if (nd->cloud_x) {
+  NodeCloud& c = nd->pc;
+  if (c.x) {
     set_error("node_set_depth: the node keeps the organised cloud it was built from (KEEP_CLOUD)");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
+  if (c.rgb) {
+    set_error("node_set_depth: the node keeps the colour cloud it was built from (STORE_CLOUD)");
     return RGBDSLAM_B200_ERR_STATE;
   }
   State& s = g_state;
   int rc;
   if ((rc = s.d_f32_a.ensure(sizeof(float) * (size_t)w * h))) return rc;
   RB200_CUDA(cudaMemcpyAsync(s.d_f32_a.ptr, depth_m, sizeof(float) * (size_t)w * h, cudaMemcpyHostToDevice, s.stream));
-  if ((rc = node_build_cloud(nd, (const float*)s.d_f32_a.ptr, w, h, K4, s.stream))) return rc;
+  const int step = s.params.cloud_creation_skip_step > 0 ? s.params.cloud_creation_skip_step : 1;
+  const int cw = (w + step - 1) / step, ch = (h + step - 1) / step;  // ceil(cols / skip), misc.cpp:482-483
+  if (!(c.slab && c.slab->refs == 1 && c.w == cw && c.h == ch)) {  // else the node alone owns a z-plane of this raster
+    NodeSlab* slab = new NodeSlab();
+    cudaError_t e = cudaMalloc(&slab->base, sizeof(float) * (size_t)cw * ch);
+    if (e != cudaSuccess) {
+      delete slab;
+      return cuda_fail(e, "cudaMalloc(cloud)");
+    }
+    slab->refs = 1;
+    release_slab(c.slab);
+    c.slab = slab;
+    c.z = (float*)slab->base;
+    c.w = cw;
+    c.h = ch;
+  }
+  c.step = step;
+  for (int k = 0; k < 4; k++) c.K[k] = K4[k];
+  RB200_CUDA(launch_store_depth_cloud(1, (const float*)s.d_f32_a.ptr, nullptr, 0, false, w, h, step, s.params.depth_scaling_factor,
+                                      s.params.minimum_depth, c.z, (size_t)cw * ch, s.stream));
+  s.launches += 1;
   RB200_CUDA(cudaStreamSynchronize(s.stream));
   return 0;
 }
@@ -751,11 +736,12 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
     set_error("observation_likelihood: bad arguments");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if (!a->cloud_z || !b->cloud_z) {
-    set_error("observation_likelihood: both nodes need a depth cloud (nodes_create with observability_threshold > 0 or node_set_depth)");
+  if (!a->pc.z || !b->pc.z) {
+    set_error("observation_likelihood: both nodes need a depth cloud (nodes_create with observability_threshold > 0 or STORE_CLOUD, "
+              "or node_set_depth)");
     return RGBDSLAM_B200_ERR_STATE;
   }
-  if (!a->cloud_x != !b->cloud_x) {
+  if (!a->pc.x != !b->pc.x) {
     set_error("observation_likelihood: a node that keeps its point cloud (KEEP_CLOUD) and a depth-image node cannot be compared");
     return RGBDSLAM_B200_ERR_STATE;
   }
@@ -770,10 +756,8 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
   if ((rc = s.d_f32_b.ensure(128))) return rc;
   cudaError_t e = cudaMemcpyAsync(s.d_f32_b.ptr, T, 64, cudaMemcpyHostToDevice, s.stream);
   if (e == cudaSuccess)
-    e = launch_emm_single(EmmNode{a->cloud_z, a->cloud_x, a->cloud_y, a->cw, a->ch, a->K},
-                          EmmNode{b->cloud_z, b->cloud_x, b->cloud_y, b->cw, b->ch, b->K}, a->cloud_x != nullptr,
-                          (const float*)s.d_f32_b.ptr, s.params.cloud_creation_skip_step, s.params.emm_skip_step, s.dp.cov_z_const,
-                          s.params.sigma_depth, (unsigned*)((char*)s.d_f32_b.ptr + 64), s.stream);
+    e = launch_emm_single(a->pc.view(), b->pc.view(), (const float*)s.d_f32_b.ptr, s.params.cloud_creation_skip_step,
+                          s.params.emm_skip_step, s.dp.cov_z_const, s.params.sigma_depth, (unsigned*)((char*)s.d_f32_b.ptr + 64), s.stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(counts, (char*)s.d_f32_b.ptr + 64, 16, cudaMemcpyDeviceToHost, s.stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
   if (e != cudaSuccess) return cuda_fail(e, "observation_likelihood");

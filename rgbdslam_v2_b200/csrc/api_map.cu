@@ -38,23 +38,20 @@ static int map_ensure_streams() {
 
 // The stored cloud of nd as the map kernels read it, with transform T (row-major 3 x 4 float; may be NULL).
 static MapNode map_node(const NodeDev* nd, const float* T) {
+  const NodeCloud& c = nd->pc;
   MapNode m;
   memset(&m, 0, sizeof(m));
-  m.rgb = nd->pc_rgb;
-  m.cw = nd->pc_w;
-  m.ch = nd->pc_h;
-  m.step = nd->pc_step;
-  if (nd->pc_z) {
-    m.z = nd->pc_z;
-    m.fxinv = (float)(1.0 / (double)nd->pc_K[0]);  // getCameraIntrinsicsInverseFocalLength (misc.cpp:64-69)
-    m.fyinv = (float)(1.0 / (double)nd->pc_K[1]);
-    m.cx = nd->pc_K[2];
-    m.cy = nd->pc_K[3];
-  } else {
-    m.x = nd->cloud_x;
-    m.y = nd->cloud_y;
-    m.z = nd->cloud_z;
-  }
+  m.x = c.x;
+  m.y = c.y;
+  m.z = c.z;
+  m.rgb = c.rgb;
+  m.cw = c.w;
+  m.ch = c.h;
+  m.step = c.step;
+  m.fxinv = (float)(1.0 / (double)c.K[0]);  // getCameraIntrinsicsInverseFocalLength (misc.cpp:64-69); unused by organised clouds
+  m.fyinv = (float)(1.0 / (double)c.K[1]);
+  m.cx = c.K[2];
+  m.cy = c.K[3];
   if (T) memcpy(m.m, T, sizeof(m.m));
   return m;
 }
@@ -143,16 +140,16 @@ int rgbdslam_b200_node_download_cloud(uint64_t node_handle, int point_bytes, voi
     set_error("node_download_cloud: point_bytes must be 16 or 32, w and h non-null");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if (!nd->pc_rgb) {
+  if (!nd->pc.rgb) {
     set_error("node_download_cloud: the node has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
     return RGBDSLAM_B200_ERR_STATE;
   }
-  *w = nd->pc_w;
-  *h = nd->pc_h;
+  *w = nd->pc.w;
+  *h = nd->pc.h;
   if (!out) return 0;
   const MapArgs a{0.f, 0, 1, 0, point_bytes};  // every point, as stored
   int64_t n = 0;
-  return map_emit(std::vector<MapNode>(1, map_node(nd, nullptr)), a, out, (int64_t)nd->pc_w * nd->pc_h, &n);
+  return map_emit(std::vector<MapNode>(1, map_node(nd, nullptr)), a, out, (int64_t)nd->pc.w * nd->pc.h, &n);
 }
 
 int rgbdslam_b200_render_cloud(int n, const uint64_t* nodes, const double* transforms12, double maximum_depth, int preserve_raster,
@@ -175,7 +172,7 @@ int rgbdslam_b200_render_cloud(int n, const uint64_t* nodes, const double* trans
   for (int k = 0; k < n; k++) {
     NodeDev* nd = get_node(nodes[k]);
     if (!nd) return RGBDSLAM_B200_ERR_ARG;
-    if (!nd->pc_rgb) {
+    if (!nd->pc.rgb) {
       set_error("render_cloud: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
       return RGBDSLAM_B200_ERR_STATE;
     }

@@ -425,14 +425,11 @@ struct NodeBatch {
   int* n = nullptr;
   size_t n_bytes = 0;
   rgbdslam_b200_keypoint* kp = nullptr;
-  std::vector<NodeDev*> made;  // nodes that own device memory before they are published (depth or kept clouds)
-  // RGBDSLAM_B200_STORE_CLOUD: one allocation for the stored clouds of all nodes, pc_node_bytes per node -- depth-image input
-  // [z | colour] at pc_w x pc_h, cloud input [x | y | z | colour] at w x h
-  NodeSlab* pc_slab = nullptr;
-  size_t pc_node_bytes = 0;
-  bool pc_cloud = false;
-  int pc_w = 0, pc_h = 0, pc_step = 0;
-  float pc_K[4] = {0, 0, 0, 0};
+  // Node::pc_col of every node in one more allocation (pc.slab; none when the call keeps no cloud), pc_node_words 4-byte words
+  // per node: depth-image input [z] at the skip-step raster, cloud input [x | y | z] at w x h, each plus [colour] for
+  // STORE_CLOUD.  pc holds frame 0's planes.
+  NodeCloud pc;
+  size_t pc_node_words = 0;
 };
 
 static int batch_alloc(NodeBatch& nb, int nodes, int kp_frames, int K) {
@@ -459,15 +456,11 @@ static int batch_alloc(NodeBatch& nb, int nodes, int kp_frames, int K) {
 static int batch_fail(NodeBatch& nb, int code) {
   cudaStreamSynchronize(g_orb.copy_stream);
   cudaStreamSynchronize(g_state.stream);
-  for (NodeDev* x : nb.made) {
-    free_node_cloud(x);
-    delete x;
-  }
   cudaFree(nb.slab->base);
   delete nb.slab;
-  if (nb.pc_slab) {
-    cudaFree(nb.pc_slab->base);
-    delete nb.pc_slab;
+  if (nb.pc.slab) {
+    cudaFree(nb.pc.slab->base);
+    delete nb.pc.slab;
   }
   return code;
 }
@@ -584,7 +577,7 @@ static int batch_publish(NodeBatch& nb, int nframes, int kp_first, int kp_frames
   if (int rc = orb_check_err_flag(flag)) return batch_fail(nb, rc);
   const int K = nb.K, Kpad = ((K > 0 ? K : 1) + 255) / 256 * 256;
   for (int f = 0; f < nframes; f++) {
-    NodeDev* nd = nb.made.empty() ? new NodeDev() : nb.made[f];
+    NodeDev* nd = new NodeDev();
     nd->magic = NodeDev::kMagic;
     nd->id = ids ? ids[f] : f;
     nd->n = n[f];
@@ -594,27 +587,14 @@ static int batch_publish(NodeBatch& nb, int nframes, int kp_first, int kp_frames
     nd->kp = (f >= kp_first && f < kp_first + kp_frames) ? nb.kp + (size_t)(f - kp_first) * K : nullptr;
     nd->slab = nb.slab;
     nb.slab->refs++;
-    if (nb.pc_slab) {
-      uint8_t* base = (uint8_t*)nb.pc_slab->base + nb.pc_node_bytes * f;
-      const size_t P = (size_t)nb.pc_w * nb.pc_h;
-      if (nb.pc_cloud) {  // the kept organised cloud (KEEP_CLOUD's planes) plus the colour words
-        nd->cloud_x = (float*)base;
-        nd->cloud_y = nd->cloud_x + P;
-        nd->cloud_z = nd->cloud_x + 2 * P;
-        nd->cw = nb.pc_w;
-        nd->ch = nb.pc_h;
-        for (int k = 0; k < 4; k++) nd->K[k] = nb.pc_K[k];
-        nd->pc_rgb = (uint32_t*)(base + 12 * P);
-      } else {
-        nd->pc_z = (float*)base;
-        nd->pc_rgb = (uint32_t*)(base + 4 * P);
-      }
-      nd->pc_w = nb.pc_w;
-      nd->pc_h = nb.pc_h;
-      nd->pc_step = nb.pc_step;
-      for (int k = 0; k < 4; k++) nd->pc_K[k] = nb.pc_K[k];
-      nd->pc_slab = nb.pc_slab;
-      nb.pc_slab->refs++;
+    if (nb.pc.slab) {
+      NodeCloud& c = nd->pc;
+      c = nb.pc;
+      const size_t off = nb.pc_node_words * f;
+      for (float** plane : {&c.x, &c.y, &c.z})
+        if (*plane) *plane += off;
+      if (c.rgb) c.rgb += off;
+      nb.pc.slab->refs++;
     }
     node_handles[f] = (uint64_t)(uintptr_t)nd;
     if (n_features) n_features[f] = n[f];
@@ -788,7 +768,7 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   State& s = g_state;
   const size_t px = (size_t)w * h;
   const FrameInput in(flags, px, s.params, K4, mask);
-  const bool store = (flags & RGBDSLAM_B200_STORE_CLOUD) != 0;
+  const bool store = (flags & RGBDSLAM_B200_STORE_CLOUD) != 0, model = s.params.observability_threshold > 0.0;
   // a stored cloud of cloud input is the kept cloud plus colour: the measurement model reads it as it reads KEEP_CLOUD's
   const bool keep_cloud = (flags & RGBDSLAM_B200_KEEP_CLOUD) != 0 || (store && in.cloud_stride);
   const int pc_step = s.params.cloud_creation_skip_step > 0 ? s.params.cloud_creation_skip_step : 1;
@@ -797,7 +777,7 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     set_error("nodes_create: STORE_CLOUD needs a cloud_creation_skip_step that divides the image width and height");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if (in.cloud_stride && !keep_cloud && s.params.observability_threshold > 0.0) {
+  if (in.cloud_stride && !keep_cloud && model) {
     set_error("nodes_create: the environment measurement model needs the point cloud on the node (observability_threshold > 0): "
               "pass RGBDSLAM_B200_KEEP_CLOUD");
     return RGBDSLAM_B200_ERR_STATE;
@@ -813,32 +793,30 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   const int K = std::min(o.kp_stride, s.params.max_keypoints);  // features per node (finalize mode 1 emits <= max_keypoints)
   NodeBatch nb;
   if ((rc = batch_alloc(nb, nframes, nframes, K))) return rc;
-  if (store) {  // Node::pc_col (node.cpp:126-131, 261) of every frame in one allocation, made before any work is queued
-    nb.pc_cloud = in.cloud_stride != 0;
-    nb.pc_w = nb.pc_cloud ? w : w / pc_step;
-    nb.pc_h = nb.pc_cloud ? h : h / pc_step;
-    nb.pc_step = nb.pc_cloud ? 0 : pc_step;
-    for (int k = 0; k < 4; k++) nb.pc_K[k] = K4 ? K4[k] : 0.f;
-    nb.pc_node_bytes = ((size_t)nb.pc_w * nb.pc_h * (nb.pc_cloud ? 16 : 8) + 255) / 256 * 256;
-    nb.pc_slab = new NodeSlab();
-    cudaError_t e = cudaMalloc(&nb.pc_slab->base, nb.pc_node_bytes * nframes);
+  if (store || keep_cloud || model) {  // Node::pc_col (node.cpp:126-131, 261) of every frame, allocated before any work is queued
+    NodeCloud& c = nb.pc;
+    c.step = in.cloud_stride ? 0 : pc_step;
+    c.w = in.cloud_stride ? w : (w + pc_step - 1) / pc_step;  // ceil(cols / skip), misc.cpp:482-483
+    c.h = in.cloud_stride ? h : (h + pc_step - 1) / pc_step;
+    // kept clouds: the camera the model projects into, depth_camera_fx ... cy, 0 when unset (misc.cpp:56-63)
+    for (int k = 0; k < 4; k++) c.K[k] = K4 ? K4[k] : 0.f;
+    const size_t P = (size_t)c.w * c.h;
+    nb.pc_node_words = (P * ((in.cloud_stride ? 3 : 1) + (store ? 1 : 0)) + 63) / 64 * 64;
+    c.slab = new NodeSlab();
+    cudaError_t e = cudaMalloc(&c.slab->base, 4 * nb.pc_node_words * nframes);
     if (e != cudaSuccess) {
-      delete nb.pc_slab;
-      nb.pc_slab = nullptr;
-      return batch_fail(nb, cuda_fail(e, "cudaMalloc(stored clouds)"));
+      delete c.slab;
+      c.slab = nullptr;
+      return batch_fail(nb, cuda_fail(e, "cudaMalloc(node clouds)"));
     }
-  } else if (keep_cloud) {  // Node::pc_col (node.cpp:261): x / y / z planes of every frame, allocated before any work is queued
-    for (int f = 0; f < nframes; f++) {
-      NodeDev* nd = new NodeDev();
-      nb.made.push_back(nd);
-      cudaError_t e = cudaMalloc(&nd->cloud_x, 3 * sizeof(float) * px);
-      if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "cudaMalloc(kept cloud)"));
-      nd->cloud_y = nd->cloud_x + px;
-      nd->cloud_z = nd->cloud_x + 2 * px;
-      nd->cw = w;
-      nd->ch = h;
-      for (int k = 0; k < 4; k++) nd->K[k] = K4 ? K4[k] : 0.f;  // depth_camera_fx ... cy, 0 when unset (misc.cpp:56-63)
+    float* planes = (float*)c.slab->base;
+    if (in.cloud_stride) {
+      c.x = planes;
+      c.y = planes + P;
+      planes += 2 * P;
     }
+    c.z = planes;
+    if (store) c.rgb = (uint32_t*)(planes + P);
   }
   bool pinned = false;
   if ((rc = setup_staging(gray, depth, mask, px, in, chunk, &pinned))) return batch_fail(nb, rc);
@@ -866,32 +844,18 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     const FeatureRows rows = {nb.kp + (size_t)f0 * K, nb.xyz + (size_t)f0 * K, nb.n + f0, nb.desc + (size_t)f0 * K * 32, K};
     if ((rc = select_describe(det, in, F, (const uint8_t*)o.cell_img.ptr, o.candidates(), dd, dg, rows, st, &launches)))
       return batch_fail(nb, rc);
-    if (store) {  // createXYZRGBPointCloud of the chunk's frames from the buffers it holds (misc.cpp:467-556, node.cpp:261)
-      float* pc = (float*)((uint8_t*)nb.pc_slab->base + nb.pc_node_bytes * f0);
-      const size_t words = nb.pc_node_bytes / 4;
+    if (nb.pc.slab) {  // createXYZRGBPointCloud of the chunk's frames from the buffers it holds (misc.cpp:467-556, node.cpp:261)
+      const size_t words = nb.pc_node_words;
       if (in.cloud_stride) {
-        e = launch_store_cloud_points(F, dd, in.cloud_stride, (int)px, pc, words, st);
+        e = launch_store_cloud_points(F, dd, in.cloud_stride, (int)px, store, nb.pc.x + words * f0, words, st);
       } else {
         const int vis = in.bayer ? 2 : in.rgb ? 1 : 0;
-        e = launch_store_depth_cloud(F, dd, vis ? drgb : dg, vis, (flags & RGBDSLAM_B200_ENCODING_RGB) == 0, w, h, pc_step,
-                                     s.params.depth_scaling_factor, s.params.minimum_depth, pc, words, st);
+        e = launch_store_depth_cloud(F, dd, store ? (vis ? drgb : dg) : nullptr, vis, (flags & RGBDSLAM_B200_ENCODING_RGB) == 0, w,
+                                     h, pc_step, s.params.depth_scaling_factor, s.params.minimum_depth, nb.pc.z + words * f0, words,
+                                     st);
       }
       if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "store_cloud kernel"));
       launches += 1;
-    }
-    if (keep_cloud && !store) {
-      for (int f = 0; f < F; f++) {
-        NodeDev* nd = nb.made[f0 + f];
-        e = launch_split_cloud((const float*)((const uint8_t*)dd + in.plane_bytes * f), in.cloud_stride, (int)px, nd->cloud_x,
-                               nd->cloud_y, nd->cloud_z, st);
-        if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "split_cloud kernel"));
-      }
-      launches += F;
-    } else if (!keep_cloud && s.params.observability_threshold > 0.0) {  // Node::pc_col for the environment measurement model
-      for (int f = 0; f < F; f++) {
-        nb.made.push_back(new NodeDev());
-        if ((rc = node_build_cloud(nb.made.back(), dd + (size_t)f * px, w, h, K4, st))) return batch_fail(nb, rc);
-      }
     }
     e = cudaEventRecord(o.ev_free[b], st);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "nodes_create events"));

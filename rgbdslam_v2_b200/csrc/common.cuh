@@ -11,6 +11,22 @@ constexpr int kMaxMatchesCap = RGBDSLAM_B200_MAX_MATCHES_CAP;  // 512
 constexpr int kMaxMaskWords = kMaxMatchesCap / 32;             // 16
 constexpr int kMaxFeatures = 4096;                             // per node (SiftGPU limit too: sift_gpu_wrapper.cpp:231)
 
+// One node's point cloud as the kernels read it: the z-plane of a depth-image node at the cloud_creation_skip_step raster, or
+// the x / y / z planes of an organised cloud (x != nullptr).  z == nullptr: the node has no cloud.
+struct CloudView {
+  const float *z, *x, *y;
+  int32_t w, h;
+  float K[4];  // fx, fy, cx, cy of the full-resolution camera (organised clouds: the camera the model projects into)
+};
+
+// x / y of a depth-image cloud's point at pixel (u, v) with z-plane value z, as createXYZRGBPointCloud back-projects it
+// (misc.cpp:525-533, misc2.h:62-64): a NaN z keeps x / y of the 1 m ray.  One rounding per operation: the reference does not
+// contract.
+__device__ __forceinline__ float2 depth_point_xy(float u, float v, float z, float cx, float cy, float fxinv, float fyinv) {
+  const float zs = isnan(z) ? 1.0f : z;
+  return make_float2(__fmul_rn(__fmul_rn(__fsub_rn(u, cx), zs), fxinv), __fmul_rn(__fmul_rn(__fsub_rn(v, cy), zs), fyinv));
+}
+
 // One frame pair as the kernels see it (device pointers).
 struct PairDesc {
   const uint32_t* q_desc;  // newer node descriptors, nq x 8 u32 (16 B aligned)
@@ -26,17 +42,10 @@ struct PairDesc {
   const float* t_norm;
   const rgbdslam_b200_keypoint* q_kp;  // 2-D keypoints (nullptr unless the node has them): pairwise g2o refinement only
   const rgbdslam_b200_keypoint* t_kp;
-  const float* q_cloud;  // depth-cloud z-planes (environment measurement model), nullptr if the node has none
-  const float* t_cloud;
-  const float* q_cloud_x;  // kept organised clouds (RGBDSLAM_B200_KEEP_CLOUD): x / y planes, nullptr for depth-image nodes
-  const float* q_cloud_y;
-  const float* t_cloud_x;
-  const float* t_cloud_y;
-  int32_t q_cw, q_ch, t_cw, t_ch;
-  float q_K[4], t_K[4];  // fx, fy, cx, cy of the full-resolution cameras (kept clouds: the camera the model projects into)
+  CloudView q_cloud, t_cloud;  // environment measurement model (match_pairs* only runs it on pairs of one cloud kind)
   int32_t sift_kind;   // float-descriptor nodes: 0 = RootSIFT / exact 2-NN ratio matcher, 1 = SiftGPU matcher (u8 tiles, raw rows)
-  int32_t emm_cloud;   // 1: the newer node keeps its organised cloud (match_pairs* only runs the model on pairs of one kind)
 };
+static_assert(sizeof(PairDesc) == 208, "PairDesc layout");
 
 // One work item of the tensor-core match kernels = 256 queries of one pair against all train rows.
 struct HamItem {

@@ -1,65 +1,16 @@
 // emm.cu -- Environment Measurement Model (SURVEY.md 8f rank 3; parameter observability_threshold > 0):
-//   k_build_cloud        the z-plane of createXYZRGBPointCloud (misc.cpp:467-556): every cloud_creation_skip_step-th pixel,
-//                        NaN where !(Z >= minimum_depth); x / y are recomputed from the pixel grid (backProject, misc2.h:49-65)
-//   k_split_cloud        Node::pc_col of the point-cloud constructor (node.cpp:261): x / y / z planes of an organised cloud
 //   k_emm_pairs          pairwiseObservationLikelihood (node.cpp:1520-1554) = observationLikelihood (misc.cpp:814-969) in both
 //                        directions + observation_criterion_met (misc.cpp:1136-1148) applied to the pair result
-// Both EMM kernels are instantiated per point source (EmmPoints): depth-image nodes (the sub-sampled z-plane) and nodes that
-// keep the organised cloud of the point-cloud constructor (RGBDSLAM_B200_KEEP_CLOUD).
+//   k_emm_single         the same for one pair and an explicit transformation (rgbdslam_b200_observation_likelihood)
+// The clouds are the nodes' pc_col, built by map.cu.  Both kernels are instantiated per point source (EmmPoints): depth-image
+// nodes (the sub-sampled z-plane; x / y are recomputed from the pixel grid, backProject, misc2.h:49-65) and nodes that keep the
+// organised cloud of the point-cloud constructor (RGBDSLAM_B200_KEEP_CLOUD).
 // Dense projective data association on the sub-sampled clouds: embarrassingly parallel per sampled pixel, HBM / latency bound
 // (<= 9 random depth reads per sample, 2 x (W/s/k) x (H/s/k) samples per pair: 2400 at the defaults s = 2, k = 8; kept clouds
 // are sampled at full resolution, s = 1: 9600).
 #include "kernels.h"
 
 namespace rb200 {
-
-
-__global__ void __launch_bounds__(256) k_build_cloud(const float* __restrict__ depth, int w, int h, int step, float scaling,
-                                                     float min_depth, float* __restrict__ cloud_z, int cw, int ch) {
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= cw * ch) return;
-  const int rx = i % cw, ry = i / cw;
-  const int u = rx * step, v = ry * step;
-  float z = __int_as_float(0x7fc00000);
-  if (u < w && v < h) {
-    const float Z = depth[(size_t)v * w + u] * scaling;  // misc.cpp:520
-    if (Z >= min_depth) z = Z;                            // :523 (also rejects NaN)
-  }
-  cloud_z[i] = z;
-}
-
-cudaError_t launch_build_cloud(const float* d_depth, int w, int h, int step, float scaling, float min_depth, float* cloud_z, int cw,
-                               int ch, cudaStream_t stream) {
-  if (cw <= 0 || ch <= 0) return cudaSuccess;
-  k_build_cloud<<<(cw * ch + 255) / 256, 256, 0, stream>>>(d_depth, w, h, step, scaling, min_depth, cloud_z, cw, ch);
-  return cudaGetLastError();
-}
-
-// De-interleave one organised cloud (n points of `stride` floats, x / y / z at 0 / 1 / 2) into three planes.
-__global__ void __launch_bounds__(256) k_split_cloud(const float* __restrict__ cloud, int stride, int n, float* __restrict__ x,
-                                                     float* __restrict__ y, float* __restrict__ z) {
-  const int i = blockIdx.x * 256 + threadIdx.x;
-  if (i >= n) return;
-  const float* p = cloud + (size_t)i * stride;
-  x[i] = p[0];
-  y[i] = p[1];
-  z[i] = p[2];
-}
-
-cudaError_t launch_split_cloud(const float* d_cloud, int stride, int n, float* x, float* y, float* z, cudaStream_t stream) {
-  if (n <= 0) return cudaSuccess;
-  k_split_cloud<<<(n + 255) / 256, 256, 0, stream>>>(d_cloud, stride, n, x, y, z);
-  return cudaGetLastError();
-}
-
-struct EmmView {
-  const float* z;   // cloud z-plane
-  const float* x;   // kept clouds (EmmPoints::kCloud) only: x / y planes of the organised cloud
-  const float* y;
-  int cw, ch;
-  float fx, fy, cx, cy;  // depth nodes: full-resolution intrinsics of the camera that took it; kept clouds: the camera the
-                         // model projects into (the reference's depth_camera_fx / fy / cx / cy)
-};
 
 __device__ __forceinline__ int round_like_ref(float d) { return (int)floor((double)d + 0.5); }  // misc.cpp:804-807
 // The same as x86-64 evaluates it: cvttsd2si gives INT_MIN for NaN, +-inf and values outside int32, and INT_MIN fails the
@@ -88,24 +39,24 @@ enum class EmmPoints {
 };
 
 template <EmmPoints P>
-__device__ void emm_direction(const EmmView& src, const EmmView& dst, const float R[9], const float t[3], int cloud_step_param,
+__device__ void emm_direction(const CloudView& src, const CloudView& dst, const float R[9], const float t[3], int cloud_step_param,
                               int skip_step, double cov_z_const, double sigma_depth, unsigned& good, unsigned& bad, unsigned& occl,
                               unsigned& all) {
   constexpr bool kCloud = P == EmmPoints::kCloud;
   // a direction whose two clouds differ in width contributes nothing, not even to `all` (misc.cpp:844-847).  The
   // `width <= 1 || height <= 1` branch before it (:836-843) is unreachable: nodes_create* rejects frames below 96 px for
   // both detectors (orb_prepare), and clouds only come from there.
-  if (kCloud && src.cw != dst.cw) return;
+  if (kCloud && src.w != dst.w) return;
   const int cloud_step = kCloud ? 1 : cloud_step_param;
-  const float sfxinv = (float)(1.0 / (double)src.fx), sfyinv = (float)(1.0 / (double)src.fy);  // misc.cpp:64-69
+  const float sfxinv = (float)(1.0 / (double)src.K[0]), sfyinv = (float)(1.0 / (double)src.K[1]);  // misc.cpp:64-69
   // "downsampled cloud?" branch (misc.cpp:854-861): intrinsics of the raster the old cloud lives on
-  const float fx = kCloud ? dst.fx : dst.fx / cloud_step, fy = kCloud ? dst.fy : dst.fy / cloud_step;
-  const float cx = kCloud ? dst.cx : dst.cx / cloud_step, cy = kCloud ? dst.cy : dst.cy / cloud_step;
-  const int nsx = (src.cw + skip_step - 1) / skip_step, nsy = (src.ch + skip_step - 1) / skip_step;
+  const float fx = kCloud ? dst.K[0] : dst.K[0] / cloud_step, fy = kCloud ? dst.K[1] : dst.K[1] / cloud_step;
+  const float cx = kCloud ? dst.K[2] : dst.K[2] / cloud_step, cy = kCloud ? dst.K[3] : dst.K[3] / cloud_step;
+  const int nsx = (src.w + skip_step - 1) / skip_step, nsy = (src.h + skip_step - 1) / skip_step;
   for (int sidx = threadIdx.x; sidx < nsx * nsy; sidx += blockDim.x) {
     all++;  // the loop header increments `all` for every sampled raster cell (:872)
     const int rx = (sidx % nsx) * skip_step, ry = (sidx / nsx) * skip_step;
-    const size_t si = (size_t)ry * src.cw + rx;
+    const size_t si = (size_t)ry * src.w + rx;
     float qx, qy, qz;
     if (kCloud) {
       // the stored point; pcl::transformPointCloud on a cloud that is not dense copies the input and leaves a point with any
@@ -121,13 +72,10 @@ __device__ void emm_direction(const EmmView& src, const EmmView& dst, const floa
         qz = pz;
       }
     } else {
-      const float Z = src.z[si];
-      // the source point: NaN depth keeps x / y of the 1 m ray (misc.cpp:525-529) -> the transformed z is NaN as well
-      const float u = (float)(rx * cloud_step), v = (float)(ry * cloud_step);
-      const float zs = isnan(Z) ? 1.0f : Z;
-      const float px = __fmul_rn(__fmul_rn(__fsub_rn(u, src.cx), zs), sfxinv);
-      const float py = __fmul_rn(__fmul_rn(__fsub_rn(v, src.cy), zs), sfyinv);
-      const float pz = Z;
+      // the source point; a NaN depth gives a NaN transformed z as well
+      const float pz = src.z[si];
+      const float2 pxy = depth_point_xy((float)(rx * cloud_step), (float)(ry * cloud_step), pz, src.K[2], src.K[3], sfxinv, sfyinv);
+      const float px = pxy.x, py = pxy.y;
       qx = __fadd_rn(dot3_rn(R[0], px, R[1], py, R[2], pz), t[0]);  // pcl::transformPointCloud
       qy = __fadd_rn(dot3_rn(R[3], px, R[4], py, R[5], pz), t[1]);
       qz = __fadd_rn(dot3_rn(R[6], px, R[7], py, R[8], pz), t[2]);
@@ -137,14 +85,14 @@ __device__ void emm_direction(const EmmView& src, const EmmView& dst, const floa
     const float xc = __fadd_rn(__fmul_rn(__fdiv_rn(qx, qz), fx), cx), yc = __fadd_rn(__fmul_rn(__fdiv_rn(qy, qz), fy), cy);
     const int ocx = kCloud ? round_x86(xc) : round_like_ref(xc);
     const int ocy = kCloud ? round_x86(yc) : round_like_ref(yc);
-    if (ocx >= dst.cw || ocx < 0 || ocy >= dst.ch || ocy < 0) continue;
+    if (ocx >= dst.w || ocx < 0 || ocy >= dst.h || ocy < 0) continue;
     const int nbhd = 2;
     bool good_point = false, occluded_point = false, bad_point = false;
     const int startx = max(0, ocx - nbhd), starty = max(0, ocy - nbhd);
-    const int endx = min(dst.cw, ocx + nbhd + 1), endy = min(dst.ch, ocy + nbhd + 1);
+    const int endx = min(dst.w, ocx + nbhd + 1), endy = min(dst.h, ocy + nbhd + 1);
     for (int oy = starty; oy < endy; oy += 2)
       for (int ox = startx; ox < endx; ox += 2) {
-        const float oz = dst.z[(size_t)oy * dst.cw + ox];
+        const float oz = dst.z[(size_t)oy * dst.w + ox];
         if (oz != oz) continue;
         const double sd_old = sigma_depth * (double)oz * (double)oz, sd_new = sigma_depth * (double)qz * (double)qz;
         const double old_sigma = __dmul_rn((double)cloud_step, cov_z_const >= 0.0 ? cov_z_const : sd_old * sd_old);
@@ -180,7 +128,7 @@ struct EmmArgs {
 
 // counts[4] = inlier, outlier, occluded, all points (MatchingResult, matching_result.h:40-42)
 template <EmmPoints P>
-__device__ void emm_pair(const EmmView& newer, const EmmView& older, const float* T16 /* column-major, newer -> older */,
+__device__ void emm_pair(const CloudView& newer, const CloudView& older, const float* T16 /* column-major, newer -> older */,
                          const EmmArgs& a, unsigned counts[4], unsigned* scratch) {
   float R[9], t[3], Ri[9], ti[3];
 #pragma unroll
@@ -224,11 +172,9 @@ __global__ void __launch_bounds__(256) k_emm_pairs(const PairDesc* __restrict__ 
   rgbdslam_b200_pair_result res = results[p];
   if (res.id1 < 0) return;  // the model only judges transformations RANSAC accepted (node.cpp:1336-1345)
   const PairDesc pd = pairs[p];
-  if ((pd.emm_cloud != 0) != (P == EmmPoints::kCloud)) return;
-  EmmView nv{pd.q_cloud, pd.q_cloud_x, pd.q_cloud_y, pd.q_cw, pd.q_ch, pd.q_K[0], pd.q_K[1], pd.q_K[2], pd.q_K[3]};
-  EmmView ov{pd.t_cloud, pd.t_cloud_x, pd.t_cloud_y, pd.t_cw, pd.t_ch, pd.t_K[0], pd.t_K[1], pd.t_K[2], pd.t_K[3]};
+  if ((pd.q_cloud.x != nullptr) != (P == EmmPoints::kCloud)) return;
   unsigned counts[4];
-  emm_pair<P>(nv, ov, res.ransac_trafo, a, counts, scratch);
+  emm_pair<P>(pd.q_cloud, pd.t_cloud, res.ransac_trafo, a, counts, scratch);
   if (threadIdx.x == 0) {
     res.inlier_points = counts[0];
     res.outlier_points = counts[1];
@@ -260,7 +206,7 @@ cudaError_t launch_emm_pairs(const PairDesc* pairs, int npairs, bool depth_pairs
 
 // rgbdslam_b200_observation_likelihood: one pair, explicit transformation, counts only
 template <EmmPoints P>
-__global__ void __launch_bounds__(256) k_emm_single(EmmView newer, EmmView older, const float* __restrict__ T16, EmmArgs a,
+__global__ void __launch_bounds__(256) k_emm_single(CloudView newer, CloudView older, const float* __restrict__ T16, EmmArgs a,
                                                     unsigned* __restrict__ counts_out) {
   __shared__ unsigned scratch[8];
   __shared__ float sT[16];
@@ -272,13 +218,11 @@ __global__ void __launch_bounds__(256) k_emm_single(EmmView newer, EmmView older
     for (int k = 0; k < 4; k++) counts_out[k] = counts[k];
 }
 
-cudaError_t launch_emm_single(const EmmNode& q, const EmmNode& t, bool cloud, const float* d_T16, int cloud_step, int skip_step,
+cudaError_t launch_emm_single(const CloudView& q, const CloudView& t, const float* d_T16, int cloud_step, int skip_step,
                               double cov_z_const, double sigma_depth, unsigned* d_counts, cudaStream_t stream) {
   EmmArgs a{cloud_step, skip_step, cov_z_const, sigma_depth, 0.0};
-  EmmView nv{q.z, q.x, q.y, q.cw, q.ch, q.K[0], q.K[1], q.K[2], q.K[3]};
-  EmmView ov{t.z, t.x, t.y, t.cw, t.ch, t.K[0], t.K[1], t.K[2], t.K[3]};
-  if (cloud) k_emm_single<EmmPoints::kCloud><<<1, 256, 0, stream>>>(nv, ov, d_T16, a, d_counts);
-  else k_emm_single<EmmPoints::kDepth><<<1, 256, 0, stream>>>(nv, ov, d_T16, a, d_counts);
+  if (q.x) k_emm_single<EmmPoints::kCloud><<<1, 256, 0, stream>>>(q, t, d_T16, a, d_counts);
+  else k_emm_single<EmmPoints::kDepth><<<1, 256, 0, stream>>>(q, t, d_T16, a, d_counts);
   return cudaGetLastError();
 }
 

@@ -26,26 +26,20 @@ cudaError_t launch_l2_tc256(const HamItem* d_items, int n_items, int sm_count, c
 
 // SIFT-128 path (sift_l2.cu / hamming_tc.cu MODE 1)
 cudaError_t launch_sift_prepare(const SiftJob* d_jobs, int njobs, int max_n_pad, int root_sift, int siftgpu, cudaStream_t stream);
-cudaError_t launch_build_cloud(const float* d_depth, int w, int h, int step, float scaling, float min_depth, float* cloud_z, int cw,
-                               int ch, cudaStream_t stream);
-cudaError_t launch_split_cloud(const float* d_cloud, int stride, int n, float* x, float* y, float* z, cudaStream_t stream);
 // Environment measurement model.  launch_emm_pairs launches the depth-node instantiation when depth_pairs, the kept-cloud one
 // when cloud_pairs (each skips the other kind's pairs) and adds the launches to *n_launches.
 cudaError_t launch_emm_pairs(const PairDesc* pairs, int npairs, bool depth_pairs, bool cloud_pairs, int cloud_step, int skip_step,
                              double cov_z_const, double sigma_depth, double observability_threshold,
                              rgbdslam_b200_pair_result* results, cudaStream_t stream, int* n_launches);
-struct EmmNode {  // one node's cloud as the model reads it (x / y only for kept clouds)
-  const float *z, *x, *y;
-  int cw, ch;
-  const float* K;
-};
-cudaError_t launch_emm_single(const EmmNode& q, const EmmNode& t, bool cloud, const float* d_T16, int cloud_step, int skip_step,
+// One pair, explicit transformation; the kind of q (q.x != nullptr: organised clouds) selects the instantiation.
+cudaError_t launch_emm_single(const CloudView& q, const CloudView& t, const float* d_T16, int cloud_step, int skip_step,
                               double cov_z_const, double sigma_depth, unsigned* d_counts, cudaStream_t stream);
-// Stored colour clouds (map.cu).  Per node `node_words` 4-byte words: depth-image frames [z | colour] planes at the skip-step
-// raster (w / step x h / step), clouds [x | y | z | colour] planes of n points.  vis_kind: 0 grey, 1 three-channel, 2 Bayer GRBG.
+// The nodes' clouds, Node::pc_col (map.cu).  Per node `node_words` 4-byte words: depth-image frames a z-plane at the skip-step
+// raster (ceil(w / step) x ceil(h / step)), clouds [x | y | z] planes of n points; each followed by a colour plane when
+// d_visual / rgb is given.  vis_kind: 0 grey, 1 three-channel, 2 Bayer GRBG.
 cudaError_t launch_store_depth_cloud(int nframes, const float* d_depth, const uint8_t* d_visual, int vis_kind, bool bgr, int w, int h,
                                      int step, double scaling, float min_depth, float* out, size_t node_words, cudaStream_t st);
-cudaError_t launch_store_cloud_points(int nframes, const float* d_cloud, int stride, int n, float* out, size_t node_words,
+cudaError_t launch_store_cloud_points(int nframes, const float* d_cloud, int stride, int n, bool rgb, float* out, size_t node_words,
                                       cudaStream_t st);
 // One node of a rgbdslam_b200_render_cloud / node_download_cloud call.
 struct MapNode {

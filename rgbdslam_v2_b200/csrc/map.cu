@@ -1,7 +1,10 @@
 // map.cu -- the nodes' colour point clouds and the registered map (RGBDSLAM_B200_STORE_CLOUD, rgbdslam_b200_render_cloud):
 //   k_store_depth_cloud   createXYZRGBPointCloud (misc.cpp:467-556) for every frame of a Node-constructor chunk: the z-plane
-//                         at the cloud_creation_skip_step raster and the packed colour words (x / y follow from the pixel)
-//   k_store_cloud_points  pc_col of the point-cloud constructor (node.cpp:261): x / y / z planes and the colour words
+//                         at the cloud_creation_skip_step raster and, for STORE_CLOUD, the packed colour words (x / y follow
+//                         from the pixel)
+//   k_store_cloud_points  pc_col of the point-cloud constructor (node.cpp:261): x / y / z planes and, for STORE_CLOUD, the
+//                         colour words
+// These two build every node cloud: the measurement model (emm.cu) and the map read the same planes.
 //   k_map_count           transformAndAppendPointCloud (misc.cpp:183-238): the points each 1024-point block keeps
 //   k_map_scan            exclusive scan of the block counts (output offsets, in node order then raster order)
 //   k_map_scatter         the kept points of the blocks that overlap one staging piece, transformed, as PCL records
@@ -16,11 +19,12 @@ constexpr uint32_t kOneF = 0x3f800000u;  // 1.0f: data[3] of a default-construct
 
 __device__ __forceinline__ float map_nan() { return __int_as_float(0x7fc00000); }
 
-// Visual of a depth-image frame: vis_kind 0 grey (w*h bytes), 1 three-channel (3*w*h bytes), 2 Bayer GRBG mosaic (w*h bytes,
-// debayered as the listener does before it builds the Node).  Channel c0 is blue under encoding_bgr (misc.cpp:487-489, RGBValue
-// :453-464: the word holds b, g, r, a in memory), red without it; alpha is 0.  Point 0 keeps colour word 0: its color_idx is 0,
-// which fails `color_idx > 0` (:537).  Requires w % step == 0 and h % step == 0 (checked by the caller), so point (rx, ry) is
-// pixel (rx * step, ry * step) for depth and colour alike.
+// The raster is ceil(w / step) x ceil(h / step) (misc.cpp:482-483): point (rx, ry) is pixel (rx * step, ry * step).  Visual
+// (NULL: no colour plane) of a depth-image frame: vis_kind 0 grey (w*h bytes), 1 three-channel (3*w*h bytes), 2 Bayer GRBG
+// mosaic (w*h bytes, debayered as the listener does before it builds the Node).  Channel c0 is blue under encoding_bgr
+// (misc.cpp:487-489, RGBValue :453-464: the word holds b, g, r, a in memory), red without it; alpha is 0.  Point 0 keeps
+// colour word 0: its color_idx is 0, which fails `color_idx > 0` (:537).  The reference's colour index only matches the pixel
+// when step divides w and h, which the caller requires for colour.
 __global__ void __launch_bounds__(256) k_store_depth_cloud(const float* __restrict__ depth, const uint8_t* __restrict__ visual,
                                                            int vis_kind, int bgr, int w, int h, int step, int cw, int ch,
                                                            double scaling, float min_depth, float* __restrict__ out,
@@ -35,6 +39,7 @@ __global__ void __launch_bounds__(256) k_store_depth_cloud(const float* __restri
   const float Z = __double2float_rn(__dmul_rn((double)depth[f * px + pix], scaling));
   float* z = out + f * node_words;
   z[i] = Z >= min_depth ? Z : map_nan();  // !(Z >= minimum_depth), NaN included (:525-530)
+  if (!visual) return;
   uint32_t word = 0;
   if (i > 0) {
     uint32_t c0, c1, c2;
@@ -55,16 +60,16 @@ __global__ void __launch_bounds__(256) k_store_depth_cloud(const float* __restri
 
 cudaError_t launch_store_depth_cloud(int nframes, const float* d_depth, const uint8_t* d_visual, int vis_kind, bool bgr, int w, int h,
                                      int step, double scaling, float min_depth, float* out, size_t node_words, cudaStream_t st) {
-  const int cw = w / step, ch = h / step;
+  const int cw = (w + step - 1) / step, ch = (h + step - 1) / step;
   k_store_depth_cloud<<<dim3((cw * ch + 255) / 256, nframes), 256, 0, st>>>(d_depth, d_visual, vis_kind, bgr ? 1 : 0, w, h, step, cw,
                                                                              ch, scaling, min_depth, out, node_words);
   return cudaGetLastError();
 }
 
 // Organised clouds of `stride` floats per point (8: PointXYZRGB, colour word at byte 16; 4: PointXYZ with RGB_IS_4TH_DIM,
-// colour in data[3]) -> per node [x | y | z | colour] planes of n points each.
-__global__ void __launch_bounds__(256) k_store_cloud_points(const float* __restrict__ cloud, int stride, int n, float* __restrict__ out,
-                                                            size_t node_words) {
+// colour in data[3]) -> per node [x | y | z] planes of n points each, and the colour plane when rgb.
+__global__ void __launch_bounds__(256) k_store_cloud_points(const float* __restrict__ cloud, int stride, int n, int rgb,
+                                                            float* __restrict__ out, size_t node_words) {
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n) return;
   const size_t f = blockIdx.y;
@@ -73,12 +78,12 @@ __global__ void __launch_bounds__(256) k_store_cloud_points(const float* __restr
   o[i] = p[0];
   o[n + i] = p[1];
   o[2 * (size_t)n + i] = p[2];
-  o[3 * (size_t)n + i] = p[stride == 8 ? 4 : 3];
+  if (rgb) o[3 * (size_t)n + i] = p[stride == 8 ? 4 : 3];
 }
 
-cudaError_t launch_store_cloud_points(int nframes, const float* d_cloud, int stride, int n, float* out, size_t node_words,
+cudaError_t launch_store_cloud_points(int nframes, const float* d_cloud, int stride, int n, bool rgb, float* out, size_t node_words,
                                       cudaStream_t st) {
-  k_store_cloud_points<<<dim3((n + 255) / 256, nframes), 256, 0, st>>>(d_cloud, stride, n, out, node_words);
+  k_store_cloud_points<<<dim3((n + 255) / 256, nframes), 256, 0, st>>>(d_cloud, stride, n, rgb ? 1 : 0, out, node_words);
   return cudaGetLastError();
 }
 
@@ -97,16 +102,14 @@ struct MapOut {
 __device__ __forceinline__ bool map_point(const MapNode& nd, int i, const MapArgs& a, MapOut& o) {
   float x, y, z;
   o.rgb = nd.rgb[i];
-  if (nd.step > 0) {  // depth-image node: x / y of createXYZRGBPointCloud from the pixel (misc.cpp:525-533, misc2.h:62-64)
+  if (nd.step > 0) {  // depth-image node: x / y of createXYZRGBPointCloud from the pixel
     z = nd.z[i];
-    const float u = (float)((i % nd.cw) * nd.step), v = (float)((i / nd.cw) * nd.step);
-    if (z != z) {  // (u - cx) * 1.0 * fxinv: the double product of two floats is exact, so this is the rounded float product
-      x = __fmul_rn(__fsub_rn(u, nd.cx), nd.fxinv);
-      y = __fmul_rn(__fsub_rn(v, nd.cy), nd.fyinv);
-    } else {
-      x = __fmul_rn(__fmul_rn(__fsub_rn(u, nd.cx), z), nd.fxinv);
-      y = __fmul_rn(__fmul_rn(__fsub_rn(v, nd.cy), z), nd.fyinv);
-    }
+    // for a NaN z the reference forms (u - cx) * 1.0 * fxinv in double: the product of two floats is exact there, so it is the
+    // rounded float product of the 1 m ray
+    const float2 xy = depth_point_xy((float)((i % nd.cw) * nd.step), (float)((i / nd.cw) * nd.step), z, nd.cx, nd.cy, nd.fxinv,
+                                     nd.fyinv);
+    x = xy.x;
+    y = xy.y;
     o.w16 = i == 0 ? kOneF : o.rgb;  // point 0 keeps the default-constructed data[3]
   } else {
     x = nd.x[i];

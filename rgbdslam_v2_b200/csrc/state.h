@@ -31,6 +31,18 @@ struct NodeSlab {
   int refs = 0;
 };
 
+// A node's point cloud, the reference's Node::pc_col (node.cpp:126-131, 261), read by the environment measurement model and
+// the map.  Depth-image nodes keep the z-plane of createXYZRGBPointCloud at every step-th pixel (x / y follow from the pixel
+// and K); point-cloud nodes keep the x / y / z planes of the organised cloud.
+struct NodeCloud {
+  float *x = nullptr, *y = nullptr, *z = nullptr;  // x / y only for organised (point-cloud) nodes; z == nullptr: no cloud
+  uint32_t* rgb = nullptr;      // colour words (b, g, r, a bytes): RGBDSLAM_B200_STORE_CLOUD only
+  int32_t w = 0, h = 0, step = 0;  // step > 0: depth-image raster, point (rx, ry) is pixel (rx * step, ry * step)
+  float K[4] = {0, 0, 0, 0};    // fx, fy, cx, cy of the call that built it (0 when it passed none)
+  NodeSlab* slab = nullptr;     // the allocation the planes live in
+  CloudView view() const { return CloudView{z, x, y, w, h, {K[0], K[1], K[2], K[3]}}; }
+};
+
 // Device copy of what the reference's Node keeps per frame (node.h:167-174).
 struct NodeDev {
   static constexpr uint32_t kMagic = 0x4e4f4445u;  // 'NODE'
@@ -44,24 +56,9 @@ struct NodeDev {
   float* norms = nullptr;     // SIFT nodes: n_pad |b|^2 of the bf16-rounded rows
   int8_t* desc_i8 = nullptr;  // float-descriptor nodes only: n_pad x 256 B operand tiles (bf16 RootSIFT rows / u8 SiftGPU rows)
   int32_t n_pad = 0;
-  float* cloud_z = nullptr;   // depth cloud z-plane (cw x ch) for the environment measurement model
-  // Kept organised cloud of the point-cloud constructor (RGBDSLAM_B200_KEEP_CLOUD): x / y / z planes at full resolution
-  // (cw x ch = w x h) in one allocation that starts at cloud_x (cloud_z = its third plane); nullptr for depth-image nodes.
-  float* cloud_x = nullptr;
-  float* cloud_y = nullptr;
-  int32_t cw = 0, ch = 0;
-  float K[4] = {0, 0, 0, 0};  // fx, fy, cx, cy of the full-resolution camera (kept clouds: the camera the model projects into)
   int32_t sift_kind = 0;      // SIFT nodes: 0 = RootSIFT rows + bf16 tiles, 1 = raw rows + u8 tiles (SiftGPU matcher)
-  NodeSlab* slab = nullptr;   // desc / xyz / kp live inside this shared allocation (cloud_z is always separate)
-  // Stored colour cloud (RGBDSLAM_B200_STORE_CLOUD), the reference's Node::pc_col: colour words (b, g, r, a bytes) at pc_w x
-  // pc_h; depth-image nodes also keep pc_z, the z-plane of createXYZRGBPointCloud at every pc_step-th pixel (x / y follow from
-  // the pixel and pc_K = fx, fy, cx, cy); point-cloud nodes keep x / y / z in cloud_x / cloud_y / cloud_z, inside the same
-  // allocation.  All of it lives in pc_slab, shared by the nodes of one nodes_create_ex call.
-  float* pc_z = nullptr;
-  uint32_t* pc_rgb = nullptr;
-  int32_t pc_w = 0, pc_h = 0, pc_step = 0;
-  float pc_K[4] = {0, 0, 0, 0};
-  NodeSlab* pc_slab = nullptr;
+  NodeSlab* slab = nullptr;   // desc / xyz / kp live inside this shared allocation
+  NodeCloud pc;
 };
 
 constexpr int kSlots = 8;  // independent in-flight match_pairs pipelines (stream + workspace each)
@@ -145,8 +142,6 @@ Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot
 #define RB200_ENTER_INITED()                                    \
   std::lock_guard<std::mutex> entry_lock__(rb200::g_state.mu); \
   if (int entry_rc__ = rb200::check_inited()) return entry_rc__
-int node_build_cloud(NodeDev* nd, const float* d_depth, int w, int h, const float K4[4], cudaStream_t st);
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
-void free_node_cloud(NodeDev* nd);  // frees the node's depth cloud or kept cloud (api.cu)
 
 }  // namespace rb200

@@ -22,10 +22,11 @@ CUTS = (0.001, 0.999)
 
 
 def cloud_z(depth, step=2, scaling=1.0, min_depth=0.1):
-    """misc.cpp:467-556: every step-th pixel of the depth map times the (float) scaling, NaN where !(Z >= min_depth)."""
+    """misc.cpp:467-556: every step-th pixel of the depth map times the double depth_scaling, rounded to float (:502, 522),
+    NaN where !(Z >= min_depth)."""
     d = np.asarray(depth, F32)
     h, w = d.shape
-    z = (d[::step, ::step] * F32(scaling)).astype(F32)
+    z = (d[::step, ::step].astype(F64) * F64(scaling)).astype(F32)
     with np.errstate(invalid="ignore"):
         z = np.where(z >= F32(min_depth), z, F32(np.nan)).astype(F32)
     assert z.shape == ((h + step - 1) // step, (w + step - 1) // step)

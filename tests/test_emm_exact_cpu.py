@@ -35,8 +35,9 @@ def scenes():
         out.append((f"other-K-rev/{tn}", d_b, K_B, d_c, (300.0, 301.0, 166.0, 124.5), T, cfg))
     for steps in ((3, 5), (1, 7), (4, 3)):
         out.append((f"steps{steps}", d_b, K_B, d_a, K_A, T_small, dict(cfg, cloud_step=steps[0], skip_step=steps[1])))
-    out.append(("scaling", (d_a * 1000).astype(np.float32), K_A, (d_b * 1000).astype(np.float32), K_B, T_small,
+    out.append(("scaling-0.001", (d_a * 1000).astype(np.float32), K_A, (d_b * 1000).astype(np.float32), K_B, T_small,
                 dict(cfg, scaling=0.001)))
+    out.append(("scaling-1.03", d_b, K_B, d_a, K_A, T_small, dict(cfg, scaling=1.03)))
     out.append(("min-depth", d_a, K_A, d_b, K_B, T_small, dict(cfg, min_depth=1.7)))
     out.append(("per-point", d_a, K_A, d_b, K_B, T_small, dict(cfg, z0=None)))
     out.append(("per-point/steps", d_b, K_B, d_c, (300.0, 301.0, 166.0, 124.5), T_big, dict(cfg, z0=None, cloud_step=3,
@@ -82,6 +83,31 @@ def test_restatement_reaches_projection_boundaries(oracle_mod):
         zn, zo, exp = _oracle_counts(oracle_mod, T, d, K_A, d, K_A, cfg)
         got = ee.pairwise(T, zn, K_A, zo, K_A, czc=ee.cov_const(0.01, 2.0))
         assert np.array_equal(got["counts"], exp.astype(np.int64)), (dx, got["counts"], exp)
+
+
+# A constant depth whose float product with float(1.03) is one ulp below its double product with 1.03: the reference's z.
+D_ULP = np.float32(2.0000021)
+
+
+@pytest.mark.parametrize("scaling", [1.0, 1.03, 0.001])
+def test_model_cloud_is_the_stored_cloud(oracle_mod, scaling):
+    """The model's z-plane is the z of createXYZRGBPointCloud, the stored cloud's restatement, on images the step divides; the
+    C oracle agrees.  A depth whose double product with the scaling equals minimum_depth is kept, one ulp above the float
+    product."""
+    import map_cloud_exact as mx
+    rng = np.random.default_rng(7)
+    d = ee.block_scene(rng, 640, 480, K_A) / np.float32(scaling)
+    for step in (1, 2, 4):
+        z = ee.cloud_z(d, step, scaling, 0.1)
+        assert np.array_equal(z.ravel(), mx.create_cloud(d, np.zeros(d.shape, np.uint8), K_A, step, scaling, 0.1)["z"], equal_nan=True)
+        assert np.array_equal(z, oracle_mod.create_cloud_z(d, step, scaling, 0.1), equal_nan=True)
+    md = float(np.float32(np.float64(D_ULP) * scaling))
+    flat = np.full((48, 64), D_ULP, np.float32)
+    for z in (ee.cloud_z(flat, 2, scaling, md), oracle_mod.create_cloud_z(flat, 2, scaling, md),
+              mx.create_cloud(flat, np.zeros(flat.shape, np.uint8), K_A, 2, scaling, md)["z"]):
+        assert (z == np.float32(md)).all()
+    if scaling == 1.03:
+        assert np.float32(D_ULP) * np.float32(scaling) < np.float32(md)
 
 
 # ---- the kernels keep the float chain uncontracted ------------------------------------------------------------------------

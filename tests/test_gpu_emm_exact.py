@@ -174,6 +174,39 @@ def test_latched_covariance(fe):
     _reinit(fe)
 
 
+def test_depth_scaling_is_a_double_product(fe):
+    """z = (float)((double)depth * depth_scaling_factor) (misc.cpp:502, 522).  A constant depth d = 2.0000021 at scaling 1.03
+    with minimum_depth = float(double(d) * 1.03): the reference keeps every point, where the float product, one ulp lower,
+    would drop them all.  Clouds from node_set_depth and from nodes_create with the model on, with and without STORE_CLOUD,
+    give the restatement's counts."""
+    import node_helpers as nh
+    d = np.float32(2.0000021)
+    md = float(np.float32(np.float64(d) * 1.03))
+    assert d * np.float32(1.03) < np.float32(md)
+    p = _reinit(fe, depth_scaling_factor=1.03, minimum_depth=md, observability_threshold=0.5)
+    K = nh.K4()
+    gray, _ = nh.stack(nh.render(range(2)))
+    depth = np.full(gray.shape, d, np.float32)
+    z = ee.cloud_z(depth[0], p.cloud_creation_skip_step, 1.03, md)
+    assert not np.isnan(z).any()
+    T = ee.rigid(np.random.default_rng(6), 1.0, [0.02, -0.01, 0.03]).astype(np.float32)
+    exp = ee.pairwise(T, z, K, z, K, cloud_step=p.cloud_creation_skip_step, skip_step=p.emm_skip_step, sigma_depth=p.sigma_depth,
+                      czc=_czc(fe))
+    assert exp["counts"][:3].sum() > 0, exp["counts"]
+    a, b = _feature_node(fe, 1), _feature_node(fe, 0)
+    fe.node_set_depth(a, depth[1], K)
+    fe.node_set_depth(b, depth[0], K)
+    pairs = [("node_set_depth", a, b)]
+    det = fe.detector_create()
+    for store in (False, True):
+        hs, _ = fe.nodes_create(det, gray, depth, None, K, store_cloud=store)
+        pairs.append((f"nodes_create store={store}", hs[1], hs[0]))
+    fe.detector_destroy(det)
+    for what, newer, older in pairs:
+        _assert_counts(fe.observation_likelihood(newer, older, T), exp, what)
+    _reinit(fe)
+
+
 # ---- the gate in match_node_pairs -----------------------------------------------------------------------------------------
 
 W, H = 640, 480

@@ -110,25 +110,52 @@ def test_pinned_input_and_chunking_do_not_change_the_clouds(fe, built):
     assert all(_same(x, y) for x, y in zip(a, b)) and len(a) == len(b) == 70
 
 
-@pytest.mark.parametrize("cloud_input", [False, True])
-def test_features_thresholds_and_model_counts_do_not_change(fe, frames, cloud_input):
+@pytest.mark.parametrize("cloud_input,scaling,model_later", [
+    pytest.param(False, 1.0, False, id="False"), pytest.param(True, 1.0, False, id="True"),
+    pytest.param(False, 1.03, False, id="scaled"), pytest.param(False, 1.0, True, id="model-switched-on-later")])
+def test_features_thresholds_and_model_counts_do_not_change(fe, frames, cloud_input, scaling, model_later):
+    """STORE_CLOUD changes nothing else, and the stored cloud is the model's.  model_later: the STORE_CLOUD nodes are built
+    with the model off, which is switched on before they are matched."""
     gray, depth = frames
-    kw = dict(observability_threshold=0.5)
+    kw = dict(observability_threshold=0.5, depth_scaling_factor=scaling)
     out = []
     for flags in ({}, dict(store_cloud=True)):
-        nh.reinit(fe, 0, **kw)
+        later = model_later and bool(flags)
+        nh.reinit(fe, 0, **(dict(kw, observability_threshold=-0.6) if later else kw))
         det = fe.detector_create()
         if cloud_input:
             clouds = np.stack([_cloud(d, g, 8) for g, d in zip(gray, depth)])
             hs, nf = fe.nodes_create(det, gray, clouds, None, nh.K4(), keep_cloud=True, **flags)
         else:
             hs, nf = fe.nodes_create(det, gray, depth, None, nh.K4(), **flags)
+        if later:
+            nh.reinit(fe, 0, **kw)
         res, _, _ = fe.match_node_pairs(hs[1:], hs[:-1], seed=3)
         out.append((nh.node_dump(fe, hs), fe.detector_thresholds(det).copy(), res.copy()))
         nh.destroy(fe, hs)
         fe.detector_destroy(det)
     assert nh.same_nodes(out[0][0], out[1][0]) and np.array_equal(out[0][1], out[1][1])
     assert out[0][2].tobytes() == out[1][2].tobytes() and out[0][2]["all_points"].sum() > 0
+
+
+def test_node_set_depth_leaves_a_node_cloud_alone(fe, frames):
+    """A node that keeps the cloud it was built from, stored (STORE_CLOUD) or organised (KEEP_CLOUD), refuses node_set_depth
+    with ERR_STATE before any device work, and its cloud stays as it was."""
+    gray, depth = frames
+    nh.reinit(fe, 0)
+    det = fe.detector_create()
+    stored, _ = fe.nodes_create(det, gray[:1], depth[:1], None, nh.K4(), store_cloud=True)
+    kept, _ = fe.nodes_create(det, gray[:1], _cloud(depth[0], gray[0], 8)[None], None, None, keep_cloud=True)
+    fe.detector_destroy(det)
+    before = fe.node_cloud(stored[0])
+    K = np.array(nh.K4(), np.float32)
+    d0 = np.ascontiguousarray(depth[0])
+    for h, flag in ((stored[0], b"STORE_CLOUD"), (kept[0], b"KEEP_CLOUD")):
+        n0 = fe.launch_count
+        assert fe.lib.rgbdslam_b200_node_set_depth(C.c_uint64(h), d0.ctypes.data, 640, 480, K.ctypes.data) == 3
+        assert flag in fe.lib.rgbdslam_b200_last_error() and fe.launch_count == n0
+    assert _same(fe.node_cloud(stored[0]), before)
+    nh.destroy(fe, stored + kept)
 
 
 def _mixed_nodes(fe, frames):
