@@ -7,6 +7,7 @@
 //   unsigned pruneEdgesWithErrorAbove(float)                             :1106-1246 -> rgbdslam_b200_posegraph_chi2
 //   void   saveTrajectory(filename)                                      graph_mgr_io.cpp:615-677 / logTransform misc.cpp:90-93
 //   void   saveAllClouds(filename)  == saveAllCloudsToFile               graph_mgr_io.cpp:502-583 -> rgbdslam_b200_render_cloud
+//   size_t reducePointClouds()      == reducePointCloud for every node   graph_manager.cpp:1310-1319 -> rgbdslam_b200_reduce_clouds
 // Host logic only; every compute step is a C-ABI call.  The reference draws from the global rand(); here every draw comes
 // from the library's counter-based generator keyed by (seed, node id).  g2o's HyperDijkstra (not under /root/reference) is
 // restated in geodesicBall().  The Python mirror rgbdslam_v2_b200/graph_manager.py is the tested twin of this file.
@@ -348,6 +349,32 @@ class GraphManager {
   static bool& preserve_raster_on_save() {
     static bool v = false;
     return v;
+  }
+
+  // parameter voxelfilter_size (parameter_server.cpp:159, default -1: no filter) of reducePointClouds
+  static double& voxelfilter_size() {
+    static double v = -1.0;
+    return v;
+  }
+  // Node::reducePointCloud(voxelfilter_size) of every node of graph_ in one device call.  The reference's slot
+  // (GraphManager::reducePointCloud, graph_manager.cpp:1310-1319) reduces the one node whose cloud pointer the GUI hands it after
+  // drawing it, so that in the end every drawn node is reduced; without a GUI the whole graph is reduced at once.  Nodes without a
+  // stored cloud are passed over; voxelfilter_size <= 0 warns and changes nothing.  Returns the number of nodes reduced.
+  size_t reducePointClouds() {
+    if (voxelfilter_size() <= 0.0) {
+      std::fprintf(stderr, "Point Clouds can't be reduced because of invalid voxelfilter_size\n");
+      return 0;
+    }
+    std::vector<uint64_t> handles;
+    for (auto& kv : graph_) {
+      int w = 0, h = 0;
+      if (rgbdslam_b200_node_download_cloud(kv.second->handle(), 32, nullptr, &w, &h) == 0) handles.push_back(kv.second->handle());
+    }
+    std::vector<int32_t> counts(handles.size());
+    check(rgbdslam_b200_reduce_clouds((int)handles.size(), handles.data(), voxelfilter_size(), counts.data()), "reduce_clouds");
+    size_t reduced = 0;
+    for (int32_t c : counts) reduced += c >= 0;
+    return reduced;
   }
 
   // world2cam = cam2rgb * eigenTransf2TF(estimate of node id) in double (graph_mgr_io.cpp:526-541), row-major 3 x 4: cam2rgb has

@@ -11,6 +11,7 @@
 // maintainer who has Eigen/OpenCV maps them with Eigen::Map / reinterpret_cast (see INTEGRATION.md).
 #pragma once
 #include <cstdint>
+#include <cstdio>
 #include <cstring>
 #include <memory>
 #include <stdexcept>
@@ -20,6 +21,7 @@
 
 #include "../rgbdslam_b200.h"
 #include "map.h"
+#include "voxel.h"
 #include "features.hpp"
 
 namespace rgbdslam_b200 {
@@ -308,6 +310,18 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     if (w > 0 && h > 0)
       check(rgbdslam_b200_node_download_cloud(handle_, (int)sizeof(point_type), pc->points.data(), &w, &h), "node_download_cloud");
     return pc;
+  }
+
+  // Node::reducePointCloud (node.cpp:1448-1460): pc_col becomes its voxel grid of leaf size vfs on the device
+  // (rgbdslam_b200_reduce_clouds), so pointCloud() afterwards is the n x 1 cloud of centroids.  vfs <= 0 warns and changes
+  // nothing, like the reference; a NaN or infinite vfs throws.  When the leaf size is too small for the cloud (PCL's
+  // "Leaf size is too small" warning) the cloud also stays as it is.
+  void reducePointCloud(double vfs) {
+    if (vfs <= 0.0) {
+      std::fprintf(stderr, "Point Clouds can't be reduced because of invalid voxelfilter_size\n");
+      return;
+    }
+    check(rgbdslam_b200_reduce_clouds(1, &handle_, vfs, nullptr), "reduce_clouds");
   }
 
   static int& max_connections() {  // parameter max_connections (parameter_server.cpp:104), -1 = unlimited

@@ -177,6 +177,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_node_download_keypoints.argtypes = [u64, vp]
     lib.rgbdslam_b200_node_download_cloud.argtypes = [u64, C.c_int, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
+    lib.rgbdslam_b200_reduce_clouds.argtypes = [C.c_int, vp, C.c_double, vp]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -561,6 +562,15 @@ class Frontend:
                                                         _ptr(out), cap, C.byref(n), _ptr(used)))
         return (out[:n.value] if isinstance(out, np.ndarray) and out.dtype.itemsize == point_bytes else out), \
             used.reshape(-1, 4, 4).transpose(0, 2, 1)
+
+    def reduce_clouds(self, nodes, voxelfilter_size: float) -> np.ndarray:
+        """Node::reducePointCloud(voxelfilter_size) of the nodes' stored clouds on the device: each becomes one centroid per
+        occupied voxel, a cloud of width n and height 1 for node_cloud / render_cloud.  Returns the new point counts (-1: the leaf size is too
+        small for that node's cloud, which stays as it is)."""
+        hs = np.ascontiguousarray(np.asarray(nodes, np.uint64))
+        counts = np.zeros(len(hs), np.int32)
+        self._check(self.lib.rgbdslam_b200_reduce_clouds(len(hs), _ptr(hs), float(voxelfilter_size), _ptr(counts)))
+        return counts
 
     # -- multi-GPU exchange -------------------------------------------------------------
     def comm_unique_id(self) -> np.ndarray:

@@ -335,7 +335,8 @@ static int check_pairs(const std::vector<PairDesc>& h_pairs, int64_t first_pair,
   if (s.params.observability_threshold > 0.0)
     for (const PairDesc& pd : h_pairs)
       if (!pd.q_cloud.z || !pd.t_cloud.z) {
-        set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth)");
+        set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth) that "
+                  "rgbdslam_b200_reduce_clouds has not voxel-filtered");
         return RGBDSLAM_B200_ERR_STATE;
       } else if (!pd.q_cloud.x != !pd.t_cloud.x) {
         // the reference never holds both kinds in one process (topic_points is global): there is no rule to restate
@@ -499,8 +500,7 @@ static int run_pairs(Workspace& w, const std::vector<PairDesc>& h_pairs, uint64_
   return 0;
 }
 
-// drops one node's reference to a shared allocation
-static void release_slab(NodeSlab* slab) {
+void release_slab(NodeSlab* slab) {
   if (slab && --slab->refs == 0) {
     cudaFree(slab->base);
     delete slab;
@@ -739,6 +739,10 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
   if (!a->pc.z || !b->pc.z) {
     set_error("observation_likelihood: both nodes need a depth cloud (nodes_create with observability_threshold > 0 or STORE_CLOUD, "
               "or node_set_depth)");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
+  if (a->pc.reduced || b->pc.reduced) {
+    set_error("observation_likelihood: a voxel-filtered cloud (rgbdslam_b200_reduce_clouds) has no raster for the measurement model");
     return RGBDSLAM_B200_ERR_STATE;
   }
   if (!a->pc.x != !b->pc.x) {

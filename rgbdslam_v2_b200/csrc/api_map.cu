@@ -2,14 +2,17 @@
 //   rgbdslam_b200_node_download_cloud  == Node::pc_col (node.cpp:126-131, 261) as an organised cloud
 //   rgbdslam_b200_render_cloud         == transformAndAppendPointCloud (misc.cpp:183-238) of many nodes, the loop of
 //                                         GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583)
+//   rgbdslam_b200_reduce_clouds        == Node::reducePointCloud (node.cpp:1448-1460) of many nodes (voxel.cu)
 // Both run count -> scan -> scatter (map.cu) and move the records to the host through a two-piece device staging ring: the copy
 // of piece k runs on its own stream while piece k + 1 is computed.
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <vector>
 
 #include "../../include/rgbdslam_b200/map.h"
+#include "../../include/rgbdslam_b200/voxel.h"
 #include "kernels.h"
 #include "state.h"
 
@@ -126,6 +129,125 @@ static int map_emit(const std::vector<MapNode>& nodes, const MapArgs& a, void* o
   return 0;
 }
 
+// ---- the voxel filter ------------------------------------------------------------------------------------------------------
+
+constexpr long long kVoxChunkPoints = 1 << 23;  // points of the nodes reduced together: 24 bytes of work buffers per point
+
+struct VoxCtx {
+  DevBuf segs, bounds, grid, key[2], idx[2], hist, heads;
+  void release() {
+    DevBuf* all[] = {&segs, &bounds, &grid, &key[0], &key[1], &idx[0], &idx[1], &hist, &heads};
+    for (DevBuf* b : all) b->release();
+  }
+};
+
+// A reduced cloud that is not yet its node's: the node takes it only when every chunk of the call has succeeded.
+struct VoxResult {
+  NodeDev* nd;
+  NodeCloud pc;
+};
+
+// Reduces nodes [k0, k1) of the call, whose clouds hold `points` points in all, into one new slab.  Appends a VoxResult per
+// reduced node and writes n_points[k] (-1: the leaf size is too small for node k, which keeps its cloud).
+static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1, long long points, float inv_leaf,
+                     std::vector<VoxResult>& results, std::vector<NodeSlab*>& slabs, int32_t* n_points) {
+  MapCtx& m = g_map;
+  State& s = g_state;
+  cudaStream_t st = s.stream;
+  const int nn = k1 - k0;
+  std::vector<MapNode> nodes(nn);
+  std::vector<VoxSeg> segs(nn);
+  std::vector<int2> blocks;
+  int pt = 0;
+  for (int k = 0; k < nn; k++) {
+    nodes[k] = map_node(nds[k0 + k], nullptr);
+    const int P = nodes[k].cw * nodes[k].ch;
+    segs[k].pt0 = pt;
+    segs[k].npts = P;
+    segs[k].blk0 = (int)blocks.size();
+    for (int first = 0; first < P; first += kMapBlockPoints) blocks.push_back(make_int2(k, first));
+    segs[k].nblk = (int)blocks.size() - segs[k].blk0;
+    pt += P;
+  }
+  const int nb = (int)blocks.size();
+  const size_t np = (size_t)std::max<long long>(points, 1);
+  int rc;
+  if ((rc = m.nodes.ensure(sizeof(MapNode) * nn)) || (rc = m.blocks.ensure(sizeof(int2) * std::max(nb, 1))) ||
+      (rc = m.counts.ensure(4 * (size_t)std::max(nb, 1))) || (rc = m.offs.ensure(8 * (size_t)(nb + 1))) ||
+      (rc = v.segs.ensure(sizeof(VoxSeg) * nn)) || (rc = v.bounds.ensure(24 * (size_t)nn)) ||
+      (rc = v.grid.ensure(sizeof(VoxGrid) * nn)) || (rc = v.hist.ensure(1024 * (size_t)std::max(nb, 1))) ||
+      (rc = v.heads.ensure(sizeof(int2) * np)))
+    return rc;
+  for (int b = 0; b < 2; b++)
+    if ((rc = v.key[b].ensure(4 * np)) || (rc = v.idx[b].ensure(4 * np))) return rc;
+  VoxBufs b;
+  b.nodes = (const MapNode*)m.nodes.ptr;
+  b.blocks = (const int2*)m.blocks.ptr;
+  b.segs = (const VoxSeg*)v.segs.ptr;
+  b.bmin = (uint32_t*)v.bounds.ptr;
+  b.bmax = b.bmin + 3 * (size_t)nn;
+  b.grid = (VoxGrid*)v.grid.ptr;
+  for (int i = 0; i < 2; i++) {
+    b.key[i] = (uint32_t*)v.key[i].ptr;
+    b.idx[i] = (uint32_t*)v.idx[i].ptr;
+  }
+  b.hist = (int*)v.hist.ptr;
+  b.counts = (int*)m.counts.ptr;
+  b.offs = (long long*)m.offs.ptr;
+  b.heads = (int2*)v.heads.ptr;
+  RB200_CUDA(cudaMemcpyAsync(m.nodes.ptr, nodes.data(), sizeof(MapNode) * nn, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(v.segs.ptr, segs.data(), sizeof(VoxSeg) * nn, cudaMemcpyHostToDevice, st));
+  if (nb > 0) RB200_CUDA(cudaMemcpyAsync(m.blocks.ptr, blocks.data(), sizeof(int2) * nb, cudaMemcpyHostToDevice, st));
+  int launches = 0;
+  RB200_CUDA(launch_vox_keys(b, nn, nb, inv_leaf, st, &launches));
+  // the grids decide how many radix passes the chunk needs: enough bytes to hold its largest cell count, so that every voxel
+  // index sorts below the key of the points that take no part
+  std::vector<VoxGrid> grid(nn);
+  RB200_CUDA(cudaMemcpyAsync(grid.data(), v.grid.ptr, sizeof(VoxGrid) * nn, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  s.launches += launches;
+  int passes = 1;
+  for (const VoxGrid& g : grid)
+    while (passes < 4 && ((long long)g.cells >> (8 * passes)) != 0) passes++;
+  launches = 0;
+  RB200_CUDA(launch_vox_sort(b, nn, nb, passes, st, &launches));
+  std::vector<long long> offs(nb + 1);
+  RB200_CUDA(cudaMemcpyAsync(offs.data(), b.offs, 8 * (size_t)(nb + 1), cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  s.launches += launches;
+  const long long nvox = offs[nb];
+  NodeSlab* slab = new NodeSlab();
+  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max<long long>(nvox, 1));
+  if (e != cudaSuccess) {
+    delete slab;
+    return cuda_fail(e, "cudaMalloc(reduced clouds)");
+  }
+  slabs.push_back(slab);
+  RB200_CUDA(launch_vox_centroids(b, passes, nvox, (float*)slab->base, st));
+  RB200_CUDA(cudaStreamSynchronize(st));  // the work buffers are the next chunk's
+  s.launches += nvox > 0;
+  for (int k = 0; k < nn; k++) {
+    if (grid[k].too_small) {
+      n_points[k0 + k] = -1;
+      continue;
+    }
+    const long long first = offs[segs[k].blk0], count = offs[segs[k].blk0 + segs[k].nblk] - first;
+    VoxResult r{nds[k0 + k], nds[k0 + k]->pc};
+    r.pc.x = (float*)slab->base + 4 * first;
+    r.pc.y = r.pc.x + count;
+    r.pc.z = r.pc.y + count;
+    r.pc.rgb = (uint32_t*)(r.pc.z + count);
+    r.pc.w = (int32_t)count;
+    r.pc.h = 1;
+    r.pc.step = 0;
+    r.pc.slab = slab;
+    r.pc.reduced = true;
+    results.push_back(r);
+    n_points[k0 + k] = (int32_t)count;
+  }
+  return 0;
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -191,6 +313,66 @@ int rgbdslam_b200_render_cloud(int n, const uint64_t* nodes, const double* trans
   const float maxd = (float)maximum_depth;
   const MapArgs a{maxd * maxd, maxd >= 0.f ? 1 : 0, preserve_raster ? 1 : 0, 1, point_bytes};
   return map_emit(table, a, out, capacity, n_out);
+}
+
+int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter_size, int32_t* n_points) {
+  RB200_ENTER_INITED();
+  const float leaf = (float)voxelfilter_size;
+  if (n < 0 || (n > 0 && !nodes) || !std::isfinite(voxelfilter_size) || !(leaf > 0.f) || !std::isfinite(leaf)) {
+    set_error("reduce_clouds: n >= 0, nodes non-null and a finite voxelfilter_size > 0 (as a float) are needed");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  std::vector<NodeDev*> nds(n);
+  for (int k = 0; k < n; k++) {
+    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
+    if (!nds[k]->pc.rgb) {
+      set_error("reduce_clouds: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    }
+  }
+  std::vector<uint64_t> sorted(nodes, nodes + n);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
+    set_error("reduce_clouds: a node is listed twice");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  long long limit = kVoxChunkPoints;
+  if (const char* env = std::getenv("RB200_VOX_CHUNK_POINTS")) limit = std::max(1ll, std::atoll(env));
+  const float inv_leaf = 1.0f / leaf;
+  std::vector<int32_t> counts(n);
+  std::vector<VoxResult> results;
+  std::vector<NodeSlab*> slabs;
+  VoxCtx v;
+  int rc = 0;
+  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
+    int k1 = k0;
+    long long points = 0;
+    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
+    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= limit);
+    rc = vox_chunk(v, nds, k0, k1, points, inv_leaf, results, slabs, counts.data());
+    k0 = k1;
+  }
+  v.release();
+  if (rc) {  // no node is changed
+    cudaStreamSynchronize(g_state.stream);
+    for (NodeSlab* sl : slabs) {
+      cudaFree(sl->base);
+      delete sl;
+    }
+    return rc;
+  }
+  for (const VoxResult& r : results) {
+    release_slab(r.nd->pc.slab);
+    r.nd->pc = r.pc;
+    r.pc.slab->refs++;
+  }
+  for (NodeSlab* sl : slabs)
+    if (sl->refs == 0) {  // a chunk whose nodes all kept their clouds
+      cudaFree(sl->base);
+      delete sl;
+    }
+  if (n_points) std::copy(counts.begin(), counts.end(), n_points);
+  return 0;
 }
 
 }  // extern "C"

@@ -63,6 +63,39 @@ cudaError_t launch_map_count(const MapNode* d_nodes, const int2* d_blocks, int n
 cudaError_t launch_map_scan(const int* d_counts, int nblocks, long long* d_offs, cudaStream_t st);
 cudaError_t launch_map_scatter(const MapNode* d_nodes, const int2* d_blocks, const long long* d_offs, int b0, int b1, long long lo,
                                long long hi, const MapArgs& a, void* d_out, cudaStream_t st);
+// The voxel filter of the stored clouds, Node::reducePointCloud (voxel.cu).  A call works on a chunk of whole nodes whose
+// points lie back to back in the work buffers; the (node, first point) block table is the map's.
+struct VoxSeg {        // one node of the chunk
+  int pt0, npts;       // its points are [pt0, pt0 + npts) of the chunk
+  int blk0, nblk;      // its blocks of the block table
+};
+struct VoxGrid {       // written by k_vox_grid
+  int min_b[3];        // floor(min_p * inv) per axis
+  int mul[3];          // 1, div_b.x, div_b.x * div_b.y
+  int cells;           // div_b.x * div_b.y * div_b.z; 0: no voxel (no finite point, or too many cells)
+  int too_small;       // 1: the leaf size is too small for this cloud (more than INT32_MAX cells): the cloud stays as it is
+};
+struct VoxBufs {
+  const MapNode* nodes;
+  const int2* blocks;
+  const VoxSeg* segs;
+  uint32_t *bmin, *bmax;  // nnodes x 3 ordered-integer images of the float bounds
+  VoxGrid* grid;
+  uint32_t* key[2];       // ping-pong: voxel index, 0xffffffff for a point that takes no part
+  uint32_t* idx[2];       //            raster index inside the node
+  int* hist;              // nblocks x 256 digit counts, then output positions
+  int* counts;            // run heads per block
+  long long* offs;        // their exclusive scan (nblocks + 1)
+  int2* heads;            // per voxel of the chunk: (position of its first point in the sorted chunk, node)
+};
+// bounds -> grid -> keys into key[0] / idx[0]
+cudaError_t launch_vox_keys(const VoxBufs& b, int nnodes, int nblocks, float inv_leaf, cudaStream_t st, int* n_launches);
+// `passes` stable 8-bit radix passes inside every node's segment, then the run heads and their scan; the sorted arrays are
+// key[passes & 1] / idx[passes & 1]
+cudaError_t launch_vox_sort(const VoxBufs& b, int nnodes, int nblocks, int passes, cudaStream_t st, int* n_launches);
+// One point per voxel into the chunk's slab: node k's planes [x | y | z | colour] of its n_k voxels start at word
+// 4 * offs[blk0_k]
+cudaError_t launch_vox_centroids(const VoxBufs& b, int passes, long long nvoxels, float* slab, cudaStream_t st);
 cudaError_t launch_refine_g2o(const PairDesc* pairs, int npairs, int max_matches, int iterations, const float4* mfrom,
                               const float4* mto, const int32_t* n_all, const rgbdslam_b200_dmatch* matches,
                               rgbdslam_b200_pair_result* results, rgbdslam_b200_dmatch* inlier_matches, cudaStream_t stream);

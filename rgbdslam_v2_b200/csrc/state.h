@@ -40,7 +40,13 @@ struct NodeCloud {
   int32_t w = 0, h = 0, step = 0;  // step > 0: depth-image raster, point (rx, ry) is pixel (rx * step, ry * step)
   float K[4] = {0, 0, 0, 0};    // fx, fy, cx, cy of the call that built it (0 when it passed none)
   NodeSlab* slab = nullptr;     // the allocation the planes live in
-  CloudView view() const { return CloudView{z, x, y, w, h, {K[0], K[1], K[2], K[3]}}; }
+  bool reduced = false;         // voxel-filtered (rgbdslam_b200_reduce_clouds): w x 1 points in ascending voxel index, no raster
+  // The cloud as the environment measurement model reads it: none for a reduced cloud, which has no raster to project into
+  // (the reference refuses voxelfilter_size with the model on, parameter_server.cpp:233).
+  CloudView view() const {
+    if (reduced) return CloudView{nullptr, nullptr, nullptr, 0, 0, {0, 0, 0, 0}};
+    return CloudView{z, x, y, w, h, {K[0], K[1], K[2], K[3]}};
+  }
 };
 
 // Device copy of what the reference's Node keeps per frame (node.h:167-174).
@@ -143,5 +149,6 @@ Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot
   std::lock_guard<std::mutex> entry_lock__(rb200::g_state.mu); \
   if (int entry_rc__ = rb200::check_inited()) return entry_rc__
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
+void release_slab(NodeSlab* slab);  // drops one node's reference to a shared allocation, freeing it with the last (api.cu)
 
 }  // namespace rb200
