@@ -309,7 +309,14 @@ int rgbdslam_b200_orb_compute(const uint8_t* gray, int w, int h, const rgbdslam_
  * handle and the ORB extractor (FAST keypoints keep angle -1: compute() does not orient given keypoints).
  * gray / mask: nframes*w*h bytes, depth: nframes*w*h floats (metres, NaN = invalid), K4 = fx, fy, cx, cy.  Feature order
  * inside a node: (octave, response descending, cell, y, x).  A keypoint's depth is the pixel at its rounded position, or with
- * params.use_feature_min_depth the minimum over its neighbourhood (see rgbdslam_b200_params), for _ex and _sharded too. */
+ * params.use_feature_min_depth the minimum over its neighbourhood (see rgbdslam_b200_params), for _ex and _sharded too.
+ * Frame size limits (every entry point that takes w and h, every input kind of _ex and _sharded; ERR_ARG before any device
+ * work): 96 <= w, h <= 4095, and each grid cell at least 40 px per side at pyramid level 7, so the smallest side that builds
+ * is 142 px without a grid, 222 with detector_grid_resolution 2, 333 with 3 (the default), 444 with 4.  Above 1023 px in
+ * either dimension the detector needs detector_grid_resolution >= 2 and round(1.5 * max_keypoints / cells) < 606 (the
+ * smallest per-level quota of the reference's cv::ORB, whose quotas are applied there: every 3x3 setting qualifies, 2x2 up to
+ * max_keypoints 1614).  A grid cell holds at most 12288 FAST candidates up to 1023 px, proportionally more above
+ * (ERR_STATE when exceeded). */
 int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                int w, int h, const float* K4, const int32_t* ids, uint64_t* node_handles, int32_t* n_features);
 /* The same with options.  RGBDSLAM_B200_MASK_FROM_DEPTH: the detection mask is what the caller of the reference's constructor

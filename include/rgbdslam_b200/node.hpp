@@ -140,7 +140,8 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   // detector / extractor: createDetector / createDescriptorExtractor (features.hpp); the whole constructor
   // -- detect, removeDepthless, retainBest, compute, projectTo3D -- runs as one rgbdslam_b200_nodes_create call, the
   // extractor argument only documents the pairing (ORB or FAST keypoints, ORB descriptors).  id_ stays -1 until
-  // GraphManager::addNode assigns it.
+  // GraphManager::addNode assigns it.  Frames of up to 4095 px per side (the limits of rgbdslam_b200_nodes_create; above
+  // 1023 px the detector grid must be >= 2 and round(1.5 * max_keypoints / cells) < 606).
   Node(const Mat& visual, const Mat& depth, const Mat& detection_mask, const CameraInfoConstPtr& cam_info, myHeader depth_header,
        Ptr<Feature2D> detector, Ptr<DescriptorExtractor> extractor)
       : stamp_(depth_header.stamp) {

@@ -47,6 +47,8 @@ struct OrbCtx {
   DevBuf d_ofs, d_w1;
   OrbTables tab;
   int max_per_cell = 0, min_cell = 0, max_cell = 0, kp_stride = 0;
+  int cand_cap = kOrbCandCap;  // FAST / NMS candidates per (frame, cell): orb_prepare
+  bool wide = false;           // wider or taller than kOrbNarrowMax px
   DevBuf in_gray[2], in_mask[2], in_depth[2];  // double-buffered chunk inputs (upload of chunk k+1 under the kernels of chunk k)
   DevBuf in_rgb[2];                            // colour or Bayer input, converted into in_gray on the device
   DevBuf in_raw[2];                            // 16-bit millimetre depth, converted into in_depth (and in_mask) on the device
@@ -59,7 +61,9 @@ struct OrbCtx {
   // and the per-(frame, cell) tables every rank holds for ALL frames of the sequence
   DevBuf sh_gray, sh_rgb, sh_raw, sh_depth, sh_mask, sh_cell_img, sh_cand, all_hist, all_cnt, all_many, all_thr;
   const uint8_t* last_gray = nullptr;  // device pointers of frame 0 of the last call (debug hooks)
-  OrbCandidates candidates() const { return {(const OrbCand*)cand.ptr, (const int*)cand_count.ptr, (const int*)thr.ptr, (float*)resp.ptr}; }
+  OrbCandidates candidates() const {
+    return {(const OrbCand*)cand.ptr, (const int*)cand_count.ptr, (const int*)thr.ptr, (float*)resp.ptr, cand_cap};
+  }
   void release() {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &in_rgb[0],
                      &in_rgb[1], &in_raw[0], &in_raw[1], &cell_img, &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp,
@@ -75,6 +79,9 @@ static OrbCtx g_orb;
 
 static inline int cv_round_f(float v) { return (int)lrintf(v); }
 static inline float layer_scale(int level) { return (float)std::pow((double)1.2f, (double)level); }  // ORB getScale()
+// a pyramid level's side: cvRound(n * (1.f / scale)) as cv::ORB sizes its levels (orb.cpp detectAndCompute: inv_scale); it
+// differs from n / scale for some n (489 at level 1: 408, not 407), none of them a 640x480 frame's or its grid cells' sides
+static inline int level_side(int n, int level) { return level == 0 ? n : cv_round_f((float)n * (1.f / layer_scale(level))); }
 
 // resize tables src_n -> dst_n (INTER_LINEAR_EXACT): first tap index and weight of the second tap (x256)
 static void build_table(int src_n, int dst_n, std::vector<int16_t>& ofs, std::vector<uint16_t>& w1) {
@@ -100,9 +107,24 @@ static int orb_prepare(int W, int H) {
     set_error("detector_grid_resolution > 4 is not supported");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  if (W < 96 || H < 96 || W > 1023 || H > 1023) {
-    set_error("image size must be within [96, 1023] in both dimensions");
+  if (W < 96 || H < 96 || W > kOrbMaxSide || H > kOrbMaxSide) {
+    set_error("image size must be within [96, 4095] in both dimensions");
     return RGBDSLAM_B200_ERR_ARG;
+  }
+  const bool wide = W > kOrbNarrowMax || H > kOrbNarrowMax;
+  if (wide) {
+    // adjustedGridWrapper's per-cell maximum (features.cpp:52-53), as below.  Below the smallest per-level quota of cv::ORB
+    // (nfeatures 10000: 606 at level 7) a quota that binds leaves more keypoints than that maximum, so the adjuster decides
+    // "too many" with or without it and k_adapt_thresholds needs no quotas (DESIGN.md 4.5.5)
+    const int cells = grid * grid, max_cell = (int)std::lround((int)(K * 1.5) / (float)cells);
+    if (grid < 2) {
+      set_error("frames above 1023 px per side need detector_grid_resolution >= 2");
+      return RGBDSLAM_B200_ERR_ARG;
+    }
+    if (max_cell >= 606) {
+      set_error("frames above 1023 px per side need round(1.5 * max_keypoints / cells) < 606 (cv::ORB's smallest per-level quota)");
+      return RGBDSLAM_B200_ERR_ARG;
+    }
   }
   o.release();
   OrbGeom& g = o.g;
@@ -119,7 +141,7 @@ static int orb_prepare(int W, int H) {
     int prev = n0;
     c.off[0] = 0;
     for (int l = 1; l < kOrbLevels; l++) {
-      const int nl = cv_round_f((float)n0 / layer_scale(l));
+      const int nl = level_side(n0, l);
       c.off[l] = (int)o.h_ofs.size();
       build_table(prev, nl, o.h_ofs, o.h_w1);
       prev = nl;
@@ -147,8 +169,8 @@ static int orb_prepare(int W, int H) {
       for (int l = 0; l < kOrbLevels; l++) {
         OrbPlane& p = g.cell[c][l];
         p.scale = layer_scale(l);
-        p.w = l == 0 ? w0 : cv_round_f((float)w0 / p.scale);
-        p.h = l == 0 ? h0 : cv_round_f((float)h0 / p.scale);
+        p.w = level_side(w0, l);
+        p.h = level_side(h0, l);
         p.off = off;
         p.tx = cx.off[l];
         p.ty = cy.off[l];
@@ -160,14 +182,24 @@ static int orb_prepare(int W, int H) {
       }
     }
   g.cell_bytes = off;
+  // the candidate buffer: kOrbCandCap per cell up to kOrbNarrowMax px; above, the same density per level-0 pixel of the largest
+  // cell as kOrbCandCap in the largest cell of a 640x480 frame's 3x3 grid (275 x 222 px), in multiples of 256
+  o.cand_cap = kOrbCandCap;
+  if (wide) {
+    size_t area = 0;
+    for (int c = 0; c < g.ncells; c++) area = std::max(area, (size_t)g.cell[c][0].w * g.cell[c][0].h);
+    const size_t cap = (area * kOrbCandCap + 275 * 222 - 1) / (275 * 222);
+    o.cand_cap = (int)std::max<size_t>(kOrbCandCap, (cap + 255) / 256 * 256);
+  }
+  o.wide = wide;
   {
     const Chain cx = chain_for(W), cy = chain_for(H);
     int foff = 0;
     for (int l = 0; l < kOrbLevels; l++) {
       OrbPlane& p = g.full[l];
       p.scale = layer_scale(l);
-      p.w = l == 0 ? W : cv_round_f((float)W / p.scale);
-      p.h = l == 0 ? H : cv_round_f((float)H / p.scale);
+      p.w = level_side(W, l);
+      p.h = level_side(H, l);
       p.off = foff;
       p.tx = cx.off[l];
       p.ty = cy.off[l];
@@ -270,9 +302,12 @@ struct FrameInput {
   bool raw_visual() const { return rgb || bayer; }  // the visual is uploaded into in_rgb / sh_rgb and converted into grey
   // frames per chunk: the input and staging buffers hold about as many bytes as kOrbChunk grey + depth-image frames (a
   // 640x480 XYZRGB cloud is 9.8 MB, against 1.5 MB), and never more than kOrbChunk frames, which bounds the per-frame work
-  // buffers (16-bit depth would allow 106); the chunk size does not change any result
-  int chunk(int nframes, size_t px) const {
-    const size_t cap = std::max<size_t>(1, (size_t)kOrbChunk * 5 * px / (gray_bytes + depth_bytes));
+  // buffers (16-bit depth would allow 106); the chunk size does not change any result.  Frames wider or taller than
+  // kOrbNarrowMax px: the same rule in bytes per 640x480 frame, so the buffers stay near their 640x480 grey + depth size
+  // (21 grey + depth frames of 1280x720, 9 of 1920x1080, at least one)
+  int chunk(int nframes, size_t px, bool wide) const {
+    const size_t ref = wide ? (size_t)640 * 480 : px;
+    const size_t cap = std::max<size_t>(1, (size_t)kOrbChunk * 5 * ref / (gray_bytes + depth_bytes));
     return (int)std::min<size_t>((size_t)std::min(std::max(nframes, 1), kOrbChunk), cap);
   }
 };
@@ -305,9 +340,9 @@ static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_byte
         (raw_bytes && (rc = o.in_raw[b].ensure(raw_bytes * F))))
       return rc;
   if ((rc = o.cell_img.ensure((size_t)g.cell_bytes * F)) || (rc = o.cell_mask.ensure((size_t)g.cell_bytes * F)) ||
-      (rc = o.cand.ensure(z * kOrbCandCap * sizeof(OrbCand))) ||
+      (rc = o.cand.ensure(z * o.cand_cap * sizeof(OrbCand))) ||
       (rc = o.cand_count.ensure(z * 4)) || (rc = o.hist.ensure(z * 256 * 4)) || (rc = o.mask_any.ensure(z * 4)) ||
-      (rc = o.thr.ensure(z * 4)) || (rc = o.resp.ensure(z * kOrbCandCap * 4)) ||
+      (rc = o.thr.ensure(z * 4)) || (rc = o.resp.ensure(z * o.cand_cap * 4)) ||
       (rc = o.cell_out.ensure(z * (size_t)o.max_per_cell * 8)) || (rc = o.cell_out_count.ensure(z * 4)) ||
       (rc = o.cand_z.ensure(z * (size_t)o.max_per_cell * 4)) || (rc = o.scratch.ensure((size_t)F * 2 * kOrbFrameCap * kOrbFrameKpBytes)) ||
       (rc = o.kp.ensure((size_t)F * o.kp_stride * sizeof(rgbdslam_b200_keypoint))) ||
@@ -359,10 +394,11 @@ static int orb_detect_stage(Detector* det, int F, const uint8_t* d_gray, const u
   cudaError_t e = orb_run_detect(g, o.tab, F, d_gray, d_mask, d_depth_for_mask, det->type, (uint8_t*)o.cell_img.ptr,
                                  (uint8_t*)o.cell_mask.ptr,
                                  (OrbCand*)o.cand.ptr, (int*)o.cand_count.ptr, (int*)o.hist.ptr,
-                                 (int*)o.mask_any.ptr, st, launches);
+                                 (int*)o.mask_any.ptr, o.cand_cap, st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb detect kernels");
   e = orb_run_adapt(g, F, (const int*)o.hist.ptr, (const int*)o.cand_count.ptr, (const int*)o.mask_any.ptr, (double*)det->d_state.ptr,
-                    (int*)o.thr.ptr, o.min_cell, o.max_cell, s.params.adjuster_max_iterations, (int*)o.err.ptr, st, launches);
+                    (int*)o.thr.ptr, o.min_cell, o.max_cell, s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, st,
+                    launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb threshold kernel");
   det->host_valid = false;
   return 0;
@@ -370,7 +406,7 @@ static int orb_detect_stage(Detector* det, int F, const uint8_t* d_gray, const u
 
 static int orb_check_err_flag(int flag) {
   if (flag & 1) {
-    set_error("ORB / FAST candidate buffer overflow (more than 12288 FAST corners in one grid cell)");
+    set_error("ORB / FAST candidate buffer overflow (more than " + std::to_string(g_orb.cand_cap) + " FAST corners in one grid cell)");
     return RGBDSLAM_B200_ERR_STATE;
   }
   return 0;
@@ -785,7 +821,7 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   if (!in.caller_mask) mask = nullptr;
   if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
-  const int chunk = in.chunk(nframes, px);
+  const int chunk = in.chunk(nframes, px, o.wide);
   if ((rc = orb_ensure_buffers(chunk, 2, in.mask_buffer(), in.plane_bytes, in.raw_visual() ? in.gray_bytes : 0,
                                in.depth_u16 ? in.depth_bytes : 0)))
     return rc;
@@ -900,14 +936,14 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
-  const int chunk = in.chunk(own, px);
+  const int chunk = in.chunk(own, px, o.wide);
   if ((rc = orb_ensure_buffers(chunk, 0, false))) return rc;
   const size_t nc = (size_t)g.ncells;
   const size_t own_ = (size_t)std::max(own, 1);
   if ((rc = o.sh_gray.ensure(px * own_)) || (rc = o.sh_depth.ensure(in.plane_bytes * own_)) ||
       (in.mask_buffer() && (rc = o.sh_mask.ensure(px * own_))) || (in.raw_visual() && (rc = o.sh_rgb.ensure(in.gray_bytes * own_))) ||
       (in.depth_u16 && (rc = o.sh_raw.ensure(in.depth_bytes * own_))) ||
-      (rc = o.sh_cell_img.ensure((size_t)g.cell_bytes * own_)) || (rc = o.sh_cand.ensure(own_ * nc * kOrbCandCap * sizeof(OrbCand))) ||
+      (rc = o.sh_cell_img.ensure((size_t)g.cell_bytes * own_)) || (rc = o.sh_cand.ensure(own_ * nc * o.cand_cap * sizeof(OrbCand))) ||
       (rc = o.all_hist.ensure((size_t)Wp * nc * 256 * 4)) || (rc = o.all_cnt.ensure((size_t)Wp * nc * 4)) ||
       (rc = o.all_many.ensure((size_t)Wp * nc * 4)) || (rc = o.all_thr.ensure((size_t)Wp * nc * 4)))
     return rc;
@@ -948,8 +984,8 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
       return batch_fail(nb, cuda_fail(e, "nodes_create_sharded input kernels"));
     const size_t gf = (size_t)(f0 + c0);  // global index of the chunk's first frame
     e = orb_run_detect(g, o.tab, F, dg, dm, in.mask_from_depth ? dd : nullptr, det->type,
-                       (uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0, (uint8_t*)o.cell_mask.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap,
-                       cnt_all + gf * nc, hist_all + gf * nc * 256, many_all + gf * nc, st, &launches);
+                       (uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0, (uint8_t*)o.cell_mask.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * o.cand_cap,
+                       cnt_all + gf * nc, hist_all + gf * nc * 256, many_all + gf * nc, o.cand_cap, st, &launches);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb detect kernels"));
   }
   // ---- the exchange that makes the frames independent: every rank gets every frame's score histograms, replays the
@@ -962,7 +998,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   }
   if ((rc = detector_to_device(det, st))) return batch_fail(nb, rc);
   e = orb_run_adapt(g, total_frames, hist_all, cnt_all, many_all, (double*)det->d_state.ptr, thr_all, o.min_cell, o.max_cell,
-                    s.params.adjuster_max_iterations, (int*)o.err.ptr, st, &launches);
+                    s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, st, &launches);
   if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb threshold kernel"));
   det->host_valid = false;
   // ---- pass B: Harris / keepStrongest / finalize / describe of the own frames, straight into the slab
@@ -972,8 +1008,8 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     const uint8_t* dg = (const uint8_t*)o.sh_gray.ptr + px * c0;
     const float* dd = (const float*)((const uint8_t*)o.sh_depth.ptr + in.plane_bytes * c0);
     const uint8_t* cimg = (const uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0;
-    const OrbCandidates c = {(const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * kOrbCandCap, cnt_all + gf * nc, thr_all + gf * nc,
-                             (float*)o.resp.ptr};
+    const OrbCandidates c = {(const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * o.cand_cap, cnt_all + gf * nc, thr_all + gf * nc,
+                             (float*)o.resp.ptr, o.cand_cap};
     const FeatureRows rows = {nb.kp + (size_t)c0 * K, nb.xyz + gf * K, nb.n + gf, nb.desc + gf * K * 32, K};
     if ((rc = select_describe(det, in, F, cimg, c, dd, dg, rows, st, &launches))) return batch_fail(nb, rc);
   }
@@ -1013,9 +1049,9 @@ int rgbdslam_b200_orb_debug_candidates(int cell, void* cand_out, float* resp_out
   if (e != cudaSuccess) return cuda_fail(e, "orb_debug_candidates");
   *n_out = n;
   if (thr_out) *thr_out = thr;
-  const int m = std::min(std::min(n, capacity), kOrbCandCap);
-  if (m > 0 && cand_out) cudaMemcpyAsync(cand_out, (const OrbCand*)o.cand.ptr + (size_t)cell * kOrbCandCap, 8 * (size_t)m, cudaMemcpyDeviceToHost, st);
-  if (m > 0 && resp_out) cudaMemcpyAsync(resp_out, (const float*)o.resp.ptr + (size_t)cell * kOrbCandCap, 4 * (size_t)m, cudaMemcpyDeviceToHost, st);
+  const int m = std::min(std::min(n, capacity), o.cand_cap);
+  if (m > 0 && cand_out) cudaMemcpyAsync(cand_out, (const OrbCand*)o.cand.ptr + (size_t)cell * o.cand_cap, 8 * (size_t)m, cudaMemcpyDeviceToHost, st);
+  if (m > 0 && resp_out) cudaMemcpyAsync(resp_out, (const float*)o.resp.ptr + (size_t)cell * o.cand_cap, 4 * (size_t)m, cudaMemcpyDeviceToHost, st);
   e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return cuda_fail(e, "orb_debug_candidates copy");
   return 0;

@@ -266,7 +266,7 @@ __device__ __forceinline__ uint32_t fast_score_pair(const uint16_t (*simg)[kFI_W
 template <bool kFast>
 __device__ __forceinline__ void fast_nms_tile(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
                                               OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist,
-                                              int tiles_x9) {
+                                              int tiles_x9, int cap) {
   constexpr int kEdge = kFast ? kFast9Edge : kFastEdge;
   __shared__ __align__(16) uint16_t simg[kFI_H][kFI_W];
   __shared__ __align__(16) uint8_t ssc[kFS_H][kFS_W];
@@ -336,27 +336,40 @@ __device__ __forceinline__ void fast_nms_tile(const uint8_t* __restrict__ cell_i
     if (cell_mask && cell_mask[base + (size_t)gy * pw + gx] == 0) continue;
     atomicAdd(&hist[fc * 256 + v], 1);
     const int slot = atomicAdd(&cand_count[fc], 1);
-    if (slot < kOrbCandCap) {
+    if (slot < cap) {
       OrbCand cd;
       cd.x = (uint16_t)gx;
       cd.y = (uint16_t)gy;
       cd.level = (uint8_t)level;
       cd.score = (uint8_t)v;
       cd.pad_ = 0;
-      cand[(size_t)fc * kOrbCandCap + slot] = cd;
+      cand[(size_t)fc * cap + slot] = cd;
     }
   }
 }
 
 __global__ void __launch_bounds__(256) k_fast_nms(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
                                                   OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist) {
-  fast_nms_tile<false>(cell_img, cell_mask, cand, cand_count, hist, 0);
+  fast_nms_tile<false>(cell_img, cell_mask, cand, cand_count, hist, 0, kOrbCandCap);
 }
 
 __global__ void __launch_bounds__(256) k_fast9_nms(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
                                                    OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist,
                                                    int tiles_x) {
-  fast_nms_tile<true>(cell_img, cell_mask, cand, cand_count, hist, tiles_x);
+  fast_nms_tile<true>(cell_img, cell_mask, cand, cand_count, hist, tiles_x, kOrbCandCap);
+}
+
+// frames above kOrbNarrowMax px: cap candidates per (frame, cell)
+__global__ void __launch_bounds__(256) k_fast_nms_wide(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
+                                                       OrbCand* __restrict__ cand, int* __restrict__ cand_count, int* __restrict__ hist,
+                                                       int cap) {
+  fast_nms_tile<false>(cell_img, cell_mask, cand, cand_count, hist, 0, cap);
+}
+
+__global__ void __launch_bounds__(256) k_fast9_nms_wide(const uint8_t* __restrict__ cell_img, const uint8_t* __restrict__ cell_mask,
+                                                        OrbCand* __restrict__ cand, int* __restrict__ cand_count,
+                                                        int* __restrict__ hist, int tiles_x, int cap) {
+  fast_nms_tile<true>(cell_img, cell_mask, cand, cand_count, hist, tiles_x, cap);
 }
 
 // All cell planes of one level from the previous level, image and mask together (INTER_LINEAR_EXACT, 8.8 fixed-point taps;
@@ -394,12 +407,11 @@ __global__ void __launch_bounds__(256) k_resize_cells(uint8_t* __restrict__ cell
 // The re-detect loop (x0.7 while too few, <= max_iters detections) only needs #candidates(S >= t): a histogram lookup.
 // One warp per grid cell; lane l owns score bins [8l, 8l+8).  state[c] = the detector's persistent threshold (double, as in
 // the reference); thr_out[f * ncells + c] = the integer FAST threshold of the LAST detection call of that frame.
-// err_flag bit 0: a cell overflowed the candidate buffer.
-__global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds(const int* __restrict__ hist, const int* __restrict__ cand_count,
-                                                                         const int* __restrict__ mask_any, double* __restrict__ state,
-                                                                         int* __restrict__ thr_out, int nframes, int ncells,
-                                                                         int min_features, int max_features, int max_iters,
-                                                                         int* __restrict__ err_flag) {
+// err_flag bit 0: a cell overflowed the candidate buffer (cap candidates per cell).
+__device__ __forceinline__ void adapt_thresholds(const int* __restrict__ hist, const int* __restrict__ cand_count,
+                                                 const int* __restrict__ mask_any, double* __restrict__ state,
+                                                 int* __restrict__ thr_out, int nframes, int ncells, int min_features,
+                                                 int max_features, int max_iters, int* __restrict__ err_flag, int cap) {
   const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (c >= ncells) return;
   double thresh = state[c];
@@ -412,7 +424,7 @@ __global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds(const in
       h[0] = a.x; h[1] = a.y; h[2] = a.z; h[3] = a.w; h[4] = b.x; h[5] = b.y; h[6] = b.z; h[7] = b.w;
     }
     const int cnt = cand_count[fc];
-    if (cnt > kOrbCandCap && lane == 0) atomicOr(err_flag, 1);
+    if (cnt > cap && lane == 0) atomicOr(err_flag, 1);
     const bool mask_nonzero = cnt > 0 || mask_any[fc] != 0;
     int iter = max_iters, used = 0;
     bool checked = false;
@@ -443,6 +455,25 @@ __global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds(const in
     if (lane == 0) thr_out[fc] = used;
   }
   if (lane == 0) state[c] = thresh;
+}
+
+__global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds(const int* __restrict__ hist, const int* __restrict__ cand_count,
+                                                                         const int* __restrict__ mask_any, double* __restrict__ state,
+                                                                         int* __restrict__ thr_out, int nframes, int ncells,
+                                                                         int min_features, int max_features, int max_iters,
+                                                                         int* __restrict__ err_flag) {
+  adapt_thresholds(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters, err_flag,
+                   kOrbCandCap);
+}
+
+__global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds_wide(const int* __restrict__ hist,
+                                                                              const int* __restrict__ cand_count,
+                                                                              const int* __restrict__ mask_any,
+                                                                              double* __restrict__ state, int* __restrict__ thr_out,
+                                                                              int nframes, int ncells, int min_features,
+                                                                              int max_features, int max_iters,
+                                                                              int* __restrict__ err_flag, int cap) {
+  adapt_thresholds(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters, err_flag, cap);
 }
 
 // HarrisResponses(img, pts, blockSize 7, k 0.04): Sobel-3 sums over 7x7, float formula evaluated in the same order
@@ -512,32 +543,54 @@ __device__ float ic_angle_warp(const uint8_t* __restrict__ im, int w, int x0, in
 }
 
 // Harris response for candidates with S >= the cell's final threshold; others get NaN (excluded).
-__global__ void __launch_bounds__(256) k_harris(const uint8_t* __restrict__ cell_img, const OrbCand* __restrict__ cand,
-                                                const int* __restrict__ cand_count, const int* __restrict__ thr,
-                                                float* __restrict__ resp) {
+__device__ __forceinline__ void harris(const uint8_t* __restrict__ cell_img, const OrbCand* __restrict__ cand,
+                                       const int* __restrict__ cand_count, const int* __restrict__ thr, float* __restrict__ resp,
+                                       int cap) {
   const int fc = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = min(cand_count[fc], kOrbCandCap);
+  const int n = min(cand_count[fc], cap);
   if (i >= n) return;
-  const OrbCand cd = cand[(size_t)fc * kOrbCandCap + i];
+  const OrbCand cd = cand[(size_t)fc * cap + i];
   float r = __int_as_float(0x7fc00000);
   if (cd.score >= thr[fc]) {
     const int f = fc / c_geom.ncells, c = fc % c_geom.ncells;
     const OrbPlane& p = c_geom.cell[c][cd.level];
     r = harris_response(cell_img + (size_t)f * c_geom.cell_bytes + p.off, p.w, cd.x, cd.y);
   }
-  resp[(size_t)fc * kOrbCandCap + i] = r;
+  resp[(size_t)fc * cap + i] = r;
+}
+
+__global__ void __launch_bounds__(256) k_harris(const uint8_t* __restrict__ cell_img, const OrbCand* __restrict__ cand,
+                                                const int* __restrict__ cand_count, const int* __restrict__ thr,
+                                                float* __restrict__ resp) {
+  harris(cell_img, cand, cand_count, thr, resp, kOrbCandCap);
+}
+
+__global__ void __launch_bounds__(256) k_harris_wide(const uint8_t* __restrict__ cell_img, const OrbCand* __restrict__ cand,
+                                                     const int* __restrict__ cand_count, const int* __restrict__ thr,
+                                                     float* __restrict__ resp, int cap) {
+  harris(cell_img, cand, cand_count, thr, resp, cap);
 }
 
 // FAST detector: a keypoint's response is its corner score S (cv::FAST); NaN below the cell's final threshold (excluded).
-__global__ void __launch_bounds__(256) k_fast_response(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
-                                                       const int* __restrict__ thr, float* __restrict__ resp) {
+__device__ __forceinline__ void fast_response(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                              const int* __restrict__ thr, float* __restrict__ resp, int cap) {
   const int fc = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = min(cand_count[fc], kOrbCandCap);
+  const int n = min(cand_count[fc], cap);
   if (i >= n) return;
-  const int s = cand[(size_t)fc * kOrbCandCap + i].score;
-  resp[(size_t)fc * kOrbCandCap + i] = s >= thr[fc] ? (float)s : __int_as_float(0x7fc00000);
+  const int s = cand[(size_t)fc * cap + i].score;
+  resp[(size_t)fc * cap + i] = s >= thr[fc] ? (float)s : __int_as_float(0x7fc00000);
+}
+
+__global__ void __launch_bounds__(256) k_fast_response(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                       const int* __restrict__ thr, float* __restrict__ resp) {
+  fast_response(cand, cand_count, thr, resp, kOrbCandCap);
+}
+
+__global__ void __launch_bounds__(256) k_fast_response_wide(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                            const int* __restrict__ thr, float* __restrict__ resp, int cap) {
+  fast_response(cand, cand_count, thr, resp, cap);
 }
 
 __device__ __forceinline__ uint32_t f32_ordered(float f) {  // ascending unsigned order == ascending float order
@@ -563,9 +616,27 @@ __device__ void bitonic_sort_u64(unsigned long long* keys, int N) {
   }
 }
 
+// A keypoint's position in k_cell_select's keys (bits 0-31): [level : 3][y : B][x : B] from bit 29 - 2B up, the sign of the
+// response in bit 0.  B = 10 for frames of up to kOrbNarrowMax px per side, 12 up to kOrbMaxSide (kWide).
+template <bool kWide>
+struct CellPos {
+  static constexpr int kBits = kWide ? 12 : 10, kShift = 29 - 2 * kBits;
+  static constexpr uint32_t kCoord = (1u << kBits) - 1, kMask = (1u << (3 + 2 * kBits)) - 1;
+  static_assert(kShift >= 1, "the position must stay above the sign bit");
+  __device__ static uint32_t pack(int level, int y, int x) {
+    return (((uint32_t)level << (2 * kBits)) | ((uint32_t)y << kBits) | (uint32_t)x) << kShift;
+  }
+  __device__ static void unpack(unsigned long long key, int& level, int& y, int& x) {
+    const uint32_t pos = (uint32_t)(key >> kShift) & kMask;
+    level = pos >> (2 * kBits);
+    y = (pos >> kBits) & kCoord;
+    x = pos & kCoord;
+  }
+};
+
 // keepStrongest(maxPerCell) by |response| (feature_adjuster.cpp:247-255; nth_element order is unspecified in the
 // reference -> canonical tie rule: (level, y, x) ascending).  One CTA per (frame, cell).
-// key = [~ordered(|resp|) : 32][level:3 y:10 x:10 : 23][0 : 9]
+// key = [~ordered(|resp|) : 32][level:3 y:10 x:10 : 23][0 : 9]   (CellPos<false>)
 __global__ void __launch_bounds__(1024) k_cell_select(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
                                                       const float* __restrict__ resp, int max_per_cell,
                                                       unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
@@ -597,6 +668,182 @@ __global__ void __launch_bounds__(1024) k_cell_select(const OrbCand* __restrict_
   const int keep = min(cnt, max_per_cell);
   for (int i = threadIdx.x; i < keep; i += blockDim.x) cell_out[(size_t)fc * out_stride + i] = keys[i];
   if (threadIdx.x == 0) cell_out_count[fc] = keep;
+}
+
+// Shared-memory histogram add with the lanes that hit the same bin merged (bin < 0: no add).  Called by whole warps.
+__device__ __forceinline__ void hist_add_warp(int* h, int bin) {
+  const unsigned peers = __match_any_sync(0xffffffffu, bin);
+  if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&h[bin], __popc(peers));
+}
+
+// The same selection for frames above kOrbNarrowMax px (cap candidates per cell, CellPos<true> keys), where a cell's valid
+// candidates can outnumber any shared-memory sort.  max_per_cell <= 1024 (orb_prepare: < the smallest ORB quota).
+// quotas (ORB detector): first cv::ORB's per-level culls (orb.cpp computeKeyPoints, nfeatures 10000: c_geom.n_per_level),
+//   retainBest(2 n_l) by FAST score, then retainBest(n_l) by Harris response; retainBest keeps every keypoint whose response
+//   equals the n-th largest.  The adjuster's count is unaffected while max_per_cell < min n_l (DESIGN.md 4.5.5).
+// Then keepStrongest: the max_per_cell smallest keys (|response| descending, then level, y, x) by an 8-bit radix select over
+// the 64-bit keys (unique per cell), sorted in shared memory.  One CTA of 1024 threads per (frame, cell); every pass re-reads
+// the cell's candidates (L2-resident).
+__global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                           const float* __restrict__ resp, int cap, int quotas, int max_per_cell,
+                                                           unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
+                                                           int out_stride) {
+  using Pos = CellPos<true>;
+  __shared__ int hist[kOrbLevels * 256];
+  __shared__ unsigned long long keys[1024];
+  __shared__ int s_score_cut[kOrbLevels], s_want[kOrbLevels];
+  __shared__ uint32_t s_resp_cut[kOrbLevels];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_shift, s_done, s_n;
+  const int fc = blockIdx.x;
+  if (max_per_cell <= 0) {
+    if (threadIdx.x == 0) cell_out_count[fc] = 0;
+    return;
+  }
+  const int n = min(cand_count[fc], cap);
+  const int n_warps = (n + 31) & ~31;  // loop bound for whole warps (hist_add_warp)
+  const OrbCand* cc = cand + (size_t)fc * cap;
+  const float* rr = resp + (size_t)fc * cap;
+  const int t = threadIdx.x;
+  // candidate i passes the per-level culls decided so far (all, until they are decided)
+  auto survives = [&](int i, OrbCand& cd, float& r) -> bool {
+    r = rr[i];
+    if (!(r == r)) return false;
+    cd = cc[i];
+    if (!quotas) return true;
+    return cd.score >= s_score_cut[cd.level] && f32_ordered(r + 0.f) >= s_resp_cut[cd.level];  // + 0.f: -0 ties +0
+  };
+  if (t < kOrbLevels) {
+    s_score_cut[t] = 0;
+    s_resp_cut[t] = 0;
+  }
+  if (quotas) {
+    // retainBest(2 n_l) by FAST score: cut at the (2 n_l)-th largest score of the level
+    for (int i = t; i < kOrbLevels * 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    for (int i = t; i < n_warps; i += blockDim.x) {
+      OrbCand cd;
+      float r;
+      const bool ok = i < n && survives(i, cd, r);
+      hist_add_warp(hist, ok ? cd.level * 256 + cd.score : -1);
+    }
+    __syncthreads();
+    if (t < kOrbLevels) {
+      const int q = 2 * c_geom.n_per_level[t];
+      int cum = 0, cut = 0, kept = 0;
+      for (int s = 255; s >= 0; s--) {
+        cum += hist[t * 256 + s];
+        if (cum >= q) {
+          cut = s;
+          break;
+        }
+      }
+      for (int s = cut; s < 256; s++) kept += hist[t * 256 + s];
+      s_score_cut[t] = cut;
+      // retainBest(n_l) by Harris response: radix select of the n_l-th largest ordered response (want < 0: nothing to cut)
+      s_want[t] = kept > c_geom.n_per_level[t] ? c_geom.n_per_level[t] : -1;
+    }
+    __syncthreads();
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int i = t; i < kOrbLevels * 256; i += blockDim.x) hist[i] = 0;
+      __syncthreads();
+      const uint32_t hi = shift == 24 ? 0u : ~0u << (shift + 8);
+      for (int i = t; i < n_warps; i += blockDim.x) {
+        OrbCand cd;
+        float r;
+        int bin = -1;
+        if (i < n && survives(i, cd, r) && s_want[cd.level] > 0) {
+          const uint32_t o = f32_ordered(r + 0.f);
+          if ((o & hi) == (s_resp_cut[cd.level] & hi)) bin = cd.level * 256 + ((o >> shift) & 255);
+        }
+        hist_add_warp(hist, bin);
+      }
+      __syncthreads();
+      if (t < kOrbLevels && s_want[t] > 0) {
+        int cum = 0;
+        for (int b = 255; b >= 0; b--) {
+          const int h = hist[t * 256 + b];
+          if (cum + h >= s_want[t]) {
+            s_resp_cut[t] |= (uint32_t)b << shift;  // survives() compares the full word only after the last pass
+            s_want[t] -= cum;
+            break;
+          }
+          cum += h;
+        }
+      }
+      __syncthreads();
+    }
+    // s_resp_cut is now the n_l-th largest ordered response of each level that had one to cut, 0 (keep all) elsewhere
+  }
+  // keepStrongest(max_per_cell): radix select of the max_per_cell-th smallest key, 8 bits per pass from the top; a pass whose
+  // boundary bin holds exactly the keys still wanted ends the select (every key is unique, so the last pass always does)
+  auto key_of = [&](const OrbCand& cd, float r) -> unsigned long long {
+    return ((unsigned long long)(~f32_ordered(fabsf(r))) << 32) | Pos::pack(cd.level, cd.y, cd.x) | (r < 0.f ? 1ull : 0ull);
+  };
+  if (t == 0) {
+    s_prefix = 0;
+    s_shift = 64;
+    s_done = 0;
+    s_want[0] = max_per_cell;
+    s_n = 0;
+  }
+  __syncthreads();
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int i = t; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const unsigned long long hi = shift == 56 ? 0ull : ~0ull << (shift + 8), prefix = s_prefix;
+    for (int i = t; i < n_warps; i += blockDim.x) {
+      OrbCand cd;
+      float r;
+      int bin = -1;
+      if (i < n && survives(i, cd, r)) {
+        const unsigned long long k = key_of(cd, r);
+        if ((k & hi) == (prefix & hi)) bin = (int)((k >> shift) & 255);
+      }
+      hist_add_warp(hist, bin);
+    }
+    __syncthreads();
+    if (t == 0) {
+      int cum = 0, b = 0;
+      for (; b < 256; b++) {
+        if (cum + hist[b] >= s_want[0]) break;
+        cum += hist[b];
+      }
+      if (b == 256) {  // fewer survivors than max_per_cell (first pass only): keep them all
+        s_prefix = ~0ull;
+        s_shift = 0;
+        s_done = 1;
+      } else {
+        s_prefix |= (unsigned long long)b << shift;
+        s_want[0] -= cum;
+        if (hist[b] == s_want[0]) {
+          s_shift = shift;
+          s_done = 1;
+        }
+      }
+    }
+    __syncthreads();
+    if (s_done) break;
+  }
+  const int sel_shift = s_shift;  // < 64: the last pass always ends the select
+  const unsigned long long sel = s_prefix >> sel_shift;
+  for (int i = t; i < n; i += blockDim.x) {
+    OrbCand cd;
+    float r;
+    if (survives(i, cd, r)) {
+      const unsigned long long k = key_of(cd, r);
+      if ((k >> sel_shift) <= sel) keys[atomicAdd(&s_n, 1)] = k;
+    }
+  }
+  __syncthreads();
+  const int cnt = s_n;
+  int N = 2;
+  while (N < cnt) N <<= 1;
+  for (int i = cnt + t; i < N; i += blockDim.x) keys[i] = ~0ull;
+  __syncthreads();
+  bitonic_sort_u64(keys, N);
+  for (int i = t; i < cnt; i += blockDim.x) cell_out[(size_t)fc * out_stride + i] = keys[i];
+  if (t == 0) cell_out_count[fc] = cnt;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -631,7 +878,8 @@ static_assert(kFrameCap == kOrbFrameCap && sizeof(FrameKpZ) == kOrbFrameKpBytes 
 // clamped to the image -- 2r x 2r, not centred.  Z = the minimum over the window, NaN pixels ignored (fminf), NaN when the
 // window holds no number or its minimum is 0 (the reference's FIXME branch; -0 == 0).  One warp per candidate, lanes stride
 // the columns of each window row.  cand_z[fc * out_stride + i] pairs with cell_out[fc * out_stride + i].
-__global__ void __launch_bounds__(256) k_min_depth(OrbFrameArgs a, int fast) {
+template <bool kWide>
+__device__ __forceinline__ void min_depth(const OrbFrameArgs& a, int fast) {
   const unsigned long long* __restrict__ cell_out = a.cell_out;
   const int* __restrict__ cell_out_count = a.cell_out_count;
   const float* __restrict__ depth = a.depth;
@@ -641,8 +889,8 @@ __global__ void __launch_bounds__(256) k_min_depth(OrbFrameArgs a, int fast) {
   if (i >= cell_out_count[fc]) return;
   const int W = c_geom.W, H = c_geom.H;
   const int f = fc / c_geom.ncells, c = fc % c_geom.ncells;
-  const uint32_t pos = (uint32_t)((cell_out[(size_t)fc * a.out_stride + i] >> 9) & 0x7FFFFFu);
-  const int level = pos >> 20, ly = (pos >> 10) & 1023, lx = pos & 1023;
+  int level, ly, lx;
+  CellPos<kWide>::unpack(cell_out[(size_t)fc * a.out_stride + i], level, ly, lx);
   const float sc = c_geom.cell[c][level].scale;
   const float x = __fadd_rn(__fmul_rn((float)lx, sc), (float)c_geom.cell_x0[c]);  // as k_frame_finalize
   const float y = __fadd_rn(__fmul_rn((float)ly, sc), (float)c_geom.cell_y0[c]);
@@ -659,6 +907,9 @@ __global__ void __launch_bounds__(256) k_min_depth(OrbFrameArgs a, int fast) {
   if (lane == 0) cand_z[(size_t)fc * a.out_stride + i] = m == 0.f ? __int_as_float(0x7fc00000) : m;
 }
 
+__global__ void __launch_bounds__(256) k_min_depth(OrbFrameArgs a, int fast) { min_depth<false>(a, fast); }
+__global__ void __launch_bounds__(256) k_min_depth_wide(OrbFrameArgs a, int fast) { min_depth<true>(a, fast); }
+
 // mode 0: detector output, cell-major, inside a cell |response| descending (canonical stand-in for the unspecified
 //         nth_element order), ties by (level, y, x).
 // mode 1: Node constructor: removeDepthless -> retainBest(K) by signed response (ties canonical, cut at K) ->
@@ -673,7 +924,8 @@ __global__ void __launch_bounds__(256) k_min_depth(OrbFrameArgs a, int fast) {
 // truncated position ((int)x, (int)y) has no NaN coordinate, up to max_keypoints kept; then compute()'s border filter and
 // octave sort.  Final order = (octave, cell, |response| descending, y, x).  maximum_depth is fixed at its default, +inf, so
 // the reference's z > maximum_depth test never drops a point.  `depth` is the cloud, cloud_stride floats per point.
-template <OrbPoints P>
+// kWide: the keys of k_cell_select_wide (CellPos<true>), frames above kOrbNarrowMax px.
+template <OrbPoints P, bool kWide>
 __global__ void __launch_bounds__(1024) k_frame_finalize(OrbFrameArgs a) {
   using Kp = FrameKpOf<P>;
   const int mode = P == OrbPoints::kDepthPixel ? a.mode : 1;
@@ -691,8 +943,8 @@ __global__ void __launch_bounds__(1024) k_frame_finalize(OrbFrameArgs a) {
     const int n = __ldg(&a.cell_out_count[fc]);
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const unsigned long long k = __ldg(&a.cell_out[(size_t)fc * out_stride + i]);
-      const uint32_t pos = (uint32_t)((k >> 9) & 0x7FFFFFu);
-      const int level = pos >> 20, ly = (pos >> 10) & 1023, lx = pos & 1023;
+      int level, ly, lx;
+      CellPos<kWide>::unpack(k, level, ly, lx);
       const uint32_t ord = ~(uint32_t)(k >> 32);
       float r = __uint_as_float(ord & 0x7FFFFFFFu);  // |resp| (ordered() of a non-negative float only sets bit 31)
       if (k & 1ull) r = -r;
@@ -823,9 +1075,12 @@ __global__ void __launch_bounds__(1024) k_frame_finalize(OrbFrameArgs a) {
   if (threadIdx.x == 0) a.n_out[f] = n_final;
 }
 
-template __global__ void k_frame_finalize<OrbPoints::kDepthPixel>(OrbFrameArgs);
-template __global__ void k_frame_finalize<OrbPoints::kMinDepth>(OrbFrameArgs);
-template __global__ void k_frame_finalize<OrbPoints::kCloud>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kDepthPixel, false>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kMinDepth, false>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kCloud, false>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kDepthPixel, true>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kMinDepth, true>(OrbFrameArgs);
+template __global__ void k_frame_finalize<OrbPoints::kCloud, true>(OrbFrameArgs);
 
 // One warp per output keypoint: intensity-centroid orientation on the detector's (cell) pyramid, the cv::KeyPoint record,
 // in mode 1 projectTo3D (node.cpp:900-965) + backProject (misc2.h:49-65) and the rotation (cos, sin) compute() will use.
@@ -904,13 +1159,18 @@ template __global__ void k_frame_emit<RGBDSLAM_B200_DETECTOR_FAST, OrbPoints::kC
 
 // -------------------------------------------------------------------------------------------------
 // GaussianBlur(level, 7x7, sigma 2, BORDER_REFLECT_101) as OpenCV evaluates it inside ORB: separable float filter,
-// row pass accumulated left to right, column pass symmetric, round-half-even to uint8.
+// row pass accumulated left to right, column pass symmetric, round-half-even to uint8.  kFma: every multiply-add of both
+// passes fused, as cv2 4.13's SIMD row and column filters compute them on x86-64 with FMA (RowVec_8u32f,
+// SymmColumnVec_32f8u: v_muladd); equal to cv2 on every pixel of a 4095x360 frame's pyramid where the unfused rule differs
+// at a few pixels per level.  Frames above kOrbNarrowMax px use it; the unfused rule stays for smaller frames (DESIGN.md
+// 4.5.5).
 __device__ __forceinline__ int reflect101(int i, int n) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * n - 2 - i;
   return i;
 }
 
+template <bool kFma>
 __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int frame_stride,
                                               int level) {
   const OrbPlane& p = c_geom.full[level];
@@ -930,7 +1190,12 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
   for (int r = ty; r < 22; r += 8) {
     float acc = 0.f;
 #pragma unroll
-    for (int j = 0; j < 7; j++) acc = __fadd_rn(acc, __fmul_rn(c_gauss[j], tile[r][tx + j]));  // left to right, as cv::sepFilter2D
+    for (int j = 0; j < 7; j++) {  // left to right, as cv::sepFilter2D
+      if constexpr (kFma)
+        acc = __fmaf_rn(c_gauss[j], tile[r][tx + j], acc);
+      else
+        acc = __fadd_rn(acc, __fmul_rn(c_gauss[j], tile[r][tx + j]));
+    }
     rows[r][tx] = acc;
   }
   __syncthreads();
@@ -940,7 +1205,13 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
     if (x < pw && y < ph) {
       float c = __fmul_rn(c_gauss[3], rows[r + 3][tx]);
 #pragma unroll
-      for (int j = 1; j <= 3; j++) c = __fadd_rn(c, __fmul_rn(c_gauss[3 + j], __fadd_rn(rows[r + 3 + j][tx], rows[r + 3 - j][tx])));
+      for (int j = 1; j <= 3; j++) {
+        const float pair = __fadd_rn(rows[r + 3 + j][tx], rows[r + 3 - j][tx]);
+        if constexpr (kFma)
+          c = __fmaf_rn(c_gauss[3 + j], pair, c);
+        else
+          c = __fadd_rn(c, __fmul_rn(c_gauss[3 + j], pair));
+      }
       int v = __float2int_rn(c);
       v = min(max(v, 0), 255);
       dst[(size_t)f * frame_stride + p.off + (size_t)y * pw + x] = (uint8_t)v;
@@ -994,11 +1265,12 @@ __global__ void __launch_bounds__(256) k_describe(const uint8_t* __restrict__ py
 // ================================================================================================
 // launch helpers (host)
 static inline dim3 plane_grid(int w, int h, int z) { return dim3((w + 31) / 32, (h + 7) / 8, z); }
+static inline bool is_wide(const OrbGeom& g) { return g.W > kOrbNarrowMax || g.H > kOrbNarrowMax; }
 
 cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, const uint8_t* d_mask,
                            const float* d_depth_for_mask, int detector, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
-                           int* d_cand_count, int* d_hist, int* d_mask_any, cudaStream_t st, int* launches) {
-  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST;
+                           int* d_cand_count, int* d_hist, int* d_mask_any, int cand_cap, cudaStream_t st, int* launches) {
+  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST, wide = is_wide(g);
   int maxw = 0, maxh = 0;
   for (int c = 0; c < g.ncells; c++) {
     maxw = g.cell[c][0].w > maxw ? g.cell[c][0].w : maxw;
@@ -1022,11 +1294,15 @@ cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, 
   }
   const int tiles = g_fast_tiles[fast ? RGBDSLAM_B200_DETECTOR_FAST : RGBDSLAM_B200_DETECTOR_ORB];
   if (tiles > 0) {
-    if (fast)
-      k_fast9_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, d_cand, d_cand_count, d_hist,
-                                                  g_fast9_tiles_x);
+    const uint8_t* m = all_valid ? nullptr : d_cell_mask;
+    if (fast && wide)
+      k_fast9_nms_wide<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, g_fast9_tiles_x, cand_cap);
+    else if (fast)
+      k_fast9_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, g_fast9_tiles_x);
+    else if (wide)
+      k_fast_nms_wide<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, cand_cap);
     else
-      k_fast_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, all_valid ? nullptr : d_cell_mask, d_cand, d_cand_count, d_hist);
+      k_fast_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist);
     (*launches)++;
   }
   return cudaGetLastError();
@@ -1063,19 +1339,26 @@ cudaError_t orb_run_bayer_gr_to_gray(int nframes, int w, int h, const uint8_t* d
 
 cudaError_t orb_run_adapt(const OrbGeom& g, int nframes, const int* d_hist, const int* d_cand_count, const int* d_mask_any,
                           double* d_state, int* d_thr, int min_features, int max_features, int max_iters, int* d_err,
-                          cudaStream_t st, int* launches) {
-  k_adapt_thresholds<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
-                                                      min_features, max_features, max_iters, d_err);
+                          int cand_cap, cudaStream_t st, int* launches) {
+  if (is_wide(g))
+    k_adapt_thresholds_wide<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
+                                                             min_features, max_features, max_iters, d_err, cand_cap);
+  else
+    k_adapt_thresholds<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
+                                                        min_features, max_features, max_iters, d_err);
   (*launches)++;
   return cudaGetLastError();
 }
 
-// k_frame_finalize<P> and the detector's k_frame_emit<D, P>
+// k_frame_finalize<P, wide> and the detector's k_frame_emit<D, P>
 template <OrbPoints P>
-static void launch_frames(int nframes, bool fast, const OrbFrameArgs& a, cudaStream_t st, int* launches) {
+static void launch_frames(int nframes, bool fast, bool wide, const OrbFrameArgs& a, cudaStream_t st, int* launches) {
   const int max_out = a.mode == 1 && a.max_keypoints < a.kp_stride ? a.max_keypoints : a.kp_stride;
   const dim3 grid((max_out + 7) / 8, nframes);
-  k_frame_finalize<P><<<nframes, 1024, 0, st>>>(a);
+  if (wide)
+    k_frame_finalize<P, true><<<nframes, 1024, 0, st>>>(a);
+  else
+    k_frame_finalize<P, false><<<nframes, 1024, 0, st>>>(a);
   if (fast)
     k_frame_emit<RGBDSLAM_B200_DETECTOR_FAST, P><<<grid, 256, 0, st>>>(a);
   else
@@ -1085,32 +1368,48 @@ static void launch_frames(int nframes, bool fast, const OrbFrameArgs& a, cudaStr
 
 cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
                            const OrbFrameArgs& a, cudaStream_t st, int* launches) {
-  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST;
+  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST, wide = is_wide(g);
   const int z = nframes * g.ncells, max_per_cell = a.out_stride;
-  if (fast)
-    k_fast_response<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(c.cand, c.count, c.thr, c.resp);
-  else
-    k_harris<<<dim3((kOrbCandCap + 255) / 256, z), 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp);
-  (*launches)++;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(k_cell_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
-    if (e != cudaSuccess) return e;
-    attr = true;
+  const dim3 rgrid((c.cap + 255) / 256, z);
+  if (wide) {
+    if (fast)
+      k_fast_response_wide<<<rgrid, 256, 0, st>>>(c.cand, c.count, c.thr, c.resp, c.cap);
+    else
+      k_harris_wide<<<rgrid, 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp, c.cap);
+    (*launches)++;
+    // the FAST detector has no quotas (cv::FastFeatureDetector)
+    k_cell_select_wide<<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, fast ? 0 : 1, max_per_cell, a.cell_out, a.cell_out_count,
+                                           max_per_cell);
+    (*launches)++;
+  } else {
+    if (fast)
+      k_fast_response<<<rgrid, 256, 0, st>>>(c.cand, c.count, c.thr, c.resp);
+    else
+      k_harris<<<rgrid, 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp);
+    (*launches)++;
+    static bool attr = false;
+    if (!attr) {
+      cudaError_t e = cudaFuncSetAttribute(k_cell_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
+      if (e != cudaSuccess) return e;
+      attr = true;
+    }
+    k_cell_select<<<z, 1024, 16384 * 8, st>>>(c.cand, c.count, c.resp, max_per_cell, a.cell_out, a.cell_out_count, max_per_cell);
+    (*launches)++;
   }
-  k_cell_select<<<z, 1024, 16384 * 8, st>>>(c.cand, c.count, c.resp, max_per_cell, a.cell_out, a.cell_out_count, max_per_cell);
-  (*launches)++;
   switch (points) {
     case OrbPoints::kDepthPixel:
-      launch_frames<OrbPoints::kDepthPixel>(nframes, fast, a, st, launches);
+      launch_frames<OrbPoints::kDepthPixel>(nframes, fast, wide, a, st, launches);
       break;
     case OrbPoints::kMinDepth:
-      k_min_depth<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(a, fast);
+      if (wide)
+        k_min_depth_wide<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(a, fast);
+      else
+        k_min_depth<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(a, fast);
       (*launches)++;
-      launch_frames<OrbPoints::kMinDepth>(nframes, fast, a, st, launches);
+      launch_frames<OrbPoints::kMinDepth>(nframes, fast, wide, a, st, launches);
       break;
     case OrbPoints::kCloud:
-      launch_frames<OrbPoints::kCloud>(nframes, fast, a, st, launches);
+      launch_frames<OrbPoints::kCloud>(nframes, fast, wide, a, st, launches);
       break;
   }
   return cudaGetLastError();
@@ -1128,7 +1427,11 @@ cudaError_t orb_run_describe(const OrbGeom& g, const OrbTables& tab, int nframes
     (*launches)++;
   }
   for (int l = 0; l < levels; l++) {
-    k_blur<<<dim3((g.full[l].w + 31) / 32, (g.full[l].h + 15) / 16, nframes), 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
+    const dim3 grid((g.full[l].w + 31) / 32, (g.full[l].h + 15) / 16, nframes);
+    if (is_wide(g))
+      k_blur<true><<<grid, 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
+    else
+      k_blur<false><<<grid, 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
     (*launches)++;
   }
   k_describe<<<dim3((max_kp + 7) / 8, nframes), 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, d_kp, d_n, kp_stride, d_trig, d_desc);

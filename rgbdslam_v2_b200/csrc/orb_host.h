@@ -11,14 +11,15 @@ cudaError_t orb_upload_constants(const OrbGeom& g, const int* umax, cudaStream_t
 
 // d_depth_for_mask != nullptr: detection mask = depthToCV8UC1(depth) != 0 (misc.cpp:414-418), d_mask ignored.
 // detector: RGBDSLAM_B200_DETECTOR_ORB (8-level cell pyramids) or _FAST (level 0 only, cv::FAST's 3 px border).
+// cand_cap: candidates per (frame, cell) in d_cand, kOrbCandCap unless the frame is wider or taller than kOrbNarrowMax.
 cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, const uint8_t* d_mask,
                            const float* d_depth_for_mask, int detector, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
-                           int* d_cand_count, int* d_hist, int* d_mask_any, cudaStream_t st, int* launches);
+                           int* d_cand_count, int* d_hist, int* d_mask_any, int cand_cap, cudaStream_t st, int* launches);
 
 // the adaptive-threshold recurrence of the F frames of a chunk, on the device (no host round trip)
 cudaError_t orb_run_adapt(const OrbGeom& g, int nframes, const int* d_hist, const int* d_cand_count, const int* d_mask_any,
                           double* d_state, int* d_thr, int min_features, int max_features, int max_iters, int* d_err,
-                          cudaStream_t st, int* launches);
+                          int cand_cap, cudaStream_t st, int* launches);
 
 // cvtColor(CV_RGB2GRAY) of nframes packed w*h*3 colour images into grey (node.cpp:139-144, 275-277).
 cudaError_t orb_run_rgb_to_gray(int nframes, size_t px, const uint8_t* d_rgb, uint8_t* d_gray, cudaStream_t st, int* launches);
@@ -45,6 +46,7 @@ struct OrbCandidates {
   const int* count;
   const int* thr;
   float* resp;
+  int cap;  // candidates per (frame, cell): the stride of cand and resp
 };
 
 // What k_min_depth, k_frame_finalize and k_frame_emit read and write, passed by value.
@@ -69,6 +71,7 @@ struct OrbFrameArgs {
 };
 
 // detector ORB: Harris responses, orientation, size 31 * scale; FAST: response = corner score, angle -1, size 7.
+// Frames wider or taller than kOrbNarrowMax px also apply cv::ORB's per-level quotas (ORB detector; k_cell_select_wide).
 cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
                            const OrbFrameArgs& a, cudaStream_t st, int* launches);
 

@@ -249,13 +249,21 @@ def _texture(seed: int, size: int = 1024) -> np.ndarray:
     return _TEX[key]
 
 
-def render_frame(pose_wc: np.ndarray, tex_seed: int = 7, nan_frac: float = 0.03, seed: int = 0, depth_noise: float = 0.0):
+def intrinsics(w: int = W, h: int = H):
+    """(fx, fy, cx, cy) of a w x h rendering: the 640x480 camera's field of view at w x h pixels"""
+    return FX * w / W, FY * h / H, (w - 1) / 2, (h - 1) / 2
+
+
+def render_frame(pose_wc: np.ndarray, tex_seed: int = 7, nan_frac: float = 0.03, seed: int = 0, depth_noise: float = 0.0,
+                 shape: tuple[int, int] = (H, W)):
     """pose_wc: 4x4 camera-to-world.  Scene: back wall z=4, floor y=1.3, left wall x=-3, right wall x=3 (world frame).
-    Returns gray u8 [480,640], depth f32 [480,640] (metres, NaN holes)."""
+    Returns gray u8 [h,w], depth f32 [h,w] (metres, NaN holes) for shape (h, w), camera intrinsics(w, h)."""
     import cv2
     rng = np.random.default_rng(seed)
+    H, W = shape
+    fx, fy, cx, cy = intrinsics(W, H)
     v, u = np.mgrid[0:H, 0:W].astype(np.float64)
-    rays_c = np.stack([(u - CX) / FX, (v - CY) / FY, np.ones_like(u)], -1)
+    rays_c = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], -1)
     R, t = pose_wc[:3, :3], pose_wc[:3, 3]
     rays_w = rays_c @ R.T
     planes = [((0, 0, 1.0), 4.0, 0), ((0, 1.0, 0), 1.3, 1), ((-1.0, 0, 0), 3.0, 2), ((1.0, 0, 0), 3.0, 3)]  # n.x = d
@@ -280,8 +288,8 @@ def render_frame(pose_wc: np.ndarray, tex_seed: int = 7, nan_frac: float = 0.03,
     depth[~np.isfinite(depth)] = np.nan
     if depth_noise > 0:
         depth = (depth + rng.normal(size=depth.shape) * depth_noise * depth * depth).astype(np.float32)
-    holes = rng.random((H // 8, W // 8)) < nan_frac
-    depth[np.kron(holes, np.ones((8, 8), bool))] = np.nan
+    holes = rng.random(((H + 7) // 8, (W + 7) // 8)) < nan_frac
+    depth[np.kron(holes, np.ones((8, 8), bool))[:H, :W]] = np.nan
     depth[rng.random(depth.shape) < nan_frac / 3] = np.nan
     return np.ascontiguousarray(gray), np.ascontiguousarray(depth)
 
