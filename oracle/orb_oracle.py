@@ -26,6 +26,11 @@ def layer_scale(level: int) -> np.float32:
     return np.float32(np.float64(np.float32(1.2)) ** level)
 
 
+def level_side(n: int, level: int) -> int:
+    """a pyramid level's side as cv::ORB sizes it: cvRound(n * (1.f / scale)) in float (orb.cpp detectAndCompute)"""
+    return n if level == 0 else int(np.rint(np.float32(n) * (np.float32(1) / layer_scale(level))))
+
+
 def depth_to_mask(depth: np.ndarray) -> np.ndarray:
     """depthToCV8UC1 (misc.cpp:414-418): depth.convertTo(mono8, CV_8UC1, 100, 0) = saturate_cast<uchar>(cvRound(d * 100)),
     NaN -> 0, negative -> 0.  cv2's Python API has no Mat::convertTo; convertScaleAbs is the same conversion of |d * 100|,

@@ -512,10 +512,11 @@ class Frontend:
         return [int(h) for h in handles], nf
 
     def orb_debug_plane(self, which: int, cell: int, level: int) -> np.ndarray:
-        buf = np.zeros(1024 * 1024, np.uint8)
         w, h = C.c_int(), C.c_int()
+        self._check(self.lib.rgbdslam_b200_orb_debug_plane(which, cell, level, None, 0, C.byref(w), C.byref(h)))
+        buf = np.zeros((h.value, w.value), np.uint8)
         self._check(self.lib.rgbdslam_b200_orb_debug_plane(which, cell, level, _ptr(buf), buf.size, C.byref(w), C.byref(h)))
-        return buf[: w.value * h.value].reshape(h.value, w.value).copy()
+        return buf
 
     def orb_debug_candidates(self, cell: int):
         dt = np.dtype([("x", "<u2"), ("y", "<u2"), ("level", "u1"), ("score", "u1"), ("pad", "<u2")])

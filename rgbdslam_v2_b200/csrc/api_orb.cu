@@ -49,6 +49,7 @@ struct OrbCtx {
   int max_per_cell = 0, min_cell = 0, max_cell = 0, kp_stride = 0;
   int cand_cap = kOrbCandCap;  // FAST / NMS candidates per (frame, cell): orb_prepare
   bool wide = false;           // wider or taller than kOrbNarrowMax px
+  bool quotas = false;         // the ORB detector applies cv::ORB's per-level quotas: orb_prepare
   DevBuf in_gray[2], in_mask[2], in_depth[2];  // double-buffered chunk inputs (upload of chunk k+1 under the kernels of chunk k)
   DevBuf in_rgb[2];                            // colour or Bayer input, converted into in_gray on the device
   DevBuf in_raw[2];                            // 16-bit millimetre depth, converted into in_depth (and in_mask) on the device
@@ -85,7 +86,9 @@ static inline int level_side(int n, int level) { return level == 0 ? n : cv_roun
 
 // resize tables src_n -> dst_n (INTER_LINEAR_EXACT): first tap index and weight of the second tap (x256)
 static void build_table(int src_n, int dst_n, std::vector<int16_t>& ofs, std::vector<uint16_t>& w1) {
-  const double scale = (double)src_n / dst_n;
+  // cv::resize's scale_x = 1. / inv_scale_x with inv_scale_x = (double)dst / src, not src / dst: the two differ in the last
+  // bit for some sides, and at 3993 -> 3328 (level 1) that moves one tap weight across a rounding boundary
+  const double scale = 1.0 / ((double)dst_n / src_n);
   for (int d = 0; d < dst_n; d++) {
     const double f = (d + 0.5) * scale - 0.5;
     int i = (int)std::floor(f);
@@ -246,6 +249,11 @@ static int orb_prepare(int W, int H) {
     return RGBDSLAM_B200_ERR_ARG;
   }
   o.kp_stride = std::min(kOrbFrameCap, o.max_per_cell * g.ncells);
+  // cv::ORB's per-level quotas where a binding one leaves more keypoints than the cell's maximum (smallest quota 606), so that
+  // the adjuster's "too many" stands with or without them and k_adapt_thresholds stays exact.  At or above 606 per cell (the
+  // ungridded detector, 2x2 above K = 1614; only frames of up to kOrbNarrowMax px get here) a binding quota can change the
+  // adjuster's count, and the quotas are not applied (DESIGN.md 4.5.5).
+  o.quotas = grid > 1 && o.max_cell < 606;
   o.W = W; o.H = H; o.grid = grid; o.max_kp = K;
   int rc;
   if ((rc = o.d_ofs.ensure(o.h_ofs.size() * 2 + 16)) || (rc = o.d_w1.ensure(o.h_w1.size() * 2 + 16))) return rc;
@@ -587,7 +595,7 @@ static int select_describe(const Detector* det, const FrameInput& in, int F, con
   a.kp_stride = out.stride;
   a.max_keypoints = g_state.params.max_keypoints;
   a.mode = in.mode;
-  cudaError_t e = orb_run_select(o.g, F, det->type, in.points, c, a, st, launches);
+  cudaError_t e = orb_run_select(o.g, F, det->type, o.quotas, in.points, c, a, st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb select kernels");
   if (in.mode == 1) {
     e = orb_run_describe(o.g, o.tab, F, det->describe_levels(), dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, out.kp, out.n,

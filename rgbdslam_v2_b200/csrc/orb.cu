@@ -676,19 +676,21 @@ __device__ __forceinline__ void hist_add_warp(int* h, int bin) {
   if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&h[bin], __popc(peers));
 }
 
-// The same selection for frames above kOrbNarrowMax px (cap candidates per cell, CellPos<true> keys), where a cell's valid
-// candidates can outnumber any shared-memory sort.  max_per_cell <= 1024 (orb_prepare: < the smallest ORB quota).
+// The same selection with cv::ORB's per-level quotas: every ORB geometry with round(1.5 K / cells) < 606, and frames above
+// kOrbNarrowMax px (cap candidates per cell, CellPos<true> keys), where a cell's valid candidates can outnumber any
+// shared-memory sort.  max_per_cell <= 1024 (orb_prepare: < the smallest ORB quota).
 // quotas (ORB detector): first cv::ORB's per-level culls (orb.cpp computeKeyPoints, nfeatures 10000: c_geom.n_per_level),
 //   retainBest(2 n_l) by FAST score, then retainBest(n_l) by Harris response; retainBest keeps every keypoint whose response
 //   equals the n-th largest.  The adjuster's count is unaffected while max_per_cell < min n_l (DESIGN.md 4.5.5).
 // Then keepStrongest: the max_per_cell smallest keys (|response| descending, then level, y, x) by an 8-bit radix select over
 // the 64-bit keys (unique per cell), sorted in shared memory.  One CTA of 1024 threads per (frame, cell); every pass re-reads
 // the cell's candidates (L2-resident).
+template <bool kWide>
 __global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
                                                            const float* __restrict__ resp, int cap, int quotas, int max_per_cell,
                                                            unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
                                                            int out_stride) {
-  using Pos = CellPos<true>;
+  using Pos = CellPos<kWide>;
   __shared__ int hist[kOrbLevels * 256];
   __shared__ unsigned long long keys[1024];
   __shared__ int s_score_cut[kOrbLevels], s_want[kOrbLevels];
@@ -1159,10 +1161,10 @@ template __global__ void k_frame_emit<RGBDSLAM_B200_DETECTOR_FAST, OrbPoints::kC
 
 // -------------------------------------------------------------------------------------------------
 // GaussianBlur(level, 7x7, sigma 2, BORDER_REFLECT_101) as OpenCV evaluates it inside ORB: separable float filter,
-// row pass accumulated left to right, column pass symmetric, round-half-even to uint8.  kFma: every multiply-add of both
-// passes fused, as cv2 4.13's SIMD row and column filters compute them on x86-64 with FMA (RowVec_8u32f,
-// SymmColumnVec_32f8u: v_muladd); equal to cv2 on every pixel of a 4095x360 frame's pyramid where the unfused rule differs
-// at a few pixels per level.  Frames above kOrbNarrowMax px use it; the unfused rule stays for smaller frames (DESIGN.md
+// row pass accumulated left to right, column pass symmetric, round-half-even to uint8.  The multiply-adds are fused, as
+// cv2 4.13's SIMD row and column filters compute them on x86-64 with FMA (RowVec_8u32f, SymmColumnVec_32f8u: v_muladd),
+// except in the row pass of the columns past the last whole 32-column block, which cv2's row filter leaves to its scalar
+// loop: there each product and sum is rounded.  Either rule alone differs from cv2 at a few pixels per million (DESIGN.md
 // 4.5.5).
 __device__ __forceinline__ int reflect101(int i, int n) {
   if (i < 0) i = -i;
@@ -1170,7 +1172,6 @@ __device__ __forceinline__ int reflect101(int i, int n) {
   return i;
 }
 
-template <bool kFma>
 __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int frame_stride,
                                               int level) {
   const OrbPlane& p = c_geom.full[level];
@@ -1187,14 +1188,15 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
     tile[r][c] = (float)im[yy * pw + xx];
   }
   __syncthreads();
+  const bool row_tail = x0 + 32 > pw;  // the columns past the level's last whole 32-column block
   for (int r = ty; r < 22; r += 8) {
     float acc = 0.f;
+    if (row_tail) {
 #pragma unroll
-    for (int j = 0; j < 7; j++) {  // left to right, as cv::sepFilter2D
-      if constexpr (kFma)
-        acc = __fmaf_rn(c_gauss[j], tile[r][tx + j], acc);
-      else
-        acc = __fadd_rn(acc, __fmul_rn(c_gauss[j], tile[r][tx + j]));
+      for (int j = 0; j < 7; j++) acc = __fadd_rn(acc, __fmul_rn(c_gauss[j], tile[r][tx + j]));
+    } else {
+#pragma unroll
+      for (int j = 0; j < 7; j++) acc = __fmaf_rn(c_gauss[j], tile[r][tx + j], acc);  // left to right, as cv::sepFilter2D
     }
     rows[r][tx] = acc;
   }
@@ -1207,10 +1209,7 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
 #pragma unroll
       for (int j = 1; j <= 3; j++) {
         const float pair = __fadd_rn(rows[r + 3 + j][tx], rows[r + 3 - j][tx]);
-        if constexpr (kFma)
-          c = __fmaf_rn(c_gauss[3 + j], pair, c);
-        else
-          c = __fadd_rn(c, __fmul_rn(c_gauss[3 + j], pair));
+        c = __fmaf_rn(c_gauss[3 + j], pair, c);
       }
       int v = __float2int_rn(c);
       v = min(max(v, 0), 255);
@@ -1366,27 +1365,33 @@ static void launch_frames(int nframes, bool fast, bool wide, const OrbFrameArgs&
   (*launches) += 2;
 }
 
-cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
+cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quotas, OrbPoints points, const OrbCandidates& c,
                            const OrbFrameArgs& a, cudaStream_t st, int* launches) {
   const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST, wide = is_wide(g);
   const int z = nframes * g.ncells, max_per_cell = a.out_stride;
   const dim3 rgrid((c.cap + 255) / 256, z);
+  quotas = quotas && !fast;  // the FAST detector has no quotas (cv::FastFeatureDetector)
   if (wide) {
     if (fast)
       k_fast_response_wide<<<rgrid, 256, 0, st>>>(c.cand, c.count, c.thr, c.resp, c.cap);
     else
       k_harris_wide<<<rgrid, 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp, c.cap);
-    (*launches)++;
-    // the FAST detector has no quotas (cv::FastFeatureDetector)
-    k_cell_select_wide<<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, fast ? 0 : 1, max_per_cell, a.cell_out, a.cell_out_count,
-                                           max_per_cell);
-    (*launches)++;
   } else {
     if (fast)
       k_fast_response<<<rgrid, 256, 0, st>>>(c.cand, c.count, c.thr, c.resp);
     else
       k_harris<<<rgrid, 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp);
+  }
+  (*launches)++;
+  if (wide) {
+    k_cell_select_wide<true><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, quotas ? 1 : 0, max_per_cell, a.cell_out,
+                                                 a.cell_out_count, max_per_cell);
     (*launches)++;
+  } else if (quotas) {
+    k_cell_select_wide<false><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, 1, max_per_cell, a.cell_out, a.cell_out_count,
+                                                  max_per_cell);
+    (*launches)++;
+  } else {  // the FAST detector, and ORB geometries where a binding quota could change the adjuster's count (DESIGN.md 4.5.5)
     static bool attr = false;
     if (!attr) {
       cudaError_t e = cudaFuncSetAttribute(k_cell_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
@@ -1428,10 +1433,7 @@ cudaError_t orb_run_describe(const OrbGeom& g, const OrbTables& tab, int nframes
   }
   for (int l = 0; l < levels; l++) {
     const dim3 grid((g.full[l].w + 31) / 32, (g.full[l].h + 15) / 16, nframes);
-    if (is_wide(g))
-      k_blur<true><<<grid, 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
-    else
-      k_blur<false><<<grid, 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
+    k_blur<<<grid, 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, l);
     (*launches)++;
   }
   k_describe<<<dim3((max_kp + 7) / 8, nframes), 256, 0, st>>>(d_pyr_raw, d_pyr_blur, g.full_bytes, d_kp, d_n, kp_stride, d_trig, d_desc);

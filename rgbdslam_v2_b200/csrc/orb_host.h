@@ -71,8 +71,9 @@ struct OrbFrameArgs {
 };
 
 // detector ORB: Harris responses, orientation, size 31 * scale; FAST: response = corner score, angle -1, size 7.
-// Frames wider or taller than kOrbNarrowMax px also apply cv::ORB's per-level quotas (ORB detector; k_cell_select_wide).
-cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
+// quotas: also apply cv::ORB's per-level quotas (ORB detector; k_cell_select_wide), which orb_prepare allows where
+// round(1.5 * max_keypoints / cells) < 606 with a grid (DESIGN.md 4.5.5).
+cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quotas, OrbPoints points, const OrbCandidates& c,
                            const OrbFrameArgs& a, cudaStream_t st, int* launches);
 
 // levels: extractor pyramid levels built and blurred (cv::ORB::compute builds 1 + the largest keypoint octave)

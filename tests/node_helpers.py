@@ -57,6 +57,33 @@ def seq(n):
     return gray, depth, np.stack([orb_oracle.depth_to_mask(d) for d in depth])
 
 
+def textured(h, w, n, seed=0, sigma=2.0):
+    """n frames of dense texture: band-limited noise (uniform noise blurred with sigma) wrapped four times over 0..255"""
+    import cv2
+    rng = np.random.default_rng(seed)
+    out = []
+    for _ in range(n):
+        t = cv2.GaussianBlur(rng.random((h, w)).astype(np.float32), (0, 0), sigma)
+        out.append((t * 1024 % 256).astype(np.uint8))
+    return np.stack(out)
+
+
+class UnboundOrb:
+    """cv2 with the detector's cv::ORB(10000, ...) replaced by cv::ORB(10^6, ...), whose per-level quotas never bind here:
+    the reference's glue in the oracle without the quotas (monkeypatched over orb_oracle.cv2)"""
+
+    def __getattr__(self, name):
+        import cv2
+        return getattr(cv2, name)
+
+    @staticmethod
+    def ORB_create(*a, **kw):
+        import cv2
+        if a and a[0] == 10000:
+            a = (10 ** 6,) + a[1:]
+        return cv2.ORB_create(*a, **kw)
+
+
 def node_dump(fe, handles):
     return [(fe.node_keypoints(h), *fe.node_download(h)) for h in handles]
 

@@ -132,35 +132,6 @@ def test_input_kinds_at_1280x720(fe):
         lambda k, st: md.node_construct(gray[k], depth[k], mask[k], K4, st, max_keypoints=K), use_feature_min_depth=1)
 
 
-def _textured(h, w, n, seed=0):
-    """frames of dense texture (band-limited noise wrapped four times over 0..255): at threshold 20 cv::ORB's per-level
-    quotas change which keypoints every cell keeps, and a 702 x 422 cell under the rendered mask has at most about
-    39 000 FAST / NMS candidates (the buffer holds 59 648)"""
-    import cv2
-    rng = np.random.default_rng(seed)
-    out = []
-    for _ in range(n):
-        t = cv2.GaussianBlur(rng.random((h, w)).astype(np.float32), (0, 0), 2.0)
-        out.append((t * 1024 % 256).astype(np.uint8))
-    return np.stack(out)
-
-
-class _UnboundOrb:
-    """cv2 with the detector's cv::ORB(10000, ...) replaced by cv::ORB(10^6, ...), whose per-level quotas never bind here:
-    the reference's glue in the oracle without the quotas"""
-
-    def __getattr__(self, name):
-        import cv2
-        return getattr(cv2, name)
-
-    @staticmethod
-    def ORB_create(*a, **kw):
-        import cv2
-        if a and a[0] == 10000:
-            a = (10 ** 6,) + a[1:]
-        return cv2.ORB_create(*a, **kw)
-
-
 @pytest.mark.parametrize("detector", [0, 1], ids=["ORB", "FAST"])
 def test_quotas_decide_the_nodes_when_the_adjuster_ends_on_too_many(fe, detector, monkeypatch):
     """1920x1080 frames of dense texture with adjuster_max_iterations 1: every detection ends on "too many", the nodes equal
@@ -171,7 +142,9 @@ def test_quotas_decide_the_nodes_when_the_adjuster_ends_on_too_many(fe, detector
     import orb_quota_oracle as qo
     from oracle import orb_oracle
     h, w = 1080, 1920
-    gray = _textured(h, w, 3)
+    # at threshold 20 cv::ORB's per-level quotas change which keypoints every cell keeps, and a 702 x 422 cell under the
+    # rendered mask has at most about 39 000 FAST / NMS candidates (the buffer holds 59 648)
+    gray = nh.textured(h, w, 3)
     _, depth, mask, K4 = frames(h, w)
     K = 2000
     per_cell = int(K * 1.5) // 9
@@ -195,7 +168,7 @@ def test_quotas_decide_the_nodes_when_the_adjuster_ends_on_too_many(fe, detector
             if c == 4:
                 _, stats = qo.quota_rule(sub, smask, 20)
                 assert any(f > 0 for _, f, _, _ in stats)  # ties at the 2 n_l cut, all kept
-        monkeypatch.setattr(orb_oracle, "cv2", _UnboundOrb())
+        monkeypatch.setattr(orb_oracle, "cv2", nh.UnboundOrb())
         st_free = orb_oracle.DetectorState()
         for k in range(3):
             okp, _, _ = orb_oracle.node_construct(gray[k], depth[k], mask[k], K4, st_free, max_keypoints=K, max_iters=1)

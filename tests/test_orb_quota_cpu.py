@@ -58,13 +58,16 @@ def test_quota_under_a_mask_and_a_level_below_its_quota():
 
 
 def test_a_cell_of_a_640x480_frame_can_reach_a_binding_quota():
-    """Frames of up to 1023 px run without the quotas.  The largest 3x3 grid cell of a 640 x 480 frame (275 x 222 px) of
-    dense texture at the adjuster's initial threshold 20 has fewer FAST / NMS candidates than the candidate buffer holds
-    (12288) and still more than 2 n_0 at level 0, so cv2's quota binds and the narrow path's keypoints differ from cv2's.
-    This pins that such a cell exists; the narrow path does not apply the quotas."""
-    img = _noise((222, 275), 11, 0.7)
+    """The largest 3x3 grid cell of a 640 x 480 frame (275 x 222 px) of dense texture at the adjuster's initial threshold 20:
+    the candidate buffer (12288 per cell) holds every candidate the device stores -- each strict 3x3 maximum of the
+    threshold-free FAST score with score >= 2 at least 15 px inside its level, at every level -- and levels 0 and 1 still have
+    more than n_l corners at threshold 20, so cv2's Harris quotas bind in a frame the narrow kernels accept."""
+    import orb_pyramid_oracle as po
+    img = _noise((222, 275), 11, 1.0)
     mine, stats = quota_rule(img, None, 20)
-    cands = sum(c for c, *_ in stats)
+    corners = sum(c for c, *_ in stats)
+    stored = sum(len(d) for d in po.orb_candidates(po.pyramid(img), po.mask_pyramid(np.full(img.shape, 255, np.uint8))))
     assert mine == cv2_quota(img, None, 20)
-    assert cands <= 12288 and stats[0][0] > 2 * N_PER_LEVEL[0]
-    assert len(mine) < cands
+    assert corners <= stored <= 12288
+    assert all(stats[l][0] > N_PER_LEVEL[l] and stats[l][3] == N_PER_LEVEL[l] for l in (0, 1))
+    assert len(mine) < corners
