@@ -105,6 +105,15 @@ PAIR_RESULT_DTYPE = np.dtype([
     ("valid_iterations", "<i4"), ("ransac_trafo", "<f4", (16,)), ("info_scale", "<f8"), ("used_identity", "<i4"),
     ("inlier_points", "<u4"), ("outlier_points", "<u4"), ("occluded_points", "<u4"), ("all_points", "<u4"), ("reserved_", "<i4"),
 ])
+class IcpResult(C.Structure):  # == rgbdslam_b200_icp_result (include/rgbdslam_b200/icp.h)
+    _fields_ = [("T", C.c_float * 16), ("converged", C.c_int32), ("iterations", C.c_int32), ("criterion", C.c_int32),
+                ("n_source", C.c_int32), ("n_target", C.c_int32), ("n_correspondences", C.c_int32), ("mse", C.c_double)]
+
+
+ICP_RESULT_DTYPE = np.dtype([("T", "<f4", (16,)), ("converged", "<i4"), ("iterations", "<i4"), ("criterion", "<i4"),
+                             ("n_source", "<i4"), ("n_target", "<i4"), ("n_correspondences", "<i4"), ("mse", "<f8")],
+                            align=True)
+assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 96
 assert PAIR_RESULT_DTYPE.itemsize == C.sizeof(PairResult) == 120
 assert DMATCH_DTYPE.itemsize == C.sizeof(DMatch) == 16
 assert KEYPOINT_DTYPE.itemsize == C.sizeof(KeyPoint) == 28
@@ -178,6 +187,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_node_download_cloud.argtypes = [u64, C.c_int, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
     lib.rgbdslam_b200_reduce_clouds.argtypes = [C.c_int, vp, C.c_double, vp]
+    lib.rgbdslam_b200_icp_align.argtypes = [C.c_int, vp, vp, C.c_int, vp]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -572,6 +582,18 @@ class Frontend:
         counts = np.zeros(len(hs), np.int32)
         self._check(self.lib.rgbdslam_b200_reduce_clouds(len(hs), _ptr(hs), float(voxelfilter_size), _ptr(counts)))
         return counts
+
+    def icp_align(self, source_handles, target_handles, max_cloud_size: int = 10000) -> np.ndarray:
+        """icpAlignment(filterCloud(source), filterCloud(target), Identity) of the nodes' stored clouds, pair by pair, on the
+        device (the ICP fallback of matchNodePair).  Returns ICP_RESULT_DTYPE records; T (column-major, as ransac_trafo) maps
+        the source cloud onto the target cloud and is the identity unless converged."""
+        s = np.ascontiguousarray(np.asarray(source_handles, np.uint64).reshape(-1))
+        t = np.ascontiguousarray(np.asarray(target_handles, np.uint64).reshape(-1))
+        if len(s) != len(t):
+            raise ValueError("one target per source")
+        out = np.zeros(len(s), ICP_RESULT_DTYPE)
+        self._check(self.lib.rgbdslam_b200_icp_align(len(s), _ptr(s), _ptr(t), int(max_cloud_size), _ptr(out)))
+        return out
 
     # -- multi-GPU exchange -------------------------------------------------------------
     def comm_unique_id(self) -> np.ndarray:

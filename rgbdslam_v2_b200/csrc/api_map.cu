@@ -3,14 +3,17 @@
 //   rgbdslam_b200_render_cloud         == transformAndAppendPointCloud (misc.cpp:183-238) of many nodes, the loop of
 //                                         GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583)
 //   rgbdslam_b200_reduce_clouds        == Node::reducePointCloud (node.cpp:1448-1460) of many nodes (voxel.cu)
-// Both run count -> scan -> scatter (map.cu) and move the records to the host through a two-piece device staging ring: the copy
-// of piece k runs on its own stream while piece k + 1 is computed.
+//   rgbdslam_b200_icp_align            == icpAlignment(filterCloud(..), filterCloud(..)) (icp.cpp:20-89) of many pairs (icp.cu)
+// The first two run count -> scan -> scatter (map.cu) and move the records to the host through a two-piece device staging
+// ring: the copy of piece k runs on its own stream while piece k + 1 is computed.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <unordered_map>
 #include <vector>
 
+#include "../../include/rgbdslam_b200/icp.h"
 #include "../../include/rgbdslam_b200/map.h"
 #include "../../include/rgbdslam_b200/voxel.h"
 #include "kernels.h"
@@ -248,6 +251,101 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
   return 0;
 }
 
+// ---- the ICP fallback of matchNodePair -------------------------------------------------------------------------------------
+
+constexpr long long kIcpChunkPoints = 1 << 24;  // raster points of the nodes one filter launch treats: 4 bytes of scratch each
+
+struct IcpCtx {
+  DevBuf nodes, pairs, targets, scratch, pts, nf, nfin, key[2], idx[2], work, corr, dist, results;
+};
+static IcpCtx g_icp;
+
+// Room for the points filterCloud keeps of a cloud of P points: at most desired + 1 with an exact step, and the float sum
+// i += step may run behind by up to about desired^2 * 2^-24 steps.
+static int icp_capacity(int P, int desired) {
+  const long long d = desired;
+  return (int)std::min<long long>(P, d + 2 + d * (d + 4) / (1ll << 23));
+}
+
+static int icp_run(const std::vector<NodeDev*>& nds, std::vector<IcpPair>& pairs, int desired, rgbdslam_b200_icp_result* out) {
+  IcpCtx& c = g_icp;
+  State& s = g_state;
+  cudaStream_t st = s.stream;
+  const int U = (int)nds.size(), n = (int)pairs.size();
+  std::vector<IcpNode> nodes(U);
+  std::vector<int> first_of_chunk;  // the node each filter launch starts at
+  long long f = 0, scratch = 0, chunk = 0, max_chunk = 1;
+  for (int u = 0; u < U; u++) {
+    IcpNode& x = nodes[u];
+    x.src = map_node(nds[u], nullptr);
+    if (!x.src.rgb) x.src.rgb = reinterpret_cast<const uint32_t*>(x.src.z);  // map_point reads a colour word ICP never uses
+    x.P = x.src.cw * x.src.ch;
+    x.cap = icp_capacity(x.P, desired);
+    x.f0 = f;
+    f += x.cap;
+    if (u == 0 || chunk + x.P > kIcpChunkPoints) {
+      first_of_chunk.push_back(u);
+      chunk = 0;
+    }
+    x.scratch0 = chunk;
+    chunk += x.P;
+    max_chunk = std::max(max_chunk, chunk);
+  }
+  first_of_chunk.push_back(U);
+  scratch = max_chunk;
+  const long long plane = std::max(f, 1ll);
+  std::vector<char> is_target(U, 0);
+  std::vector<int> targets;
+  long long w = 0;
+  for (IcpPair& p : pairs) {
+    if (!is_target[p.t]) targets.push_back(p.t);
+    is_target[p.t] = 1;
+    p.w0 = w;
+    w += nodes[p.s].cap;
+  }
+  const long long wplane = std::max(w, 1ll);
+  int rc;
+  if ((rc = c.nodes.ensure(sizeof(IcpNode) * U)) || (rc = c.pairs.ensure(sizeof(IcpPair) * n)) ||
+      (rc = c.targets.ensure(sizeof(int) * targets.size())) || (rc = c.scratch.ensure(sizeof(int) * scratch)) ||
+      (rc = c.pts.ensure(3 * sizeof(float) * plane)) || (rc = c.nf.ensure(sizeof(int) * U)) || (rc = c.nfin.ensure(sizeof(int) * U)) ||
+      (rc = c.work.ensure(3 * sizeof(float) * wplane)) || (rc = c.corr.ensure(sizeof(int) * wplane)) ||
+      (rc = c.dist.ensure(sizeof(float) * wplane)) || (rc = c.results.ensure(sizeof(rgbdslam_b200_icp_result) * n)))
+    return rc;
+  for (int b = 0; b < 2; b++)
+    if ((rc = c.key[b].ensure(sizeof(unsigned long long) * plane)) || (rc = c.idx[b].ensure(sizeof(int) * plane))) return rc;
+  RB200_CUDA(cudaMemcpyAsync(c.nodes.ptr, nodes.data(), sizeof(IcpNode) * U, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(c.pairs.ptr, pairs.data(), sizeof(IcpPair) * n, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(c.targets.ptr, targets.data(), sizeof(int) * targets.size(), cudaMemcpyHostToDevice, st));
+  const IcpNode* d_nodes = (const IcpNode*)c.nodes.ptr;
+  float* pts = (float*)c.pts.ptr;
+  int* nf = (int*)c.nf.ptr;
+  int launches = 0;
+  for (size_t k = 0; k + 1 < first_of_chunk.size(); k++) {
+    const int u0 = first_of_chunk[k], u1 = first_of_chunk[k + 1];
+    RB200_CUDA(launch_icp_filter(d_nodes + u0, u1 - u0, desired, (int*)c.scratch.ptr, pts, plane, nf + u0, st));
+    launches++;
+  }
+  unsigned long long* key[2] = {(unsigned long long*)c.key[0].ptr, (unsigned long long*)c.key[1].ptr};
+  int* idx[2] = {(int*)c.idx[0].ptr, (int*)c.idx[1].ptr};
+  RB200_CUDA(launch_icp_cells(d_nodes, (const int*)c.targets.ptr, (int)targets.size(), pts, plane, nf, key, idx, (int*)c.nfin.ptr, st));
+  RB200_CUDA(launch_icp_align((const IcpPair*)c.pairs.ptr, n, d_nodes, pts, plane, nf, key[0], idx[0], (const int*)c.nfin.ptr,
+                              (float*)c.work.ptr, wplane, (int*)c.corr.ptr, (float*)c.dist.ptr,
+                              (rgbdslam_b200_icp_result*)c.results.ptr, st));
+  launches += 2;
+  std::vector<int> kept(U);
+  RB200_CUDA(cudaMemcpyAsync(kept.data(), nf, sizeof(int) * U, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaMemcpyAsync(out, c.results.ptr, sizeof(rgbdslam_b200_icp_result) * n, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  s.launches += launches;
+  for (int u = 0; u < U; u++)
+    if (kept[u] > nodes[u].cap) {
+      set_error("icp_align: filterCloud kept " + std::to_string(kept[u]) + " points, more than the " + std::to_string(nodes[u].cap) +
+                " allowed for");
+      return RGBDSLAM_B200_ERR_CUDA;
+    }
+  return 0;
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -373,6 +471,40 @@ int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter
     }
   if (n_points) std::copy(counts.begin(), counts.end(), n_points);
   return 0;
+}
+
+int rgbdslam_b200_icp_align(int n, const uint64_t* source, const uint64_t* target, int max_cloud_size,
+                            rgbdslam_b200_icp_result* out) {
+  RB200_ENTER_INITED();
+  if (n < 0 || max_cloud_size < 1 || (n > 0 && (!source || !target || !out))) {
+    set_error("icp_align: n >= 0, max_cloud_size >= 1 and non-null source, target and out are needed");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  std::vector<NodeDev*> nds;  // the distinct nodes of the call, in order of first appearance
+  std::unordered_map<uint64_t, int> slot;
+  std::vector<IcpPair> pairs(n);
+  for (int k = 0; k < 2 * n; k++) {
+    const uint64_t h = (k & 1 ? target : source)[k >> 1];
+    auto it = slot.find(h);
+    int u;
+    if (it != slot.end()) {
+      u = it->second;
+    } else {
+      NodeDev* nd = get_node(h);
+      if (!nd) return RGBDSLAM_B200_ERR_ARG;
+      u = (int)nds.size();
+      slot.emplace(h, u);
+      nds.push_back(nd);
+    }
+    (k & 1 ? pairs[k >> 1].t : pairs[k >> 1].s) = u;
+  }
+  for (size_t u = 0; u < nds.size(); u++)
+    if (!nds[u]->pc.z) {
+      set_error("icp_align: a node has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD or KEEP_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    }
+  if (n == 0) return 0;
+  return icp_run(nds, pairs, max_cloud_size, out);
 }
 
 }  // extern "C"

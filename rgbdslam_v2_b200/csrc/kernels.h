@@ -1,5 +1,6 @@
 // kernels.h -- host-side launchers of the sm_90a kernels (implemented in *.cu).
 #pragma once
+#include "../../include/rgbdslam_b200/icp.h"
 #include "common.cuh"
 
 namespace rb200 {
@@ -96,6 +97,28 @@ cudaError_t launch_vox_sort(const VoxBufs& b, int nnodes, int nblocks, int passe
 // One point per voxel into the chunk's slab: node k's planes [x | y | z | colour] of its n_k voxels start at word
 // 4 * offs[blk0_k]
 cudaError_t launch_vox_centroids(const VoxBufs& b, int passes, long long nvoxels, float* slab, cudaStream_t st);
+// The ICP fallback of matchNodePair (icp.cu).  The kept points of every distinct node of a call lie in three planes of `plane`
+// floats each (x | y | z), node u's at [f0, f0 + cap).
+struct IcpNode {
+  MapNode src;          // its stored cloud, as stored
+  int P;                // src.cw * src.ch
+  int cap;              // room for its kept points
+  long long f0;         // their first slot in the point planes (and in the cell arrays)
+  long long scratch0;   // its non-NaN index list in the scratch of the filter launch that treats it
+};
+struct IcpPair {
+  int s, t;             // source and target node
+  long long w0;         // the pair's working source, correspondences and distances: [w0, w0 + cap of s)
+};
+// filterCloud of nnodes nodes: kept points into pts, their counts into nf (one CTA per node)
+cudaError_t launch_icp_filter(const IcpNode* d_nodes, int nnodes, int desired, int* scratch, float* pts, long long plane, int* nf,
+                              cudaStream_t st);
+// the cell keys of the finite kept points of the listed nodes, sorted, into key[0] / idx[0] at f0; counts into nfin
+cudaError_t launch_icp_cells(const IcpNode* d_nodes, const int* targets, int ntargets, const float* pts, long long plane, const int* nf,
+                             unsigned long long* key[2], int* idx[2], int* nfin, cudaStream_t st);
+cudaError_t launch_icp_align(const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane, const int* nf,
+                             const unsigned long long* key, const int* idx, const int* nfin, float* work, long long wplane, int* corr,
+                             float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st);
 cudaError_t launch_refine_g2o(const PairDesc* pairs, int npairs, int max_matches, int iterations, const float4* mfrom,
                               const float4* mto, const int32_t* n_all, const rgbdslam_b200_dmatch* matches,
                               rgbdslam_b200_pair_result* results, rgbdslam_b200_dmatch* inlier_matches, cudaStream_t stream);
