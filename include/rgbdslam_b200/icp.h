@@ -16,8 +16,9 @@ extern "C" {
 typedef struct rgbdslam_b200_icp_result {
   float T[16];                /* getFinalTransformation(), column-major like pair_result.ransac_trafo; identity unless converged */
   int32_t converged;          /* hasConverged() */
-  int32_t iterations;         /* nr_iterations_ */
-  int32_t criterion;          /* 0 fewer than 3 correspondences, 1 iterations, 2 transform, 3 absolute MSE, 4 relative MSE */
+  int32_t iterations;         /* nr_iterations_: ICP iterations */
+  int32_t criterion;          /* 0 fewer than the method's minimum (3 for icp, 4 for icp_nl), 1 iterations, 2 transform,
+                                 3 absolute MSE, 4 relative MSE */
   int32_t n_source, n_target; /* points after filterCloud */
   int32_t n_correspondences;  /* of the last iteration */
   double mse;                 /* calculateMSE of the last completed iteration, 0 when none completed */
@@ -52,6 +53,44 @@ typedef struct rgbdslam_b200_icp_result {
  * device work: a node without a stored cloud. */
 int rgbdslam_b200_icp_align(int n, const uint64_t* source, const uint64_t* target, int max_cloud_size,
                             rgbdslam_b200_icp_result* out);
+
+/* icp_method (parameter_server.cpp:110, icp.cpp:50-58): "icp" is IterativeClosestPoint, "icp_nl" IterativeClosestPointNonLinear */
+#define RGBDSLAM_B200_ICP_METHOD_ICP 0
+#define RGBDSLAM_B200_ICP_METHOD_ICP_NL 1
+
+/* rgbdslam_b200_icp_align with the estimator chosen by method; rgbdslam_b200_icp_align(...) == _ex(..., METHOD_ICP).
+ * METHOD_ICP_NL is pcl::IterativeClosestPointNonLinear<PointXYZRGB, PointXYZRGB> (PCL 1.7, float): the loop, filterCloud, the
+ * correspondences, the move, final = T_inc final, the MSE and the convergence test are those above, except:
+ *   - fewer than 4 correspondences stop ICP, not converged (criterion 0);
+ *   - T_inc comes from TransformationEstimationLM over the correspondences in source order: x in R^6 from 0, read through
+ *     WarpPointRigid6D as (tx, ty, tz, qx, qy, qz); q.q = (qx qx + qz qz) + qy qy (the order of Eigen's SSE reduction of a
+ *     Vector4 with w = 0), w = sqrt(1 - q.q), q is not renormalised (PCL 1.7.2), the rotation is Quaternion::
+ *     toRotationMatrix's formula; q.q > 1 makes w and every residual NaN, and every comparison with NaN is false, as written;
+ *   - residual i = sqrt((dx dx + dz dz) + dy dy) of warp(src_i) - tgt_i, warp(p) = ((r0 x + r1 y) + r2 z) + t;
+ *   - Eigen's LevenbergMarquardt<NumericalDiff<.>, float>::minimize with the defaults (factor 100, maxfev 400,
+ *     ftol = xtol = sqrt(FLT_EPSILON), gtol 0): forward differences h = sqrt(FLT_EPSILON) |x_j| (sqrt(FLT_EPSILON) when 0),
+ *     column (f(x + h e_j) - f(x)) / h; NumericalDiff's f(x) equals the current residual vector bit for bit, so it is reused,
+ *     and every Jacobian counts 7 evaluations against maxfev.  With 4 or 5 correspondences Eigen refuses (fewer rows than
+ *     parameters): T_inc is the identity and the transform criterion (2) ends ICP;
+ *   - ColPivHouseholderQR as in Eigen 3.2 (and 3.3-beta1, ROS kinetic's): squared column norms, the chosen column's
+ *     squared norm recomputed over its rows >= k, downdated by subtracting the squared new row-k entries, pivot ties to the
+ *     first maximum, no stop at a small pivot (only the count of nonzero pivots), rank() = the diagonal entries among them
+ *     above |max pivot| * 6 FLT_EPSILON; Householder vectors as makeHouseholderInPlace (tail squared norm <= FLT_MIN: tau 0);
+ *     Q^T f applies H_0 first; lmpar2 and qrsolv (MINPACK's order: the rotated diagonal is solved, then R's restored);
+ *   - stableNorm as Eigen 3.3 (blocks of 4096 in index order, scale updated per block); blueNorm as Eigen with float's
+ *     constants (b1 2^-63, b2 2^52, s1m 2^63, s2m 2^-76, relerr sqrt(FLT_EPSILON));
+ *   - sums over the m correspondences (stableNorm's and blueNorm's sums of squares, column norms, Householder tails and dot
+ *     products, Q^T f) run in the fixed order above: 256 partials, partial j adding the rows j, j + 256, ... in order from +0
+ *     (rows outside the operated range add nothing), then the pairwise tree; a stableNorm block of 4096 rows is summed the
+ *     same way on its own.  Sums of six values (the norms of 6-vectors) take that order too: ((v0 + v4) + v2) + ((v1 + v5)
+ *     + v3).  Other 6-term dot products add their products in index order starting from the first; triangular solves run as
+ *     Eigen's column-major (back substitution, a zero right-hand side skipped) and row-major (dot product, then divide) ones;
+ *   - mixed literals follow C++ promotion: actred = 1. - (fnorm1 / fnorm)^2 is a double subtraction rounded to float;
+ *     std::max / std::min are (a < b) ? b : a and (b < a) ? b : a.
+ * The LM's status and function evaluations are not reported.  The arguments are checked as above, and a method that is
+ * neither ICP nor ICP_NL is ERR_ARG, before any device work. */
+int rgbdslam_b200_icp_align_ex(int n, const uint64_t* source, const uint64_t* target, int max_cloud_size, int method,
+                               rgbdslam_b200_icp_result* out);
 
 #ifdef __cplusplus
 }

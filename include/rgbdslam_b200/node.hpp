@@ -296,7 +296,10 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
         }
       }
       std::vector<rgbdslam_b200_icp_result> r(at.size());
-      if (!at.empty() && rgbdslam_b200_icp_align((int)at.size(), src.data(), tgt.data(), gicp_max_cloud_size(), r.data()) == 0)
+      // icp_method (icp.cpp:50-58): "icp_nl" is IterativeClosestPointNonLinear; any other name, "gicp" included, is "icp"
+      const int method = icp_method() == "icp_nl" ? RGBDSLAM_B200_ICP_METHOD_ICP_NL : RGBDSLAM_B200_ICP_METHOD_ICP;
+      if (!at.empty() &&
+          rgbdslam_b200_icp_align_ex((int)at.size(), src.data(), tgt.data(), gicp_max_cloud_size(), method, r.data()) == 0)
         for (size_t k = 0; k < at.size(); k++) {
           icp[at[k]] = 1;
           icp_res[at[k]] = r[k];
@@ -332,6 +335,12 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   }
   static int& gicp_max_cloud_size() {
     static int v = 10000;
+    return v;
+  }
+  // icp_method (parameter_server.cpp:110): "icp" (IterativeClosestPoint) or "icp_nl" (IterativeClosestPointNonLinear); any
+  // other name takes "icp", as icp.cpp:55-57 does.  Read in matchNodePair.
+  static std::string& icp_method() {
+    static std::string v = "icp";
     return v;
   }
 

@@ -114,6 +114,7 @@ ICP_RESULT_DTYPE = np.dtype([("T", "<f4", (16,)), ("converged", "<i4"), ("iterat
                              ("n_source", "<i4"), ("n_target", "<i4"), ("n_correspondences", "<i4"), ("mse", "<f8")],
                             align=True)
 assert ICP_RESULT_DTYPE.itemsize == C.sizeof(IcpResult) == 96
+ICP_METHODS = {"icp": 0, "icp_nl": 1}  # RGBDSLAM_B200_ICP_METHOD_* (include/rgbdslam_b200/icp.h)
 assert PAIR_RESULT_DTYPE.itemsize == C.sizeof(PairResult) == 120
 assert DMATCH_DTYPE.itemsize == C.sizeof(DMatch) == 16
 assert KEYPOINT_DTYPE.itemsize == C.sizeof(KeyPoint) == 28
@@ -188,6 +189,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
     lib.rgbdslam_b200_reduce_clouds.argtypes = [C.c_int, vp, C.c_double, vp]
     lib.rgbdslam_b200_icp_align.argtypes = [C.c_int, vp, vp, C.c_int, vp]
+    lib.rgbdslam_b200_icp_align_ex.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -583,16 +585,20 @@ class Frontend:
         self._check(self.lib.rgbdslam_b200_reduce_clouds(len(hs), _ptr(hs), float(voxelfilter_size), _ptr(counts)))
         return counts
 
-    def icp_align(self, source_handles, target_handles, max_cloud_size: int = 10000) -> np.ndarray:
+    def icp_align(self, source_handles, target_handles, max_cloud_size: int = 10000, method: str = "icp") -> np.ndarray:
         """icpAlignment(filterCloud(source), filterCloud(target), Identity) of the nodes' stored clouds, pair by pair, on the
-        device (the ICP fallback of matchNodePair).  Returns ICP_RESULT_DTYPE records; T (column-major, as ransac_trafo) maps
-        the source cloud onto the target cloud and is the identity unless converged."""
+        device (the ICP fallback of matchNodePair).  method is icp_method: "icp" (IterativeClosestPoint) or "icp_nl"
+        (IterativeClosestPointNonLinear).  Returns ICP_RESULT_DTYPE records; T (column-major, as ransac_trafo) maps the
+        source cloud onto the target cloud and is the identity unless converged."""
+        if method not in ICP_METHODS:
+            raise ValueError(f"icp method must be one of {sorted(ICP_METHODS)}, not {method!r}")
         s = np.ascontiguousarray(np.asarray(source_handles, np.uint64).reshape(-1))
         t = np.ascontiguousarray(np.asarray(target_handles, np.uint64).reshape(-1))
         if len(s) != len(t):
             raise ValueError("one target per source")
         out = np.zeros(len(s), ICP_RESULT_DTYPE)
-        self._check(self.lib.rgbdslam_b200_icp_align(len(s), _ptr(s), _ptr(t), int(max_cloud_size), _ptr(out)))
+        self._check(self.lib.rgbdslam_b200_icp_align_ex(len(s), _ptr(s), _ptr(t), int(max_cloud_size), ICP_METHODS[method],
+                                                         _ptr(out)))
         return out
 
     # -- multi-GPU exchange -------------------------------------------------------------
