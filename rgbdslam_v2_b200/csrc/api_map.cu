@@ -310,7 +310,7 @@ static int icp_run(const std::vector<NodeDev*>& nds, std::vector<IcpPair>& pairs
   if ((rc = c.nodes.ensure(sizeof(IcpNode) * U)) || (rc = c.pairs.ensure(sizeof(IcpPair) * n)) ||
       (rc = c.targets.ensure(sizeof(int) * targets.size())) || (rc = c.scratch.ensure(sizeof(int) * scratch)) ||
       (rc = c.pts.ensure(3 * sizeof(float) * plane)) || (rc = c.nf.ensure(sizeof(int) * U)) || (rc = c.nfin.ensure(sizeof(int) * U)) ||
-      (rc = c.work.ensure((method == RGBDSLAM_B200_ICP_METHOD_ICP_NL ? kIcpNlPlanes : 3) * sizeof(float) * wplane)) || (rc = c.corr.ensure(sizeof(int) * wplane)) ||
+      (rc = c.work.ensure(icp_work_planes(method) * sizeof(float) * wplane)) || (rc = c.corr.ensure(sizeof(int) * wplane)) ||
       (rc = c.dist.ensure(sizeof(float) * wplane)) || (rc = c.results.ensure(sizeof(rgbdslam_b200_icp_result) * n)))
     return rc;
   for (int b = 0; b < 2; b++)
@@ -330,9 +330,8 @@ static int icp_run(const std::vector<NodeDev*>& nds, std::vector<IcpPair>& pairs
   unsigned long long* key[2] = {(unsigned long long*)c.key[0].ptr, (unsigned long long*)c.key[1].ptr};
   int* idx[2] = {(int*)c.idx[0].ptr, (int*)c.idx[1].ptr};
   RB200_CUDA(launch_icp_cells(d_nodes, (const int*)c.targets.ptr, (int)targets.size(), pts, plane, nf, key, idx, (int*)c.nfin.ptr, st));
-  RB200_CUDA((method == RGBDSLAM_B200_ICP_METHOD_ICP_NL ? launch_icp_nl_align : launch_icp_align)(
-      (const IcpPair*)c.pairs.ptr, n, d_nodes, pts, plane, nf, key[0], idx[0], (const int*)c.nfin.ptr, (float*)c.work.ptr, wplane,
-      (int*)c.corr.ptr, (float*)c.dist.ptr, (rgbdslam_b200_icp_result*)c.results.ptr, st));
+  RB200_CUDA(launch_icp_align(method, (const IcpPair*)c.pairs.ptr, n, d_nodes, pts, plane, nf, key[0], idx[0], (const int*)c.nfin.ptr,
+                              (float*)c.work.ptr, wplane, (int*)c.corr.ptr, (float*)c.dist.ptr, (rgbdslam_b200_icp_result*)c.results.ptr, st));
   launches += 2;
   std::vector<int> kept(U);
   RB200_CUDA(cudaMemcpyAsync(kept.data(), nf, sizeof(int) * U, cudaMemcpyDeviceToHost, st));

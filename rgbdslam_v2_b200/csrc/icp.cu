@@ -4,8 +4,7 @@
 //                 (one thread: it is a chain of float additions), then the kept points' coordinates
 //   k_icp_cells   one CTA per distinct target: the finite kept points' cells of side 1/16 m, stably sorted by cell key
 //                 (8-bit LSD radix passes in global memory), so that a cell's points stay in index order
-//   k_icp_align   one CTA per pair runs every iteration: nearest target in the 27 cells around each source point, the
-//                 Umeyama sums, then on thread 0 the 3 x 3 Jacobi SVD, the accumulation and the convergence test
+//   IcpSvd        the estimator of k_icp_align<IcpSvd> (icp.cuh): the Umeyama sums, then on thread 0 the 3 x 3 Jacobi SVD
 // Points are read through map_point (map.cuh), as stored.  Every float operation is an explicit _rn intrinsic (no
 // contraction, no approximate division or square root), so tests/icp_exact.py replays the kernels bit for bit.
 #include "icp.cuh"
@@ -301,169 +300,68 @@ __device__ __forceinline__ void icp_umeyama(const float (&sigma)[3][3], const fl
   for (int i = 0; i < 3; i++) T[4 * i + 3] = __fsub_rn(dm[i], icp_dot3(T[4 * i], sm[0], T[4 * i + 1], sm[1], T[4 * i + 2], sm[2]));
 }
 
-__global__ void __launch_bounds__(kIcpThreads) k_icp_align(const IcpPair* __restrict__ pairs, const IcpNode* __restrict__ nodes,
-                                                           const float* __restrict__ pts, long long plane, const int* __restrict__ nf,
-                                                           const unsigned long long* __restrict__ key, const int* __restrict__ idx,
-                                                           const int* __restrict__ nfin, float* __restrict__ work, long long wplane,
-                                                           int* __restrict__ corr, float* __restrict__ dist,
-                                                           rgbdslam_b200_icp_result* __restrict__ results) {
-  __shared__ float red[9][kIcpThreads];
-  __shared__ float s_T[12];
-  __shared__ int s_cnt, s_stop;
-  const IcpPair pr = pairs[blockIdx.x];
-  const long long fs = nodes[pr.s].f0, ft = nodes[pr.t].f0;
-  const int ns = nf[pr.s];
-  IcpTarget tg;
-  tg.key = key + ft;
-  tg.idx = idx + ft;
-  tg.m = nfin[pr.t];
-  tg.x = pts + ft;
-  tg.y = tg.x + plane;
-  tg.z = tg.y + plane;
-  float* wx = work + pr.w0;  // the source as the iterations move it
-  float* wy = wx + wplane;
-  float* wz = wy + wplane;
-  int* cr = corr + pr.w0;
-  float* ds = dist + pr.w0;
-  for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-    wx[i] = pts[fs + i];
-    wy[i] = pts[plane + fs + i];
-    wz[i] = pts[2 * plane + fs + i];
+// TransformationEstimationSVD for k_icp_align: the means (summed in the search) and sigma, then Umeyama on thread 0.
+struct IcpSvd {
+  static constexpr int kMinCorrespondences = 3;
+  static constexpr int kMinBlocks = 3;  // at most 80 registers, without spills
+  static constexpr int kPlanes = 3;  // the moving source only
+  struct Shared {
+    float red[9][kIcpThreads];
+    int cnt;
+  };
+  float v[6];  // this thread's sums of the source and target coordinates
+  float inv_n, sm[3], dm[3];
+
+  __device__ IcpSvd(Shared& sh, float*, long long) : v{0.f, 0.f, 0.f, 0.f, 0.f, 0.f} {
+    if (threadIdx.x == 0) sh.cnt = 0;
   }
-  // thread 0's bookkeeping
-  float final_T[16];
+  __device__ void add(float x, float y, float z, float tx, float ty, float tz) {
+    v[0] = __fadd_rn(v[0], x);
+    v[1] = __fadd_rn(v[1], y);
+    v[2] = __fadd_rn(v[2], z);
+    v[3] = __fadd_rn(v[3], tx);
+    v[4] = __fadd_rn(v[4], ty);
+    v[5] = __fadd_rn(v[5], tz);
+  }
+  __device__ int count(Shared& sh, const IcpPass&, int c) {
+    if (c) atomicAdd(&sh.cnt, c);
+    icp_tree<6>(sh.red, v);
 #pragma unroll
-  for (int k = 0; k < 16; k++) final_T[k] = k % 5 == 0 ? 1.f : 0.f;
-  double prev = 1.7976931348623157e308, mse = 0.0;
-  int iterations = 0, criterion = 0, cnt = 0;
-  if (threadIdx.x == 0) s_cnt = 0;
-  __syncthreads();
-#pragma unroll 1
-  for (;;) {
-    // 1. correspondences in source order, and the partial sums of the means
-    float v[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    int c = 0;
-    for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-      const float x = wx[i], y = wy[i], z = wz[i];
-      float d = INFINITY;
-      int j = icp_finite(x, y, z) ? icp_nearest(tg, x, y, z, d) : -1;
-      if (j >= 0 && !((double)d <= kIcpMaxD2)) j = -1;
-      cr[i] = j;
-      ds[i] = d;
-      if (j >= 0) {
-        c++;
-        v[0] = __fadd_rn(v[0], x);
-        v[1] = __fadd_rn(v[1], y);
-        v[2] = __fadd_rn(v[2], z);
-        v[3] = __fadd_rn(v[3], tg.x[j]);
-        v[4] = __fadd_rn(v[4], tg.y[j]);
-        v[5] = __fadd_rn(v[5], tg.z[j]);
-      }
-    }
-    if (c) atomicAdd(&s_cnt, c);
-    float m6[6] = {v[0], v[1], v[2], v[3], v[4], v[5]};
-    icp_tree<6>(red, m6);
-    cnt = s_cnt;
-    if (cnt < 3) {  // too few correspondences: not converged
-      criterion = 0;
-      break;
-    }
-    const float inv_n = __fdiv_rn(1.f, (float)cnt);
-    float sm[3], dm[3];
+    for (int k = 0; k < 6; k++) v[k] = 0.f;
+    return sh.cnt;
+  }
+  __device__ void estimate(Shared& sh, const IcpPass& p, int n) {
+    inv_n = __fdiv_rn(1.f, (float)n);
 #pragma unroll
     for (int k = 0; k < 3; k++) {
-      sm[k] = __fmul_rn(red[k][0], inv_n);
-      dm[k] = __fmul_rn(red[3 + k][0], inv_n);
+      sm[k] = __fmul_rn(sh.red[k][0], inv_n);
+      dm[k] = __fmul_rn(sh.red[3 + k][0], inv_n);
     }
     __syncthreads();
-    // 2. sigma = (1/n) dst_demean src_demean^T
-#pragma unroll
-    for (int k = 0; k < 9; k++) v[k] = 0.f;
-    for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-      const int j = cr[i];
+    // sigma = (1/n) dst_demean src_demean^T
+    float s[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int i = threadIdx.x; i < p.ns; i += kIcpThreads) {
+      const int j = p.cr[i];
       if (j < 0) continue;
-      const float sd[3] = {__fsub_rn(wx[i], sm[0]), __fsub_rn(wy[i], sm[1]), __fsub_rn(wz[i], sm[2])};
-      const float dd[3] = {__fsub_rn(tg.x[j], dm[0]), __fsub_rn(tg.y[j], dm[1]), __fsub_rn(tg.z[j], dm[2])};
+      const float sd[3] = {__fsub_rn(p.x[i], sm[0]), __fsub_rn(p.y[i], sm[1]), __fsub_rn(p.z[i], sm[2])};
+      const float dd[3] = {__fsub_rn(p.tg.x[j], dm[0]), __fsub_rn(p.tg.y[j], dm[1]), __fsub_rn(p.tg.z[j], dm[2])};
 #pragma unroll
       for (int r = 0; r < 3; r++)
 #pragma unroll
-        for (int q = 0; q < 3; q++) v[3 * r + q] = __fadd_rn(v[3 * r + q], __fmul_rn(dd[r], sd[q]));
+        for (int q = 0; q < 3; q++) s[3 * r + q] = __fadd_rn(s[3 * r + q], __fmul_rn(dd[r], sd[q]));
     }
-    icp_tree<9>(red, v);
-    // 3. thread 0: T_inc, final = T_inc final, calculateMSE and DefaultConvergenceCriteria
-    if (threadIdx.x == 0) {
-      float sigma[3][3], T[12];
-#pragma unroll
-      for (int r = 0; r < 3; r++)
-#pragma unroll
-        for (int q = 0; q < 3; q++) sigma[r][q] = __fmul_rn(inv_n, red[3 * r + q][0]);
-      icp_umeyama(sigma, sm, dm, T);
-      float nf_T[16];
-#pragma unroll
-      for (int r = 0; r < 4; r++)
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const float a0 = r < 3 ? T[4 * r] : 0.f, a1 = r < 3 ? T[4 * r + 1] : 0.f, a2 = r < 3 ? T[4 * r + 2] : 0.f,
-                      a3 = r < 3 ? T[4 * r + 3] : 1.f;
-          nf_T[4 * r + q] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a0, final_T[q]), __fmul_rn(a1, final_T[4 + q])),
-                                                __fmul_rn(a2, final_T[8 + q])),
-                                      __fmul_rn(a3, final_T[12 + q]));
-        }
-#pragma unroll
-      for (int k = 0; k < 16; k++) final_T[k] = nf_T[k];
-      iterations++;
-      double acc = 0.0;
-#pragma unroll 4
-      for (int i = 0; i < ns; i++)
-        if (cr[i] >= 0) acc = __dadd_rn(acc, (double)ds[i]);
-      mse = __ddiv_rn(acc, (double)cnt);
-      int stop = 0;
-      const double cos_angle = __dmul_rn(0.5, (double)__fsub_rn(__fadd_rn(__fadd_rn(T[0], T[5]), T[10]), 1.f));
-      const double trans2 = (double)__fadd_rn(__fadd_rn(__fmul_rn(T[3], T[3]), __fmul_rn(T[7], T[7])), __fmul_rn(T[11], T[11]));
-      const double dmse = fabs(__dsub_rn(mse, prev));
-      if (iterations >= kIcpMaxIterations) stop = 1;
-      else if (cos_angle >= 1.0 - kIcpTransformEps && trans2 <= kIcpTransformEps) stop = 2;
-      else if (dmse < 1e-12) stop = 3;
-      else if (__ddiv_rn(dmse, prev) < kIcpFitnessEps) stop = 4;
-      else prev = mse;
-      criterion = stop;
-#pragma unroll
-      for (int k = 0; k < 12; k++) s_T[k] = T[k];
-      s_stop = stop;
-      s_cnt = 0;
-    }
-    __syncthreads();
-    if (s_stop) break;
-    // 4. move the source: ((r0 x + r1 y) + r2 z) + t of every finite point
-    float T[12];
-#pragma unroll
-    for (int k = 0; k < 12; k++) T[k] = s_T[k];
-    for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-      const float x = wx[i], y = wy[i], z = wz[i];
-      if (!icp_finite(x, y, z)) continue;
-      wx[i] = __fadd_rn(icp_dot3(T[0], x, T[1], y, T[2], z), T[3]);
-      wy[i] = __fadd_rn(icp_dot3(T[4], x, T[5], y, T[6], z), T[7]);
-      wz[i] = __fadd_rn(icp_dot3(T[8], x, T[9], y, T[10], z), T[11]);
-    }
-    __syncthreads();
+    icp_tree<9>(sh.red, s);
   }
-  if (threadIdx.x == 0) {
-    rgbdslam_b200_icp_result r;
-    const bool converged = criterion != 0;
+  __device__ void increment(Shared& sh, float (&T)[12]) {
+    float sigma[3][3];
 #pragma unroll
-    for (int q = 0; q < 4; q++)
+    for (int r = 0; r < 3; r++)
 #pragma unroll
-      for (int p = 0; p < 4; p++) r.T[4 * q + p] = converged ? final_T[4 * p + q] : (p == q ? 1.f : 0.f);
-    r.converged = converged ? 1 : 0;
-    r.iterations = iterations;
-    r.criterion = criterion;
-    r.n_source = ns;
-    r.n_target = nf[pr.t];
-    r.n_correspondences = cnt;
-    r.mse = mse;
-    results[blockIdx.x] = r;
+      for (int q = 0; q < 3; q++) sigma[r][q] = __fmul_rn(inv_n, sh.red[3 * r + q][0]);
+    icp_umeyama(sigma, sm, dm, T);
+    sh.cnt = 0;  // every thread read it before estimate's barriers
   }
-}
+};
 
 // ---- launchers -------------------------------------------------------------------------------------------------------------
 
@@ -481,12 +379,15 @@ cudaError_t launch_icp_cells(const IcpNode* d_nodes, const int* targets, int nta
   return cudaGetLastError();
 }
 
-cudaError_t launch_icp_align(const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane, const int* nf,
-                             const unsigned long long* key, const int* idx, const int* nfin, float* work, long long wplane, int* corr,
-                             float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st) {
-  if (npairs <= 0) return cudaSuccess;
-  k_icp_align<<<npairs, kIcpThreads, 0, st>>>(pairs, d_nodes, pts, plane, nf, key, idx, nfin, work, wplane, corr, dist, results);
-  return cudaGetLastError();
+int icp_work_planes(int method) {
+  return method == RGBDSLAM_B200_ICP_METHOD_ICP_NL ? IcpAlign<IcpLm>::planes() : IcpAlign<IcpSvd>::planes();
+}
+
+cudaError_t launch_icp_align(int method, const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane,
+                             const int* nf, const unsigned long long* key, const int* idx, const int* nfin, float* work,
+                             long long wplane, int* corr, float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st) {
+  return (method == RGBDSLAM_B200_ICP_METHOD_ICP_NL ? IcpAlign<IcpLm>::launch : IcpAlign<IcpSvd>::launch)(
+      pairs, npairs, d_nodes, pts, plane, nf, key, idx, nfin, work, wplane, corr, dist, results, st);
 }
 
 }  // namespace rb200

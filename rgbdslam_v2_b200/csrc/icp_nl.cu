@@ -2,8 +2,8 @@
 // pcl::IterativeClosestPointNonLinear<PointXYZRGB, PointXYZRGB>, whose increments come from TransformationEstimationLM:
 // Eigen's LevenbergMarquardt (MINPACK lmder) over NumericalDiff's forward differences of |warp(src_i) - tgt_i|, with
 // WarpPointRigid6D's parameters (tx, ty, tz, qx, qy, qz).  The clouds come from icp.cu's k_icp_filter and k_icp_cells.
-//   k_icp_nl_align  one persistent CTA per pair runs every ICP iteration: the correspondences (icp_nearest), compacted in
-//                   source order into the pair's work rows, then the LM, then the move and PCL's convergence test.
+//   IcpLm  the estimator of k_icp_align<IcpLm> (icp.cuh): the correspondences, compacted in source order into the pair's
+//          work rows, then the LM.
 // The length-m work of the LM is spread over the CTA: residuals, Jacobian columns, blueNorm and squared column norms, the
 // Householder tails and their updates, Q^T f and stableNorm.  Thread 0 does the 6 x 6 work: pivots, Householder scalars,
 // lmpar2 / qrsolv and the LM bookkeeping.  Every length-m float sum is the fixed-order block sum of icp_tree over the row
@@ -16,15 +16,14 @@
 namespace rb200 {
 
 constexpr int kNlN = 6;                 // WarpPointRigid6D's dimension
-constexpr int kNlMinCorrespondences = 4;
 constexpr int kNlMaxfev = 400;
 constexpr int kNlStableBlock = 4096;    // stableNorm's block
 constexpr float kNlEps = 0x1p-23f;  // NumTraits<float>::epsilon()
 constexpr float kNlFactor = 100.f;
 constexpr float kNlB1 = 0x1p-63f, kNlB2 = 0x1p52f, kNlS1m = 0x1p63f, kNlS2m = 0x1p-76f;  // blueNorm's constants for float
 
-// The work planes of a pair (kIcpNlPlanes, at w0 in each, wplane apart)
-enum { kWx = 0, kSx = 3, kTx = 6, kF0 = 9, kQf = 11, kJ0 = 12 };
+// The work planes of a pair after k_icp_align's moving source (planes 0-2)
+enum { kSx = 3, kTx = 6, kF0 = 9, kQf = 11, kJ0 = 12 };
 
 struct NlLm {  // thread 0's 6 x 6 state and what it broadcasts
   float R[kNlN][kNlN], S[kNlN][kNlN];
@@ -171,7 +170,7 @@ __device__ __forceinline__ float nl_residual(const float (&T)[12], float sx, flo
 
 // The compact correspondences of a pair and its work rows
 struct NlRows {
-  const float *sx, *sy, *sz, *tx, *ty, *tz;
+  float *sx, *sy, *sz, *tx, *ty, *tz;
   float* f[2];
   float* q;
   float* J[kNlN];
@@ -662,186 +661,78 @@ __device__ void nl_minimize(const NlRows& r, float (*red)[kIcpThreads], NlLm& L)
   }
 }
 
-// ---- alignment ------------------------------------------------------------------------------------------------------------
+// ---- the estimator -----------------------------------------------------------------------------------------------------------
 
-__global__ void __launch_bounds__(kIcpThreads) k_icp_nl_align(const IcpPair* __restrict__ pairs, const IcpNode* __restrict__ nodes,
-                                                              const float* __restrict__ pts, long long plane, const int* __restrict__ nf,
-                                                              const unsigned long long* __restrict__ key, const int* __restrict__ idx,
-                                                              const int* __restrict__ nfin, float* __restrict__ work, long long wplane,
-                                                              int* __restrict__ corr, float* __restrict__ dist,
-                                                              rgbdslam_b200_icp_result* __restrict__ results) {
-  __shared__ float red[4 * kNlN][kIcpThreads];
-  __shared__ NlLm L;
-  __shared__ float s_T[12];
-  __shared__ int s_warp[kIcpThreads / 32];
-  __shared__ int s_stop;
-  const IcpPair pr = pairs[blockIdx.x];
-  const long long fs = nodes[pr.s].f0, ft = nodes[pr.t].f0;
-  const int ns = nf[pr.s];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  IcpTarget tg;
-  tg.key = key + ft;
-  tg.idx = idx + ft;
-  tg.m = nfin[pr.t];
-  tg.x = pts + ft;
-  tg.y = tg.x + plane;
-  tg.z = tg.y + plane;
-  float* w = work + pr.w0;
-  float* wx = w + kWx * wplane;  // the source as the iterations move it
-  float* wy = wx + wplane;
-  float* wz = wy + wplane;
+// TransformationEstimationLM for k_icp_align: the correspondences compacted in source order into the pair's work rows, the
+// LM from x = 0, and T_inc = WarpPointRigid6D(x).  With fewer rows than parameters Eigen refuses and x stays 0.
+struct IcpLm {
+  static constexpr int kMinCorrespondences = 4;
+  static constexpr int kMinBlocks = 2;  // at most 128 registers: the LM fits them without spills
+  static constexpr int kPlanes = kJ0 + kNlN;
+  struct Shared {
+    float red[4 * kNlN][kIcpThreads];
+    NlLm L;
+    int warp[kIcpThreads / 32];
+  };
   NlRows rows;
-  float* cs[6];
+
+  __device__ IcpLm(Shared&, float* w, long long wplane) {
+    const auto plane = [&](int k) { return w + k * wplane; };
+    rows.sx = plane(kSx), rows.sy = plane(kSx + 1), rows.sz = plane(kSx + 2);
+    rows.tx = plane(kTx), rows.ty = plane(kTx + 1), rows.tz = plane(kTx + 2);
+    rows.f[0] = plane(kF0);
+    rows.f[1] = plane(kF0 + 1);
+    rows.q = plane(kQf);
 #pragma unroll
-  for (int c = 0; c < 6; c++) cs[c] = w + (kSx + c) * wplane;  // the compact correspondences: source x y z, target x y z
-  rows.sx = cs[0], rows.sy = cs[1], rows.sz = cs[2], rows.tx = cs[3], rows.ty = cs[4], rows.tz = cs[5];
-  rows.f[0] = w + kF0 * wplane;
-  rows.f[1] = w + (kF0 + 1) * wplane;
-  rows.q = w + kQf * wplane;
-#pragma unroll
-  for (int c = 0; c < kNlN; c++) rows.J[c] = w + (kJ0 + c) * wplane;
-  int* cr = corr + pr.w0;
-  float* ds = dist + pr.w0;
-  for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-    wx[i] = pts[fs + i];
-    wy[i] = pts[plane + fs + i];
-    wz[i] = pts[2 * plane + fs + i];
+    for (int c = 0; c < kNlN; c++) rows.J[c] = plane(kJ0 + c);
   }
-  // thread 0's bookkeeping
-  float final_T[16];
-#pragma unroll
-  for (int k = 0; k < 16; k++) final_T[k] = k % 5 == 0 ? 1.f : 0.f;
-  double prev = 1.7976931348623157e308, mse = 0.0;
-  int iterations = 0, criterion = 0, cnt = 0;
-  __syncthreads();
-#pragma unroll 1
-  for (;;) {
-    // 1. correspondences, compacted in source order
+  __device__ void add(float, float, float, float, float, float) {}
+  __device__ int count(Shared& sh, const IcpPass& p, int) {  // the compaction; this thread reads only the cr it wrote in the search
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     int m = 0;
 #pragma unroll 1
-    for (int base = 0; base < ns; base += kIcpThreads) {
+    for (int base = 0; base < p.ns; base += kIcpThreads) {
       const int i = base + threadIdx.x;
-      int j = -1;
-      float x = 0.f, y = 0.f, z = 0.f;
-      if (i < ns) {
-        x = wx[i], y = wy[i], z = wz[i];
-        float d = INFINITY;
-        j = icp_finite(x, y, z) ? icp_nearest(tg, x, y, z, d) : -1;
-        if (j >= 0 && !((double)d <= kIcpMaxD2)) j = -1;
-        cr[i] = j;
-        ds[i] = d;
-      }
+      const int j = i < p.ns ? p.cr[i] : -1;
       const unsigned bal = __ballot_sync(0xffffffffu, j >= 0);
-      if (lane == 0) s_warp[wid] = __popc(bal);
+      if (lane == 0) sh.warp[wid] = __popc(bal);
       __syncthreads();
       int before = 0, sum = 0;
 #pragma unroll
       for (int q = 0; q < kIcpThreads / 32; q++) {
-        const int c = s_warp[q];
+        const int c = sh.warp[q];
         before += q < wid ? c : 0;
         sum += c;
       }
       if (j >= 0) {
         const int at = m + before + __popc(bal & ((1u << lane) - 1u));
-        cs[0][at] = x;
-        cs[1][at] = y;
-        cs[2][at] = z;
-        cs[3][at] = tg.x[j];
-        cs[4][at] = tg.y[j];
-        cs[5][at] = tg.z[j];
+        rows.sx[at] = p.x[i];
+        rows.sy[at] = p.y[i];
+        rows.sz[at] = p.z[i];
+        rows.tx[at] = p.tg.x[j];
+        rows.ty[at] = p.tg.y[j];
+        rows.tz[at] = p.tg.z[j];
       }
       m += sum;
       __syncthreads();
     }
-    cnt = m;
-    if (cnt < kNlMinCorrespondences) {  // too few correspondences: not converged
-      criterion = 0;
-      break;
-    }
-    // 2. T_inc: the LM's x through WarpPointRigid6D; with fewer rows than parameters Eigen refuses and x stays 0
-    rows.m = m;
-    if (m >= kNlN) {
-      nl_minimize(rows, red, L);
+    return m;
+  }
+  __device__ void estimate(Shared& sh, const IcpPass&, int n) {
+    if (n >= kNlN) {
+      rows.m = n;
+      nl_minimize(rows, sh.red, sh.L);
     } else if (threadIdx.x == 0) {
-      for (int k = 0; k < kNlN; k++) L.x[k] = 0.f;
+      for (int k = 0; k < kNlN; k++) sh.L.x[k] = 0.f;
     }
-    // 3. thread 0: final = T_inc final, calculateMSE and DefaultConvergenceCriteria
-    if (threadIdx.x == 0) {
-      float x[kNlN], T[12];
-      for (int k = 0; k < kNlN; k++) x[k] = L.x[k];
-      nl_warp(x, T);
-      float nf_T[16];
-#pragma unroll
-      for (int r = 0; r < 4; r++)
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const float a0 = r < 3 ? T[4 * r] : 0.f, a1 = r < 3 ? T[4 * r + 1] : 0.f, a2 = r < 3 ? T[4 * r + 2] : 0.f,
-                      a3 = r < 3 ? T[4 * r + 3] : 1.f;
-          nf_T[4 * r + q] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(a0, final_T[q]), __fmul_rn(a1, final_T[4 + q])),
-                                                __fmul_rn(a2, final_T[8 + q])),
-                                      __fmul_rn(a3, final_T[12 + q]));
-        }
-#pragma unroll
-      for (int k = 0; k < 16; k++) final_T[k] = nf_T[k];
-      iterations++;
-      double acc = 0.0;
-#pragma unroll 4
-      for (int i = 0; i < ns; i++)
-        if (cr[i] >= 0) acc = __dadd_rn(acc, (double)ds[i]);
-      mse = __ddiv_rn(acc, (double)cnt);
-      int stop = 0;
-      const double cos_angle = __dmul_rn(0.5, (double)__fsub_rn(__fadd_rn(__fadd_rn(T[0], T[5]), T[10]), 1.f));
-      const double trans2 = (double)__fadd_rn(__fadd_rn(__fmul_rn(T[3], T[3]), __fmul_rn(T[7], T[7])), __fmul_rn(T[11], T[11]));
-      const double dmse = fabs(__dsub_rn(mse, prev));
-      if (iterations >= kIcpMaxIterations) stop = 1;
-      else if (cos_angle >= 1.0 - kIcpTransformEps && trans2 <= kIcpTransformEps) stop = 2;
-      else if (dmse < 1e-12) stop = 3;
-      else if (__ddiv_rn(dmse, prev) < kIcpFitnessEps) stop = 4;
-      else prev = mse;
-      criterion = stop;
-#pragma unroll
-      for (int k = 0; k < 12; k++) s_T[k] = T[k];
-      s_stop = stop;
-    }
-    __syncthreads();
-    if (s_stop) break;
-    // 4. move the source: ((r0 x + r1 y) + r2 z) + t of every finite point
-    float T[12];
-#pragma unroll
-    for (int k = 0; k < 12; k++) T[k] = s_T[k];
-    for (int i = threadIdx.x; i < ns; i += kIcpThreads) {
-      const float x = wx[i], y = wy[i], z = wz[i];
-      if (!icp_finite(x, y, z)) continue;
-      wx[i] = __fadd_rn(icp_dot3(T[0], x, T[1], y, T[2], z), T[3]);
-      wy[i] = __fadd_rn(icp_dot3(T[4], x, T[5], y, T[6], z), T[7]);
-      wz[i] = __fadd_rn(icp_dot3(T[8], x, T[9], y, T[10], z), T[11]);
-    }
-    __syncthreads();
   }
-  if (threadIdx.x == 0) {
-    rgbdslam_b200_icp_result r;
-    const bool converged = criterion != 0;
-#pragma unroll
-    for (int q = 0; q < 4; q++)
-#pragma unroll
-      for (int p = 0; p < 4; p++) r.T[4 * q + p] = converged ? final_T[4 * p + q] : (p == q ? 1.f : 0.f);
-    r.converged = converged ? 1 : 0;
-    r.iterations = iterations;
-    r.criterion = criterion;
-    r.n_source = ns;
-    r.n_target = nf[pr.t];
-    r.n_correspondences = cnt;
-    r.mse = mse;
-    results[blockIdx.x] = r;
+  __device__ void increment(Shared& sh, float (&T)[12]) {
+    float x[kNlN];
+    for (int k = 0; k < kNlN; k++) x[k] = sh.L.x[k];
+    nl_warp(x, T);
   }
-}
+};
 
-cudaError_t launch_icp_nl_align(const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane,
-                                const int* nf, const unsigned long long* key, const int* idx, const int* nfin, float* work,
-                                long long wplane, int* corr, float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st) {
-  if (npairs <= 0) return cudaSuccess;
-  k_icp_nl_align<<<npairs, kIcpThreads, 0, st>>>(pairs, d_nodes, pts, plane, nf, key, idx, nfin, work, wplane, corr, dist, results);
-  return cudaGetLastError();
-}
+template struct IcpAlign<IcpLm>;
 
 }  // namespace rb200

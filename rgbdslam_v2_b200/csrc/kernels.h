@@ -116,14 +116,12 @@ cudaError_t launch_icp_filter(const IcpNode* d_nodes, int nnodes, int desired, i
 // the cell keys of the finite kept points of the listed nodes, sorted, into key[0] / idx[0] at f0; counts into nfin
 cudaError_t launch_icp_cells(const IcpNode* d_nodes, const int* targets, int ntargets, const float* pts, long long plane, const int* nf,
                              unsigned long long* key[2], int* idx[2], int* nfin, cudaStream_t st);
-cudaError_t launch_icp_align(const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane, const int* nf,
-                             const unsigned long long* key, const int* idx, const int* nfin, float* work, long long wplane, int* corr,
-                             float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st);
-// icp_method "icp_nl" (icp_nl.cu): the same arguments; work holds kIcpNlPlanes planes of wplane floats
-constexpr int kIcpNlPlanes = 18;
-cudaError_t launch_icp_nl_align(const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane,
-                                const int* nf, const unsigned long long* key, const int* idx, const int* nfin, float* work,
-                                long long wplane, int* corr, float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st);
+// the alignment of every pair by icp_method `method` (RGBDSLAM_B200_ICP_METHOD_*, one CTA per pair); work holds
+// icp_work_planes(method) planes of wplane floats
+int icp_work_planes(int method);
+cudaError_t launch_icp_align(int method, const IcpPair* pairs, int npairs, const IcpNode* d_nodes, const float* pts, long long plane,
+                             const int* nf, const unsigned long long* key, const int* idx, const int* nfin, float* work,
+                             long long wplane, int* corr, float* dist, rgbdslam_b200_icp_result* results, cudaStream_t st);
 cudaError_t launch_refine_g2o(const PairDesc* pairs, int npairs, int max_matches, int iterations, const float4* mfrom,
                               const float4* mto, const int32_t* n_all, const rgbdslam_b200_dmatch* matches,
                               rgbdslam_b200_pair_result* results, rgbdslam_b200_dmatch* inlier_matches, cudaStream_t stream);

@@ -1,10 +1,12 @@
-// The ICP fallback through the shim (Node::pcl_icp(), USE_PCL_ICP in the reference).  RANSAC is made to fail with a tiny
-// max_dist_for_inliers.  Input (argv[1]): int32 W, H, F, F grey images (W x H bytes), F float depth images (W x H floats).
-// Prints "ICP SHIM OK" when every check holds.  (CPU: compile + link; GPU: run.)
+// The ICP fallback through the shim (Node::pcl_icp(), USE_PCL_ICP in the reference) and its icp_method (Node::icp_method(),
+// icp.cpp:50-58).  RANSAC is made to fail with a tiny max_dist_for_inliers.  Input (argv[1]): int32 W, H, F, F grey images
+// (W x H bytes), F float depth images (W x H floats).  Prints "ICP SHIM OK" when every check holds.  (CPU: compile + link;
+// GPU: run.)
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <memory>
+#include <string>
 #include <vector>
 
 #include "rgbdslam_b200/graph_manager.hpp"
@@ -24,6 +26,14 @@ static bool zero_info(const MatchingResult& m) {
   for (double v : m.edge.informationMatrix.m)
     if (v != 0.0) return false;
   return true;
+}
+
+// the edge of an ICP result as matchNodePair fills it
+static bool is_icp_edge(const MatchingResult& mr, const rgbdslam_b200_icp_result& ir, int id1, int id2) {
+  bool tr = true;
+  for (int k = 0; k < 16; k++) tr &= mr.edge.transform.m[k] == (double)ir.T[k];
+  return tr && mr.edge.id1 == id1 && mr.edge.id2 == id2 && !std::memcmp(mr.icp_trafo.m, ir.T, sizeof(ir.T)) &&
+         !std::memcmp(mr.final_trafo.m, ir.T, sizeof(ir.T));
 }
 
 static bool same(const MatchingResult& a, const MatchingResult& b) {
@@ -100,6 +110,29 @@ int main(int argc, char** argv) {
       CHECK(std::fabs(ir.T[12]) + std::fabs(ir.T[13]) + std::fabs(ir.T[14]) > 1e-4);
       std::printf("icp edge 0->1: iterations %d criterion %d correspondences %d t = (%g %g %g)\n", ir.iterations, ir.criterion,
                   ir.n_correspondences, ir.T[12], ir.T[13], ir.T[14]);
+    }
+    // icp_method: "icp_nl" gives rgbdslam_b200_icp_align_ex(..., ICP_NL)'s edge; "gicp" or an unknown name the "icp" edge
+    {
+      CHECK(Node::icp_method() == "icp");
+      uint64_t src = n0->handle(), tgt = n1->handle();
+      rgbdslam_b200_icp_result icp, icp_nl, plain;
+      check(rgbdslam_b200_icp_align_ex(1, &src, &tgt, Node::gicp_max_cloud_size(), RGBDSLAM_B200_ICP_METHOD_ICP, &icp), "icp");
+      check(rgbdslam_b200_icp_align_ex(1, &src, &tgt, Node::gicp_max_cloud_size(), RGBDSLAM_B200_ICP_METHOD_ICP_NL, &icp_nl),
+            "icp_nl");
+      check(rgbdslam_b200_icp_align(1, &src, &tgt, Node::gicp_max_cloud_size(), &plain), "icp_align");
+      CHECK(!std::memcmp(&plain, &icp, sizeof(icp)) && icp_nl.converged == 1);
+      std::printf("icp: iterations %d criterion %d; icp_nl: iterations %d criterion %d\n", icp.iterations, icp.criterion,
+                  icp_nl.iterations, icp_nl.criterion);
+      const char* names[] = {"icp_nl", "icp", "gicp", "no_such_method"};
+      for (const char* name : names) {
+        Node::icp_method() = name;
+        std::unique_ptr<Node> n = make(1, 1);
+        const MatchingResult mr = n->matchNodePair(n0.get(), 3, 0);
+        const bool nl = std::string(name) == "icp_nl";
+        CHECK(is_icp_edge(mr, nl ? icp_nl : icp, 0, 1) && n->initial_node_matches_ == 1);
+        if (!is_icp_edge(mr, nl ? icp_nl : icp, 0, 1)) std::printf("  method %s\n", name);
+      }
+      Node::icp_method() = "icp";
     }
     // non-adjacent: no ICP
     CHECK(n3->matchNodePair(n0.get(), 3, 0).edge.id1 == -1 && n3->initial_node_matches_ == 0);

@@ -207,9 +207,11 @@ def matmul4(A, B):
     return C
 
 
-def align_points(src, tgt, max_iterations=MAX_ITERATIONS):
-    """IterativeClosestPoint::align of filtered (3, n) float32 clouds with an identity guess.  Returns a dict with the fields of
-    rgbdslam_b200_icp_result (T as a 4 x 4 row-major matrix) and the per-iteration correspondences `corr`."""
+def align_points(src, tgt, max_iterations=MAX_ITERATIONS, estimate=umeyama, min_correspondences=3):
+    """IterativeClosestPoint::align of filtered (3, n) float32 clouds with an identity guess, with the transformation
+    estimator estimate(source, dst, mask) -> T_inc, where dst holds at the masked source points their corresponding target
+    points.  Returns a dict with the fields of rgbdslam_b200_icp_result (T as a 4 x 4 row-major matrix) and the
+    per-iteration correspondences `corr`."""
     src = np.asarray(src, F32)
     tgt = np.asarray(tgt, F32)
     ws = src.copy()
@@ -222,12 +224,12 @@ def align_points(src, tgt, max_iterations=MAX_ITERATIONS):
         ok = (idx >= 0) & (dist.astype(np.float64) <= MAX_D2)
         cnt = int(ok.sum())
         corr.append(np.where(ok, idx, -1))
-        if cnt < 3:
+        if cnt < min_correspondences:
             crit = 0
             break
         dst = np.zeros_like(ws)
         dst[:, ok] = tgt[:, idx[ok]]
-        Tinc = umeyama(ws, dst, ok)
+        Tinc = estimate(ws, dst, ok)
         ws = transform(Tinc, ws)
         final = matmul4(Tinc, final)
         it += 1

@@ -8,7 +8,8 @@ The length-m work (residuals, the Jacobian, column norms, the Householder tails,
 (pivots, lmpar, qrsolv, the LM bookkeeping) is scalar, as on the device's thread 0."""
 import numpy as np
 
-from icp_exact import DBL_MAX, FITNESS_EPS, MAX_D2, MAX_ITERATIONS, TRANSFORM_EPS, block_sum, filter_cloud, matmul4, nearest, transform
+import icp_exact as ix
+from icp_exact import MAX_ITERATIONS, block_sum, filter_cloud, transform
 
 F32 = np.float32
 N = 6  # WarpPointRigid6D's parameters (tx, ty, tz, qx, qy, qz)
@@ -492,55 +493,16 @@ def lm_estimate(src, dst):
                     break
 
 
-# ---- IterativeClosestPointNonLinear::align ------------------------------------------------------------------------------------
-
 def align_points(src, tgt, max_iterations=MAX_ITERATIONS):
-    """IterativeClosestPointNonLinear::align of filtered (3, n) float32 clouds with an identity guess.  Returns a dict with
-    the fields of rgbdslam_b200_icp_result (T as a 4 x 4 row-major matrix), the per-iteration correspondences `corr` and
-    the estimator's (status, nfev, iterations) per ICP iteration in `lm`."""
-    src = np.asarray(src, F32)
-    tgt = np.asarray(tgt, F32)
-    ws = src.copy()
-    final = np.eye(4, dtype=F32)
-    prev = DBL_MAX
-    it, mse, cnt, crit = 0, 0.0, 0, 0
-    corr, lm = [], []
-    while True:
-        idx, dist = nearest(ws, tgt)
-        ok = (idx >= 0) & (dist.astype(np.float64) <= MAX_D2)
-        cnt = int(ok.sum())
-        corr.append(np.where(ok, idx, -1))
-        if cnt < MIN_CORRESPONDENCES:
-            crit = 0
-            break
-        Tinc, status, nfev, lm_it = lm_estimate(ws[:, ok], tgt[:, idx[ok]])
-        lm.append((status, nfev, lm_it))
-        ws = transform(Tinc, ws)
-        final = matmul4(Tinc, final)
-        it += 1
-        acc = 0.0
-        for d in dist[ok]:
-            acc += float(d)
-        mse = acc / cnt
-        if it >= max_iterations:
-            crit = 1
-            break
-        cos = 0.5 * float(F32(F32(F32(Tinc[0, 0] + Tinc[1, 1]) + Tinc[2, 2]) - F32(1.0)))
-        tr = float(F32(F32(F32(Tinc[0, 3] * Tinc[0, 3]) + F32(Tinc[1, 3] * Tinc[1, 3])) + F32(Tinc[2, 3] * Tinc[2, 3])))
-        if cos >= 1.0 - TRANSFORM_EPS and tr <= TRANSFORM_EPS:
-            crit = 2
-            break
-        with np.errstate(divide="ignore", invalid="ignore"):
-            if abs(mse - prev) < 1e-12:
-                crit = 3
-                break
-            if np.float64(abs(mse - prev)) / np.float64(prev) < FITNESS_EPS:
-                crit = 4
-                break
-        prev = mse
-    converged = crit != 0
-    return dict(T=final if converged else np.eye(4, dtype=F32), converged=int(converged), iterations=it, criterion=crit,
-                n_source=src.shape[1], n_target=tgt.shape[1], n_correspondences=cnt, mse=mse, corr=corr, lm=lm)
+    """IterativeClosestPointNonLinear::align: icp_exact.align_points with lm_estimate, plus the estimator's (status, nfev,
+    iterations) per ICP iteration in `lm`"""
+    lm = []
+
+    def estimate(ws, dst, ok):
+        T, *record = lm_estimate(ws[:, ok], dst[:, ok])
+        lm.append(tuple(record))
+        return T
+    return dict(ix.align_points(src, tgt, max_iterations, estimate, MIN_CORRESPONDENCES), lm=lm)
 
 
 def align(source_pc, target_pc, max_cloud_size=10000):

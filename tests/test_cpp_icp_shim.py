@@ -1,7 +1,9 @@
 """The C++ shim's ICP fallback (tests/cpp/test_icp_shim.cpp): CPU: compile + link + 'no CPU fallback' exit path; GPU: with
 RANSAC made to fail, the adjacent pair takes the ICP edge in the reference's direction with a zero information matrix, the
 non-adjacent pair and the pair with too few matches stay invalid, max_connections is honoured in order, the online
-GraphManager over 30 frames optimises to finite poses, and with Node::pcl_icp() off the results are those of the RANSAC path."""
+GraphManager over 30 frames optimises to finite poses, and with Node::pcl_icp() off the results are those of the RANSAC path;
+with Node::icp_method() = "icp_nl" the ICP edge equals rgbdslam_b200_icp_align_ex(..., ICP_NL), and "gicp" or an unknown
+name gives the "icp" edge."""
 import subprocess
 from pathlib import Path
 

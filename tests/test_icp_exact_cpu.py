@@ -259,27 +259,35 @@ def _nvcc():
     return None
 
 
+PTX_OPS = ("fma.rn.f32", "fma.rn.f64", "mul.rn.f32", "add.rn.f32", "sub.rn.f32", "div.rn.f32", "sqrt.rn.f32", "mul.rn.f64",
+           "add.rn.f64", "sub.rn.f64", "div.rn.f64")
+
+
 def _kernel_ops(ptx):
+    """{kernel: op counts} of the k_icp_* entries; the align kernel is named by its estimator, as align<IcpSvd>"""
     out = {}
     for m in re.finditer(r"\.entry\s+(\S*k_icp_\S*)\(.*?\n}\n", ptx, re.S):
-        body = m.group(0)
-        out[m.group(1)] = tuple(body.count(op) for op in ("fma.rn.f32", "fma.rn.f64", "mul.rn.f32", "add.rn.f32", "mul.rn.f64",
-                                                           "add.rn.f64", "div.rn.f32", "div.rn.f64", "sqrt.rn.f32"))
+        k = re.search(r"k_icp_(filter|cells|align)(?:INS_\d+(\w+?)EE)?", m.group(1))
+        out[k.group(1) + (f"<{k.group(2)}>" if k.group(2) else "")] = tuple(m.group(0).count(op) for op in PTX_OPS)
     return out
 
 
 @pytest.mark.skipif(_nvcc() is None, reason="nvcc not available")
 def test_icp_ptx_has_no_contracted_or_approximate_operations(tmp_path):
+    """both ICP sources: every k_icp_* entry has no fma, the same operations under --fmad=false, and no approximate
+    operation; the entries are filterCloud, the cells and one align kernel per estimator"""
     from rgbdslam_v2_b200.build import NVCC_FLAGS
     flags = [f for f in NVCC_FLAGS if f not in ("-shared", "-ldl", "-Xcompiler", "-fPIC")]
-    src = ROOT / "rgbdslam_v2_b200" / "csrc" / "icp.cu"
-    counts, texts = [], []
-    for extra in ([], ["--fmad=false"]):
-        out = tmp_path / f"icp{len(extra)}.ptx"
-        subprocess.run([_nvcc(), *flags, *extra, "-ptx", "-o", str(out), str(src)], check=True, capture_output=True)
-        texts.append(out.read_text())
-        counts.append(_kernel_ops(texts[-1]))
-    assert len(counts[0]) == 3, counts[0]
-    assert counts[0] == counts[1], counts
-    assert all(c[0] == c[1] == 0 for c in counts[0].values())
-    assert not re.search(r"\b(rcp|rsqrt|sqrt\.approx|div\.approx|div\.full|ex2|lg2)\b", texts[0])
+    entries = {"icp.cu": {"filter", "cells", "align<IcpSvd>"}, "icp_nl.cu": {"align<IcpLm>"}}
+    for name, expected in entries.items():
+        src = ROOT / "rgbdslam_v2_b200" / "csrc" / name
+        counts, texts = [], []
+        for extra in ([], ["--fmad=false"]):
+            out = tmp_path / f"{name}{len(extra)}.ptx"
+            subprocess.run([_nvcc(), *flags, *extra, "-ptx", "-o", str(out), str(src)], check=True, capture_output=True)
+            texts.append(out.read_text())
+            counts.append(_kernel_ops(texts[-1]))
+        assert set(counts[0]) == expected and len(re.findall(r"\.entry", texts[0])) == len(expected), (name, counts[0])
+        assert counts[0] == counts[1], (name, counts)
+        assert all(c[0] == c[1] == 0 for c in counts[0].values()), (name, counts[0])
+        assert not re.search(r"\b(rcp|rsqrt|sqrt\.approx|div\.approx|div\.full|ex2|lg2)\b", texts[0]), name

@@ -133,9 +133,11 @@ def measure(fe, hs, pcs, method, args, n, nb, hp, ix, nx):
         fe.synchronize()
     kern = {}
     for e in prof.events():
-        mm = re.search(r"rb200::(k_icp_\w+)", e.name) if e.device_type.name == "CUDA" else None
+        # k_icp_filter, k_icp_cells and the align kernel of the method's estimator: k_icp_align<IcpSvd> or <IcpLm>
+        mm = re.search(r"rb200::(k_icp_\w+(?:<rb200::\w+>)?)", e.name) if e.device_type.name == "CUDA" else None
         if mm:
-            kern[mm.group(1)] = kern.get(mm.group(1), 0.0) + e.device_time
+            k = mm.group(1).replace("rb200::", "")
+            kern[k] = kern.get(k, 0.0) + e.device_time
     res["batch_device_kernel_ms"] = {k: round(v / 1e3, 3) for k, v in sorted(kern.items())}
     res["batch_device_kernel_ms_total"] = round(sum(kern.values()) / 1e3, 3)
     clouds = [ix.filter_cloud(pc, 10000) for pc in pcs]
