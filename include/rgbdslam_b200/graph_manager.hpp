@@ -8,6 +8,8 @@
 //   void   saveTrajectory(filename)                                      graph_mgr_io.cpp:615-677 / logTransform misc.cpp:90-93
 //   void   saveAllClouds(filename)  == saveAllCloudsToFile               graph_mgr_io.cpp:502-583 -> rgbdslam_b200_render_cloud
 //   size_t reducePointClouds()      == reducePointCloud for every node   graph_manager.cpp:1310-1319 -> rgbdslam_b200_reduce_clouds
+//   void   saveOctomap(filename)    == saveOctomapImpl                   graph_mgr_io.cpp:253-310 -> rgbdslam_b200_octomap_*
+//   void   renderToOctomap(Node*), writeOctomap(filename)              graph_mgr_io.cpp:312-329
 // Host logic only; every compute step is a C-ABI call.  The reference draws from the global rand(); here every draw comes
 // from the library's counter-based generator keyed by (seed, node id).  g2o's HyperDijkstra (not under /root/reference) is
 // restated in geodesicBall().  The Python mirror rgbdslam_v2_b200/graph_manager.py is the tested twin of this file.
@@ -58,6 +60,68 @@ inline void rotToQuat(const double R[9], double* q) {  // Eigen::Quaternion(Matr
   const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
   for (int a = 0; a < 4; a++) q[a] /= n;
 }
+// The float 3 x 4 (row-major, node -> map) saveOctomap applies to a node whose estimate has rotation R (row-major, double)
+// and translation t: updateCloudOrigin stores R cast to float as an Eigen Quaternionf (Eigen's trace -- its unrolled
+// reduction m00 + (m11 + m22) -- and largest-diagonal algorithm, in float) and t as float; insertCloudCallback widens the
+// quaternion to a tf::Quaternion, tf::Matrix3x3::setRotation builds the basis in double, pcl_ros::transformPointCloud takes it
+// back with getRotation (tf's branch and tie rule), narrows it to a Quaternionf and applies toRotationMatrix (float).  The
+// ray origin is the translation column.  rgbdslam_v2_b200._capi.octomap_pose is the same chain in numpy.
+inline void octomapPose(const double R[9], const double t[3], float T[12]) {
+  float r[9], q[4];  // q: x, y, z, w
+  for (int i = 0; i < 9; i++) r[i] = (float)R[i];
+  const float tr = r[0] + (r[4] + r[8]);
+  if (tr > 0.0f) {
+    float s = std::sqrt(tr + 1.0f);
+    q[3] = 0.5f * s;
+    s = 0.5f / s;
+    q[0] = (r[7] - r[5]) * s; q[1] = (r[2] - r[6]) * s; q[2] = (r[3] - r[1]) * s;
+  } else {
+    int i = 0;
+    if (r[4] > r[0]) i = 1;
+    if (r[8] > r[4 * i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    float s = std::sqrt(r[4 * i] - r[4 * j] - r[4 * k] + 1.0f);
+    q[i] = 0.5f * s;
+    s = 0.5f / s;
+    q[3] = (r[3 * k + j] - r[3 * j + k]) * s;
+    q[j] = (r[3 * j + i] + r[3 * i + j]) * s;
+    q[k] = (r[3 * k + i] + r[3 * i + k]) * s;
+  }
+  // tf::Matrix3x3::setRotation(tf::Quaternion(x, y, z, w)) in double
+  const double x = q[0], y = q[1], z = q[2], w = q[3];
+  const double d = x * x + y * y + z * z + w * w, s2 = 2.0 / d;
+  const double xs = x * s2, ys = y * s2, zs = z * s2, wx = w * xs, wy = w * ys, wz = w * zs;
+  const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
+  const double M[9] = {1.0 - (yy + zz), xy - wz, xz + wy, xy + wz, 1.0 - (xx + zz), yz - wx, xz - wy, yz + wx, 1.0 - (xx + yy)};
+  // tf::Matrix3x3::getRotation
+  double g[4];
+  const double mt = M[0] + M[4] + M[8];
+  if (mt > 0.0) {
+    double s = std::sqrt(mt + 1.0);
+    g[3] = s * 0.5;
+    s = 0.5 / s;
+    g[0] = (M[7] - M[5]) * s; g[1] = (M[2] - M[6]) * s; g[2] = (M[3] - M[1]) * s;
+  } else {
+    const int i = M[0] < M[4] ? (M[4] < M[8] ? 2 : 1) : (M[0] < M[8] ? 2 : 0);
+    const int j = (i + 1) % 3, k = (i + 2) % 3;
+    double s = std::sqrt(M[4 * i] - M[4 * j] - M[4 * k] + 1.0);
+    g[i] = s * 0.5;
+    s = 0.5 / s;
+    g[3] = (M[3 * k + j] - M[3 * j + k]) * s;
+    g[j] = (M[3 * j + i] + M[3 * i + j]) * s;
+    g[k] = (M[3 * k + i] + M[3 * i + k]) * s;
+  }
+  // Quaternionf::toRotationMatrix
+  const float fx = (float)g[0], fy = (float)g[1], fz = (float)g[2], fw = (float)g[3];
+  const float tx = 2.0f * fx, ty = 2.0f * fy, tz = 2.0f * fz;
+  const float twx = tx * fw, twy = ty * fw, twz = tz * fw, txx = tx * fx, txy = ty * fx, txz = tz * fx;
+  const float tyy = ty * fy, tyz = tz * fy, tzz = tz * fz;
+  const float out[12] = {1.0f - (tyy + tzz), txy - twz, txz + twy, (float)t[0],
+                         txy + twz, 1.0f - (txx + tzz), tyz - twx, (float)t[1],
+                         txz - twy, tyz + twx, 1.0f - (txx + tyy), (float)t[2]};
+  std::memcpy(T, out, sizeof(out));
+}
+
 inline Pose7 poseFromIsometry(const Isometry3d& T) {  // column-major 4x4
   double R[9];
   for (int r = 0; r < 3; r++)
@@ -122,8 +186,9 @@ class GraphManager {
   int earliest_loop_closure_node_ = 0;         // graph_manager.h:356
   std::set<int> fixed_ids_;                    // vertices with setFixed(true) (persist between optimisations like g2o's flags)
 
-  ~GraphManager() {
+  virtual ~GraphManager() {
     for (auto& kv : graph_) delete kv.second;
+    if (octomap_) rgbdslam_b200_octomap_destroy(octomap_);
   }
 
   bool isBigTrafo(const Isometry3d& t) const {
@@ -450,6 +515,77 @@ class GraphManager {
     return pts.size();
   }
 
+  // parameters octomap_* (parameter_server.cpp:56-65) that ColorOctomapServer::reset and saveOctomapImpl read;
+  // octomap_occupancy_threshold does not change the file
+  static double& octomap_resolution() { static double v = 0.05; return v; }
+  static double& octomap_prob_hit() { static double v = 0.9; return v; }
+  static double& octomap_prob_miss() { static double v = 0.4; return v; }
+  static double& octomap_clamping_min() { static double v = 0.001; return v; }
+  static double& octomap_clamping_max() { static double v = 0.999; return v; }
+  static double& octomap_occupancy_threshold() { static double v = 0.5; return v; }
+  static int& octomap_autosave_step() { static int v = 50; return v; }
+  static bool& octomap_clear_after_save() { static bool v = false; return v; }
+  static bool& octomap_clear_raycasted_clouds() { static bool v = false; return v; }
+
+  // GraphManager::updateCloudOrigin (graph_mgr_io.cpp:216-235): the node has a valid estimate, a vertex and a non-empty stored
+  // cloud.  (The reference's function lacks its final `return true`; true is its evident intent.)
+  bool updateCloudOrigin(const Node* node) const {
+    if (!node->valid_tf_estimate_ || !estimates_.count(node->vertex_id_)) return false;
+    int w = 0, h = 0;
+    return rgbdslam_b200_node_download_cloud(node->handle(), 32, nullptr, &w, &h) == 0 && (long long)w * h > 0;
+  }
+  // octomapPose of the node's estimate
+  void octomapTransform(int vertex_id, float T[12]) const {
+    const Pose7& p = estimates_.at(vertex_id);
+    double R[9];
+    quatToRot(p.v + 3, R);  // the VertexSE3 estimate's rotation as an Isometry3d holds it
+    octomapPose(R, p.v, T);
+  }
+  // ColorOctomapServer::reset: an empty map with the current octomap_* parameters
+  void resetOctomap() {
+    if (octomap_) check(rgbdslam_b200_octomap_destroy(octomap_), "octomap_destroy");
+    octomap_ = 0;
+    rgbdslam_b200_octomap_params p{octomap_resolution(), octomap_prob_hit(), octomap_prob_miss(), octomap_clamping_min(),
+                                   octomap_clamping_max()};
+    check(rgbdslam_b200_octomap_create(&p, &octomap_), "octomap_create");
+  }
+  // GraphManager::renderToOctomap (graph_mgr_io.cpp:318-329): insertCloudCallback of the node when updateCloudOrigin passes,
+  // then, with octomap_clear_raycasted_clouds, Node::clearPointCloud whether it was rendered or not
+  void renderToOctomap(Node* node) { renderToOctomap(std::vector<Node*>(1, node)); }
+  // GraphManager::writeOctomap / ColorOctomapServer::save: the .ot file.  Virtual so that a caller can observe every write,
+  // saveOctomap's autosaves included.
+  virtual void writeOctomap(const std::string& filename) const {
+    if (!octomap_) const_cast<GraphManager*>(this)->resetOctomap();
+    int64_t n = 0;
+    check(rgbdslam_b200_octomap_write(octomap_, nullptr, 0, &n), "octomap_write");
+    std::vector<char> buf((size_t)n);
+    check(rgbdslam_b200_octomap_write(octomap_, buf.data(), n, &n), "octomap_write");
+    FILE* f = std::fopen(filename.c_str(), "wb");
+    if (!f) throw std::runtime_error("cannot open " + filename);
+    const bool ok = std::fwrite(buf.data(), 1, buf.size(), f) == buf.size();
+    if (std::fclose(f) != 0 || !ok) throw std::runtime_error("cannot write " + filename);
+  }
+  // GraphManager::saveOctomapImpl (graph_mgr_io.cpp:253-310): the nodes passing updateCloudOrigin in ascending id order, a reset
+  // map, each node rendered (octomap_clear_raycasted_clouds applied after it), the file written after every
+  // octomap_autosave_step-th node (<= 0: never; the reference divides by it) and once more at the end, then with
+  // octomap_clear_after_save a reset.  The nodes between two autosaves go to the device in one insert call: how many one
+  // call takes does not change the map.
+  void saveOctomap(const std::string& filename) {
+    std::vector<Node*> nodes;
+    for (auto& kv : graph_)
+      if (updateCloudOrigin(kv.second)) nodes.push_back(kv.second);
+    resetOctomap();
+    const int step = octomap_autosave_step();
+    for (size_t k0 = 0; k0 < nodes.size();) {
+      const size_t k1 = step > 0 ? std::min(nodes.size(), (k0 / step + 1) * (size_t)step) : nodes.size();
+      renderToOctomap(std::vector<Node*>(nodes.begin() + k0, nodes.begin() + k1));
+      if (step > 0 && k1 % step == 0) writeOctomap(filename);
+      k0 = k1;
+    }
+    writeOctomap(filename);
+    if (octomap_clear_after_save()) resetOctomap();
+  }
+
   // TUM trajectory "timestamp tx ty tz qx qy qz qw" (logTransform, misc.cpp:90-93)
   void saveTrajectory(const std::string& filename) const {
     FILE* f = std::fopen(filename.c_str(), "w");
@@ -464,6 +600,22 @@ class GraphManager {
 
  private:
   std::map<int, std::set<int>> adj_;
+  uint64_t octomap_ = 0;  // ColorOctomapServer co_server_ (graph_manager.h), created at the first reset or write
+
+  void renderToOctomap(const std::vector<Node*>& nodes) {
+    if (!octomap_) resetOctomap();
+    std::vector<uint64_t> handles;
+    std::vector<float> T;
+    for (Node* n : nodes) {
+      if (!updateCloudOrigin(n)) continue;
+      handles.push_back(n->handle());
+      T.resize(T.size() + 12);
+      octomapTransform(n->vertex_id_, &T[T.size() - 12]);
+    }
+    check(rgbdslam_b200_octomap_insert(octomap_, (int)handles.size(), handles.data(), T.data(), maximum_depth()), "octomap_insert");
+    if (octomap_clear_raycasted_clouds())
+      for (Node* n : nodes) n->clearPointCloud();
+  }
 
   static void tfMatrix(const double* q, double M[12]) {  // tf::Matrix3x3::setRotation, into the rotation part of a 3 x 4
     const double x = q[0], y = q[1], z = q[2], w = q[3];

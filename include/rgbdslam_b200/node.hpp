@@ -22,6 +22,7 @@
 #include "../rgbdslam_b200.h"
 #include "icp.h"
 #include "map.h"
+#include "octomap.h"
 #include "voxel.h"
 #include "features.hpp"
 
@@ -382,6 +383,10 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     }
     check(rgbdslam_b200_reduce_clouds(1, &handle_, vfs, nullptr), "reduce_clouds");
   }
+
+  // Node::clearPointCloud (octomap_clear_raycasted_clouds): the node drops pc_col on the device
+  // (rgbdslam_b200_node_clear_cloud); pointCloud() afterwards is empty.
+  void clearPointCloud() { check(rgbdslam_b200_node_clear_cloud(handle_), "node_clear_cloud"); }
 
   static int& max_connections() {  // parameter max_connections (parameter_server.cpp:104), -1 = unlimited
     static int v = -1;

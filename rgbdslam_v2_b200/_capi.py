@@ -119,6 +119,93 @@ assert PAIR_RESULT_DTYPE.itemsize == C.sizeof(PairResult) == 120
 assert DMATCH_DTYPE.itemsize == C.sizeof(DMatch) == 16
 assert KEYPOINT_DTYPE.itemsize == C.sizeof(KeyPoint) == 28
 
+class OctomapParams(C.Structure):  # == rgbdslam_b200_octomap_params (include/rgbdslam_b200/octomap.h)
+    _fields_ = [("resolution", C.c_double), ("prob_hit", C.c_double), ("prob_miss", C.c_double), ("clamping_min", C.c_double),
+                ("clamping_max", C.c_double)]
+
+
+def octomap_pose_steps(T) -> dict:
+    """The pose chain of saveOctomap step by step (see octomap_pose): q_eigen (x, y, z, w, float32) and eigen_branch of
+    Eigen's Quaternion(Matrix3f), M (the tf::Matrix3x3 of setRotation, float64), q_tf and tf_branch of its getRotation,
+    and T, the float 3 x 4.  A branch is -1 for the positive-trace formula, else the index of the diagonal entry used."""
+    f, d = np.float32, np.float64
+    T = np.asarray(T, d)
+    R = T[:3, :3].astype(f)
+    # Eigen's Quaternion(Matrix3f): trace as its unrolled reduction m00 + (m11 + m22), then the positive-trace or the
+    # largest-diagonal branch (strict >), in float
+    tr = R[0, 0] + (R[1, 1] + R[2, 2])
+    q = np.zeros(4, f)  # x, y, z, w
+    if tr > f(0):
+        eb = -1
+        t = np.sqrt(tr + f(1))
+        q[3] = f(0.5) * t
+        t = f(0.5) / t
+        q[0], q[1], q[2] = (R[2, 1] - R[1, 2]) * t, (R[0, 2] - R[2, 0]) * t, (R[1, 0] - R[0, 1]) * t
+    else:
+        i = 0
+        if R[1, 1] > R[0, 0]:
+            i = 1
+        if R[2, 2] > R[i, i]:
+            i = 2
+        eb = i
+        j, k = (i + 1) % 3, (i + 2) % 3
+        t = np.sqrt(((R[i, i] - R[j, j]) - R[k, k]) + f(1))
+        q[i] = f(0.5) * t
+        t = f(0.5) / t
+        q[3] = (R[k, j] - R[j, k]) * t
+        q[j] = (R[j, i] + R[i, j]) * t
+        q[k] = (R[k, i] + R[i, k]) * t
+    # tf::Matrix3x3::setRotation in double
+    x, y, z, w = (d(v) for v in q)
+    s = d(2.0) / (((x * x + y * y) + z * z) + w * w)
+    xs, ys, zs = x * s, y * s, z * s
+    wx, wy, wz = w * xs, w * ys, w * zs
+    xx, xy, xz = x * xs, x * ys, x * zs
+    yy, yz, zz = y * ys, y * zs, z * zs
+    M = np.array([[d(1.0) - (yy + zz), xy - wz, xz + wy], [xy + wz, d(1.0) - (xx + zz), yz - wx],
+                  [xz - wy, yz + wx, d(1.0) - (xx + yy)]])
+    # tf::Matrix3x3::getRotation (strict <, in double)
+    tr = (M[0, 0] + M[1, 1]) + M[2, 2]
+    g = np.zeros(4, d)
+    if tr > 0.0:
+        tb = -1
+        sq = np.sqrt(tr + 1.0)
+        g[3] = sq * 0.5
+        sq = 0.5 / sq
+        g[0], g[1], g[2] = (M[2, 1] - M[1, 2]) * sq, (M[0, 2] - M[2, 0]) * sq, (M[1, 0] - M[0, 1]) * sq
+    else:
+        i = (2 if M[1, 1] < M[2, 2] else 1) if M[0, 0] < M[1, 1] else (2 if M[0, 0] < M[2, 2] else 0)
+        tb = i
+        j, k = (i + 1) % 3, (i + 2) % 3
+        sq = np.sqrt(((M[i, i] - M[j, j]) - M[k, k]) + 1.0)
+        g[i] = sq * 0.5
+        sq = 0.5 / sq
+        g[3] = (M[k, j] - M[j, k]) * sq
+        g[j] = (M[j, i] + M[i, j]) * sq
+        g[k] = (M[k, i] + M[i, k]) * sq
+    # Quaternionf::toRotationMatrix in float
+    x, y, z, w = (f(v) for v in g)
+    tx, ty, tz = f(2) * x, f(2) * y, f(2) * z
+    twx, twy, twz = tx * w, ty * w, tz * w
+    txx, txy, txz = tx * x, ty * x, tz * x
+    tyy, tyz, tzz = ty * y, tz * y, tz * z
+    out = np.zeros((3, 4), f)
+    out[:, :3] = [[f(1) - (tyy + tzz), txy - twz, txz + twy], [txy + twz, f(1) - (txx + tzz), tyz - twx],
+                  [txz - twy, tyz + twx, f(1) - (txx + tyy)]]
+    out[:, 3] = T[:3, 3].astype(f)
+    return dict(q_eigen=q, eigen_branch=eb, M=M, q_tf=g, tf_branch=tb, T=out)
+
+
+def octomap_pose(T) -> np.ndarray:
+    """The float 3 x 4 (row-major, node -> map) that the reference's saveOctomap applies to a node whose VertexSE3 estimate is
+    T (4 x 4 or 3 x 4, double): updateCloudOrigin stores the rotation cast to float as an Eigen Quaternionf and the translation
+    as float; insertCloudCallback widens the quaternion to tf (double), builds a tf::Matrix3x3 from it (setRotation) and
+    pcl_ros::transformPointCloud takes it back with getRotation, narrows it to a Quaternionf and uses toRotationMatrix.  The
+    ray origin is the translation column.  Every operation is one numpy operation on float32 or float64 scalars; the C++ shim's
+    octomapPose (include/rgbdslam_b200/graph_manager.hpp) is the same chain in native arithmetic."""
+    return octomap_pose_steps(T)["T"]
+
+
 _lib = None
 
 
@@ -190,6 +277,15 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_reduce_clouds.argtypes = [C.c_int, vp, C.c_double, vp]
     lib.rgbdslam_b200_icp_align.argtypes = [C.c_int, vp, vp, C.c_int, vp]
     lib.rgbdslam_b200_icp_align_ex.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp]
+    lib.rgbdslam_b200_octomap_default_params.argtypes = [C.POINTER(OctomapParams)]
+    lib.rgbdslam_b200_octomap_default_params.restype = None
+    lib.rgbdslam_b200_octomap_create.argtypes = [C.POINTER(OctomapParams), C.POINTER(u64)]
+    lib.rgbdslam_b200_octomap_insert.argtypes = [u64, C.c_int, vp, vp, C.c_double]
+    lib.rgbdslam_b200_octomap_write.argtypes = [u64, vp, i64, C.POINTER(i64)]
+    lib.rgbdslam_b200_octomap_stats.argtypes = [u64, C.POINTER(i64), C.POINTER(i64)]
+    lib.rgbdslam_b200_octomap_clear.argtypes = [u64]
+    lib.rgbdslam_b200_octomap_destroy.argtypes = [u64]
+    lib.rgbdslam_b200_node_clear_cloud.argtypes = [u64]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -600,6 +696,46 @@ class Frontend:
         self._check(self.lib.rgbdslam_b200_icp_align_ex(len(s), _ptr(s), _ptr(t), int(max_cloud_size), ICP_METHODS[method],
                                                          _ptr(out)))
         return out
+
+    # -- the colour OctoMap ----------------------------------------------------------------
+    def octomap_create(self, resolution: float = 0.05, prob_hit: float = 0.9, prob_miss: float = 0.4, clamping_min: float = 0.001,
+                       clamping_max: float = 0.999) -> int:
+        """An empty colour OctoMap on the device (ColorOctomapServer::reset with these parameters)."""
+        p = OctomapParams(resolution, prob_hit, prob_miss, clamping_min, clamping_max)
+        h = C.c_uint64()
+        self._check(self.lib.rgbdslam_b200_octomap_create(C.byref(p), C.byref(h)))
+        return h.value
+
+    def octomap_insert(self, octomap: int, nodes, transforms12, max_range: float = float("inf")):
+        """insertCloudCallback of the nodes' stored clouds in order; transforms12: (n, 3, 4) float32 node -> map, e.g.
+        octomap_pose of each estimate; max_range is maximum_depth (< 0 or inf: none)."""
+        hs = np.ascontiguousarray(np.asarray(nodes, np.uint64).reshape(-1))
+        T = np.ascontiguousarray(np.asarray(transforms12, np.float32).reshape(len(hs), 12))
+        self._check(self.lib.rgbdslam_b200_octomap_insert(C.c_uint64(octomap), len(hs), _ptr(hs), _ptr(T), float(max_range)))
+
+    def octomap_write(self, octomap: int) -> bytes:
+        """The .ot file (ColorOcTree::write) as bytes."""
+        n = C.c_int64()
+        self._check(self.lib.rgbdslam_b200_octomap_write(C.c_uint64(octomap), None, 0, C.byref(n)))
+        buf = np.zeros(n.value, np.uint8)
+        self._check(self.lib.rgbdslam_b200_octomap_write(C.c_uint64(octomap), _ptr(buf), n.value, C.byref(n)))
+        return buf.tobytes()
+
+    def octomap_stats(self, octomap: int) -> tuple[int, int]:
+        """(tree nodes with the root, leaves)"""
+        a, b = C.c_int64(), C.c_int64()
+        self._check(self.lib.rgbdslam_b200_octomap_stats(C.c_uint64(octomap), C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def octomap_clear(self, octomap: int):
+        self._check(self.lib.rgbdslam_b200_octomap_clear(C.c_uint64(octomap)))
+
+    def octomap_destroy(self, octomap: int):
+        self._check(self.lib.rgbdslam_b200_octomap_destroy(C.c_uint64(octomap)))
+
+    def node_clear_cloud(self, h: int):
+        """Node::clearPointCloud: the node drops its stored cloud"""
+        self._check(self.lib.rgbdslam_b200_node_clear_cloud(C.c_uint64(int(h))))
 
     # -- multi-GPU exchange -------------------------------------------------------------
     def comm_unique_id(self) -> np.ndarray:

@@ -44,7 +44,7 @@ static int map_ensure_streams() {
 }
 
 // The stored cloud of nd as the map kernels read it, with transform T (row-major 3 x 4 float; may be NULL).
-static MapNode map_node(const NodeDev* nd, const float* T) {
+MapNode map_node(const NodeDev* nd, const float* T) {
   const NodeCloud& c = nd->pc;
   MapNode m;
   memset(&m, 0, sizeof(m));

@@ -150,5 +150,6 @@ Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot
   if (int entry_rc__ = rb200::check_inited()) return entry_rc__
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
 void release_slab(NodeSlab* slab);  // drops one node's reference to a shared allocation, freeing it with the last (api.cu)
+MapNode map_node(const NodeDev* nd, const float* T);  // nd's stored cloud as map_point reads it, transform T (api_map.cu)
 
 }  // namespace rb200
