@@ -5,6 +5,7 @@
 //   MatchingResult               src/matching_result.h:24-46
 //   Node (feature members, matchNodePair, featureMatching-free ctor from features)   src/node.h:64-178
 //   the two image constructors (depth image node.cpp:101-240, point cloud :252-369) and pcl::PointCloud / PointXYZ[RGB]
+//   listenerNode: the listener's depth-image handling and Node construction (openni_listener.cpp:633-659, 779)
 //   bruteForceSearchORB          src/features.h:13, src/features.cpp:168-182
 // The reference types Eigen::Matrix4f / Eigen::Isometry3d / cv::DMatch / cv::KeyPoint are replaced by
 // layout-compatible PODs (column-major float[16] etc.) so this header has no third-party dependency; a
@@ -20,6 +21,7 @@
 #include <vector>
 
 #include "../rgbdslam_b200.h"
+#include "depth_resize.h"
 #include "icp.h"
 #include "map.h"
 #include "octomap.h"
@@ -162,11 +164,7 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
     const uint8_t* m = detection_mask.empty() ? nullptr : detail::packed<uint8_t>(detection_mask, tm);
     const CameraInfo ci = cam_info ? *cam_info : CameraInfo();
     const float K4[4] = {(float)ci.K[0], (float)ci.K[4], (float)ci.K[2], (float)ci.K[5]};  // node.cpp:913-916
-    const int flags = (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) | (u16 ? RGBDSLAM_B200_DEPTH_U16 : 0) |
-                      (u16 && !m ? RGBDSLAM_B200_MASK_FROM_DEPTH : 0) |
-                      (store_pointclouds() || pcl_icp() ? RGBDSLAM_B200_STORE_CLOUD | (encoding_bgr() ? 0 : RGBDSLAM_B200_ENCODING_RGB)
-                                                        : 0);
-    construct(g, d, m, visual.cols, visual.rows, K4, detector->handle(), flags);
+    construct(g, d, m, visual.cols, visual.rows, K4, detector->handle(), image_flags(visual, u16, u16 && !m));
   }
   // The reference's point-cloud constructor, argument for argument (node.h:74-78, call site openni_listener.cpp:754):
   //   Node(visual, detector, extractor, point_cloud, detection_mask)
@@ -223,12 +221,32 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   Node(const Node&) = delete;
   Node& operator=(const Node&) = delete;
 
+  // the nodes_create flags of a depth-image Node: the visual's channels, the depth's type, the mask derived from the depth, and
+  // the stored cloud of store_pointclouds() / pcl_icp()
+  static int image_flags(const Mat& visual, bool depth_u16, bool mask_from_depth) {
+    return (visual.type() == RB_8UC3 ? RGBDSLAM_B200_VISUAL_RGB : 0) | (depth_u16 ? RGBDSLAM_B200_DEPTH_U16 : 0) |
+           (mask_from_depth ? RGBDSLAM_B200_MASK_FROM_DEPTH : 0) |
+           (store_pointclouds() || pcl_icp() ? RGBDSLAM_B200_STORE_CLOUD | (encoding_bgr() ? 0 : RGBDSLAM_B200_ENCODING_RGB) : 0);
+  }
   // flags: rgbdslam_b200_nodes_create_ex's (colour visual, point cloud in place of the depth image)
   void construct(const uint8_t* gray, const float* depth_m, const uint8_t* detection_mask, int w, int h, const float K4[4],
                  uint64_t detector, int flags = 0) {
     int32_t n = 0, id32 = id_ < 0 ? 0 : id_;
     check(rgbdslam_b200_nodes_create_ex(detector, 1, gray, depth_m, detection_mask, w, h, K4, &id32, flags, &handle_, &n),
           "nodes_create");
+    download_features(n);
+  }
+  // the same for a depth image of depth_w x depth_h pixels, resized to w x h on the device (rgbdslam_b200_nodes_create_resized)
+  void construct_resized(const uint8_t* gray, const void* depth, int depth_w, int depth_h, const uint8_t* detection_mask, int w,
+                         int h, const float K4[4], uint64_t detector, int flags) {
+    int32_t n = 0, id32 = id_ < 0 ? 0 : id_;
+    check(rgbdslam_b200_nodes_create_resized(detector, 1, gray, depth, depth_w, depth_h, detection_mask, w, h, K4, &id32, flags,
+                                             &handle_, &n),
+          "nodes_create_resized");
+    download_features(n);
+  }
+  // the public feature members from the node's n features on the device
+  void download_features(int n) {
     feature_locations_2d_.resize(n);
     feature_locations_3d_.resize(n);
     feature_descriptors_.resize((size_t)n * 32);
@@ -403,6 +421,37 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
  private:
   uint64_t handle_ = 0;
 };
+
+// OpenNIListener::noCloudCallback's image handling (openni_listener.cpp:633-659) and noCloudCameraCallback's
+// new Node(visual, depth, depth_mono8_img_, cam_info, depth_header, detector, extractor) (:779) in one call.  visual CV_8UC1 or
+// CV_8UC3 as for the Node constructor; depth CV_32FC1 metres or the raw CV_16UC1 millimetres, of any size up to 4095 px per side.
+// A depth of another size than the visual is resized to the visual's size as the listener does, cv::resize(depth, depth,
+// visual.size(), 0, 0, INTER_NEAREST) (:651-656), on the device (rgbdslam_b200/depth_resize.h); the 16-bit depth is converted
+// as the Node constructor converts it.  The detection mask is depthToCV8UC1 of that depth (:659; RGBDSLAM_B200_MASK_FROM_DEPTH),
+// which the listener always builds.  cam_info is the visual camera's.  store_pointclouds(), pcl_icp() and encoding_bgr() apply
+// as in the constructor.  The caller owns the returned Node.  The Node constructor itself keeps refusing a depth of another size:
+// in the reference the resize is the listener's step, not the Node's.
+inline Node* listenerNode(const Mat& visual, const Mat& depth, const CameraInfoConstPtr& cam_info, myHeader depth_header,
+                          Ptr<Feature2D> detector, Ptr<DescriptorExtractor> extractor) {
+  if (!detector || !detector->handle()) throw std::invalid_argument("listenerNode: detector must come from createDetector(\"ORB\" or \"FAST\")");
+  if (!extractor) throw std::invalid_argument("listenerNode: null extractor");
+  const bool u16 = depth.type() == RB_16UC1;
+  if ((visual.type() != RB_8UC1 && visual.type() != RB_8UC3) || (depth.type() != RB_32FC1 && !u16) || depth.empty())
+    throw std::invalid_argument("listenerNode: visual must be CV_8UC1 or CV_8UC3 and depth CV_32FC1 or CV_16UC1");
+  std::unique_ptr<Node> node(new Node());
+  node->stamp_ = depth_header.stamp;
+  node->seq_id_ = (int)depth_header.seq;
+  std::vector<uint8_t> tg;
+  std::vector<float> td;
+  std::vector<uint16_t> tr;
+  const uint8_t* g = detail::packed<uint8_t>(visual, tg);
+  const void* d = u16 ? static_cast<const void*>(detail::packed<uint16_t>(depth, tr)) : detail::packed<float>(depth, td);
+  const CameraInfo ci = cam_info ? *cam_info : CameraInfo();
+  const float K4[4] = {(float)ci.K[0], (float)ci.K[4], (float)ci.K[2], (float)ci.K[5]};  // node.cpp:913-916
+  node->construct_resized(g, d, depth.cols, depth.rows, nullptr, visual.cols, visual.rows, K4, detector->handle(),
+                          Node::image_flags(visual, u16, true));
+  return node.release();
+}
 
 }  // namespace rgbdslam_b200
 

@@ -88,6 +88,16 @@ def node_input_flags(gray_shape, depth_shape, mask_from_depth=False, mask_from_c
     return flags
 
 
+def resized_input_flags(gray_shape, depth_shape, **kw) -> int:
+    """node_input_flags for nodes_create_resized: gray (F,H,W) or (F,H,W,3), depth (F,dh,dw) a depth image of any size with
+    the same frame count (clouds of another size than the visual are not taken)."""
+    if len(depth_shape) != 3:
+        raise ValueError(f"depth must be a depth image (F,dh,dw) (clouds of another size are not taken), got {tuple(depth_shape)}")
+    if depth_shape[0] != gray_shape[0]:
+        raise ValueError(f"gray {tuple(gray_shape)} and depth {tuple(depth_shape)} differ in frames")
+    return node_input_flags(gray_shape, tuple(gray_shape[:3]), **kw)
+
+
 class PairResult(C.Structure):
     _fields_ = [
         ("id1", C.c_int32), ("id2", C.c_int32), ("n_all_matches", C.c_int32), ("n_inliers", C.c_int32),
@@ -271,6 +281,10 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_nodes_create.argtypes = [u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.rgbdslam_b200_nodes_create_ex.argtypes = [u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_nodes_create_sharded.argtypes = [u64, u64, C.c_int, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]
+    lib.rgbdslam_b200_nodes_create_resized.argtypes = [u64, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int,
+                                                       vp, vp]
+    lib.rgbdslam_b200_nodes_create_sharded_resized.argtypes = [u64, u64, C.c_int, vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp,
+                                                               vp, C.c_int, vp, vp]
     lib.rgbdslam_b200_node_download_keypoints.argtypes = [u64, vp]
     lib.rgbdslam_b200_node_download_cloud.argtypes = [u64, C.c_int, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
@@ -616,6 +630,56 @@ class Frontend:
             det, C.c_uint64(comm), total_frames, _ptr(gray) if own else None, _ptr(depth) if own else None,
             _ptr(None if (mask_from_depth or mask_from_cloud or not own) else mask), W, H, _ptr(K4), _ptr(ids), flags, _ptr(handles),
             _ptr(nf)))
+        self._nodes += [int(h) for h in handles]
+        return [int(h) for h in handles], nf
+
+    @staticmethod
+    def _depth_image_inputs(gray, depth, mask):
+        depth_u16 = _is_u16(depth)
+        if isinstance(gray, np.ndarray):
+            gray = np.ascontiguousarray(gray, np.uint8)
+            depth = np.ascontiguousarray(depth, np.uint16 if depth_u16 else np.float32)
+            mask = None if mask is None else np.ascontiguousarray(mask, np.uint8)
+        return gray, depth, mask, depth_u16
+
+    def nodes_create_resized(self, det: int, gray, depth, mask, K4, ids=None, mask_from_depth: bool = False, bayer: bool = False,
+                             store_cloud: bool = False, encoding_rgb: bool = False):
+        """nodes_create for a depth image of another size than the visual (include/rgbdslam_b200/depth_resize.h): gray [F,H,W]
+        u8 or [F,H,W,3] colour, depth [F,dh,dw] f32 metres or u16 millimetres, resized on the device to H x W as the listener's
+        cv::resize(INTER_NEAREST) does; mask [F,H,W] u8 or None; K4 the visual camera's.  The nodes equal nodes_create's on
+        cv2.resize(depth, (W, H), interpolation=cv2.INTER_NEAREST).  Raises ValueError for cloud-shaped depth or another frame
+        count."""
+        gray, depth, mask, depth_u16 = self._depth_image_inputs(gray, depth, mask)
+        flags = resized_input_flags(gray.shape, depth.shape, mask_from_depth=mask_from_depth, depth_u16=depth_u16, bayer=bayer,
+                                    store_cloud=store_cloud, encoding_rgb=encoding_rgb)
+        F, H, W = gray.shape[:3]
+        dh, dw = depth.shape[1:3]
+        K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
+        ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
+        handles = np.zeros(F, np.uint64)
+        nf = np.zeros(F, np.int32)
+        self._check(self.lib.rgbdslam_b200_nodes_create_resized(det, F, _ptr(gray), _ptr(depth), dw, dh,
+                                                                _ptr(None if mask_from_depth else mask), W, H, _ptr(K4), _ptr(ids),
+                                                                flags, _ptr(handles), _ptr(nf)))
+        self._nodes += [int(h) for h in handles]
+        return [int(h) for h in handles], nf
+
+    def nodes_create_sharded_resized(self, det: int, comm: int, total_frames: int, gray, depth, mask, K4, ids=None,
+                                     mask_from_depth: bool = False, bayer: bool = False):
+        """nodes_create_sharded for depth images of another size than the visual: gray / depth / mask hold THIS rank's frames,
+        depth [F,dh,dw] as in nodes_create_resized; returns handles and feature counts of ALL total_frames nodes."""
+        gray, depth, mask, depth_u16 = self._depth_image_inputs(gray, depth, mask)
+        flags = resized_input_flags(gray.shape, depth.shape, mask_from_depth=mask_from_depth, depth_u16=depth_u16, bayer=bayer)
+        H, W = gray.shape[1:3]
+        dh, dw = depth.shape[1:3]
+        K4 = None if K4 is None else np.ascontiguousarray(K4, np.float32)
+        ids = None if ids is None else np.ascontiguousarray(ids, np.int32)
+        handles = np.zeros(total_frames, np.uint64)
+        nf = np.zeros(total_frames, np.int32)
+        own = gray.shape[0] > 0
+        self._check(self.lib.rgbdslam_b200_nodes_create_sharded_resized(
+            det, C.c_uint64(comm), total_frames, _ptr(gray) if own else None, _ptr(depth) if own else None, dw, dh,
+            _ptr(None if (mask_from_depth or not own) else mask), W, H, _ptr(K4), _ptr(ids), flags, _ptr(handles), _ptr(nf)))
         self._nodes += [int(h) for h in handles]
         return [int(h) for h in handles], nf
 

@@ -10,12 +10,15 @@
 //                                 with DEPTH_U16 / VISUAL_BAYER_GR the listener's conversions of its raw 16UC1 depth and
 //                                 bayer_grbg8 images (openni_listener.cpp:633-659), with STORE_CLOUD the colour cloud pc_col
 //                                 (createXYZRGBPointCloud, node.cpp:126-131, misc.cpp:467-556) for the map
+//   rgbdslam_b200_nodes_create_resized / _sharded_resized == the same after the listener's nearest-neighbour resize of a depth
+//                                 image of another size than the visual (openni_listener.cpp:651-656; rgbdslam_b200/depth_resize.h)
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <mutex>
 #include <vector>
 
+#include "../../include/rgbdslam_b200/depth_resize.h"
 #include "comm.h"
 #include "kernels.h"
 #include "orb_host.h"
@@ -52,7 +55,13 @@ struct OrbCtx {
   bool quotas = false;         // the ORB detector applies cv::ORB's per-level quotas: orb_prepare
   DevBuf in_gray[2], in_mask[2], in_depth[2];  // double-buffered chunk inputs (upload of chunk k+1 under the kernels of chunk k)
   DevBuf in_rgb[2];                            // colour or Bayer input, converted into in_gray on the device
-  DevBuf in_raw[2];                            // 16-bit millimetre depth, converted into in_depth (and in_mask) on the device
+  DevBuf in_raw[2];  // depth as the caller passes it when it is not the w x h float plane (16-bit millimetres, or another size),
+                     // gathered / converted into in_depth (and in_mask) on the device
+  // the nearest-neighbour resize tables of a depth image of nn_dw x nn_dh into nn_w x nn_h (nn_resize_tables): w source columns,
+  // then h source rows
+  std::vector<uint16_t> h_nn;
+  DevBuf d_nn;
+  int nn_w = 0, nn_h = 0, nn_dw = 0, nn_dh = 0;
   PinBuf stage[2];                             // pinned staging for callers that pass pageable memory
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
@@ -69,8 +78,9 @@ struct OrbCtx {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &in_rgb[0],
                      &in_rgb[1], &in_raw[0], &in_raw[1], &cell_img, &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp,
                      &cell_out, &cell_out_count, &cand_z, &scratch, &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray,
-                     &sh_rgb, &sh_raw, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr};
+                     &sh_rgb, &sh_raw, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr, &d_nn};
     for (DevBuf* b : all) b->release();
+    nn_w = nn_h = nn_dw = nn_dh = 0;
     stage[0].release();
     stage[1].release();
     ready = false;
@@ -269,6 +279,30 @@ static int orb_prepare(int W, int H) {
   return 0;
 }
 
+// cv::resize(depth, depth, visual.size(), 0, 0, INTER_NEAREST) (openni_listener.cpp:651-656) of a dw x dh depth image to the
+// w x h visual, as cv2 4.13's resizeNN indexes it: ifx = 1.0 / ((double)w / dw) in double, source column
+// min((int)floor(x * ifx), dw - 1), rows likewise (the exact quotient x * dw / w picks another pixel at some sizes).  Built on
+// the host and uploaded once per (w, h, dw, dh), as orb_prepare's pyramid tables are per frame size.
+static int nn_resize_tables(int w, int h, int dw, int dh) {
+  OrbCtx& o = g_orb;
+  if (o.nn_w == w && o.nn_h == h && o.nn_dw == dw && o.nn_dh == dh) return 0;
+  auto axis = [&](int n, int dn) {
+    const double ifx = 1.0 / ((double)n / dn);
+    for (int x = 0; x < n; x++) o.h_nn.push_back((uint16_t)std::min((int)std::floor(x * ifx), dn - 1));
+  };
+  o.h_nn.clear();
+  axis(w, dw);
+  axis(h, dh);
+  int rc;
+  if ((rc = o.d_nn.ensure(o.h_nn.size() * 2))) return rc;
+  cudaStream_t st = g_state.stream;
+  cudaError_t e = cudaMemcpyAsync(o.d_nn.ptr, o.h_nn.data(), o.h_nn.size() * 2, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return cuda_fail(e, "nn_resize_tables upload");
+  o.nn_w = w; o.nn_h = h; o.nn_dw = dw; o.nn_dh = dh;
+  return 0;
+}
+
 constexpr int kOrbChunk = 64;  // frames per pass of nodes_create for grey + depth-image input
 
 // The recipe of a call: what one frame brings (from the flags of nodes_create*, include/rgbdslam_b200.h) and how its keypoints
@@ -276,7 +310,9 @@ constexpr int kOrbChunk = 64;  // frames per pass of nodes_create for grey + dep
 struct FrameInput {
   int mode = 0;                               // 0: detector output, 1: Node constructor
   bool rgb = false, bayer = false, mask_from_depth = false, mask_from_cloud = false;
-  bool depth_u16 = false, mask_from_u16 = false;  // 16-bit millimetres; its mask is written into the mask buffer (k_depth_u16)
+  bool depth_u16 = false, mask_from_u16 = false;  // 16-bit millimetres; its mask is written into the mask buffer (k_depth_gather)
+  bool resize = false;                        // the depth image is dw x dh, not w x h (nodes_create_resized): k_depth_gather resizes it
+  int dw = 0, dh = 0;                         // the depth image's size as the caller passes it
   bool caller_mask = false;                   // the caller's mask is uploaded (not replaced by one derived on the device)
   int cloud_stride = 0;                       // floats per cloud point (4: PointXYZ, 8: PointXYZRGB); 0 = depth image
   size_t gray_bytes = 0, depth_bytes = 0;     // per frame, as the caller passes them: the visual image, the depth image or cloud
@@ -285,8 +321,13 @@ struct FrameInput {
   float depth_scaling = 1.f;
   float4 Kinv = {0.f, 0.f, 0.f, 0.f};         // projectTo3D intrinsics (node.cpp:913-916): float(1./fx), float(1./fy), cx, cy
   FrameInput() = default;
-  FrameInput(int flags, size_t px, const rgbdslam_b200_params& p, const float* K4, const uint8_t* mask) {
+  // w x h frames whose depth image is dw x dh (nodes_create_resized; the same size for every other call)
+  FrameInput(int flags, int w, int h, const rgbdslam_b200_params& p, const float* K4, const uint8_t* mask, int dw_, int dh_) {
+    const size_t px = (size_t)w * h, dpx = (size_t)dw_ * dh_;
     mode = 1;
+    dw = dw_;
+    dh = dh_;
+    resize = dw != w || dh != h;
     rgb = (flags & RGBDSLAM_B200_VISUAL_RGB) != 0;
     bayer = (flags & RGBDSLAM_B200_VISUAL_BAYER_GR) != 0;
     depth_u16 = (flags & RGBDSLAM_B200_DEPTH_U16) != 0;
@@ -297,7 +338,7 @@ struct FrameInput {
     caller_mask = mask && !from_depth && !mask_from_cloud;
     cloud_stride = (flags & RGBDSLAM_B200_CLOUD_XYZRGB) ? 8 : (flags & RGBDSLAM_B200_CLOUD_XYZ) ? 4 : 0;
     gray_bytes = rgb ? 3 * px : px;
-    depth_bytes = cloud_stride ? px * cloud_stride * 4 : depth_u16 ? px * 2 : px * 4;
+    depth_bytes = cloud_stride ? px * cloud_stride * 4 : depth_u16 ? dpx * 2 : dpx * 4;
     plane_bytes = cloud_stride ? depth_bytes : px * 4;
     // getMinDepthInNeighborhood (node.cpp:82-83, 940-941) is a depth-image rule: the point-cloud constructor does not read it
     points = cloud_stride ? OrbPoints::kCloud : p.use_feature_min_depth ? OrbPoints::kMinDepth : OrbPoints::kDepthPixel;
@@ -308,6 +349,7 @@ struct FrameInput {
   }
   bool mask_buffer() const { return caller_mask || mask_from_cloud || mask_from_u16; }  // a device mask per frame
   bool raw_visual() const { return rgb || bayer; }  // the visual is uploaded into in_rgb / sh_rgb and converted into grey
+  bool raw_depth() const { return depth_u16 || resize; }  // the depth is uploaded into in_raw / sh_raw and gathered into the plane
   // frames per chunk: the input and staging buffers hold about as many bytes as kOrbChunk grey + depth-image frames (a
   // 640x480 XYZRGB cloud is 9.8 MB, against 1.5 MB), and never more than kOrbChunk frames, which bounds the per-frame work
   // buffers (16-bit depth would allow 106); the chunk size does not change any result.  Frames wider or taller than
@@ -335,7 +377,7 @@ static int orb_ensure_streams() {
 
 // work buffers for F frames per pass; nbuf input buffers (1: synchronous single-frame entry points, 2: nodes_create)
 // depth_bytes: per frame (0 = a w*h float depth image); visual_bytes / raw_bytes: per frame of the colour or Bayer input
-// buffers / of the 16-bit depth input buffers (0 = none)
+// buffers / of the raw depth input buffers, 16-bit or of another size (0 = none)
 static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_bytes = 0, size_t visual_bytes = 0, size_t raw_bytes = 0) {
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
@@ -511,7 +553,7 @@ static int batch_fail(NodeBatch& nb, int code) {
 
 // Frame input of a nodes_create* call: the caller's buffers are copied from directly when they are pinned, else through the two
 // pinned staging buffers (chunk frames each).
-static int setup_staging(const uint8_t* gray, const float* depth, const uint8_t* mask, size_t px, const FrameInput& in, int chunk,
+static int setup_staging(const uint8_t* gray, const void* depth, const uint8_t* mask, size_t px, const FrameInput& in, int chunk,
                          bool* pinned) {
   OrbCtx& o = g_orb;
   *pinned = is_pinned(gray) && is_pinned(depth) && (!mask || is_pinned(mask));
@@ -551,14 +593,19 @@ static int upload_chunk(int ci, int F, int chunk, size_t px, const FrameInput& i
   return 0;
 }
 
-// The input kernels of a chunk of F frames: cvtColor of the colour or Bayer visuals drgb into dg, the conversion of the 16-bit
-// depth images draw into dd (and their mask into dm), calculateDepthMask of the clouds dd into dm.
-static cudaError_t chunk_inputs(const FrameInput& in, int F, size_t px, const uint8_t* drgb, uint8_t* dg, const uint16_t* draw,
+// The input kernels of a chunk of F frames: cvtColor of the colour or Bayer visuals drgb into dg, the resize and / or conversion
+// of the raw depth images draw into dd (and the 16-bit mask into dm), calculateDepthMask of the clouds dd into dm.
+static cudaError_t chunk_inputs(const FrameInput& in, int F, size_t px, const uint8_t* drgb, uint8_t* dg, const void* draw,
                                 float* dd, uint8_t* dm, cudaStream_t st, int* launches) {
+  const OrbCtx& o = g_orb;
   cudaError_t e = cudaSuccess;
   if (in.rgb) e = orb_run_rgb_to_gray(F, px, drgb, dg, st, launches);
-  if (in.bayer) e = orb_run_bayer_gr_to_gray(F, g_orb.g.W, g_orb.g.H, drgb, dg, st, launches);
-  if (e == cudaSuccess && in.depth_u16) e = orb_run_depth_u16(F, px, draw, dd, in.mask_from_u16 ? dm : nullptr, st, launches);
+  if (in.bayer) e = orb_run_bayer_gr_to_gray(F, o.g.W, o.g.H, drgb, dg, st, launches);
+  if (e == cudaSuccess && in.raw_depth()) {
+    const uint16_t* col = in.resize ? (const uint16_t*)o.d_nn.ptr : nullptr;
+    e = orb_run_depth_gather(F, o.g.W, o.g.H, draw, in.depth_u16, in.dw, in.dh, col, col ? col + o.g.W : nullptr, dd,
+                             in.mask_from_u16 ? dm : nullptr, st, launches);
+  }
   if (e == cudaSuccess && in.mask_from_cloud) e = orb_run_cloud_mask(F, px, dd, in.cloud_stride, dm, st, launches);
   return e;
 }
@@ -791,27 +838,32 @@ int rgbdslam_b200_orb_compute(const uint8_t* gray, int w, int h, const rgbdslam_
   return 0;
 }
 
+}  // extern "C"
+
+namespace rb200 {
+
 // Node::Node for nframes frames in order.  Pipeline per chunk of kOrbChunk frames:
 //   copy stream    : host -> device of the chunk's gray / depth / mask into one of two input buffers (straight from the caller's
 //                    buffers when they are pinned, else through pinned staging filled by this thread)
 //   compute stream : detect kernels -> threshold recurrence (device) -> Harris / keepStrongest / finalize -> describe, writing
 //                    straight into the slab that holds all nodes of the call (no per-node allocation, no device->device copy)
 // The only host synchronisation is the download of the feature counts at the end.
-int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
-                                  int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
-                                  int32_t* n_features) {
-  RB200_ENTER_INITED();
+// nodes_create_ex and nodes_create_resized (depth images of dw x dh; dw == w and dh == h is nodes_create_ex), with the entry
+// lock held.
+static int nodes_create_run(const char* what, uint64_t detector, int nframes, const uint8_t* gray, const void* depth, int dw, int dh,
+                            const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
+                            int32_t* n_features) {
   Detector* det = get_detector(detector);
   int rc;
-  if ((rc = check_nodes_args("nodes_create", det, nframes, K4, node_handles, flags))) return rc;
+  if ((rc = check_nodes_args(what, det, nframes, K4, node_handles, flags))) return rc;
   if (nframes > 0 && (!gray || !depth)) {
-    set_error("nodes_create: null image buffers");
+    set_error(std::string(what) + ": null image buffers");
     return RGBDSLAM_B200_ERR_ARG;
   }
   if (nframes == 0) return 0;
   State& s = g_state;
   const size_t px = (size_t)w * h;
-  const FrameInput in(flags, px, s.params, K4, mask);
+  const FrameInput in(flags, w, h, s.params, K4, mask, dw, dh);
   const bool store = (flags & RGBDSLAM_B200_STORE_CLOUD) != 0, model = s.params.observability_threshold > 0.0;
   // a stored cloud of cloud input is the kept cloud plus colour: the measurement model reads it as it reads KEEP_CLOUD's
   const bool keep_cloud = (flags & RGBDSLAM_B200_KEEP_CLOUD) != 0 || (store && in.cloud_stride);
@@ -827,11 +879,11 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     return RGBDSLAM_B200_ERR_STATE;
   }
   if (!in.caller_mask) mask = nullptr;
-  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams()) || (in.resize && (rc = nn_resize_tables(w, h, dw, dh)))) return rc;
   OrbCtx& o = g_orb;
   const int chunk = in.chunk(nframes, px, o.wide);
   if ((rc = orb_ensure_buffers(chunk, 2, in.mask_buffer(), in.plane_bytes, in.raw_visual() ? in.gray_bytes : 0,
-                               in.depth_u16 ? in.depth_bytes : 0)))
+                               in.raw_depth() ? in.depth_bytes : 0)))
     return rc;
   cudaStream_t st = s.stream;
   const int K = std::min(o.kp_stride, s.params.max_keypoints);  // features per node (finalize mode 1 emits <= max_keypoints)
@@ -875,10 +927,10 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
     uint8_t* dg = (uint8_t*)o.in_gray[b].ptr;
     float* dd = (float*)o.in_depth[b].ptr;
     uint8_t* drgb = (uint8_t*)o.in_rgb[b].ptr;
-    uint16_t* draw = (uint16_t*)o.in_raw[b].ptr;
+    void* draw = o.in_raw[b].ptr;
     uint8_t* dm = in.mask_buffer() ? (uint8_t*)o.in_mask[b].ptr : nullptr;
     if ((rc = upload_chunk(ci, F, chunk, px, in, pinned, gray + in.gray_bytes * f0, (const float*)((const uint8_t*)depth + in.depth_bytes * f0),
-                           mask ? mask + px * f0 : nullptr, in.raw_visual() ? drgb : dg, in.depth_u16 ? (void*)draw : dd,
+                           mask ? mask + px * f0 : nullptr, in.raw_visual() ? drgb : dg, in.raw_depth() ? draw : dd,
                            mask ? dm : nullptr, o.ev_free[b])))
       return batch_fail(nb, rc);
     if (f0 == 0) o.last_gray = dg;
@@ -909,21 +961,33 @@ int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t*
   return 0;
 }
 
-// Frame-sharded Node construction: see include/rgbdslam_b200.h.  Two passes over the rank's own frames around ONE exchange of
-// the score histograms; then one exchange of the finished features.
-int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
-                                       const float* depth, const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids,
-                                       int flags, uint64_t* node_handles, int32_t* n_features) {
-  RB200_ENTER_INITED();
+// nodes_create_resized's own checks, before any device work: the depth size, and no cloud input (the listener drops clouds of
+// another size than the visual, openni_listener.cpp:713-719)
+static int check_resized_args(const char* what, int dw, int dh, int flags) {
+  const char* bad = nullptr;
+  if (dw < 1 || dh < 1 || dw > kOrbMaxSide || dh > kOrbMaxSide) bad = "depth_w and depth_h must be within [1, 4095]";
+  else if (flags & (RGBDSLAM_B200_CLOUD_XYZRGB | RGBDSLAM_B200_CLOUD_XYZ | RGBDSLAM_B200_MASK_FROM_CLOUD | RGBDSLAM_B200_KEEP_CLOUD))
+    bad = "takes depth images only (CLOUD_XYZRGB, CLOUD_XYZ, MASK_FROM_CLOUD and KEEP_CLOUD are rejected)";
+  if (bad) {
+    set_error(std::string(what) + ": " + bad);
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  return 0;
+}
+
+// nodes_create_sharded and nodes_create_sharded_resized (own depth images of dw x dh), with the entry lock held.
+static int nodes_create_sharded_run(const char* what, uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
+                                    const void* depth, int dw, int dh, const uint8_t* mask, int w, int h, const float* K4,
+                                    const int32_t* ids, int flags, uint64_t* node_handles, int32_t* n_features) {
   if (flags & (RGBDSLAM_B200_KEEP_CLOUD | RGBDSLAM_B200_STORE_CLOUD)) {
-    set_error("nodes_create_sharded: KEEP_CLOUD and STORE_CLOUD are not supported (the clouds are not exchanged between ranks)");
+    set_error(std::string(what) + ": KEEP_CLOUD and STORE_CLOUD are not supported (the clouds are not exchanged between ranks)");
     return RGBDSLAM_B200_ERR_ARG;
   }
   Comm* cm = get_comm(comm_handle);
   if (!cm) return RGBDSLAM_B200_ERR_ARG;
   Detector* det = get_detector(detector);
   int rc;
-  if ((rc = check_nodes_args("nodes_create_sharded", det, total_frames, K4, node_handles, flags))) return rc;
+  if ((rc = check_nodes_args(what, det, total_frames, K4, node_handles, flags))) return rc;
   if (total_frames == 0) return 0;
   State& s = g_state;
   if (s.params.observability_threshold > 0.0) {
@@ -935,13 +999,13 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   const int f0 = std::min(rank * per, total_frames), f1 = std::min((rank + 1) * per, total_frames);
   const int own = f1 - f0, Wp = world * per;
   if (own > 0 && (!gray || !depth)) {
-    set_error("nodes_create_sharded: null image buffers");
+    set_error(std::string(what) + ": null image buffers");
     return RGBDSLAM_B200_ERR_ARG;
   }
   const size_t px = (size_t)w * h;
-  const FrameInput in(flags, px, s.params, K4, mask);
+  const FrameInput in(flags, w, h, s.params, K4, mask, dw, dh);
   if (!in.caller_mask) mask = nullptr;
-  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams())) return rc;
+  if ((rc = orb_prepare(w, h)) || (rc = orb_ensure_streams()) || (in.resize && (rc = nn_resize_tables(w, h, dw, dh)))) return rc;
   OrbCtx& o = g_orb;
   const OrbGeom& g = o.g;
   const int chunk = in.chunk(own, px, o.wide);
@@ -950,7 +1014,7 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   const size_t own_ = (size_t)std::max(own, 1);
   if ((rc = o.sh_gray.ensure(px * own_)) || (rc = o.sh_depth.ensure(in.plane_bytes * own_)) ||
       (in.mask_buffer() && (rc = o.sh_mask.ensure(px * own_))) || (in.raw_visual() && (rc = o.sh_rgb.ensure(in.gray_bytes * own_))) ||
-      (in.depth_u16 && (rc = o.sh_raw.ensure(in.depth_bytes * own_))) ||
+      (in.raw_depth() && (rc = o.sh_raw.ensure(in.depth_bytes * own_))) ||
       (rc = o.sh_cell_img.ensure((size_t)g.cell_bytes * own_)) || (rc = o.sh_cand.ensure(own_ * nc * o.cand_cap * sizeof(OrbCand))) ||
       (rc = o.all_hist.ensure((size_t)Wp * nc * 256 * 4)) || (rc = o.all_cnt.ensure((size_t)Wp * nc * 4)) ||
       (rc = o.all_many.ensure((size_t)Wp * nc * 4)) || (rc = o.all_thr.ensure((size_t)Wp * nc * 4)))
@@ -980,11 +1044,11 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
     const int F = std::min(chunk, own - c0);
     uint8_t* dg = (uint8_t*)o.sh_gray.ptr + px * c0;
     uint8_t* drgb = in.raw_visual() ? (uint8_t*)o.sh_rgb.ptr + in.gray_bytes * c0 : nullptr;
-    uint16_t* draw = in.depth_u16 ? (uint16_t*)o.sh_raw.ptr + px * c0 : nullptr;
+    void* draw = in.raw_depth() ? (uint8_t*)o.sh_raw.ptr + in.depth_bytes * c0 : nullptr;
     float* dd = (float*)((uint8_t*)o.sh_depth.ptr + in.plane_bytes * c0);
     uint8_t* dm = in.mask_buffer() ? (uint8_t*)o.sh_mask.ptr + px * c0 : nullptr;
     if ((rc = upload_chunk(ci, F, chunk, px, in, pinned, gray + in.gray_bytes * c0, (const float*)((const uint8_t*)depth + in.depth_bytes * c0),
-                           mask ? mask + px * c0 : nullptr, in.raw_visual() ? drgb : dg, in.depth_u16 ? (void*)draw : dd,
+                           mask ? mask + px * c0 : nullptr, in.raw_visual() ? drgb : dg, in.raw_depth() ? draw : dd,
                            mask ? dm : nullptr, nullptr)))
       return batch_fail(nb, rc);
     if (c0 == 0) o.last_gray = dg;
@@ -1031,6 +1095,46 @@ int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, 
   if ((rc = batch_publish(nb, total_frames, f0, own, ids, node_handles, n_features, "nodes_create_sharded finish"))) return rc;
   s.launches += launches;
   return 0;
+}
+
+}  // namespace rb200
+
+extern "C" {
+
+int rgbdslam_b200_nodes_create_ex(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
+                                  int w, int h, const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
+                                  int32_t* n_features) {
+  RB200_ENTER_INITED();
+  return nodes_create_run("nodes_create", detector, nframes, gray, depth, w, h, mask, w, h, K4, ids, flags, node_handles, n_features);
+}
+
+int rgbdslam_b200_nodes_create_resized(uint64_t detector, int nframes, const uint8_t* gray, const void* depth, int depth_w, int depth_h,
+                                       const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids, int flags,
+                                       uint64_t* node_handles, int32_t* n_features) {
+  RB200_ENTER_INITED();
+  if (int rc = check_resized_args("nodes_create_resized", depth_w, depth_h, flags)) return rc;
+  return nodes_create_run("nodes_create_resized", detector, nframes, gray, depth, depth_w, depth_h, mask, w, h, K4, ids, flags,
+                          node_handles, n_features);
+}
+
+// Frame-sharded Node construction: see include/rgbdslam_b200.h.  Two passes over the rank's own frames around ONE exchange of
+// the score histograms; then one exchange of the finished features.
+int rgbdslam_b200_nodes_create_sharded(uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
+                                       const float* depth, const uint8_t* mask, int w, int h, const float* K4, const int32_t* ids,
+                                       int flags, uint64_t* node_handles, int32_t* n_features) {
+  RB200_ENTER_INITED();
+  return nodes_create_sharded_run("nodes_create_sharded", detector, comm_handle, total_frames, gray, depth, w, h, mask, w, h, K4, ids,
+                                  flags, node_handles, n_features);
+}
+
+int rgbdslam_b200_nodes_create_sharded_resized(uint64_t detector, uint64_t comm_handle, int total_frames, const uint8_t* gray,
+                                               const void* depth, int depth_w, int depth_h, const uint8_t* mask, int w, int h,
+                                               const float* K4, const int32_t* ids, int flags, uint64_t* node_handles,
+                                               int32_t* n_features) {
+  RB200_ENTER_INITED();
+  if (int rc = check_resized_args("nodes_create_sharded_resized", depth_w, depth_h, flags)) return rc;
+  return nodes_create_sharded_run("nodes_create_sharded_resized", detector, comm_handle, total_frames, gray, depth, depth_w, depth_h,
+                                  mask, w, h, K4, ids, flags, node_handles, n_features);
 }
 
 int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,

@@ -380,7 +380,7 @@ def main_raw(args):
     out["h2d_bytes_per_frame"] = {k: c[3] for k, c in base.items()}
 
     # ---- the conversion kernels' device time per frame (torch.profiler, separate pass)
-    kernels = ("k_depth_u16", "k_bayer_gr_to_gray", "k_rgb_to_gray")
+    kernels = ("k_depth_gather", "k_bayer_gr_to_gray", "k_rgb_to_gray")
     prof_frames = min(64, nt)
     ktimes = {}
     for c in ("bayer_u16_pinned", "rgb_float_pinned"):
