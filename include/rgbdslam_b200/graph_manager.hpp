@@ -10,6 +10,7 @@
 //   size_t reducePointClouds()      == reducePointCloud for every node   graph_manager.cpp:1310-1319 -> rgbdslam_b200_reduce_clouds
 //   void   saveOctomap(filename)    == saveOctomapImpl                   graph_mgr_io.cpp:253-310 -> rgbdslam_b200_octomap_*
 //   void   renderToOctomap(Node*), writeOctomap(filename)              graph_mgr_io.cpp:312-329
+//   void   occupancyFilterClouds()                                      graph_manager.cpp:1372-1381 -> rgbdslam_b200_octomap_filter_clouds
 // Host logic only; every compute step is a C-ABI call.  The reference draws from the global rand(); here every draw comes
 // from the library's counter-based generator keyed by (seed, node id).  g2o's HyperDijkstra (not under /root/reference) is
 // restated in geodesicBall().  The Python mirror rgbdslam_v2_b200/graph_manager.py is the tested twin of this file.
@@ -60,14 +61,12 @@ inline void rotToQuat(const double R[9], double* q) {  // Eigen::Quaternion(Matr
   const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
   for (int a = 0; a < 4; a++) q[a] /= n;
 }
-// The float 3 x 4 (row-major, node -> map) saveOctomap applies to a node whose estimate has rotation R (row-major, double)
-// and translation t: updateCloudOrigin stores R cast to float as an Eigen Quaternionf (Eigen's trace -- its unrolled
-// reduction m00 + (m11 + m22) -- and largest-diagonal algorithm, in float) and t as float; insertCloudCallback widens the
-// quaternion to a tf::Quaternion, tf::Matrix3x3::setRotation builds the basis in double, pcl_ros::transformPointCloud takes it
-// back with getRotation (tf's branch and tie rule), narrows it to a Quaternionf and applies toRotationMatrix (float).  The
-// ray origin is the translation column.  rgbdslam_v2_b200._capi.octomap_pose is the same chain in numpy.
-inline void octomapPose(const double R[9], const double t[3], float T[12]) {
-  float r[9], q[4];  // q: x, y, z, w
+// What updateCloudOrigin stores in a node's cloud for an estimate with rotation R (row-major, double) and translation t:
+// sensor_orientation_ q (x, y, z, w), R cast to float as an Eigen Quaternionf (Eigen's trace -- its unrolled reduction
+// m00 + (m11 + m22) -- and largest-diagonal algorithm, in float), and sensor_origin_ o, t as float.
+// rgbdslam_v2_b200._capi.cloud_sensor_pose is the same step in numpy.
+inline void cloudSensorPose(const double R[9], const double t[3], float q[4], float o[3]) {
+  float r[9];
   for (int i = 0; i < 9; i++) r[i] = (float)R[i];
   const float tr = r[0] + (r[4] + r[8]);
   if (tr > 0.0f) {
@@ -87,6 +86,16 @@ inline void octomapPose(const double R[9], const double t[3], float T[12]) {
     q[j] = (r[3 * j + i] + r[3 * i + j]) * s;
     q[k] = (r[3 * k + i] + r[3 * i + k]) * s;
   }
+  for (int i = 0; i < 3; i++) o[i] = (float)t[i];
+}
+// The float 3 x 4 (row-major, node -> map) saveOctomap applies to a node whose estimate has rotation R (row-major, double)
+// and translation t: cloudSensorPose, then insertCloudCallback widens the quaternion to a tf::Quaternion,
+// tf::Matrix3x3::setRotation builds the basis in double, pcl_ros::transformPointCloud takes it back with getRotation (tf's
+// branch and tie rule), narrows it to a Quaternionf and applies toRotationMatrix (float).  The ray origin is the translation
+// column.  rgbdslam_v2_b200._capi.octomap_pose is the same chain in numpy.
+inline void octomapPose(const double R[9], const double t[3], float T[12]) {
+  float q[4], o[3];  // q: x, y, z, w
+  cloudSensorPose(R, t, q, o);
   // tf::Matrix3x3::setRotation(tf::Quaternion(x, y, z, w)) in double
   const double x = q[0], y = q[1], z = q[2], w = q[3];
   const double d = x * x + y * y + z * z + w * w, s2 = 2.0 / d;
@@ -116,9 +125,9 @@ inline void octomapPose(const double R[9], const double t[3], float T[12]) {
   const float tx = 2.0f * fx, ty = 2.0f * fy, tz = 2.0f * fz;
   const float twx = tx * fw, twy = ty * fw, twz = tz * fw, txx = tx * fx, txy = ty * fx, txz = tz * fx;
   const float tyy = ty * fy, tyz = tz * fy, tzz = tz * fz;
-  const float out[12] = {1.0f - (tyy + tzz), txy - twz, txz + twy, (float)t[0],
-                         txy + twz, 1.0f - (txx + tzz), tyz - twx, (float)t[1],
-                         txz - twy, tyz + twx, 1.0f - (txx + tyy), (float)t[2]};
+  const float out[12] = {1.0f - (tyy + tzz), txy - twz, txz + twy, o[0],
+                         txy + twz, 1.0f - (txx + tzz), tyz - twx, o[1],
+                         txz - twy, tyz + twx, 1.0f - (txx + tyy), o[2]};
   std::memcpy(T, out, sizeof(out));
 }
 
@@ -331,7 +340,10 @@ class GraphManager {
     std::vector<uint8_t> fixed;
     std::vector<int32_t> ij;
     gather(ids, poses, fixed, ij, meas, info);
-    if (ij.empty()) return 0.0;
+    if (ij.empty()) {
+      renderNewestOnline();
+      return 0.0;
+    }
     fixationOfVertices(ids, fixed);
     const double stop = break_criterion > 0.0 ? break_criterion : params.optimizer_iterations;  // :942
     double chi2 = 0;
@@ -345,6 +357,7 @@ class GraphManager {
     fixed_ids_.clear();
     if (params.pose_relative_to == "inaffected") fixed_ids_.insert(ids.begin(), ids.end());
     last_chi2 = chi2;
+    renderNewestOnline();
     return chi2;
   }
 
@@ -526,13 +539,41 @@ class GraphManager {
   static int& octomap_autosave_step() { static int v = 50; return v; }
   static bool& octomap_clear_after_save() { static bool v = false; return v; }
   static bool& octomap_clear_raycasted_clouds() { static bool v = false; return v; }
+  // octomap_online_creation (parameter_server.cpp:65): optimizeGraph ends by rendering the newest node into the map, firstNode
+  // runs optimizeGraph, and saveOctomap only writes the map
+  static bool& octomap_online_creation() { static bool v = false; return v; }
+  // occupancy_filter_threshold (parameter_server.cpp:69) of occupancyFilterClouds
+  static double& occupancy_filter_threshold() { static double v = 0.9; return v; }
 
   // GraphManager::updateCloudOrigin (graph_mgr_io.cpp:216-235): the node has a valid estimate, a vertex and a non-empty stored
-  // cloud.  (The reference's function lacks its final `return true`; true is its evident intent.)
+  // cloud; the cloud then records the estimate as its sensor pose (Node::cloud_sensor_pose_, cloudSensorPose).  (The
+  // reference's function lacks its final `return true`; true is its evident intent.)
   bool updateCloudOrigin(const Node* node) const {
     if (!node->valid_tf_estimate_ || !estimates_.count(node->vertex_id_)) return false;
     int w = 0, h = 0;
-    return rgbdslam_b200_node_download_cloud(node->handle(), 32, nullptr, &w, &h) == 0 && (long long)w * h > 0;
+    if (rgbdslam_b200_node_download_cloud(node->handle(), 32, nullptr, &w, &h) != 0 || (long long)w * h == 0) return false;
+    const Pose7& p = estimates_.at(node->vertex_id_);
+    double R[9];
+    quatToRot(p.v + 3, R);
+    cloudSensorPose(R, p.v, node->cloud_sensor_pose_, node->cloud_sensor_pose_ + 4);
+    return true;
+  }
+  // GraphManager::occupancyFilterClouds (graph_manager.cpp:1372-1381): ColorOctomapServer::occupancyFilter of every node of
+  // graph_ that has a stored cloud, each under the sensor pose its cloud holds, against the map, in one device call.  Without
+  // a map yet an empty one is made first (as writeOctomap does): every cloud is then emptied, as in the reference.
+  void occupancyFilterClouds() {
+    if (!octomap_) resetOctomap();
+    std::vector<uint64_t> handles;
+    std::vector<float> sensor;
+    for (auto& kv : graph_) {
+      int w = 0, h = 0;
+      if (rgbdslam_b200_node_download_cloud(kv.second->handle(), 32, nullptr, &w, &h) != 0) continue;
+      handles.push_back(kv.second->handle());
+      sensor.insert(sensor.end(), kv.second->cloud_sensor_pose_, kv.second->cloud_sensor_pose_ + 7);
+    }
+    check(rgbdslam_b200_octomap_filter_clouds(octomap_, (int)handles.size(), handles.data(), sensor.data(), occupancy_filter_threshold(),
+                                              nullptr),
+          "octomap_filter_clouds");
   }
   // octomapPose of the node's estimate
   void octomapTransform(int vertex_id, float T[12]) const {
@@ -569,8 +610,12 @@ class GraphManager {
   // map, each node rendered (octomap_clear_raycasted_clouds applied after it), the file written after every
   // octomap_autosave_step-th node (<= 0: never; the reference divides by it) and once more at the end, then with
   // octomap_clear_after_save a reset.  The nodes between two autosaves go to the device in one insert call: how many one
-  // call takes does not change the map.
+  // call takes does not change the map.  With octomap_online_creation the map is only written (no reset, autosave or clear).
   void saveOctomap(const std::string& filename) {
+    if (octomap_online_creation()) {  // graph_mgr_io.cpp:238-240: the map is already built
+      writeOctomap(filename);
+      return;
+    }
     std::vector<Node*> nodes;
     for (auto& kv : graph_)
       if (updateCloudOrigin(kv.second)) nodes.push_back(kv.second);
@@ -673,6 +718,15 @@ class GraphManager {
     estimates_[n->id_] = Pose7::Identity();
     adj_[n->id_];
     keyframe_ids_.push_back(n->id_);
+    if (octomap_online_creation()) optimizeGraph();  // :395-399
+  }
+
+  // the end of optimizeGraph (graph_manager.cpp:1044-1049) with octomap_online_creation: the newest node, graph_[size - 1],
+  // rendered when updateCloudOrigin passes
+  void renderNewestOnline() {
+    if (!octomap_online_creation()) return;
+    auto it = graph_.find((int)graph_.size() - 1);
+    if (it != graph_.end() && updateCloudOrigin(it->second)) renderToOctomap(it->second);
   }
 
   // ---- graph_manager.cpp:421-658

@@ -129,6 +129,9 @@ class Node {  // src/node.h: the members the hot path reads + matchNodePair
   double stamp_ = 0.0;           // header_.stamp in seconds
   bool matchable_ = true, valid_tf_estimate_ = true;  // node.h:160,178
   mutable int initial_node_matches_ = 0;              // node.h:207: accepted transformations of this node (max_connections)
+  // pc_col->sensor_orientation_ (qx qy qz qw) and sensor_origin_ (ox oy oz): PCL's default until GraphManager::updateCloudOrigin
+  // records the estimate (graph_mgr_io.cpp:232-233); occupancyFilterClouds applies it.  Mutable like the cloud header it is.
+  mutable float cloud_sensor_pose_[7] = {0, 0, 0, 1, 0, 0, 0};
   std::vector<KeyPoint> feature_locations_2d_;  // node.h:167
   std::vector<Vector4f> feature_locations_3d_;  // node.h:174
   std::vector<uint8_t> feature_descriptors_;    // N x 32 (cv::Mat CV_8U rows), node.h:169

@@ -61,6 +61,30 @@ int rgbdslam_b200_octomap_destroy(uint64_t map);
  * Features and keypoints stay.  A node without a cloud is left as it is. */
 int rgbdslam_b200_node_clear_cloud(uint64_t node_handle);
 
+/* ColorOctomapServer::occupancyFilter(pc_col, pc_col, occupancy_threshold) (ColorOctomapServer.cpp:132-185) for n nodes, in
+ * place: GraphManager::occupancyFilterClouds (graph_manager.cpp:1372-1381).  sensor7: per node qx qy qz qw ox oy oz, the
+ * cloud's sensor_orientation_ / sensor_origin_ (updateCloudOrigin; PCL's default is 0 0 0 1 0 0 0).  n_points may be NULL,
+ * else it receives each node's new point count.  The rule (DESIGN.md 4.15), for each point p of the cloud in storage order --
+ * p as node_download_cloud returns it:
+ *   1. in = q * p + t in float, q * p Eigen's _transformVector: uv = q.vec() x p; uv += uv; v = p + q.w() * uv + q.vec() x uv,
+ *      each component left to right without contraction, then + t.
+ *   2. in.z NaN: the point is dropped.
+ *   3. k = coordToKey(in.c) per axis, unchecked: (uint16)((int)floor((1 / res) * (double)c) + 32768), (int) as x86-64
+ *      converts (INT_MIN for NaN, +-inf and out of range).
+ *   4. a = k - 1 per axis: the reference's nested loops never reset y_a and z_a, so only the cells (ax, ay, az + d), d = 0, 1,
+ *      2, are visited, every key taken back to uint16 (-1 is 65535).
+ *   5. for each visited cell that is a leaf of the map: d. = keyToCoord(key.) - (double)in., w = (dx dx + dy dy) + dz dz,
+ *      occ = 1 - 1 / (1 + exp((double)lo)) as glibc computes it; sum_occ += occ / w, sum_w += w (double).
+ *   6. the point is kept iff sum_occ < threshold * sum_w: a point with no visited leaf (e.g. every point of an empty map) is
+ *      dropped.
+ * Kept points keep their records, in order.  A node that keeps every point keeps its cloud as it is (same raster, no copy);
+ * any other becomes an unorganised n x 1 cloud (0 x 1 when nothing is kept) that render_cloud, octomap_insert, reduce_clouds,
+ * icp_align and this call read, and that the measurement model refuses (ERR_STATE) for want of a raster.  How many nodes one
+ * call takes changes nothing.  ERR_ARG before any device work for a bad map or node handle, a node listed twice, a non-finite
+ * sensor7 entry or a NaN threshold; ERR_STATE for a node without a stored cloud.  A failed call changes no node. */
+int rgbdslam_b200_octomap_filter_clouds(uint64_t map, int n, const uint64_t* nodes, const float* sensor7, double occupancy_threshold,
+                                        int32_t* n_points);
+
 #ifdef __cplusplus
 }
 #endif

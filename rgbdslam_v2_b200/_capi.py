@@ -134,15 +134,11 @@ class OctomapParams(C.Structure):  # == rgbdslam_b200_octomap_params (include/rg
                 ("clamping_max", C.c_double)]
 
 
-def octomap_pose_steps(T) -> dict:
-    """The pose chain of saveOctomap step by step (see octomap_pose): q_eigen (x, y, z, w, float32) and eigen_branch of
-    Eigen's Quaternion(Matrix3f), M (the tf::Matrix3x3 of setRotation, float64), q_tf and tf_branch of its getRotation,
-    and T, the float 3 x 4.  A branch is -1 for the positive-trace formula, else the index of the diagonal entry used."""
-    f, d = np.float32, np.float64
-    T = np.asarray(T, d)
-    R = T[:3, :3].astype(f)
-    # Eigen's Quaternion(Matrix3f): trace as its unrolled reduction m00 + (m11 + m22), then the positive-trace or the
-    # largest-diagonal branch (strict >), in float
+def _eigen_quaternion(T):
+    """Eigen's Quaternion(Matrix3f) of T's rotation cast to float: (q (x, y, z, w) float32, branch) -- the trace as its unrolled
+    reduction m00 + (m11 + m22), then the positive-trace (branch -1) or the largest-diagonal branch (strict >), in float."""
+    f = np.float32
+    R = np.asarray(T, np.float64)[:3, :3].astype(f)
     tr = R[0, 0] + (R[1, 1] + R[2, 2])
     q = np.zeros(4, f)  # x, y, z, w
     if tr > f(0):
@@ -165,6 +161,23 @@ def octomap_pose_steps(T) -> dict:
         q[3] = (R[k, j] - R[j, k]) * t
         q[j] = (R[j, i] + R[i, j]) * t
         q[k] = (R[k, i] + R[i, k]) * t
+    return q, eb
+
+
+def cloud_sensor_pose(T) -> tuple[np.ndarray, np.ndarray]:
+    """What GraphManager::updateCloudOrigin stores in a node's cloud for a VertexSE3 estimate T (4 x 4 or 3 x 4, double):
+    sensor_orientation_, Eigen's Quaternionf of the rotation cast to float (x, y, z, w), and sensor_origin_, the translation
+    as float -- the sensor pose occupancyFilter applies (Frontend.octomap_filter_clouds), and the first step of octomap_pose."""
+    return _eigen_quaternion(T)[0], np.asarray(T, np.float64)[:3, 3].astype(np.float32)
+
+
+def octomap_pose_steps(T) -> dict:
+    """The pose chain of saveOctomap step by step (see octomap_pose): q_eigen (x, y, z, w, float32) and eigen_branch of
+    Eigen's Quaternion(Matrix3f), M (the tf::Matrix3x3 of setRotation, float64), q_tf and tf_branch of its getRotation,
+    and T, the float 3 x 4.  A branch is -1 for the positive-trace formula, else the index of the diagonal entry used."""
+    f, d = np.float32, np.float64
+    T = np.asarray(T, d)
+    q, eb = _eigen_quaternion(T)
     # tf::Matrix3x3::setRotation in double
     x, y, z, w = (d(v) for v in q)
     s = d(2.0) / (((x * x + y * y) + z * z) + w * w)
@@ -300,6 +313,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_octomap_clear.argtypes = [u64]
     lib.rgbdslam_b200_octomap_destroy.argtypes = [u64]
     lib.rgbdslam_b200_node_clear_cloud.argtypes = [u64]
+    lib.rgbdslam_b200_octomap_filter_clouds.argtypes = [u64, C.c_int, vp, vp, C.c_double, vp]
     lib.rgbdslam_b200_orb_debug_plane.argtypes = [C.c_int, C.c_int, C.c_int, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_orb_debug_candidates.argtypes = [C.c_int, vp, vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_node_create_from_sift.argtypes = [C.c_int32, vp, vp, C.c_int, C.POINTER(u64)]
@@ -796,6 +810,17 @@ class Frontend:
 
     def octomap_destroy(self, octomap: int):
         self._check(self.lib.rgbdslam_b200_octomap_destroy(C.c_uint64(octomap)))
+
+    def octomap_filter_clouds(self, octomap: int, nodes, sensor7, threshold: float = 0.9) -> np.ndarray:
+        """ColorOctomapServer::occupancyFilter of the nodes' stored clouds against the map, in place (occupancyFilterClouds).
+        sensor7: (n, 7) float32 per node qx qy qz qw ox oy oz -- cloud_sensor_pose of its estimate, or 0 0 0 1 0 0 0 for a
+        cloud updateCloudOrigin never saw; threshold is occupancy_filter_threshold.  Returns the new point counts."""
+        hs = np.ascontiguousarray(np.asarray(nodes, np.uint64).reshape(-1))
+        S = np.ascontiguousarray(np.asarray(sensor7, np.float32).reshape(len(hs), 7))
+        counts = np.zeros(len(hs), np.int32)
+        self._check(self.lib.rgbdslam_b200_octomap_filter_clouds(C.c_uint64(octomap), len(hs), _ptr(hs), _ptr(S), float(threshold),
+                                                                 _ptr(counts)))
+        return counts
 
     def node_clear_cloud(self, h: int):
         """Node::clearPointCloud: the node drops its stored cloud"""

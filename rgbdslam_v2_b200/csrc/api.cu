@@ -336,7 +336,8 @@ static int check_pairs(const std::vector<PairDesc>& h_pairs, int64_t first_pair,
     for (const PairDesc& pd : h_pairs)
       if (!pd.q_cloud.z || !pd.t_cloud.z) {
         set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth) that "
-                  "rgbdslam_b200_reduce_clouds has not voxel-filtered");
+                  "rgbdslam_b200_reduce_clouds has not voxel-filtered and rgbdslam_b200_octomap_filter_clouds has not left "
+                  "without a raster");
         return RGBDSLAM_B200_ERR_STATE;
       } else if (!pd.q_cloud.x != !pd.t_cloud.x) {
         // the reference never holds both kinds in one process (topic_points is global): there is no rule to restate
@@ -741,8 +742,9 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
               "or node_set_depth)");
     return RGBDSLAM_B200_ERR_STATE;
   }
-  if (a->pc.reduced || b->pc.reduced) {
-    set_error("observation_likelihood: a voxel-filtered cloud (rgbdslam_b200_reduce_clouds) has no raster for the measurement model");
+  if (a->pc.unorganised || b->pc.unorganised) {
+    set_error("observation_likelihood: a voxel-filtered (rgbdslam_b200_reduce_clouds) or occupancy-filtered "
+              "(rgbdslam_b200_octomap_filter_clouds) cloud has no raster for the measurement model");
     return RGBDSLAM_B200_ERR_STATE;
   }
   if (!a->pc.x != !b->pc.x) {

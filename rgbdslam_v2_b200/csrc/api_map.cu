@@ -55,12 +55,34 @@ MapNode map_node(const NodeDev* nd, const float* T) {
   m.cw = c.w;
   m.ch = c.h;
   m.step = c.step;
+  m.point0_one = c.point0_one ? 1 : 0;
   m.fxinv = (float)(1.0 / (double)c.K[0]);  // getCameraIntrinsicsInverseFocalLength (misc.cpp:64-69); unused by organised clouds
   m.fyinv = (float)(1.0 / (double)c.K[1]);
   m.cx = c.K[2];
   m.cy = c.K[3];
   if (T) memcpy(m.m, T, sizeof(m.m));
   return m;
+}
+
+void adopt_clouds(const std::vector<CloudResult>& results, const std::vector<NodeSlab*>& slabs) {
+  for (const CloudResult& r : results) {
+    release_slab(r.nd->pc.slab);
+    r.nd->pc = r.pc;
+    r.pc.slab->refs++;
+  }
+  for (NodeSlab* sl : slabs)
+    if (sl->refs == 0) {  // a chunk whose nodes all kept their clouds
+      cudaFree(sl->base);
+      delete sl;
+    }
+}
+
+void drop_slabs(const std::vector<NodeSlab*>& slabs) {
+  cudaStreamSynchronize(g_state.stream);
+  for (NodeSlab* sl : slabs) {
+    cudaFree(sl->base);
+    delete sl;
+  }
 }
 
 // Count, scan and (unless out is NULL) scatter the records of `nodes` into the host buffer out (capacity records).
@@ -145,16 +167,10 @@ struct VoxCtx {
   }
 };
 
-// A reduced cloud that is not yet its node's: the node takes it only when every chunk of the call has succeeded.
-struct VoxResult {
-  NodeDev* nd;
-  NodeCloud pc;
-};
-
-// Reduces nodes [k0, k1) of the call, whose clouds hold `points` points in all, into one new slab.  Appends a VoxResult per
+// Reduces nodes [k0, k1) of the call, whose clouds hold `points` points in all, into one new slab.  Appends a CloudResult per
 // reduced node and writes n_points[k] (-1: the leaf size is too small for node k, which keeps its cloud).
 static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1, long long points, float inv_leaf,
-                     std::vector<VoxResult>& results, std::vector<NodeSlab*>& slabs, int32_t* n_points) {
+                     std::vector<CloudResult>& results, std::vector<NodeSlab*>& slabs, int32_t* n_points) {
   MapCtx& m = g_map;
   State& s = g_state;
   cudaStream_t st = s.stream;
@@ -236,7 +252,7 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
       continue;
     }
     const long long first = offs[segs[k].blk0], count = offs[segs[k].blk0 + segs[k].nblk] - first;
-    VoxResult r{nds[k0 + k], nds[k0 + k]->pc};
+    CloudResult r{nds[k0 + k], nds[k0 + k]->pc};
     r.pc.x = (float*)slab->base + 4 * first;
     r.pc.y = r.pc.x + count;
     r.pc.z = r.pc.y + count;
@@ -245,7 +261,8 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
     r.pc.h = 1;
     r.pc.step = 0;
     r.pc.slab = slab;
-    r.pc.reduced = true;
+    r.pc.unorganised = true;
+    r.pc.point0_one = false;
     results.push_back(r);
     n_points[k0 + k] = (int32_t)count;
   }
@@ -439,7 +456,7 @@ int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter
   if (const char* env = std::getenv("RB200_VOX_CHUNK_POINTS")) limit = std::max(1ll, std::atoll(env));
   const float inv_leaf = 1.0f / leaf;
   std::vector<int32_t> counts(n);
-  std::vector<VoxResult> results;
+  std::vector<CloudResult> results;
   std::vector<NodeSlab*> slabs;
   VoxCtx v;
   int rc = 0;
@@ -453,23 +470,10 @@ int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter
   }
   v.release();
   if (rc) {  // no node is changed
-    cudaStreamSynchronize(g_state.stream);
-    for (NodeSlab* sl : slabs) {
-      cudaFree(sl->base);
-      delete sl;
-    }
+    drop_slabs(slabs);
     return rc;
   }
-  for (const VoxResult& r : results) {
-    release_slab(r.nd->pc.slab);
-    r.nd->pc = r.pc;
-    r.pc.slab->refs++;
-  }
-  for (NodeSlab* sl : slabs)
-    if (sl->refs == 0) {  // a chunk whose nodes all kept their clouds
-      cudaFree(sl->base);
-      delete sl;
-    }
+  adopt_clouds(results, slabs);
   if (n_points) std::copy(counts.begin(), counts.end(), n_points);
   return 0;
 }

@@ -2,12 +2,15 @@
 //   insert: count every node's entries once, then per batch of whole nodes (bounded by kOctBatchEntries) emit -> sort ->
 //           one update per (cell, scan) -> fold per cell -> merge the new leaves into the sorted leaf array
 //   write / stats: the inner levels from the leaves, bottom up; pre-order offsets top down; the records
+//   filter_clouds: the leaves' occupancy from the host's libm (cached until the map changes), then per chunk of whole nodes
+//           keep flags -> block scan -> the kept points of the nodes that lose some into one new slab
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/rgbdslam_b200/octomap.h"
@@ -18,6 +21,7 @@ namespace rb200 {
 
 constexpr long long kOctBatchEntries = 1ll << 26;  // sort entries per batch: about 1.6 GB of work buffers (24 bytes each)
 constexpr int kOctDepth = 16;
+constexpr long long kOcfChunkPoints = 1ll << 25;  // points one filter chunk flags and scatters: 1 byte of flags each
 
 struct OctoMap {
   static constexpr uint32_t kMagic = 0x4f43544du;  // 'OCTM'
@@ -28,6 +32,9 @@ struct OctoMap {
   int cur = 0;
   DevBuf lk[2], llo[2], lrgb[2];  // the leaves, sorted by Morton code: ping-pong for the merge
   DevBuf nodes, blocks, counts, pcount, offs, key[2], val[2], flags, scan, tsum, toffs, bits, starts, nk, nlo, nrgb, newk;
+  // the filter: per leaf its occupancy (valid while occ_ok; insert and clear reset it), and the work buffers
+  DevBuf occ, sensor, pflags, keep0, outs;
+  bool occ_ok = false;
   // the writer's levels 0..15 (level 16 is the leaves): key, lo, rgb, first, mask, size, off
   DevBuf lvl[kOctDepth + 1][7];
   void release() {
@@ -38,10 +45,12 @@ struct OctoMap {
       key[b].release();
       val[b].release();
     }
-    DevBuf* all[] = {&nodes, &blocks, &counts, &pcount, &offs, &flags, &scan, &tsum, &toffs, &bits, &starts, &nk, &nlo, &nrgb, &newk};
+    DevBuf* all[] = {&nodes, &blocks, &counts, &pcount, &offs, &flags, &scan, &tsum, &toffs, &bits, &starts, &nk, &nlo, &nrgb, &newk,
+                     &occ, &sensor, &pflags, &keep0, &outs};
     for (DevBuf* b : all) b->release();
     for (auto& l : lvl)
       for (DevBuf& b : l) b.release();
+    occ_ok = false;
   }
 };
 
@@ -193,6 +202,115 @@ static int oct_insert(OctoMap& m, const std::vector<MapNode>& table) {
   return 0;
 }
 
+// The occupancy of every leaf, OcTreeNode::getOccupancy = 1 - 1 / (1 + exp(lo)), computed here with the host's libm so that
+// the filter's decisions are glibc's (CUDA's double exp is only faithful to within 1 ulp).  Each distinct log-odds value is
+// evaluated once: the clamped float sums of a few increments take few values.
+static int oct_occupancy(OctoMap& m) {
+  if (m.occ_ok || m.nleaves == 0) return 0;
+  cudaStream_t st = g_state.stream;
+  const size_t n = (size_t)m.nleaves;
+  std::vector<uint32_t> lo(n);
+  RB200_CUDA(cudaMemcpyAsync(lo.data(), m.llo[m.cur].ptr, 4 * n, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  std::vector<double> occ(n);
+  std::unordered_map<uint32_t, double> seen;
+  for (size_t i = 0; i < n; i++) {
+    auto it = seen.find(lo[i]);
+    if (it == seen.end()) {
+      float l;
+      std::memcpy(&l, &lo[i], 4);
+      it = seen.emplace(lo[i], 1.0 - 1.0 / (1.0 + std::exp((double)l))).first;
+    }
+    occ[i] = it->second;
+  }
+  int rc;
+  if ((rc = m.occ.ensure(8 * n))) return rc;
+  RB200_CUDA(cudaMemcpyAsync(m.occ.ptr, occ.data(), 8 * n, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  m.occ_ok = true;
+  return 0;
+}
+
+// Filters nodes [k0, k1) of the call into one new slab.  Appends a CloudResult per node that loses
+// points and writes n_points[k].
+static int ocf_chunk(OctoMap& m, const std::vector<NodeDev*>& nds, const float* sensor7, int k0, int k1, const OcfArgs& a,
+                     std::vector<CloudResult>& results, std::vector<NodeSlab*>& slabs, int32_t* n_points) {
+  State& s = g_state;
+  cudaStream_t st = s.stream;
+  const int nn = k1 - k0;
+  std::vector<MapNode> nodes(nn);
+  std::vector<int2> blocks;
+  std::vector<int> blk0(nn + 1);
+  for (int k = 0; k < nn; k++) {
+    nodes[k] = map_node(nds[k0 + k], nullptr);
+    blk0[k] = (int)blocks.size();
+    const int P = nodes[k].cw * nodes[k].ch;
+    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2(k, f));
+  }
+  const int nb = (int)blocks.size();
+  blk0[nn] = nb;
+  int rc;
+  if ((rc = m.nodes.ensure(sizeof(MapNode) * nn)) || (rc = m.blocks.ensure(sizeof(int2) * std::max(nb, 1))) ||
+      (rc = m.counts.ensure(4 * (size_t)std::max(nb, 1))) || (rc = m.offs.ensure(8 * ((size_t)nb + 1))) ||
+      (rc = m.sensor.ensure(28 * (size_t)nn)) || (rc = m.pflags.ensure((size_t)kMapBlockPoints * std::max(nb, 1))) ||
+      (rc = m.keep0.ensure((size_t)nn)) || (rc = m.outs.ensure(sizeof(OcfOut) * nn)))
+    return rc;
+  RB200_CUDA(cudaMemcpyAsync(m.nodes.ptr, nodes.data(), sizeof(MapNode) * nn, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(m.sensor.ptr, sensor7 + 7 * (size_t)k0, 28 * (size_t)nn, cudaMemcpyHostToDevice, st));
+  if (nb > 0) RB200_CUDA(cudaMemcpyAsync(m.blocks.ptr, blocks.data(), sizeof(int2) * nb, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemsetAsync(m.keep0.ptr, 0, (size_t)nn, st));
+  RB200_CUDA(launch_ocf_flags((const MapNode*)m.nodes.ptr, (const int2*)m.blocks.ptr, nb, (const float*)m.sensor.ptr, a,
+                              (uint8_t*)m.pflags.ptr, (int*)m.counts.ptr, (uint8_t*)m.keep0.ptr, st));
+  RB200_CUDA(launch_map_scan((const int*)m.counts.ptr, nb, (long long*)m.offs.ptr, st));
+  std::vector<long long> offs(nb + 1);
+  std::vector<uint8_t> keep0(nn);
+  RB200_CUDA(cudaMemcpyAsync(offs.data(), m.offs.ptr, 8 * ((size_t)nb + 1), cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaMemcpyAsync(keep0.data(), m.keep0.ptr, (size_t)nn, cudaMemcpyDeviceToHost, st));
+  RB200_CUDA(cudaStreamSynchronize(st));
+  s.launches += (nb > 0) + 1;
+  // the nodes that lose points get their planes in the new slab, back to back; the others keep their clouds
+  std::vector<OcfOut> out(nn);
+  long long dst = 0;
+  for (int k = 0; k < nn; k++) {
+    const long long first = offs[blk0[k]], count = offs[blk0[k + 1]] - first;
+    const bool changed = count < (long long)nodes[k].cw * nodes[k].ch;
+    out[k] = OcfOut{changed ? dst : -1, first, count};
+    if (changed) dst += count;
+    n_points[k0 + k] = (int32_t)count;
+  }
+  if (std::none_of(out.begin(), out.end(), [](const OcfOut& o) { return o.dst >= 0; })) return 0;
+  NodeSlab* slab = new NodeSlab();
+  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max(dst, 1ll));
+  if (e != cudaSuccess) {
+    delete slab;
+    return cuda_fail(e, "cudaMalloc(occupancy-filtered clouds)");
+  }
+  slabs.push_back(slab);
+  RB200_CUDA(cudaMemcpyAsync(m.outs.ptr, out.data(), sizeof(OcfOut) * nn, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(launch_ocf_scatter((const MapNode*)m.nodes.ptr, (const int2*)m.blocks.ptr, nb, (const uint8_t*)m.pflags.ptr,
+                                (const long long*)m.offs.ptr, (const OcfOut*)m.outs.ptr, (float*)slab->base, st));
+  RB200_CUDA(cudaStreamSynchronize(st));  // the work buffers are the next chunk's
+  s.launches += nb > 0;
+  for (int k = 0; k < nn; k++) {
+    if (out[k].dst < 0) continue;
+    NodeDev* nd = nds[k0 + k];
+    CloudResult r{nd, nd->pc};
+    const long long c = out[k].count;
+    r.pc.x = (float*)slab->base + 4 * out[k].dst;
+    r.pc.y = r.pc.x + c;
+    r.pc.z = r.pc.y + c;
+    r.pc.rgb = (uint32_t*)(r.pc.z + c);
+    r.pc.w = (int32_t)c;
+    r.pc.h = 1;
+    r.pc.step = 0;
+    r.pc.slab = slab;
+    r.pc.unorganised = true;
+    r.pc.point0_one = (nd->pc.step > 0 || nd->pc.point0_one) && keep0[k];  // the kept point 0 stays point 0
+    results.push_back(r);
+  }
+  return 0;
+}
+
 // The levels of the tree in m.lvl (level 16: the leaves); returns the node count (0 for an empty map) through *count.
 static int oct_levels(OctoMap& m, OctLevel* lv, long long* count) {
   cudaStream_t st = g_state.stream;
@@ -306,7 +424,64 @@ int rgbdslam_b200_octomap_insert(uint64_t map, int n, const uint64_t* nodes, con
     table[k] = map_node(nd, transforms12 + (size_t)k * 12);
   }
   m->a.max_range = max_range;
+  m->occ_ok = false;
   return oct_insert(*m, table);
+}
+
+int rgbdslam_b200_octomap_filter_clouds(uint64_t map, int n, const uint64_t* nodes, const float* sensor7, double occupancy_threshold,
+                                        int32_t* n_points) {
+  RB200_ENTER_INITED();
+  OctoMap* m = get_octomap(map);
+  if (!m) return RGBDSLAM_B200_ERR_ARG;
+  if (n < 0 || (n > 0 && (!nodes || !sensor7)) || std::isnan(occupancy_threshold)) {
+    set_error("octomap_filter_clouds: n >= 0, non-null nodes and sensor poses and a threshold that is not NaN are needed");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  for (size_t i = 0; i < (size_t)n * 7; i++)
+    if (!std::isfinite(sensor7[i])) {
+      set_error("octomap_filter_clouds: sensor pose " + std::to_string(i / 7) + " has a non-finite entry");
+      return RGBDSLAM_B200_ERR_ARG;
+    }
+  std::vector<NodeDev*> nds(n);
+  for (int k = 0; k < n; k++) {
+    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
+    if (!nds[k]->pc.rgb) {
+      set_error("octomap_filter_clouds: node " + std::to_string(k) +
+                " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    }
+  }
+  std::vector<uint64_t> sorted(nodes, nodes + n);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
+    set_error("octomap_filter_clouds: a node is listed twice");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  if (n == 0) return 0;
+  int rc;
+  if ((rc = oct_occupancy(*m))) return rc;
+  const OcfArgs a{m->p.resolution, m->a.rf, occupancy_threshold, (const unsigned long long*)m->lk[m->cur].ptr, (const double*)m->occ.ptr,
+                  m->nleaves};
+  long long limit = kOcfChunkPoints;
+  if (const char* env = std::getenv("RB200_OCF_CHUNK_POINTS")) limit = std::max(1ll, std::atoll(env));
+  std::vector<int32_t> counts(n);
+  std::vector<CloudResult> results;
+  std::vector<NodeSlab*> slabs;
+  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
+    int k1 = k0;
+    long long points = 0;
+    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
+    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= limit);
+    rc = ocf_chunk(*m, nds, sensor7, k0, k1, a, results, slabs, counts.data());
+    k0 = k1;
+  }
+  if (rc) {  // no node is changed
+    drop_slabs(slabs);
+    return rc;
+  }
+  adopt_clouds(results, slabs);
+  if (n_points) std::copy(counts.begin(), counts.end(), n_points);
+  return 0;
 }
 
 int rgbdslam_b200_octomap_write(uint64_t map, void* out, int64_t capacity, int64_t* n_bytes) {

@@ -48,6 +48,7 @@ struct MapNode {
   const uint32_t* rgb;     // colour words
   int cw, ch;
   int step;                // > 0: depth-image node (x / y from pixel (rx * step, ry * step)); 0: x / y planes stored
+  int point0_one;          // x / y planes: point 0 came from a depth image, its data[3] is 1.0f
   float fxinv, fyinv, cx, cy;
   float m[12];             // row-major 3 x 4 float transform
 };

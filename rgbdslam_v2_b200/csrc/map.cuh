@@ -35,7 +35,7 @@ __device__ __forceinline__ bool map_point(const MapNode& nd, int i, const MapArg
     x = nd.x[i];
     y = nd.y[i];
     z = nd.z[i];
-    o.w16 = o.rgb;
+    o.w16 = i == 0 && nd.point0_one ? kOneF : o.rgb;
   }
   // squaredEuclideanDistance(p, origin) > max_Depth^2 (PCL: ((dx dx + dy dy) + dz dz), dx = 0 - x)
   if (a.filter && __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)) > a.maxd2) {

@@ -7,8 +7,11 @@
 //   k_oct_merge               the new leaves into the sorted leaf array
 //   k_oct_reduce / _offsets / _records
 //                             the writer: inner nodes level by level, pre-order record offsets top down, 8-byte records
+//   k_ocf_flags / _scatter    the occupancy filter of the stored clouds: per point its keep flag from three leaf lookups,
+//                             then the kept points of the changed nodes into new x / y / z / colour planes, in order
 // The float and double chains are written with explicit _rn intrinsics: octomap on x86-64 does not contract.
 #include <cfloat>
+#include <climits>
 
 #include "map.cuh"
 #include "octomap.cuh"
@@ -509,7 +512,138 @@ __global__ void k_oct_records(OctLevel l, uint2* __restrict__ out) {
                              (rgb >> 16) | (((rgb >> 8) & 0xff) << 8) | ((rgb & 0xff) << 16) | ((uint32_t)l.mask[i] << 24));
 }
 
+// ---- the occupancy filter --------------------------------------------------------------------------------------------------
+
+// coordToKey unchecked: (uint16)((int)floor(rf * c) + 32768), (int) as x86-64's cvttsd2si (INT_MIN for NaN, +-inf and out of
+// range)
+__device__ __forceinline__ uint32_t ocf_key(double rf, float c) {
+  const double v = floor(__dmul_rn(rf, (double)c));
+  const int k = v >= -2147483648.0 && v < 2147483648.0 ? (int)v : INT_MIN;
+  return ((uint32_t)k + 32768u) & 0xffffu;
+}
+
+// keyToCoord: (double((int)key - 32768) + 0.5) * res
+__device__ __forceinline__ double ocf_coord(double res, uint32_t k) { return __dmul_rn(__dadd_rn((double)((int)k - 32768), 0.5), res); }
+
+// ColorOctomapServer::occupancyFilter for one point p (as stored) under the sensor pose s (qx qy qz qw ox oy oz)
+__device__ __forceinline__ bool ocf_keep(const OcfArgs& a, const float* s, float px, float py, float pz) {
+  const float qx = s[0], qy = s[1], qz = s[2], qw = s[3];
+  // Eigen's _transformVector: uv = q.vec() x p; uv += uv; v = p + w uv + q.vec() x uv; then + t
+  float ux = __fsub_rn(__fmul_rn(qy, pz), __fmul_rn(qz, py));
+  float uy = __fsub_rn(__fmul_rn(qz, px), __fmul_rn(qx, pz));
+  float uz = __fsub_rn(__fmul_rn(qx, py), __fmul_rn(qy, px));
+  ux = __fadd_rn(ux, ux);
+  uy = __fadd_rn(uy, uy);
+  uz = __fadd_rn(uz, uz);
+  const float ix = __fadd_rn(__fadd_rn(__fadd_rn(px, __fmul_rn(qw, ux)), __fsub_rn(__fmul_rn(qy, uz), __fmul_rn(qz, uy))), s[4]);
+  const float iy = __fadd_rn(__fadd_rn(__fadd_rn(py, __fmul_rn(qw, uy)), __fsub_rn(__fmul_rn(qz, ux), __fmul_rn(qx, uz))), s[5]);
+  const float iz = __fadd_rn(__fadd_rn(__fadd_rn(pz, __fmul_rn(qw, uz)), __fsub_rn(__fmul_rn(qx, uy), __fmul_rn(qy, ux))), s[6]);
+  if (isnan(iz)) return false;
+  // the reference's nested loops never reset y_a / z_a: only (kx - 1, ky - 1, kz - 1 + d), d = 0, 1, 2, are visited
+  const uint32_t k[3] = {(ocf_key(a.rf, ix) + 0xffffu) & 0xffffu, (ocf_key(a.rf, iy) + 0xffffu) & 0xffffu,
+                         (ocf_key(a.rf, iz) + 0xffffu) & 0xffffu};
+  const double dx = __dsub_rn(ocf_coord(a.res, k[0]), (double)ix);
+  const double dy = __dsub_rn(ocf_coord(a.res, k[1]), (double)iy);
+  const double dxy = __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy));
+  double so = 0.0, sw = 0.0;
+#pragma unroll 1
+  for (int d = 0; d < 3; d++) {
+    const uint32_t c[3] = {k[0], k[1], (k[2] + d) & 0xffffu};
+    const unsigned long long key = oct_morton(c);
+    const long long idx = oct_lower_bound(a.lk, a.nleaves, key);
+    if (idx < a.nleaves && a.lk[idx] == key) {
+      const double dz = __dsub_rn(ocf_coord(a.res, c[2]), (double)iz);
+      const double w = __dadd_rn(dxy, __dmul_rn(dz, dz));
+      so = __dadd_rn(so, __ddiv_rn(a.occ[idx], w));
+      sw = __dadd_rn(sw, w);
+    }
+  }
+  return so < __dmul_rn(a.threshold, sw);
+}
+
+__global__ void __launch_bounds__(kOctThreads) k_ocf_flags(const MapNode* __restrict__ nodes, const int2* __restrict__ blocks,
+                                                           const float* __restrict__ sensor7, OcfArgs a, uint8_t* __restrict__ flags,
+                                                           int* __restrict__ counts, uint8_t* __restrict__ keep0) {
+  __shared__ int warp_sum[kOctThreads / 32];
+  const int2 blk = blocks[blockIdx.x];
+  const MapNode& nd = nodes[blk.x];
+  const float* s = sensor7 + 7 * (size_t)blk.x;
+  const int P = nd.cw * nd.ch;
+  const MapArgs ma{0.f, 0, 1, 0, 32};  // every point, as stored
+  int c = 0;
+#pragma unroll 1
+  for (int r = 0; r < kMapBlockPoints / kOctThreads; r++) {
+    const int i = blk.y + r * kOctThreads + threadIdx.x;
+    bool keep = false;
+    if (i < P) {
+      MapOut p;
+      map_point(nd, i, ma, p);
+      keep = ocf_keep(a, s, p.x, p.y, p.z);
+    }
+    flags[(size_t)blockIdx.x * kMapBlockPoints + r * kOctThreads + threadIdx.x] = keep;
+    if (i == 0) keep0[blk.x] = keep;
+    c += keep;
+  }
+  const int t = oct_block_sum(c, warp_sum);
+  if (threadIdx.x == 0) counts[blockIdx.x] = t;
+}
+
+__global__ void __launch_bounds__(kOctThreads) k_ocf_scatter(const MapNode* __restrict__ nodes, const int2* __restrict__ blocks,
+                                                             const uint8_t* __restrict__ flags, const long long* __restrict__ offs,
+                                                             const OcfOut* __restrict__ out, float* __restrict__ slab) {
+  __shared__ int warp_cnt[kOctThreads / 32];
+  const int2 blk = blocks[blockIdx.x];
+  const OcfOut o = out[blk.x];
+  if (o.dst < 0) return;  // the whole CTA: the node keeps its cloud
+  const MapNode& nd = nodes[blk.x];
+  const int P = nd.cw * nd.ch;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  float* x = slab + 4 * o.dst;
+  long long next = offs[blockIdx.x] - o.first;
+  const MapArgs ma{0.f, 0, 1, 0, 32};
+#pragma unroll 1
+  for (int r = 0; r < kMapBlockPoints / kOctThreads; r++) {
+    const int i = blk.y + r * kOctThreads + threadIdx.x;
+    const bool keep = i < P && flags[(size_t)blockIdx.x * kMapBlockPoints + r * kOctThreads + threadIdx.x];
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) warp_cnt[wid] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kOctThreads / 32; w++) {
+      const int c = warp_cnt[w];
+      before += w < wid ? c : 0;
+      total += c;
+    }
+    if (keep) {
+      MapOut p;
+      map_point(nd, i, ma, p);
+      const long long j = next + before + __popc(bal & ((1u << lane) - 1u));
+      x[j] = p.x;
+      x[o.count + j] = p.y;
+      x[2 * o.count + j] = p.z;
+      reinterpret_cast<uint32_t*>(x)[3 * o.count + j] = p.rgb;
+    }
+    next += total;
+    __syncthreads();
+  }
+}
+
 // ---- launchers -------------------------------------------------------------------------------------------------------------
+
+cudaError_t launch_ocf_flags(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const float* d_sensor7, const OcfArgs& a,
+                             uint8_t* d_flags, int* d_counts, uint8_t* d_keep0, cudaStream_t st) {
+  if (nblocks <= 0) return cudaSuccess;
+  k_ocf_flags<<<nblocks, kOctThreads, 0, st>>>(d_nodes, d_blocks, d_sensor7, a, d_flags, d_counts, d_keep0);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_ocf_scatter(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const uint8_t* d_flags, const long long* d_offs,
+                               const OcfOut* d_out, float* slab, cudaStream_t st) {
+  if (nblocks <= 0) return cudaSuccess;
+  k_ocf_scatter<<<nblocks, kOctThreads, 0, st>>>(d_nodes, d_blocks, d_flags, d_offs, d_out, slab);
+  return cudaGetLastError();
+}
 
 static inline unsigned grid_of(long long n) { return (unsigned)std::max<long long>(1, (n + kOctThreads - 1) / kOctThreads); }
 

@@ -74,4 +74,26 @@ cudaError_t launch_oct_offsets(OctLevel p, OctLevel c, cudaStream_t st);
 cudaError_t launch_oct_records(OctLevel l, uint8_t* out, cudaStream_t st);
 cudaError_t launch_oct_leaf_level(OctLevel l, cudaStream_t st);  // size 1, mask 0
 
+// ---- the occupancy filter (ColorOctomapServer::occupancyFilter, DESIGN.md 4.15) --------------------------------------------
+struct OcfArgs {
+  double res, rf;      // resolution and 1 / resolution
+  double threshold;    // occupancy_filter_threshold
+  const unsigned long long* lk;  // the map's leaves (Morton keys, sorted) and their occupancy 1 - 1 / (1 + exp(lo)), libm's
+  const double* occ;
+  long long nleaves;
+};
+// Where the kept points of one node of the chunk go: its planes at slab point dst (dst < 0: the node keeps its cloud), the
+// first of its offsets (map scan of the block counts) and its kept count.
+struct OcfOut {
+  long long dst, first;
+  long long count;
+};
+// The keep flag of every point of the blocks (node, first point), flags[block * 1024 + point - first point]; per block the
+// kept count; keep0[node] = the flag of the node's point 0.  sensor7: per node qx qy qz qw ox oy oz.
+cudaError_t launch_ocf_flags(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const float* d_sensor7, const OcfArgs& a,
+                             uint8_t* d_flags, int* d_counts, uint8_t* d_keep0, cudaStream_t st);
+// The kept points of the blocks, as stored, into the x / y / z / colour planes of their node at slab + 4 * out[node].dst floats.
+cudaError_t launch_ocf_scatter(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const uint8_t* d_flags, const long long* d_offs,
+                               const OcfOut* d_out, float* slab, cudaStream_t st);
+
 }  // namespace rb200
