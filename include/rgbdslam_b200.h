@@ -293,7 +293,9 @@ int rgbdslam_b200_detector_thresholds(uint64_t detector, double* thresholds16, i
  * cv::FastFeatureDetector::create(int(thresh)) (FAST-9/16 with non-max suppression, :88-91) for a FAST detector: integer
  * positions in [3, n-4] of each cell, size 7, angle -1, octave 0, response = corner score.  gray/mask: w*h bytes (mask may
  * be NULL).  Output order: cell-major, |response| descending inside a cell, ties by (octave, y, x) (the reference's
- * nth_element order is unspecified).  *n_out = number found; at most `capacity` are written. */
+ * nth_element order is unspecified).  *n_out = number found; at most `capacity` are written.  The detector is the one the
+ * parameters name (see rgbdslam_b200_nodes_create); at most 4096 keypoints per call: a whole-frame detector (grid <= 1 or
+ * adjuster_max_iterations <= 0) that returns more fails with ERR_STATE.  The Node constructor has no such limit. */
 int rgbdslam_b200_orb_detect(uint64_t detector, const uint8_t* gray, const uint8_t* mask, int w, int h,
                              rgbdslam_b200_keypoint* kp_out, int capacity, int* n_out);
 
@@ -313,10 +315,14 @@ int rgbdslam_b200_orb_compute(const uint8_t* gray, int w, int h, const rgbdslam_
  * Frame size limits (every entry point that takes w and h, every input kind of _ex and _sharded; ERR_ARG before any device
  * work): 96 <= w, h <= 4095, and each grid cell at least 40 px per side at pyramid level 7, so the smallest side that builds
  * is 142 px without a grid, 222 with detector_grid_resolution 2, 333 with 3 (the default), 444 with 4.  Above 1023 px in
- * either dimension the detector needs detector_grid_resolution >= 2 and round(1.5 * max_keypoints / cells) < 606 (the
- * smallest per-level quota of the reference's cv::ORB, whose quotas are applied there: every 3x3 setting qualifies, 2x2 up to
- * max_keypoints 1614).  A grid cell holds at most 12288 FAST candidates up to 1023 px, proportionally more above
- * (ERR_STATE when exceeded). */
+ * either dimension the detector needs detector_grid_resolution >= 2, adjuster_max_iterations > 0 and
+ * round(1.5 * max_keypoints / cells) < 606 (the smallest per-level quota of the reference's cv::ORB: every 3x3 setting
+ * qualifies, 2x2 up to max_keypoints 1614).  The detector is createDetector's (features.cpp:101-112): the grid adjuster
+ * (grid > 1, iterations > 0), the whole-frame adjuster (grid <= 1, iterations > 0, no keepStrongest) or, with
+ * adjuster_max_iterations <= 0, one whole-frame detection at the handle's cell-0 threshold, which never changes.  The ORB
+ * detector applies cv::ORB's per-level quotas everywhere, in the adjuster's counts too.  A grid cell holds at most 12288 FAST
+ * candidates up to 1023 px and a cell above 1023 px proportionally more (ERR_STATE when exceeded); a whole-frame cell, or
+ * one whose maximum reaches 606, holds every FAST / NMS maximum its pixels can have. */
 int rgbdslam_b200_nodes_create(uint64_t detector, int nframes, const uint8_t* gray, const float* depth, const uint8_t* mask,
                                int w, int h, const float* K4, const int32_t* ids, uint64_t* node_handles, int32_t* n_features);
 /* The same with options.  RGBDSLAM_B200_MASK_FROM_DEPTH: the detection mask is what the caller of the reference's constructor

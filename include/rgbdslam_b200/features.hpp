@@ -119,7 +119,9 @@ using Ptr = std::shared_ptr<T>;  // cv::Ptr
 
 // features.cpp:63-113.  The grid / dynamic wrappers are part of the detector here (detector_grid_resolution,
 // adjuster_max_iterations and max_keypoints are read from the library's parameters like the reference reads its
-// ParameterServer).  "ORB" and "FAST" need the library's feature_detector_type to name the same detector.  "SIFTGPU"
+// ParameterServer): the grid adjuster, the whole-frame adjuster (detector_grid_resolution <= 1) or, with
+// adjuster_max_iterations <= 0, the bare DetectorAdjuster on the whole frame at a fixed threshold, as the reference
+// chooses.  "ORB" and "FAST" need the library's feature_detector_type to name the same detector.  "SIFTGPU"
 // returns NULL like the reference (:69-71).
 inline Feature2D* createDetector(const std::string& detectorType) {
   if (detectorType == "SIFTGPU") return nullptr;

@@ -52,7 +52,8 @@ struct OrbCtx {
   int max_per_cell = 0, min_cell = 0, max_cell = 0, kp_stride = 0;
   int cand_cap = kOrbCandCap;  // FAST / NMS candidates per (frame, cell): orb_prepare
   bool wide = false;           // wider or taller than kOrbNarrowMax px
-  bool quotas = false;         // the ORB detector applies cv::ORB's per-level quotas: orb_prepare
+  bool regular = false;        // adjuster_max_iterations <= 0: the bare DetectorAdjuster (one whole-frame cell, fixed threshold)
+  bool quota_table = false;    // the ORB adjuster counts through orb_run_quota_counts: a cell's maximum reaches cv::ORB's smallest quota
   DevBuf in_gray[2], in_mask[2], in_depth[2];  // double-buffered chunk inputs (upload of chunk k+1 under the kernels of chunk k)
   DevBuf in_rgb[2];                            // colour or Bayer input, converted into in_gray on the device
   DevBuf in_raw[2];  // depth as the caller passes it when it is not the w x h float plane (16-bit millimetres, or another size),
@@ -67,6 +68,7 @@ struct OrbCtx {
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
   DevBuf cell_img, cell_mask, cand, cand_count, hist, mask_any, thr, resp, cell_out, cell_out_count, cand_z, scratch, kp, xyz, n,
       pyr_raw, pyr_blur, desc, err, trig;
+  DevBuf all_keys, all_count, all_z;  // whole-frame detectors: the survivors of every frame before k_frame_precap (OrbSurvivors)
   // rgbdslam_b200_nodes_create_sharded: what must survive between the detection pass and the finishing pass of ALL own frames,
   // and the per-(frame, cell) tables every rank holds for ALL frames of the sequence
   DevBuf sh_gray, sh_rgb, sh_raw, sh_depth, sh_mask, sh_cell_img, sh_cand, all_hist, all_cnt, all_many, all_thr;
@@ -78,7 +80,8 @@ struct OrbCtx {
     DevBuf* all[] = {&d_ofs, &d_w1, &in_gray[0], &in_gray[1], &in_mask[0], &in_mask[1], &in_depth[0], &in_depth[1], &in_rgb[0],
                      &in_rgb[1], &in_raw[0], &in_raw[1], &cell_img, &cell_mask, &cand, &cand_count, &hist, &mask_any, &thr, &resp,
                      &cell_out, &cell_out_count, &cand_z, &scratch, &kp, &xyz, &n, &pyr_raw, &pyr_blur, &desc, &err, &trig, &sh_gray,
-                     &sh_rgb, &sh_raw, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr, &d_nn};
+                     &sh_rgb, &sh_raw, &sh_depth, &sh_mask, &sh_cell_img, &sh_cand, &all_hist, &all_cnt, &all_many, &all_thr, &d_nn,
+                     &all_keys, &all_count, &all_z};
     for (DevBuf* b : all) b->release();
     nn_w = nn_h = nn_dw = nn_dh = 0;
     stage[0].release();
@@ -113,9 +116,11 @@ static void build_table(int src_n, int dst_n, std::vector<int16_t>& ofs, std::ve
 static int orb_prepare(int W, int H) {
   State& s = g_state;
   OrbCtx& o = g_orb;
-  const int grid = s.params.detector_grid_resolution > 1 ? s.params.detector_grid_resolution : 1;
+  // createDetector (features.cpp:101-112): without adaptation the bare DetectorAdjuster runs on the whole frame, grid or not
+  const bool regular = s.params.adjuster_max_iterations <= 0;
+  const int grid = !regular && s.params.detector_grid_resolution > 1 ? s.params.detector_grid_resolution : 1;
   const int K = s.params.max_keypoints;
-  if (o.ready && o.W == W && o.H == H && o.grid == grid && o.max_kp == K) return 0;
+  if (o.ready && o.W == W && o.H == H && o.grid == grid && o.max_kp == K && o.regular == regular) return 0;
   if (grid * grid > kOrbMaxCells) {
     set_error("detector_grid_resolution > 4 is not supported");
     return RGBDSLAM_B200_ERR_ARG;
@@ -131,7 +136,7 @@ static int orb_prepare(int W, int H) {
     // "too many" with or without it and k_adapt_thresholds needs no quotas (DESIGN.md 4.5.5)
     const int cells = grid * grid, max_cell = (int)std::lround((int)(K * 1.5) / (float)cells);
     if (grid < 2) {
-      set_error("frames above 1023 px per side need detector_grid_resolution >= 2");
+      set_error("frames above 1023 px per side need detector_grid_resolution >= 2 and adjuster_max_iterations > 0");
       return RGBDSLAM_B200_ERR_ARG;
     }
     if (max_cell >= 606) {
@@ -195,13 +200,29 @@ static int orb_prepare(int W, int H) {
       }
     }
   g.cell_bytes = off;
+  // adjustedGridWrapper's per-cell maximum (features.cpp:52-53); adjusterWrapper's is 1.5 K (features.cpp:101-112)
+  const int mx = (int)(K * 1.5), max_cell = grid > 1 ? (int)std::lround(mx / (float)g.ncells) : mx;
   // the candidate buffer: kOrbCandCap per cell up to kOrbNarrowMax px; above, the same density per level-0 pixel of the largest
-  // cell as kOrbCandCap in the largest cell of a 640x480 frame's 3x3 grid (275 x 222 px), in multiples of 256
+  // cell as kOrbCandCap in the largest cell of a 640x480 frame's 3x3 grid (275 x 222 px), in multiples of 256.  A whole-frame
+  // cell or one whose maximum reaches cv::ORB's smallest quota (606), up to kOrbNarrowMax px, holds every candidate its pixels
+  // can have: a strict 3x3 maximum has no maximum among its 8 neighbours, so each 2x2 block of a level's scored pixels holds at
+  // most one (the larger of the ORB detector's 8 levels inside the 15 px border and the FAST detector's level 0 inside 3 px).
   o.cand_cap = kOrbCandCap;
   if (wide) {
     size_t area = 0;
     for (int c = 0; c < g.ncells; c++) area = std::max(area, (size_t)g.cell[c][0].w * g.cell[c][0].h);
     const size_t cap = (area * kOrbCandCap + 275 * 222 - 1) / (275 * 222);
+    o.cand_cap = (int)std::max<size_t>(kOrbCandCap, (cap + 255) / 256 * 256);
+  } else if (grid == 1 || max_cell >= 606) {
+    auto blocks = [](int w, int h, int edge) -> size_t {
+      return w > 2 * edge && h > 2 * edge ? (size_t)((w - 2 * edge + 1) / 2) * ((h - 2 * edge + 1) / 2) : 0;
+    };
+    size_t cap = 0;
+    for (int c = 0; c < g.ncells; c++) {
+      size_t orb = 0;
+      for (int l = 0; l < kOrbLevels; l++) orb += blocks(g.cell[c][l].w, g.cell[c][l].h, 15);
+      cap = std::max({cap, orb, blocks(g.cell[c][0].w, g.cell[c][0].h, 3)});
+    }
     o.cand_cap = (int)std::max<size_t>(kOrbCandCap, (cap + 255) / 256 * 256);
   }
   o.wide = wide;
@@ -244,7 +265,7 @@ static int orb_prepare(int W, int H) {
     }
   }
   // adjustedGridWrapper (features.cpp:43-60)
-  const int mn = K, mx = (int)(K * 1.5);
+  const int mn = K;
   if (grid > 1) {
     o.min_cell = (int)std::lround(mn / (float)g.ncells);
     o.max_cell = (int)std::lround(mx / (float)g.ncells);
@@ -252,18 +273,18 @@ static int orb_prepare(int W, int H) {
   } else {
     o.min_cell = mn;
     o.max_cell = mx;
-    o.max_per_cell = kOrbFrameCap;  // no keepStrongest without the grid wrapper
+    o.max_per_cell = kOrbFrameCap;  // no keepStrongest without the grid wrapper: k_frame_precap's output
   }
   if (o.max_per_cell * g.ncells > kOrbFrameCap && grid > 1) {
     set_error("max_keypoints too large for the per-frame staging buffer (1.5 * max_keypoints <= 4096)");
     return RGBDSLAM_B200_ERR_ARG;
   }
   o.kp_stride = std::min(kOrbFrameCap, o.max_per_cell * g.ncells);
-  // cv::ORB's per-level quotas where a binding one leaves more keypoints than the cell's maximum (smallest quota 606), so that
-  // the adjuster's "too many" stands with or without them and k_adapt_thresholds stays exact.  At or above 606 per cell (the
-  // ungridded detector, 2x2 above K = 1614; only frames of up to kOrbNarrowMax px get here) a binding quota can change the
-  // adjuster's count, and the quotas are not applied (DESIGN.md 4.5.5).
-  o.quotas = grid > 1 && o.max_cell < 606;
+  // Below 606 per cell a binding quota leaves more keypoints than the cell's maximum, so the adjuster's "too many" stands with
+  // or without it and the score histogram decides.  At or above 606 (the ungridded adjuster, 2x2 above K = 1614; only frames
+  // of up to kOrbNarrowMax px get here) the ORB adjuster counts what cv::ORB returns, quotas included (DESIGN.md 4.5.7).
+  o.quota_table = !regular && o.max_cell >= 606;
+  o.regular = regular;
   o.W = W; o.H = H; o.grid = grid; o.max_kp = K;
   int rc;
   if ((rc = o.d_ofs.ensure(o.h_ofs.size() * 2 + 16)) || (rc = o.d_w1.ensure(o.h_w1.size() * 2 + 16))) return rc;
@@ -401,7 +422,17 @@ static int orb_ensure_buffers(int F, int nbuf, bool want_mask, size_t depth_byte
       (rc = o.desc.ensure((size_t)F * o.kp_stride * 32)) || (rc = o.err.ensure(16)) ||
       (rc = o.trig.ensure((size_t)F * o.kp_stride * 8)))
     return rc;
+  if (g.ncells == 1 && ((rc = o.all_keys.ensure((size_t)F * o.cand_cap * 8)) || (rc = o.all_count.ensure((size_t)F * 4)) ||
+                        (rc = o.all_z.ensure((size_t)F * o.cand_cap * 4))))
+    return rc;
   return 0;
+}
+
+// how the thresholds of a call come about (orb_run_adapt)
+static OrbThresholds threshold_mode(const Detector* det) {
+  const OrbCtx& o = g_orb;
+  if (o.regular) return OrbThresholds::kFixed;
+  return o.quota_table && det->type == RGBDSLAM_B200_DETECTOR_ORB ? OrbThresholds::kQuotaTable : OrbThresholds::kHistogram;
 }
 
 static Detector* get_detector(uint64_t h) {
@@ -446,9 +477,15 @@ static int orb_detect_stage(Detector* det, int F, const uint8_t* d_gray, const u
                                  (OrbCand*)o.cand.ptr, (int*)o.cand_count.ptr, (int*)o.hist.ptr,
                                  (int*)o.mask_any.ptr, o.cand_cap, st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb detect kernels");
+  const OrbThresholds mode = threshold_mode(det);
+  if (mode == OrbThresholds::kQuotaTable) {  // the tables take the histograms' place
+    e = orb_run_quota_counts(g, F, (const uint8_t*)o.cell_img.ptr, (const OrbCand*)o.cand.ptr, (const int*)o.cand_count.ptr,
+                             (int*)o.thr.ptr, (float*)o.resp.ptr, o.cand_cap, (int*)o.hist.ptr, st, launches);
+    if (e != cudaSuccess) return cuda_fail(e, "orb quota count kernels");
+  }
   e = orb_run_adapt(g, F, (const int*)o.hist.ptr, (const int*)o.cand_count.ptr, (const int*)o.mask_any.ptr, (double*)det->d_state.ptr,
-                    (int*)o.thr.ptr, o.min_cell, o.max_cell, s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, st,
-                    launches);
+                    (int*)o.thr.ptr, o.min_cell, o.max_cell, s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, mode,
+                    st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb threshold kernel");
   det->host_valid = false;
   return 0;
@@ -457,6 +494,10 @@ static int orb_detect_stage(Detector* det, int F, const uint8_t* d_gray, const u
 static int orb_check_err_flag(int flag) {
   if (flag & 1) {
     set_error("ORB / FAST candidate buffer overflow (more than " + std::to_string(g_orb.cand_cap) + " FAST corners in one grid cell)");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
+  if (flag & 2) {
+    set_error("orb_detect: the whole-frame detector returned more than " + std::to_string(kOrbFrameCap) + " keypoints");
     return RGBDSLAM_B200_ERR_STATE;
   }
   return 0;
@@ -642,7 +683,8 @@ static int select_describe(const Detector* det, const FrameInput& in, int F, con
   a.kp_stride = out.stride;
   a.max_keypoints = g_state.params.max_keypoints;
   a.mode = in.mode;
-  cudaError_t e = orb_run_select(o.g, F, det->type, o.quotas, in.points, c, a, st, launches);
+  const OrbSurvivors all = {(unsigned long long*)o.all_keys.ptr, (int*)o.all_count.ptr, (float*)o.all_z.ptr, o.cand_cap};
+  cudaError_t e = orb_run_select(o.g, F, det->type, in.points, c, a, o.g.ncells == 1 ? &all : nullptr, (int*)o.err.ptr, st, launches);
   if (e != cudaSuccess) return cuda_fail(e, "orb select kernels");
   if (in.mode == 1) {
     e = orb_run_describe(o.g, o.tab, F, det->describe_levels(), dg, (uint8_t*)o.pyr_raw.ptr, (uint8_t*)o.pyr_blur.ptr, out.kp, out.n,
@@ -1039,6 +1081,7 @@ static int nodes_create_sharded_run(const char* what, uint64_t detector, uint64_
   if (e == cudaSuccess) e = cudaStreamWaitEvent(cs, o.ev_free[0], 0);
   if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "nodes_create_sharded setup"));
   int launches = 0, ci = 0;
+  const OrbThresholds mode = threshold_mode(det);
   // ---- pass A: upload + pyramids + FAST / NMS candidates + score histograms of the own frames
   for (int c0 = 0; c0 < own; c0 += chunk, ci++) {
     const int F = std::min(chunk, own - c0);
@@ -1059,6 +1102,12 @@ static int nodes_create_sharded_run(const char* what, uint64_t detector, uint64_
                        (uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0, (uint8_t*)o.cell_mask.ptr, (OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * o.cand_cap,
                        cnt_all + gf * nc, hist_all + gf * nc * 256, many_all + gf * nc, o.cand_cap, st, &launches);
     if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb detect kernels"));
+    if (mode == OrbThresholds::kQuotaTable) {  // the tables take the histograms' place
+      e = orb_run_quota_counts(g, F, (const uint8_t*)o.sh_cell_img.ptr + (size_t)g.cell_bytes * c0,
+                               (const OrbCand*)o.sh_cand.ptr + (size_t)c0 * nc * o.cand_cap, cnt_all + gf * nc, (int*)o.thr.ptr,
+                               (float*)o.resp.ptr, o.cand_cap, hist_all + gf * nc * 256, st, &launches);
+      if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb quota count kernels"));
+    }
   }
   // ---- the exchange that makes the frames independent: every rank gets every frame's score histograms, replays the
   //      threshold recurrence of the whole sequence (feature_adjuster.cpp:131-150, 185-224) and keeps its own frames' thresholds
@@ -1070,7 +1119,7 @@ static int nodes_create_sharded_run(const char* what, uint64_t detector, uint64_
   }
   if ((rc = detector_to_device(det, st))) return batch_fail(nb, rc);
   e = orb_run_adapt(g, total_frames, hist_all, cnt_all, many_all, (double*)det->d_state.ptr, thr_all, o.min_cell, o.max_cell,
-                    s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, st, &launches);
+                    s.params.adjuster_max_iterations, (int*)o.err.ptr, o.cand_cap, mode, st, &launches);
   if (e != cudaSuccess) return batch_fail(nb, cuda_fail(e, "orb threshold kernel"));
   det->host_valid = false;
   // ---- pass B: Harris / keepStrongest / finalize / describe of the own frames, straight into the slab

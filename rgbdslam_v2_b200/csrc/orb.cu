@@ -423,6 +423,9 @@ __global__ void __launch_bounds__(256) k_resize_cells(uint8_t* __restrict__ cell
 // One warp per grid cell; lane l owns score bins [8l, 8l+8).  state[c] = the detector's persistent threshold (double, as in
 // the reference); thr_out[f * ncells + c] = the integer FAST threshold of the LAST detection call of that frame.
 // err_flag bit 0: a cell overflowed the candidate buffer (cap candidates per cell).
+// kTable: hist holds, per (frame, cell), the count cv::ORB's detect returns at each threshold t = 0..255 (k_quota_counts) in
+// place of the score histogram.
+template <bool kTable>
 __device__ __forceinline__ void adapt_thresholds(const int* __restrict__ hist, const int* __restrict__ cand_count,
                                                  const int* __restrict__ mask_any, double* __restrict__ state,
                                                  int* __restrict__ thr_out, int nframes, int ncells, int min_features,
@@ -433,7 +436,7 @@ __device__ __forceinline__ void adapt_thresholds(const int* __restrict__ hist, c
   for (int f = 0; f < nframes; f++) {
     const int fc = f * ncells + c;
     int h[8];
-    {
+    if constexpr (!kTable) {
       const int4 a = reinterpret_cast<const int4*>(hist + (size_t)fc * 256)[lane * 2];
       const int4 b = reinterpret_cast<const int4*>(hist + (size_t)fc * 256)[lane * 2 + 1];
       h[0] = a.x; h[1] = a.y; h[2] = a.z; h[3] = a.w; h[4] = b.x; h[5] = b.y; h[6] = b.z; h[7] = b.w;
@@ -447,10 +450,14 @@ __device__ __forceinline__ void adapt_thresholds(const int* __restrict__ hist, c
       const int t = (int)thresh;  // static_cast<int>(thresh_) feature_adjuster.cpp:94
       used = t;
       int part = 0;
+      if constexpr (kTable) {
+        part = t < 256 ? hist[(size_t)fc * 256 + t] : 0;
+      } else {
 #pragma unroll
-      for (int k = 0; k < 8; k++) part += (lane * 8 + k >= t) ? h[k] : 0;
+        for (int k = 0; k < 8; k++) part += (lane * 8 + k >= t) ? h[k] : 0;
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+        for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+      }
       const int found = part;  // t > 255 -> 0
       if (found < min_features) {
         thresh = __dmul_rn(thresh, 0.7);  // tooFew
@@ -477,8 +484,31 @@ __global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds(const in
                                                                          int* __restrict__ thr_out, int nframes, int ncells,
                                                                          int min_features, int max_features, int max_iters,
                                                                          int* __restrict__ err_flag) {
-  adapt_thresholds(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters, err_flag,
-                   kOrbCandCap);
+  adapt_thresholds<false>(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters,
+                          err_flag, kOrbCandCap);
+}
+
+// The same recurrence on k_quota_counts' tables: ORB geometries whose per-cell maximum reaches cv::ORB's smallest quota.
+__global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds_quota(const int* __restrict__ table,
+                                                                               const int* __restrict__ cand_count,
+                                                                               const int* __restrict__ mask_any,
+                                                                               double* __restrict__ state, int* __restrict__ thr_out,
+                                                                               int nframes, int ncells, int min_features,
+                                                                               int max_features, int max_iters,
+                                                                               int* __restrict__ err_flag, int cap) {
+  adapt_thresholds<true>(table, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters,
+                         err_flag, cap);
+}
+
+// The bare DetectorAdjuster (adjuster_max_iterations <= 0, features.cpp:101-112): every frame is detected once at the
+// persistent threshold, which never changes.  One thread per (frame, cell); err_flag bit 0 as in adapt_thresholds.
+__global__ void __launch_bounds__(256) k_fixed_thresholds(const int* __restrict__ cand_count, const double* __restrict__ state,
+                                                          int* __restrict__ thr_out, int n, int ncells, int* __restrict__ err_flag,
+                                                          int cap) {
+  const int fc = blockIdx.x * blockDim.x + threadIdx.x;
+  if (fc >= n) return;
+  if (cand_count[fc] > cap) atomicOr(err_flag, 1);
+  thr_out[fc] = (int)state[fc % ncells];
 }
 
 __global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds_wide(const int* __restrict__ hist,
@@ -488,7 +518,8 @@ __global__ void __launch_bounds__(32 * kOrbMaxCells) k_adapt_thresholds_wide(con
                                                                               int nframes, int ncells, int min_features,
                                                                               int max_features, int max_iters,
                                                                               int* __restrict__ err_flag, int cap) {
-  adapt_thresholds(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters, err_flag, cap);
+  adapt_thresholds<false>(hist, cand_count, mask_any, state, thr_out, nframes, ncells, min_features, max_features, max_iters,
+                          err_flag, cap);
 }
 
 // HarrisResponses(img, pts, blockSize 7, k 0.04): Sobel-3 sums over 7x7, float formula evaluated in the same order
@@ -691,6 +722,99 @@ __device__ __forceinline__ void hist_add_warp(int* h, int bin) {
   if (bin >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&h[bin], __popc(peers));
 }
 
+// The count cv::ORB(10000, 1.2, 8, 15, 0, 2, HARRIS, 31, t).detect returns on a cell, for every t = 0..255, from the cell's
+// threshold-free candidates and their Harris responses (resp, every candidate: k_harris with a threshold of 0).  With
+// B_l(t) = {S >= max(t, s_l)}, s_l the 2 n_l-th largest score of level l (0 when it has fewer candidates: retainBest(2 n_l)
+// does not cut), level l keeps q_l(t) = |B_l| when |B_l| <= n_l and otherwise the keypoints of B_l whose Harris response is
+// at least the n_l-th largest of B_l (retainBest keeps ties); k_cell_select_wide applies the same rule at one threshold.
+// One CTA per (frame, cell, level): the level's score histogram gives s_l and every |B_l|; each warp then finds the n_l-th
+// largest response of one B_l (radix select, 8 bits per pass, over the cell's candidates) for the thresholds in
+// [s_l, u_hi], the ones where |B_l| > n_l.  table[fc * 256 + t] += q_l(t) (zeroed by the caller).
+__global__ void __launch_bounds__(1024) k_quota_counts(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                       const float* __restrict__ resp, int cap, int* __restrict__ table) {
+  __shared__ int s_n[256];  // the level's score histogram, then |{S >= u}|
+  __shared__ int s_q[256];  // q_l(u) for u >= s_l
+  __shared__ int s_wh[32][256];
+  __shared__ int s_cut, s_hi;
+  const int fc = blockIdx.x, l = blockIdx.y, t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  const int n = min(cand_count[fc], cap), nl = c_geom.n_per_level[l];
+  const OrbCand* cc = cand + (size_t)fc * cap;
+  const float* rr = resp + (size_t)fc * cap;
+  if (t < 256) s_n[t] = 0;
+  __syncthreads();
+  for (int i = t; i < ((n + 31) & ~31); i += blockDim.x) {
+    int bin = -1;
+    if (i < n) {
+      const OrbCand cd = cc[i];
+      if (cd.level == l) bin = cd.score;
+    }
+    hist_add_warp(s_n, bin);
+  }
+  __syncthreads();
+  if (t == 0) {
+    int cum = 0, cut = -1;
+    for (int u = 255; u >= 0; u--) {
+      cum += s_n[u];
+      s_n[u] = cum;
+      if (cut < 0 && cum >= 2 * nl) cut = u;
+    }
+    if (cut < 0) cut = 0;
+    int hi = cut - 1;
+    while (hi < 255 && s_n[hi + 1] > nl) hi++;
+    s_cut = cut;
+    s_hi = hi;
+  }
+  __syncthreads();
+  const int cut = s_cut, hi = s_hi;
+  if (t < 256) s_q[t] = s_n[t];  // |B_l(u)| <= n_l above u_hi
+  __syncthreads();
+  int* wh = s_wh[warp];
+  for (int v = cut + warp; v <= hi; v += 32) {
+    uint32_t prefix = 0;
+    int want = nl;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int b = lane; b < 256; b += 32) wh[b] = 0;
+      __syncwarp();
+      const uint32_t mask = shift == 24 ? 0u : ~0u << (shift + 8);
+      for (int i = lane; i < n; i += 32) {
+        const OrbCand cd = cc[i];
+        if (cd.level == l && cd.score >= v) {
+          const uint32_t o = f32_ordered(rr[i] + 0.f);  // + 0.f: -0 ties +0, as k_cell_select_wide
+          if ((o & mask) == (prefix & mask)) atomicAdd(&wh[(o >> shift) & 255], 1);
+        }
+      }
+      __syncwarp();
+      if (lane == 0) {
+        int cum = 0;
+        for (int b = 255; b >= 0; b--) {
+          if (cum + wh[b] >= want) {
+            prefix |= (uint32_t)b << shift;
+            want -= cum;
+            break;
+          }
+          cum += wh[b];
+        }
+      }
+      prefix = __shfl_sync(0xffffffffu, prefix, 0);
+      want = __shfl_sync(0xffffffffu, want, 0);
+      __syncwarp();
+    }
+    int q = 0;
+    for (int i = lane; i < n; i += 32) {
+      const OrbCand cd = cc[i];
+      q += (cd.level == l && cd.score >= v && f32_ordered(rr[i] + 0.f) >= prefix) ? 1 : 0;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+    if (lane == 0) s_q[v] = q;
+  }
+  __syncthreads();
+  if (t < 256) {
+    const int q = s_q[max(t, cut)];
+    if (q) atomicAdd(&table[(size_t)fc * 256 + t], q);
+  }
+}
+
 // The same selection with cv::ORB's per-level quotas: every ORB geometry with round(1.5 K / cells) < 606, and frames above
 // kOrbNarrowMax px (cap candidates per cell, CellPos<true> keys), where a cell's valid candidates can outnumber any
 // shared-memory sort.  max_per_cell <= 1024 (orb_prepare: < the smallest ORB quota).
@@ -700,11 +824,12 @@ __device__ __forceinline__ void hist_add_warp(int* h, int bin) {
 // Then keepStrongest: the max_per_cell smallest keys (|response| descending, then level, y, x) by an 8-bit radix select over
 // the 64-bit keys (unique per cell), sorted in shared memory.  One CTA of 1024 threads per (frame, cell); every pass re-reads
 // the cell's candidates (L2-resident).
-template <bool kWide>
-__global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
-                                                           const float* __restrict__ resp, int cap, int quotas, int max_per_cell,
-                                                           unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
-                                                           int out_stride) {
+// kAll (k_cell_quota_all): no keepStrongest; every survivor of the quotas goes to cell_out, unsorted.
+template <bool kWide, bool kAll>
+__device__ __forceinline__ void cell_select(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                            const float* __restrict__ resp, int cap, int quotas, int max_per_cell,
+                                            unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
+                                            int out_stride) {
   using Pos = CellPos<kWide>;
   __shared__ int hist[kOrbLevels * 256];
   __shared__ unsigned long long keys[1024];
@@ -797,6 +922,18 @@ __global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __rest
   auto key_of = [&](const OrbCand& cd, float r) -> unsigned long long {
     return ((unsigned long long)(~f32_ordered(fabsf(r))) << 32) | Pos::pack(cd.level, cd.y, cd.x) | (r < 0.f ? 1ull : 0ull);
   };
+  if constexpr (kAll) {
+    if (t == 0) s_n = 0;
+    __syncthreads();
+    for (int i = t; i < n; i += blockDim.x) {
+      OrbCand cd;
+      float r;
+      if (survives(i, cd, r)) cell_out[(size_t)fc * out_stride + atomicAdd(&s_n, 1)] = key_of(cd, r);
+    }
+    __syncthreads();
+    if (t == 0) cell_out_count[fc] = s_n;
+    return;
+  }
   if (t == 0) {
     s_prefix = 0;
     s_shift = 64;
@@ -861,6 +998,23 @@ __global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __rest
   bitonic_sort_u64(keys, N);
   for (int i = t; i < cnt; i += blockDim.x) cell_out[(size_t)fc * out_stride + i] = keys[i];
   if (t == 0) cell_out_count[fc] = cnt;
+}
+
+template <bool kWide>
+__global__ void __launch_bounds__(1024) k_cell_select_wide(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                           const float* __restrict__ resp, int cap, int quotas, int max_per_cell,
+                                                           unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
+                                                           int out_stride) {
+  cell_select<kWide, false>(cand, cand_count, resp, cap, quotas, max_per_cell, cell_out, cell_out_count, out_stride);
+}
+
+// Whole-frame detectors (one cell, up to kOrbNarrowMax px): cv::ORB's quotas (quotas != 0) or none (FAST), no keepStrongest;
+// out_stride >= cap.  k_frame_precap then caps each frame's survivors for k_frame_finalize.
+__global__ void __launch_bounds__(1024) k_cell_quota_all(const OrbCand* __restrict__ cand, const int* __restrict__ cand_count,
+                                                         const float* __restrict__ resp, int cap, int quotas,
+                                                         unsigned long long* __restrict__ cell_out, int* __restrict__ cell_out_count,
+                                                         int out_stride) {
+  cell_select<false, true>(cand, cand_count, resp, cap, quotas, 1, cell_out, cell_out_count, out_stride);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1099,6 +1253,119 @@ template __global__ void k_frame_finalize<OrbPoints::kDepthPixel, true>(OrbFrame
 template __global__ void k_frame_finalize<OrbPoints::kMinDepth, true>(OrbFrameArgs);
 template __global__ void k_frame_finalize<OrbPoints::kCloud, true>(OrbFrameArgs);
 
+// Whole-frame detectors return up to about 10^4 keypoints (ORB) or more (FAST), k_frame_finalize holds kFrameCap.  Per frame
+// (one cell), from k_cell_quota_all's survivors src[f * src_stride ...] (and, kMinDepth, their depths src_z), this keeps the
+// kFrameCap first of the keypoints k_frame_finalize would keep, in the order of its cut at max_keypoints: mode 1 the
+// removeDepthless / cloud test of its step A, then signed response descending (retainBest) or, kCloud, |response| descending
+// (the detector order projectTo3D walks), ties by (level, y, x).  max_keypoints <= 2730 < kFrameCap, so finalize's result is
+// unchanged.  Mode 0 (the detector output itself) cannot be cut: more than kFrameCap keypoints sets err_flag bit 1.  The
+// kept keys (and depths) go to a.cell_out (a.cand_z) at stride a.out_stride; radix select of the kFrameCap-th smallest
+// order key as in k_cell_select_wide.
+template <OrbPoints P>
+__global__ void __launch_bounds__(1024) k_frame_precap(OrbFrameArgs a, const unsigned long long* __restrict__ src,
+                                                       const int* __restrict__ src_count, const float* __restrict__ src_z,
+                                                       int src_stride, int* __restrict__ err_flag) {
+  using Pos = CellPos<false>;
+  __shared__ int hist[256];
+  __shared__ unsigned long long s_prefix;
+  __shared__ int s_shift, s_done, s_want, s_n;
+  const int mode = P == OrbPoints::kDepthPixel ? a.mode : 1;
+  const int f = blockIdx.x, t = threadIdx.x, W = c_geom.W, H = c_geom.H;
+  const int n = src_count[f];
+  const unsigned long long* sk = src + (size_t)f * src_stride;
+  if (mode == 0 && n > kFrameCap) {
+    if (t == 0) {
+      atomicOr(err_flag, 2);
+      a.cell_out_count[f] = 0;
+    }
+    return;
+  }
+  // order key of survivor i, ~0 when k_frame_finalize's step A would drop it
+  auto order = [&](int i) -> unsigned long long {
+    const unsigned long long k = sk[i];
+    if (mode == 0) return k;
+    int level, ly, lx;
+    Pos::unpack(k, level, ly, lx);
+    const float sc = c_geom.cell[0][level].scale;
+    const float x = __fadd_rn(__fmul_rn((float)lx, sc), (float)c_geom.cell_x0[0]);
+    const float y = __fadd_rn(__fmul_rn((float)ly, sc), (float)c_geom.cell_y0[0]);
+    bool ok = !(x >= W || x < 0 || y >= H || y < 0);
+    if constexpr (P == OrbPoints::kMinDepth) {
+      const float z = src_z[(size_t)f * src_stride + i];
+      ok = ok && !(z != z);
+    } else if constexpr (P == OrbPoints::kCloud) {
+      if (ok) {
+        const float* p = a.depth + ((size_t)f * W * H + (size_t)__float2int_rz(y) * W + __float2int_rz(x)) * a.cloud_stride;
+        ok = !(p[0] != p[0] || p[1] != p[1] || p[2] != p[2]);
+      }
+    } else if (ok) {
+      const int rx = (int)floorf(x + 0.5f), ry = (int)floorf(y + 0.5f);
+      const size_t idx = (size_t)ry * W + rx;
+      ok = idx < (size_t)W * H && !(a.depth[(size_t)f * W * H + idx] != a.depth[(size_t)f * W * H + idx]);
+    }
+    if (!ok) return ~0ull;
+    const uint32_t ord = ~(uint32_t)(k >> 32);  // ordered |response|
+    float r = __uint_as_float(ord & 0x7FFFFFFFu);
+    if (P != OrbPoints::kCloud && (k & 1ull)) r = -r;
+    return ((unsigned long long)(~f32_ordered(r)) << 32) | Pos::pack(level, ly, lx);
+  };
+  if (t == 0) {
+    s_prefix = 0;
+    s_shift = 64;
+    s_done = 0;
+    s_want = kFrameCap;
+    s_n = 0;
+  }
+  __syncthreads();
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int i = t; i < 256; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const unsigned long long hi = shift == 56 ? 0ull : ~0ull << (shift + 8), prefix = s_prefix;
+    for (int i = t; i < ((n + 31) & ~31); i += blockDim.x) {
+      int bin = -1;
+      if (i < n) {
+        const unsigned long long k = order(i);
+        if (k != ~0ull && (k & hi) == (prefix & hi)) bin = (int)((k >> shift) & 255);
+      }
+      hist_add_warp(hist, bin);
+    }
+    __syncthreads();
+    if (t == 0) {
+      int cum = 0, b = 0;
+      for (; b < 256; b++) {
+        if (cum + hist[b] >= s_want) break;
+        cum += hist[b];
+      }
+      if (b == 256) {  // at most kFrameCap kept (first pass only): all of them
+        s_prefix = ~0ull;
+        s_shift = 0;
+        s_done = 1;
+      } else {
+        s_prefix |= (unsigned long long)b << shift;
+        s_want -= cum;
+        if (hist[b] == s_want) {
+          s_shift = shift;
+          s_done = 1;
+        }
+      }
+    }
+    __syncthreads();
+    if (s_done) break;
+  }
+  const int sel_shift = s_shift;
+  const unsigned long long sel = s_prefix >> sel_shift;
+  for (int i = t; i < n; i += blockDim.x) {
+    const unsigned long long k = order(i);
+    if (k != ~0ull && (k >> sel_shift) <= sel) {
+      const int slot = atomicAdd(&s_n, 1);
+      a.cell_out[(size_t)f * a.out_stride + slot] = sk[i];
+      if constexpr (P == OrbPoints::kMinDepth) a.cand_z[(size_t)f * a.out_stride + slot] = src_z[(size_t)f * src_stride + i];
+    }
+  }
+  __syncthreads();
+  if (t == 0) a.cell_out_count[f] = s_n;
+}
+
 // One warp per output keypoint: intensity-centroid orientation on the detector's (cell) pyramid, the cv::KeyPoint record,
 // in mode 1 projectTo3D (node.cpp:900-965) + backProject (misc2.h:49-65) and the rotation (cos, sin) compute() will use.
 // Detector FAST: cv::FAST's KeyPoint(x, y, 7.f, -1, score) -- no orientation; compute() steers the pattern by the angle as
@@ -1309,11 +1576,13 @@ cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, 
   const int tiles = g_fast_tiles[fast ? RGBDSLAM_B200_DETECTOR_FAST : RGBDSLAM_B200_DETECTOR_ORB];
   if (tiles > 0) {
     const uint8_t* m = all_valid ? nullptr : d_cell_mask;
-    if (fast && wide)
+    // the capped kernels: frames above kOrbNarrowMax px, and cells whose candidate buffer orb_prepare sizes by area
+    const bool capped = wide || cand_cap != kOrbCandCap;
+    if (fast && capped)
       k_fast9_nms_wide<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, g_fast9_tiles_x, cand_cap);
     else if (fast)
       k_fast9_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, g_fast9_tiles_x);
-    else if (wide)
+    else if (capped)
       k_fast_nms_wide<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist, cand_cap);
     else
       k_fast_nms<<<dim3(tiles, z), 256, 0, st>>>(d_cell_img, m, d_cand, d_cand_count, d_hist);
@@ -1356,14 +1625,33 @@ cudaError_t orb_run_bayer_gr_to_gray(int nframes, int w, int h, const uint8_t* d
 
 cudaError_t orb_run_adapt(const OrbGeom& g, int nframes, const int* d_hist, const int* d_cand_count, const int* d_mask_any,
                           double* d_state, int* d_thr, int min_features, int max_features, int max_iters, int* d_err,
-                          int cand_cap, cudaStream_t st, int* launches) {
-  if (is_wide(g))
+                          int cand_cap, OrbThresholds mode, cudaStream_t st, int* launches) {
+  if (mode == OrbThresholds::kFixed)
+    k_fixed_thresholds<<<(nframes * g.ncells + 255) / 256, 256, 0, st>>>(d_cand_count, d_state, d_thr, nframes * g.ncells, g.ncells,
+                                                                        d_err, cand_cap);
+  else if (mode == OrbThresholds::kQuotaTable)
+    k_adapt_thresholds_quota<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
+                                                              min_features, max_features, max_iters, d_err, cand_cap);
+  else if (is_wide(g) || cand_cap != kOrbCandCap)
     k_adapt_thresholds_wide<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
                                                              min_features, max_features, max_iters, d_err, cand_cap);
   else
     k_adapt_thresholds<<<1, 32 * kOrbMaxCells, 0, st>>>(d_hist, d_cand_count, d_mask_any, d_state, d_thr, nframes, g.ncells,
                                                         min_features, max_features, max_iters, d_err);
   (*launches)++;
+  return cudaGetLastError();
+}
+
+cudaError_t orb_run_quota_counts(const OrbGeom& g, int nframes, const uint8_t* d_cell_img, const OrbCand* d_cand,
+                                 const int* d_cand_count, int* d_thr_scratch, float* d_resp, int cand_cap, int* d_table,
+                                 cudaStream_t st, int* launches) {
+  const int z = nframes * g.ncells;
+  cudaError_t e = cudaMemsetAsync(d_thr_scratch, 0, sizeof(int) * z, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_table, 0, sizeof(int) * 256 * z, st);
+  if (e != cudaSuccess) return e;
+  k_harris_wide<<<dim3((cand_cap + 255) / 256, z), 256, 0, st>>>(d_cell_img, d_cand, d_cand_count, d_thr_scratch, d_resp, cand_cap);
+  k_quota_counts<<<dim3(z, kOrbLevels), 1024, 0, st>>>(d_cand, d_cand_count, d_resp, cand_cap, d_table);
+  (*launches) += 2;
   return cudaGetLastError();
 }
 
@@ -1383,13 +1671,13 @@ static void launch_frames(int nframes, bool fast, bool wide, const OrbFrameArgs&
   (*launches) += 2;
 }
 
-cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quotas, OrbPoints points, const OrbCandidates& c,
-                           const OrbFrameArgs& a, cudaStream_t st, int* launches) {
-  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST, wide = is_wide(g);
+cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
+                           const OrbFrameArgs& a, const OrbSurvivors* all, int* d_err, cudaStream_t st, int* launches) {
+  const bool fast = detector == RGBDSLAM_B200_DETECTOR_FAST, wide = is_wide(g), capped = wide || c.cap != kOrbCandCap;
   const int z = nframes * g.ncells, max_per_cell = a.out_stride;
   const dim3 rgrid((c.cap + 255) / 256, z);
-  quotas = quotas && !fast;  // the FAST detector has no quotas (cv::FastFeatureDetector)
-  if (wide) {
+  const int quotas = fast ? 0 : 1;  // the FAST detector has no quotas (cv::FastFeatureDetector)
+  if (capped) {
     if (fast)
       k_fast_response_wide<<<rgrid, 256, 0, st>>>(c.cand, c.count, c.thr, c.resp, c.cap);
     else
@@ -1401,15 +1689,36 @@ cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quo
       k_harris<<<rgrid, 256, 0, st>>>(a.cell_img, c.cand, c.count, c.thr, c.resp);
   }
   (*launches)++;
-  if (wide) {
-    k_cell_select_wide<true><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, quotas ? 1 : 0, max_per_cell, a.cell_out,
+  if (all) {  // whole-frame detectors: no keepStrongest; k_frame_precap caps what k_frame_finalize receives
+    k_cell_quota_all<<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, quotas, all->keys, all->count, all->stride);
+    OrbFrameArgs pre = a;
+    pre.cell_out = all->keys;
+    pre.cell_out_count = all->count;
+    pre.out_stride = all->stride;
+    pre.cand_z = all->z;
+    (*launches) += 2;
+    switch (points) {
+      case OrbPoints::kDepthPixel:
+        k_frame_precap<OrbPoints::kDepthPixel><<<nframes, 1024, 0, st>>>(a, all->keys, all->count, all->z, all->stride, d_err);
+        break;
+      case OrbPoints::kMinDepth:
+        k_min_depth<<<dim3((all->stride + 7) / 8, z), 256, 0, st>>>(pre, fast);
+        (*launches)++;
+        k_frame_precap<OrbPoints::kMinDepth><<<nframes, 1024, 0, st>>>(a, all->keys, all->count, all->z, all->stride, d_err);
+        break;
+      case OrbPoints::kCloud:
+        k_frame_precap<OrbPoints::kCloud><<<nframes, 1024, 0, st>>>(a, all->keys, all->count, all->z, all->stride, d_err);
+        break;
+    }
+  } else if (wide) {
+    k_cell_select_wide<true><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, quotas, max_per_cell, a.cell_out,
                                                  a.cell_out_count, max_per_cell);
     (*launches)++;
-  } else if (quotas) {
-    k_cell_select_wide<false><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, 1, max_per_cell, a.cell_out, a.cell_out_count,
+  } else if (quotas || capped) {
+    k_cell_select_wide<false><<<z, 1024, 0, st>>>(c.cand, c.count, c.resp, c.cap, quotas, max_per_cell, a.cell_out, a.cell_out_count,
                                                   max_per_cell);
     (*launches)++;
-  } else {  // the FAST detector, and ORB geometries where a binding quota could change the adjuster's count (DESIGN.md 4.5.5)
+  } else {  // the FAST detector's cells of up to kOrbCandCap candidates
     static bool attr = false;
     if (!attr) {
       cudaError_t e = cudaFuncSetAttribute(k_cell_select, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
@@ -1424,11 +1733,14 @@ cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quo
       launch_frames<OrbPoints::kDepthPixel>(nframes, fast, wide, a, st, launches);
       break;
     case OrbPoints::kMinDepth:
-      if (wide)
+      if (all) {  // k_min_depth ran on the survivors, before k_frame_precap
+      } else if (wide) {
         k_min_depth_wide<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(a, fast);
-      else
+        (*launches)++;
+      } else {
         k_min_depth<<<dim3((max_per_cell + 7) / 8, z), 256, 0, st>>>(a, fast);
-      (*launches)++;
+        (*launches)++;
+      }
       launch_frames<OrbPoints::kMinDepth>(nframes, fast, wide, a, st, launches);
       break;
     case OrbPoints::kCloud:

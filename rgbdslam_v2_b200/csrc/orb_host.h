@@ -16,10 +16,24 @@ cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, 
                            const float* d_depth_for_mask, int detector, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
                            int* d_cand_count, int* d_hist, int* d_mask_any, int cand_cap, cudaStream_t st, int* launches);
 
-// the adaptive-threshold recurrence of the F frames of a chunk, on the device (no host round trip)
+// How a call's detection thresholds come about (createDetector, features.cpp:101-112)
+enum class OrbThresholds {
+  kHistogram,   // the adjuster's recurrence on the score histograms (FAST, and ORB where no quota can change its count)
+  kQuotaTable,  // the same recurrence on orb_run_quota_counts' tables: ORB where a cell's maximum reaches cv::ORB's smallest quota
+  kFixed,       // adjuster_max_iterations <= 0: the bare DetectorAdjuster detects once at its persistent threshold
+};
+
+// the thresholds of the F frames of a chunk, on the device (no host round trip): d_hist holds the score histograms or, for
+// kQuotaTable, the count tables
 cudaError_t orb_run_adapt(const OrbGeom& g, int nframes, const int* d_hist, const int* d_cand_count, const int* d_mask_any,
                           double* d_state, int* d_thr, int min_features, int max_features, int max_iters, int* d_err,
-                          int cand_cap, cudaStream_t st, int* launches);
+                          int cand_cap, OrbThresholds mode, cudaStream_t st, int* launches);
+
+// d_table[(f * ncells + c) * 256 + t] = the number of keypoints cv::ORB(10000, ..., t).detect returns on cell c of frame f,
+// t = 0..255 (k_quota_counts), from the candidates of orb_run_detect.  Overwrites d_thr_scratch (nframes x ncells) and d_resp.
+cudaError_t orb_run_quota_counts(const OrbGeom& g, int nframes, const uint8_t* d_cell_img, const OrbCand* d_cand,
+                                 const int* d_cand_count, int* d_thr_scratch, float* d_resp, int cand_cap, int* d_table,
+                                 cudaStream_t st, int* launches);
 
 // cvtColor(CV_RGB2GRAY) of nframes packed w*h*3 colour images into grey (node.cpp:139-144, 275-277).
 cudaError_t orb_run_rgb_to_gray(int nframes, size_t px, const uint8_t* d_rgb, uint8_t* d_gray, cudaStream_t st, int* launches);
@@ -72,11 +86,19 @@ struct OrbFrameArgs {
   int mode;                      // 0: detector output (OrbPoints::kDepthPixel), 1: Node constructor
 };
 
-// detector ORB: Harris responses, orientation, size 31 * scale; FAST: response = corner score, angle -1, size 7.
-// quotas: also apply cv::ORB's per-level quotas (ORB detector; k_cell_select_wide), which orb_prepare allows where
-// round(1.5 * max_keypoints / cells) < 606 with a grid (DESIGN.md 4.5.5).
-cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, bool quotas, OrbPoints points, const OrbCandidates& c,
-                           const OrbFrameArgs& a, cudaStream_t st, int* launches);
+// Whole-frame detectors: every frame's keypoints before k_frame_precap caps them at kOrbFrameCap (stride >= cand_cap)
+struct OrbSurvivors {
+  unsigned long long* keys;
+  int* count;
+  float* z;  // OrbPoints::kMinDepth
+  int stride;
+};
+
+// detector ORB: Harris responses, cv::ORB's per-level quotas (k_cell_select_wide), orientation, size 31 * scale; FAST:
+// response = corner score, angle -1, size 7.  all != NULL (one whole-frame cell): no keepStrongest, the survivors go through
+// `all` to k_frame_precap; d_err bit 1: a detector output (mode 0) of more than kOrbFrameCap keypoints.
+cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,
+                           const OrbFrameArgs& a, const OrbSurvivors* all, int* d_err, cudaStream_t st, int* launches);
 
 // levels: extractor pyramid levels built and blurred (cv::ORB::compute builds 1 + the largest keypoint octave)
 cudaError_t orb_run_describe(const OrbGeom& g, const OrbTables& tab, int nframes, int levels, const uint8_t* d_gray,
