@@ -27,13 +27,14 @@ class OracleBackend:
     def n_features(self, handle):
         return len(handle[1])
 
-    def match_one_to_many(self, node, olds, seed):
+    def match_one_to_many(self, node, olds, seed, first_pair_index=None):
         prm = self.o.make_params(depth_cov_z0=2.0)
         new = node.handle
         dn = np.concatenate([new[1]] * len(olds)); xn = np.concatenate([new[2]] * len(olds))
         do = np.concatenate([o.handle[1] for o in olds]); xo = np.concatenate([o.handle[2] for o in olds])
         res, _, _ = self.o.match_pairs(prm, dn, xn, [len(new[1])] * len(olds), do, xo, [len(o.handle[1]) for o in olds],
-                                       [node.id] * len(olds), [o.id for o in olds], seed=seed, first_pair_index=64 * node.id,
+                                       [node.id] * len(olds), [o.id for o in olds], seed=seed,
+                                       first_pair_index=64 * node.id if first_pair_index is None else first_pair_index,
                                        threads=8, want_matches=False)
         return res
 

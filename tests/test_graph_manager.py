@@ -138,3 +138,97 @@ def test_max_connections_stops_further_comparisons():
     assert max(matched.values()) == 3 and matched[11] == 3 and gm.n_const_edges > 0
     gm2, _, _ = _run(12, lambda a, b: True)
     assert max(np.bincount([b for _, b in gm2.edges])) > 4 and gm2.n_const_edges == 0
+
+
+def _run_strategy(n, visible, strategy, **kw):
+    return _run(n, visible, pose_relative_to=strategy, **kw)[0]
+
+
+def test_fixation_first_and_previous():
+    # fixationOfVertices (graph_manager.cpp:918-936): "first" fixes node 0, "previous" the node before the newest
+    for strategy, expect in [("first", lambda n: 0), ("previous", lambda n: n - 2 if n > 2 else 0)]:
+        gm = _run_strategy(10, lambda a, b: abs(a - b) <= 2, strategy)
+        for rec in gm.records[1:]:
+            (o,) = rec["optimizations"]
+            n = len(o["ids"])
+            assert list(np.nonzero(o["fixed"])[0]) == [expect(n)], (strategy, n, o["fixed"])
+
+
+def test_fixation_largest_loop_follows_the_earliest_loop_closure_node():
+    # the loop closure 9 -> 2 lowers earliest_loop_closure_node_ to 2 (:893-896): vertices 0 and 1 are fixed in that
+    # optimisation (:922-931); without a loop closure the earliest node is the new one and everything before it is fixed
+    gm = _run_strategy(12, lambda a, b: a - b == 1 or (a, b) == (9, 2), "largest_loop")
+    rec = gm.records[9]
+    assert rec["earliest"] == 2 and list(rec["optimizations"][0]["fixed"]) == [1, 1] + [0] * 8
+    rec = gm.records[10]
+    assert rec["earliest"] == 9 and list(rec["optimizations"][0]["fixed"]) == [1] * 9 + [0, 0]
+    # "first" leaves earliest_loop_closure_node_ at the new node's id
+    gm = _run_strategy(12, lambda a, b: a - b == 1 or (a, b) == (9, 2), "first")
+    assert [r["earliest"] for r in gm.records[1:]] == list(range(1, 12))
+
+
+def test_fixation_inaffected_frees_the_ends_of_new_edges():
+    # after an optimisation every vertex is fixed (:1031-1033); the edges of the next node free both their ends (:889-892)
+    gm = _run_strategy(9, lambda a, b: a - b in (1, 3), "inaffected")
+    for k in range(5, 9):
+        (o,) = gm.records[k]["optimizations"]
+        freed = {k, k - 1, k - 3}
+        assert list(o["fixed"]) == [0 if v in freed else 1 for v in o["ids"]], (k, o["fixed"])
+    assert gm.fixed_ids == set(range(9))
+    # the first optimisation frees vertex 0 too: nothing is fixed, so the first vertex anchors the solve
+    assert list(gm.records[1]["optimizations"][0]["fixed"]) == [1, 0]
+
+
+def test_keyframe_rule_reads_earliest_loop_closure_node():
+    # node 10 matches 9 and 3, neither a keyframe (keyframes 0, 2, 4, 6, 8): with "first" the earliest loop closure node is
+    # node 10 itself, newer than the last keyframe, so 9 becomes one (:731-732); with "largest_loop" the edge to 3 lowers it
+    # below keyframe 8 and no keyframe is added
+    def visible(a, b):
+        return b in (9, 3) if a == 10 else a - b in (1, 2)
+    for strategy, last in [("first", 9), ("largest_loop", 8)]:
+        gm = _run_strategy(11, visible, strategy)
+        assert gm.keyframe_ids[:5] == [0, 2, 4, 6, 8] and gm.keyframe_ids[-1] == last, (strategy, gm.keyframe_ids)
+
+
+def test_first_node_is_replaced_by_a_richer_one():
+    # addNode (:762-769): no match with the only node, which has fewer features -> resetGraph + firstNode(new node).  The
+    # constant-position edge (frames < 0.1 s apart) counts as a match, so the frames here are 0.5 s apart.
+    be = ScriptedBackend(_line(4), lambda a, b: False)
+    gm = G.GraphManager(be, G.Params(), seed=0)
+    assert gm.add_node("a", 30, 0.0) and gm.add_node("b", 500, 0.5)
+    assert list(gm.nodes) == [0] and gm.nodes[0].handle == "b" and gm.keyframe_ids == [0] and gm.fixed_ids == {0}
+    assert gm.records[1]["ret"] and gm.records[1]["id"] == 0 and gm.records[1]["edges"] == []
+    assert not gm.add_node("c", 400, 1.0)  # fewer features than the first node: not added, no replacement
+    assert list(gm.nodes) == [0] and gm.nodes[0].handle == "b"
+    # 1/30 s apart the constant-position edge keeps the new node: no replacement
+    gm = G.GraphManager(ScriptedBackend(_line(4), lambda a, b: False), G.Params(), seed=0)
+    assert gm.add_node("a", 30, 0.0) and gm.add_node("b", 500, 1 / 30)
+    assert list(gm.nodes) == [0, 1] and gm.n_const_edges == 1
+
+
+class KeyedBackend(ScriptedBackend):
+    """records the generator key of each call's first pair, resolved as pipeline.GpuBackend resolves it"""
+
+    def match_one_to_many(self, node, olds, seed, first_pair_index=None):
+        self.keys.append((node.id, len(olds), 64 * node.id if first_pair_index is None else first_pair_index))
+        return super().match_one_to_many(node, olds, seed)
+
+
+def test_initial_comparison_key_self_candidates_and_max_connections():
+    poses = _line(30)
+    be = KeyedBackend(poses, lambda a, b: abs(a - b) <= 3)
+    be.keys = []
+    gm = G.GraphManager(be, G.Params(min_translation_meter=0.01, max_connections=1), seed=3)
+    for k in range(30):
+        gm.add_node(k, 500, k / 30.0)
+    # the initial comparison is keyed 64 id + 63, the batch 64 id + k (nodeComparisons, graph_manager.hpp)
+    initial = [(i, f) for i, n, f in be.keys if n == 1 and f % 64 == 63]
+    assert len(initial) == 29 and all(f == 64 * i + 63 for i, f in initial)
+    assert all(f == 64 * i for i, n, f in be.keys if f % 64 != 63)
+    # the new node is never its own candidate (the geodesic ball around the matched predecessor holds it)
+    assert all(new not in olds for new, olds in be.calls)
+    # max_connections counts the initial comparison's transformation (node.cpp:1310-1312, :1417): with 1, the initial edge
+    # and one more
+    ident = np.array([0, 0, 0, 0, 0, 0, 1.0])
+    per_node = np.bincount([b for (a, b), z in zip(gm.edges, gm.meas) if not np.allclose(z, ident)])
+    assert (per_node[1:] == 2).all(), per_node
