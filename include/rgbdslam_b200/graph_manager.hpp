@@ -11,6 +11,8 @@
 //   void   saveOctomap(filename)    == saveOctomapImpl                   graph_mgr_io.cpp:253-310 -> rgbdslam_b200_octomap_*
 //   void   renderToOctomap(Node*), writeOctomap(filename)              graph_mgr_io.cpp:312-329
 //   void   occupancyFilterClouds()                                      graph_manager.cpp:1372-1381 -> rgbdslam_b200_octomap_filter_clouds
+//   size_t saveIndividualClouds(basename) == saveIndividualCloudsToFile graph_mgr_io.cpp:330-433 -> rgbdslam_b200_transform_clouds
+//   size_t saveAllFeatures(filename) == saveAllFeaturesToFile           graph_mgr_io.cpp:445-497 (export_text.hpp, host only)
 // Host logic only; every compute step is a C-ABI call.  The reference draws from the global rand(); here every draw comes
 // from the library's counter-based generator keyed by (seed, node id).  g2o's HyperDijkstra (not under /root/reference) is
 // restated in geodesicBall().  oracle/graph_manager_oracle.py is the Python twin of this file, decision for decision; where
@@ -26,8 +28,10 @@
 #include <functional>
 #include <map>
 #include <set>
+#include <stdexcept>
 #include <string>
 
+#include "export_text.hpp"
 #include "node.hpp"
 
 namespace rgbdslam_b200 {
@@ -93,6 +97,62 @@ inline void cloudSensorPose(const double R[9], const double t[3], float q[4], fl
   }
   for (int i = 0; i < 3; i++) o[i] = (float)t[i];
 }
+// tf and Eigen conversions, on row-major 3 x 4 transforms (rotation | origin):
+// tf::Matrix3x3::setRotation(tf::Quaternion(x, y, z, w)) in double, into the rotation part of M
+inline void tfSetRotation(const double* q, double M[12]) {
+  const double x = q[0], y = q[1], z = q[2], w = q[3];
+  const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
+  const double xs = x * s, ys = y * s, zs = z * s, wx = w * xs, wy = w * ys, wz = w * zs;
+  const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
+  M[0] = 1.0 - (yy + zz), M[1] = xy - wz, M[2] = xz + wy;
+  M[4] = xy + wz, M[5] = 1.0 - (xx + zz), M[6] = yz - wx;
+  M[8] = xz - wy, M[9] = yz + wx, M[10] = 1.0 - (xx + yy);
+}
+// tf::Matrix3x3::getRotation of the rotation part of M (tf's branch and tie rule): g (x, y, z, w)
+inline void tfGetRotation(const double M[12], double g[4]) {
+  const double mt = M[0] + M[5] + M[10];
+  if (mt > 0.0) {
+    double s = std::sqrt(mt + 1.0);
+    g[3] = s * 0.5;
+    s = 0.5 / s;
+    g[0] = (M[9] - M[6]) * s; g[1] = (M[2] - M[8]) * s; g[2] = (M[4] - M[1]) * s;
+  } else {
+    const int i = M[0] < M[5] ? (M[5] < M[10] ? 2 : 1) : (M[0] < M[10] ? 2 : 0);
+    const int j = (i + 1) % 3, k = (i + 2) % 3;
+    double s = std::sqrt(M[5 * i] - M[5 * j] - M[5 * k] + 1.0);
+    g[i] = s * 0.5;
+    s = 0.5 / s;
+    g[3] = (M[4 * k + j] - M[4 * j + k]) * s;
+    g[j] = (M[4 * j + i] + M[4 * i + j]) * s;
+    g[k] = (M[4 * k + i] + M[4 * i + k]) * s;
+  }
+}
+// Eigen's Quaternionf::toRotationMatrix of q (x, y, z, w), into the rotation part of T
+inline void quatfToRotationMatrix(const float q[4], float T[12]) {
+  const float fx = q[0], fy = q[1], fz = q[2], fw = q[3];
+  const float tx = 2.0f * fx, ty = 2.0f * fy, tz = 2.0f * fz;
+  const float twx = tx * fw, twy = ty * fw, twz = tz * fw, txx = tx * fx, txy = ty * fx, txz = tz * fx;
+  const float tyy = ty * fy, tyz = tz * fy, tzz = tz * fz;
+  T[0] = 1.0f - (tyy + tzz), T[1] = txy - twz, T[2] = txz + twy;
+  T[4] = txy + twz, T[5] = 1.0f - (txx + tzz), T[6] = tyz - twx;
+  T[8] = txz - twy, T[9] = tyz + twx, T[10] = 1.0f - (txx + tyy);
+}
+// tf::Transform * tf::Transform: (Ra Rb, Ra tb + ta), every entry a sum (a0 b0 + a1 b1) + a2 b2
+inline void tfMul(const double A[12], const double B[12], double T[12]) {
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) T[4 * r + c] = (A[4 * r] * B[c] + A[4 * r + 1] * B[4 + c]) + A[4 * r + 2] * B[8 + c];
+    T[4 * r + 3] = ((A[4 * r] * B[3] + A[4 * r + 1] * B[7]) + A[4 * r + 2] * B[11]) + A[4 * r + 3];
+  }
+}
+// tf::Transform::inverse: (R^T, R^T (-t)), -t negating every component (a zero origin becomes -0)
+inline void tfInverse(const double A[12], double T[12]) {
+  const double m[3] = {-A[3], -A[7], -A[11]};
+  for (int r = 0; r < 3; r++) {
+    for (int c = 0; c < 3; c++) T[4 * r + c] = A[4 * c + r];
+    T[4 * r + 3] = (A[r] * m[0] + A[4 + r] * m[1]) + A[8 + r] * m[2];
+  }
+}
+
 // The float 3 x 4 (row-major, node -> map) saveOctomap applies to a node whose estimate has rotation R (row-major, double)
 // and translation t: cloudSensorPose, then insertCloudCallback widens the quaternion to a tf::Quaternion,
 // tf::Matrix3x3::setRotation builds the basis in double, pcl_ros::transformPointCloud takes it back with getRotation (tf's
@@ -101,39 +161,13 @@ inline void cloudSensorPose(const double R[9], const double t[3], float q[4], fl
 inline void octomapPose(const double R[9], const double t[3], float T[12]) {
   float q[4], o[3];  // q: x, y, z, w
   cloudSensorPose(R, t, q, o);
-  // tf::Matrix3x3::setRotation(tf::Quaternion(x, y, z, w)) in double
-  const double x = q[0], y = q[1], z = q[2], w = q[3];
-  const double d = x * x + y * y + z * z + w * w, s2 = 2.0 / d;
-  const double xs = x * s2, ys = y * s2, zs = z * s2, wx = w * xs, wy = w * ys, wz = w * zs;
-  const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
-  const double M[9] = {1.0 - (yy + zz), xy - wz, xz + wy, xy + wz, 1.0 - (xx + zz), yz - wx, xz - wy, yz + wx, 1.0 - (xx + yy)};
-  // tf::Matrix3x3::getRotation
-  double g[4];
-  const double mt = M[0] + M[4] + M[8];
-  if (mt > 0.0) {
-    double s = std::sqrt(mt + 1.0);
-    g[3] = s * 0.5;
-    s = 0.5 / s;
-    g[0] = (M[7] - M[5]) * s; g[1] = (M[2] - M[6]) * s; g[2] = (M[3] - M[1]) * s;
-  } else {
-    const int i = M[0] < M[4] ? (M[4] < M[8] ? 2 : 1) : (M[0] < M[8] ? 2 : 0);
-    const int j = (i + 1) % 3, k = (i + 2) % 3;
-    double s = std::sqrt(M[4 * i] - M[4 * j] - M[4 * k] + 1.0);
-    g[i] = s * 0.5;
-    s = 0.5 / s;
-    g[3] = (M[3 * k + j] - M[3 * j + k]) * s;
-    g[j] = (M[3 * j + i] + M[3 * i + j]) * s;
-    g[k] = (M[3 * k + i] + M[3 * i + k]) * s;
-  }
-  // Quaternionf::toRotationMatrix
-  const float fx = (float)g[0], fy = (float)g[1], fz = (float)g[2], fw = (float)g[3];
-  const float tx = 2.0f * fx, ty = 2.0f * fy, tz = 2.0f * fz;
-  const float twx = tx * fw, twy = ty * fw, twz = tz * fw, txx = tx * fx, txy = ty * fx, txz = tz * fx;
-  const float tyy = ty * fy, tyz = tz * fy, tzz = tz * fz;
-  const float out[12] = {1.0f - (tyy + tzz), txy - twz, txz + twy, o[0],
-                         txy + twz, 1.0f - (txx + tzz), tyz - twx, o[1],
-                         txz - twy, tyz + twx, 1.0f - (txx + tyy), o[2]};
-  std::memcpy(T, out, sizeof(out));
+  const double qd[4] = {q[0], q[1], q[2], q[3]};
+  double M[12], g[4];
+  tfSetRotation(qd, M);
+  tfGetRotation(M, g);
+  const float gf[4] = {(float)g[0], (float)g[1], (float)g[2], (float)g[3]};
+  quatfToRotationMatrix(gf, T);
+  T[3] = o[0], T[7] = o[1], T[11] = o[2];
 }
 
 inline Pose7 poseFromIsometry(const Isometry3d& T) {  // column-major 4x4
@@ -497,23 +531,25 @@ class GraphManager {
   // rotation createQuaternionFromRPY(-1.57, 0, -1.57) (-1.57, not -pi/2) and origin (0, -0.04, 0); eigenTransf2TF takes the
   // rotation through a quaternion (Eigen's matrix -> quaternion, here normalised) and tf's quaternion -> matrix.
   void mapTransform(int id, double T[12]) const {
-    const Pose7& p = estimates_.at(id);
-    double R[9], q[4];
-    quatToRot(p.v + 3, R);  // the VertexSE3 estimate as an Isometry3d
-    rotToQuat(R, q);
     double P[12], C[12];
-    tfMatrix(q, P);
-    P[3] = p.v[0], P[7] = p.v[1], P[11] = p.v[2];
+    eigenTransf2TF(id, P);
     const double hr = -1.57 * 0.5, hp = 0.0, hy = -1.57 * 0.5;  // tf::Quaternion::setRPY(roll, pitch, yaw)
     const double cr = std::cos(hr), sr = std::sin(hr), cp = std::cos(hp), sp = std::sin(hp), cy = std::cos(hy), sy = std::sin(hy);
     const double qc[4] = {sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy,
                           cr * cp * cy + sr * sp * sy};
-    tfMatrix(qc, C);
+    tfSetRotation(qc, C);
     C[3] = 0.0, C[7] = -0.04, C[11] = 0.0;
-    for (int r = 0; r < 3; r++) {  // tf::Transform * tf::Transform: (Rc Rp, Rc tp + tc), sums (a0 b0 + a1 b1) + a2 b2
-      for (int c = 0; c < 3; c++) T[4 * r + c] = (C[4 * r] * P[c] + C[4 * r + 1] * P[4 + c]) + C[4 * r + 2] * P[8 + c];
-      T[4 * r + 3] = ((C[4 * r] * P[3] + C[4 * r + 1] * P[7]) + C[4 * r + 2] * P[11]) + C[4 * r + 3];
-    }
+    tfMul(C, P, T);
+  }
+  // eigenTransf2TF(estimate of node id) (misc.cpp), row-major 3 x 4: the VertexSE3 estimate as an Isometry3d, its rotation
+  // through Eigen's matrix -> quaternion (here normalised) and tf's quaternion -> matrix, its translation as it is
+  void eigenTransf2TF(int id, double P[12]) const {
+    const Pose7& p = estimates_.at(id);
+    double R[9], q[4];
+    quatToRot(p.v + 3, R);
+    rotToQuat(R, q);
+    tfSetRotation(q, P);
+    P[3] = p.v[0], P[7] = p.v[1], P[11] = p.v[2];
   }
 
   // GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583): the stored clouds (Node::store_pointclouds()) of the nodes
@@ -522,15 +558,8 @@ class GraphManager {
   // leaves the aggregate).  ".pcd" is appended when the name lacks it; a ".ply" name throws std::invalid_argument (PLY
   // output is not built).  Returns the number of points written.
   size_t saveAllClouds(std::string filename) const {
-    auto ends_with = [&](const char* ext) {
-      const size_t n = std::strlen(ext);
-      if (filename.size() < n) return false;
-      for (size_t i = 0; i < n; i++)
-        if (std::tolower((unsigned char)filename[filename.size() - n + i]) != ext[i]) return false;
-      return true;
-    };
-    if (ends_with(".ply")) throw std::invalid_argument("saveAllClouds: PLY output is not built (save as .pcd)");
-    if (!ends_with(".pcd")) filename += ".pcd";
+    if (endsWith(filename, ".ply")) throw std::invalid_argument("saveAllClouds: PLY output is not built (save as .pcd)");
+    if (!endsWith(filename, ".pcd")) filename += ".pcd";
     std::vector<uint64_t> handles;
     std::vector<double> T;
     for (auto& kv : graph_) {
@@ -549,21 +578,128 @@ class GraphManager {
     check(rgbdslam_b200_render_cloud((int)handles.size(), handles.data(), T.data(), maximum_depth(), preserve, 32, pts.data(), count,
                                      &count, nullptr),
           "render_cloud");
-    FILE* f = std::fopen(filename.c_str(), "wb");
-    if (!f) throw std::runtime_error("cannot open " + filename);
     const unsigned long long n = (unsigned long long)count;
-    std::fprintf(f,
-                 "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z rgb\nSIZE 4 4 4 4\nTYPE F F F F\n"
-                 "COUNT 1 1 1 1\nWIDTH %llu\nHEIGHT %llu\nVIEWPOINT 0 0 0 1 0 0 0\nPOINTS %llu\nDATA binary\n",
-                 preserve ? n : 1ull, preserve ? 1ull : n, n);
-    std::vector<float> rec(4 * (size_t)count);
-    for (size_t i = 0; i < pts.size(); i++) {
-      rec[4 * i] = pts[i].x, rec[4 * i + 1] = pts[i].y, rec[4 * i + 2] = pts[i].z;
-      std::memcpy(&rec[4 * i + 3], &pts[i].b, 4);
-    }
-    const bool ok = std::fwrite(rec.data(), 16, pts.size(), f) == pts.size();
-    if (std::fclose(f) != 0 || !ok) throw std::runtime_error("cannot write " + filename);
+    const float viewpoint[7] = {0, 0, 0, 1, 0, 0, 0};
+    writePCD(filename, pts, preserve ? n : 1ull, preserve ? 1ull : n, viewpoint);
     return pts.size();
+  }
+
+  // parameter transform_individual_clouds (parameter_server.cpp:67, default false) of saveIndividualClouds
+  static bool& transform_individual_clouds() {
+    static bool v = false;
+    return v;
+  }
+  // world2points of saveIndividualCloudsToFile (graph_mgr_io.cpp:384-396) without tf and ground truth:
+  // computeFixedToBaseTransform (:56-90) init_base_pose_ * base2points * eigenTransf2TF(estimate) * base2points.inverse(), times
+  // base2points, with init_base_pose_ and base2points identities.  The products are formed literally: an identity factor can
+  // turn the sign of a zero, which the pose text shows.
+  void worldToPoints(int id, double W[12]) const {
+    const double I[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
+    double M[12], inv[12], a[12], b[12], c[12];
+    eigenTransf2TF(id, M);
+    tfInverse(I, inv);
+    tfMul(I, I, a);
+    tfMul(a, M, b);
+    tfMul(b, inv, c);
+    tfMul(c, I, W);
+  }
+  // GraphManager::saveIndividualCloudsToFile (graph_mgr_io.cpp:330-433): in ascending id, every node with valid_tf_estimate_,
+  // an estimate and a non-empty stored cloud (the test of updateCloudOrigin) writes basename_%04d.pcd (its stored cloud, binary,
+  // x y z rgb, its own width x height, NaN points included) and basename_%04d.txt (the sensor pose as a 4 x 4, rows "R R R o ",
+  // then "0 0 0 1").  With transform_individual_clouds the clouds are first transformed in place on the device by their
+  // estimates (rgbdslam_b200_transform_clouds) and stay so; the pose is then the reference's Quaternionf(0, 0, 0, 1) --
+  // (w, x, y, z): w = 0, z = 1, a half turn about z -- at origin 0.  Without it the pose is worldToPoints'.  Either way it
+  // becomes the node's cloud sensor pose.  Floats are written as std::ostream writes them (ostreamFloat).  The _gt.pcd files
+  // of ground_truth_frame_name are not built.  Returns the number of nodes written.
+  size_t saveIndividualClouds(const std::string& basename) {
+    std::vector<Node*> nodes;
+    for (auto& kv : graph_)
+      if (hasCloud(kv.second)) nodes.push_back(kv.second);
+    const bool in_place = transform_individual_clouds();
+    if (in_place) {
+      std::vector<uint64_t> handles;
+      std::vector<double> T;
+      for (Node* n : nodes) {  // v->estimate().matrix()
+        const Pose7& p = estimates_.at(n->vertex_id_);
+        double R[9];
+        quatToRot(p.v + 3, R);
+        handles.push_back(n->handle());
+        const double t[12] = {R[0], R[1], R[2], p.v[0], R[3], R[4], R[5], p.v[1], R[6], R[7], R[8], p.v[2]};
+        T.insert(T.end(), t, t + 12);
+      }
+      check(rgbdslam_b200_transform_clouds((int)handles.size(), handles.data(), T.data()), "transform_clouds");
+    }
+    for (Node* n : nodes) {
+      float q[4] = {0, 0, 1, 0}, o[3] = {0, 0, 0};  // sensor_orientation_ (x, y, z, w), sensor_origin_
+      if (!in_place) {
+        double W[12], g[4];
+        worldToPoints(n->vertex_id_, W);
+        tfGetRotation(W, g);
+        for (int k = 0; k < 4; k++) q[k] = (float)g[k];
+        o[0] = (float)W[3], o[1] = (float)W[7], o[2] = (float)W[11];
+      }
+      float R[12];
+      quatfToRotationMatrix(q, R);
+      std::memcpy(n->cloud_sensor_pose_, q, sizeof(q));
+      std::memcpy(n->cloud_sensor_pose_ + 4, o, sizeof(o));
+      int w = 0, h = 0;
+      check(rgbdslam_b200_node_download_cloud(n->handle(), 32, nullptr, &w, &h), "node_download_cloud");
+      std::vector<PointXYZRGB> pts((size_t)w * h);
+      check(rgbdslam_b200_node_download_cloud(n->handle(), 32, pts.data(), &w, &h), "node_download_cloud");
+      char suffix[32];
+      std::snprintf(suffix, sizeof(suffix), "_%04d", n->id_);
+      const float viewpoint[7] = {o[0], o[1], o[2], q[3], q[0], q[1], q[2]};
+      writePCD(basename + suffix + ".pcd", pts, (unsigned long long)w, (unsigned long long)h, viewpoint);
+      std::string text;
+      for (int i = 0; i < 3; i++)
+        text += ostreamFloat(R[4 * i]) + " " + ostreamFloat(R[4 * i + 1]) + " " + ostreamFloat(R[4 * i + 2]) + " " + ostreamFloat(o[i]) + " ";
+      text += "0 0 0 1\n";
+      writeFile(basename + suffix + ".txt", text);
+    }
+    return nodes.size();
+  }
+
+  // GraphManager::saveAllFeaturesToFile (graph_mgr_io.cpp:445-497) as OpenCV 4.13's cv::FileStorage writes it (YamlFileStorage):
+  // Feature_Locations, a sequence of flow maps {x, y, z}, one per feature of every node with valid_tf_estimate_ in id order --
+  // mapTransform cast to float applied to (x, y, z, 1) in float, each row ((c0 x + c1 y) + c2 z) + c3, non-finite values
+  // included --, then Feature_Descriptors, the descriptors of graph_[0], graph_[1], ... graph_[size - 1] looked up by key, as one
+  // CV_8U matrix of 32 columns; like the reference this includes the nodes whose locations were skipped.  The float chain
+  // assumes a build without FMA contraction (x86-64's default; add -ffp-contract=off to -mfma builds).  A name not ending in
+  // .yml / .yaml throws std::invalid_argument (XML, JSON and .gz storage are not built); an empty graph throws
+  // std::runtime_error (the reference asserts) and an id missing from [0, size) std::out_of_range (the reference crashes),
+  // before the file is opened.  Returns the number of feature locations written.
+  size_t saveAllFeatures(const std::string& filename) const {
+    if (!endsWith(filename, ".yml") && !endsWith(filename, ".yaml"))
+      throw std::invalid_argument("saveAllFeatures: only YAML storage (.yml / .yaml) is built");
+    if (graph_.empty()) throw std::runtime_error("saveAllFeatures: the graph is empty");
+    std::vector<uint8_t> desc;
+    for (int i = 0; i < (int)graph_.size(); i++) {
+      const std::vector<uint8_t>& d = graph_.at(i)->feature_descriptors_;
+      desc.insert(desc.end(), d.begin(), d.end());
+    }
+    YamlFileStorage fs;
+    fs.startSeq("Feature_Locations");
+    size_t count = 0;
+    for (auto& kv : graph_) {
+      const Node* n = kv.second;
+      if (!n->valid_tf_estimate_) continue;
+      double T[12];
+      mapTransform(n->vertex_id_, T);
+      float M[12];
+      for (int k = 0; k < 12; k++) M[k] = (float)T[k];
+      for (const Vector4f& loc : n->feature_locations_3d_) {
+        fs.startFlowMap();
+        fs.writeReal("x", ((M[0] * loc.x + M[1] * loc.y) + M[2] * loc.z) + M[3]);
+        fs.writeReal("y", ((M[4] * loc.x + M[5] * loc.y) + M[6] * loc.z) + M[7]);
+        fs.writeReal("z", ((M[8] * loc.x + M[9] * loc.y) + M[10] * loc.z) + M[11]);
+        fs.endStruct();
+        count++;
+      }
+    }
+    fs.endStruct();
+    fs.writeMatU8("Feature_Descriptors", desc.data(), (int)(desc.size() / 32), 32);
+    writeFile(filename, fs.release());
+    return count;
   }
 
   // parameters octomap_* (parameter_server.cpp:56-65) that ColorOctomapServer::reset and saveOctomapImpl read;
@@ -587,9 +723,7 @@ class GraphManager {
   // cloud; the cloud then records the estimate as its sensor pose (Node::cloud_sensor_pose_, cloudSensorPose).  (The
   // reference's function lacks its final `return true`; true is its evident intent.)
   bool updateCloudOrigin(const Node* node) const {
-    if (!node->valid_tf_estimate_ || !estimates_.count(node->vertex_id_)) return false;
-    int w = 0, h = 0;
-    if (rgbdslam_b200_node_download_cloud(node->handle(), 32, nullptr, &w, &h) != 0 || (long long)w * h == 0) return false;
+    if (!hasCloud(node)) return false;
     const Pose7& p = estimates_.at(node->vertex_id_);
     double R[9];
     quatToRot(p.v + 3, R);
@@ -700,14 +834,41 @@ class GraphManager {
       for (Node* n : nodes) n->clearPointCloud();
   }
 
-  static void tfMatrix(const double* q, double M[12]) {  // tf::Matrix3x3::setRotation, into the rotation part of a 3 x 4
-    const double x = q[0], y = q[1], z = q[2], w = q[3];
-    const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
-    const double xs = x * s, ys = y * s, zs = z * s, wx = w * xs, wy = w * ys, wz = w * zs;
-    const double xx = x * xs, xy = x * ys, xz = x * zs, yy = y * ys, yz = y * zs, zz = z * zs;
-    M[0] = 1.0 - (yy + zz), M[1] = xy - wz, M[2] = xz + wy;
-    M[4] = xy + wz, M[5] = 1.0 - (xx + zz), M[6] = yz - wx;
-    M[8] = xz - wy, M[9] = yz + wx, M[10] = 1.0 - (xx + yy);
+  // the test updateCloudOrigin and saveIndividualClouds share: valid_tf_estimate_, an estimate and a non-empty stored cloud
+  bool hasCloud(const Node* node) const {
+    if (!node->valid_tf_estimate_ || !estimates_.count(node->vertex_id_)) return false;
+    int w = 0, h = 0;
+    return rgbdslam_b200_node_download_cloud(node->handle(), 32, nullptr, &w, &h) == 0 && (long long)w * h != 0;
+  }
+
+  static bool endsWith(const std::string& name, const char* ext) {  // ext in lower case; the name's case does not matter
+    const size_t n = std::strlen(ext);
+    if (name.size() < n) return false;
+    for (size_t i = 0; i < n; i++)
+      if (std::tolower((unsigned char)name[name.size() - n + i]) != ext[i]) return false;
+    return true;
+  }
+  static void writeFile(const std::string& filename, const std::string& text) {
+    FILE* f = std::fopen(filename.c_str(), "wb");
+    if (!f) throw std::runtime_error("cannot open " + filename);
+    const bool ok = std::fwrite(text.data(), 1, text.size(), f) == text.size();
+    if (std::fclose(f) != 0 || !ok) throw std::runtime_error("cannot write " + filename);
+  }
+  // pcl::io::savePCDFile(filename, cloud, true) of PointXYZRGB records: a binary PCD v0.7 of fields x y z rgb (16 bytes per
+  // point), width x height, viewpoint ox oy oz qw qx qy qz as std::ostream writes floats
+  static void writePCD(const std::string& filename, const std::vector<PointXYZRGB>& pts, unsigned long long width,
+                       unsigned long long height, const float viewpoint[7]) {
+    std::string head =
+        "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z rgb\nSIZE 4 4 4 4\nTYPE F F F F\nCOUNT 1 1 1 1\n"
+        "WIDTH " + std::to_string(width) + "\nHEIGHT " + std::to_string(height) + "\nVIEWPOINT";
+    for (int k = 0; k < 7; k++) head += " " + ostreamFloat(viewpoint[k]);
+    head += "\nPOINTS " + std::to_string((unsigned long long)pts.size()) + "\nDATA binary\n";
+    std::string body(16 * pts.size(), '\0');
+    for (size_t i = 0; i < pts.size(); i++) {
+      std::memcpy(&body[16 * i], &pts[i].x, 12);
+      std::memcpy(&body[16 * i + 12], &pts[i].b, 4);
+    }
+    writeFile(filename, head + body);
   }
 
   struct Rand {  // rand() stand-in: the library's splitmix64 counter generator, stream 0xC0

@@ -3,8 +3,8 @@
  * nodes built with RGBDSLAM_B200_STORE_CLOUD (rgbdslam_b200_nodes_create_ex, ../rgbdslam_b200.h) and
  * GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583).  The conventions of ../rgbdslam_b200.h hold; both calls
  * need an initialised library.
- * The voxel filter of these clouds (Node::reducePointCloud) is declared in voxel.h; both calls read a reduced cloud as
- * they read any other.
+ * The voxel filter of these clouds (Node::reducePointCloud) is declared in voxel.h and their in-place transform
+ * (transform_individual_clouds) in cloud_transform.h; both calls read a reduced or transformed cloud as they read any other.
  */
 #ifndef RGBDSLAM_B200_MAP_H
 #define RGBDSLAM_B200_MAP_H

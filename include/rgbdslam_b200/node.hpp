@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "../rgbdslam_b200.h"
+#include "cloud_transform.h"
 #include "depth_resize.h"
 #include "icp.h"
 #include "map.h"

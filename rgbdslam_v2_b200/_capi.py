@@ -302,6 +302,7 @@ def load_library(path: str | Path | None = None) -> C.CDLL:
     lib.rgbdslam_b200_node_download_cloud.argtypes = [u64, C.c_int, vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     lib.rgbdslam_b200_render_cloud.argtypes = [C.c_int, vp, vp, C.c_double, C.c_int, C.c_int, vp, i64, C.POINTER(i64), vp]
     lib.rgbdslam_b200_reduce_clouds.argtypes = [C.c_int, vp, C.c_double, vp]
+    lib.rgbdslam_b200_transform_clouds.argtypes = [C.c_int, vp, vp]
     lib.rgbdslam_b200_icp_align.argtypes = [C.c_int, vp, vp, C.c_int, vp]
     lib.rgbdslam_b200_icp_align_ex.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp]
     lib.rgbdslam_b200_octomap_default_params.argtypes = [C.POINTER(OctomapParams)]
@@ -758,6 +759,14 @@ class Frontend:
         counts = np.zeros(len(hs), np.int32)
         self._check(self.lib.rgbdslam_b200_reduce_clouds(len(hs), _ptr(hs), float(voxelfilter_size), _ptr(counts)))
         return counts
+
+    def transform_clouds(self, nodes, transforms12):
+        """pcl::transformPointCloud of the nodes' stored clouds in place on the device (transform_individual_clouds):
+        transforms12 (n, 3, 4) float64, each cast to float; points with a non-finite coordinate stay.  The nodes keep the
+        transformed clouds for node_cloud, render_cloud, reduce_clouds and the OctoMap calls."""
+        hs = np.ascontiguousarray(np.asarray(nodes, np.uint64).reshape(-1))
+        T = np.ascontiguousarray(np.asarray(transforms12, np.float64).reshape(len(hs), 12))
+        self._check(self.lib.rgbdslam_b200_transform_clouds(len(hs), _ptr(hs), _ptr(T)))
 
     def icp_align(self, source_handles, target_handles, max_cloud_size: int = 10000, method: str = "icp") -> np.ndarray:
         """icpAlignment(filterCloud(source), filterCloud(target), Identity) of the nodes' stored clouds, pair by pair, on the

@@ -336,8 +336,8 @@ static int check_pairs(const std::vector<PairDesc>& h_pairs, int64_t first_pair,
     for (const PairDesc& pd : h_pairs)
       if (!pd.q_cloud.z || !pd.t_cloud.z) {
         set_error("observability_threshold > 0 needs nodes with a depth cloud (nodes_create or node_set_depth) that "
-                  "rgbdslam_b200_reduce_clouds has not voxel-filtered and rgbdslam_b200_octomap_filter_clouds has not left "
-                  "without a raster");
+                  "rgbdslam_b200_reduce_clouds has not voxel-filtered, rgbdslam_b200_octomap_filter_clouds has not left "
+                  "without a raster and rgbdslam_b200_transform_clouds has not moved into the map frame");
         return RGBDSLAM_B200_ERR_STATE;
       } else if (!pd.q_cloud.x != !pd.t_cloud.x) {
         // the reference never holds both kinds in one process (topic_points is global): there is no rule to restate
@@ -745,6 +745,10 @@ int rgbdslam_b200_observation_likelihood(uint64_t newer, uint64_t older, const f
   if (a->pc.unorganised || b->pc.unorganised) {
     set_error("observation_likelihood: a voxel-filtered (rgbdslam_b200_reduce_clouds) or occupancy-filtered "
               "(rgbdslam_b200_octomap_filter_clouds) cloud has no raster for the measurement model");
+    return RGBDSLAM_B200_ERR_STATE;
+  }
+  if (a->pc.transformed || b->pc.transformed) {
+    set_error("observation_likelihood: a cloud moved into the map frame (rgbdslam_b200_transform_clouds) holds no camera points");
     return RGBDSLAM_B200_ERR_STATE;
   }
   if (!a->pc.x != !b->pc.x) {

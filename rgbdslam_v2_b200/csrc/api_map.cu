@@ -3,6 +3,8 @@
 //   rgbdslam_b200_render_cloud         == transformAndAppendPointCloud (misc.cpp:183-238) of many nodes, the loop of
 //                                         GraphManager::saveAllCloudsToFile (graph_mgr_io.cpp:502-583)
 //   rgbdslam_b200_reduce_clouds        == Node::reducePointCloud (node.cpp:1448-1460) of many nodes (voxel.cu)
+//   rgbdslam_b200_transform_clouds     == pcl::transformPointCloud(*pc_col, *pc_col, m) of many nodes, the
+//                                         transform_individual_clouds step of saveIndividualCloudsToFile (graph_mgr_io.cpp:372-374)
 //   rgbdslam_b200_icp_align(_ex)       == icpAlignment(filterCloud(..), filterCloud(..)) (icp.cpp:20-89) of many pairs (icp.cu,
 //                                         icp_nl.cu)
 // The first two run count -> scan -> scatter (map.cu) and move the records to the host through a two-piece device staging
@@ -14,6 +16,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "../../include/rgbdslam_b200/cloud_transform.h"
 #include "../../include/rgbdslam_b200/icp.h"
 #include "../../include/rgbdslam_b200/map.h"
 #include "../../include/rgbdslam_b200/voxel.h"
@@ -28,6 +31,7 @@ struct MapCtx {
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_done[2] = {nullptr, nullptr}, ev_copied[2] = {nullptr, nullptr};
   DevBuf nodes, blocks, counts, offs, stage[2];
+  DevBuf first;  // transform_clouds: each node's first point in its chunk's slab
 };
 static MapCtx g_map;
 
@@ -269,6 +273,67 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
   return 0;
 }
 
+// ---- transform_individual_clouds -------------------------------------------------------------------------------------------
+
+constexpr long long kXfChunkPoints = 1 << 24;  // points of the nodes transformed together: one slab of 16 bytes per point
+
+// Transforms nodes [k0, k1) of the call, whose clouds hold `points` points in all, into one new slab and appends a CloudResult
+// per node.  The new planes keep the raster; a depth-image node's x / y are stored from now on.
+static int xf_chunk(const std::vector<NodeDev*>& nds, const double* transforms12, int k0, int k1, long long points,
+                    std::vector<CloudResult>& results, std::vector<NodeSlab*>& slabs) {
+  MapCtx& m = g_map;
+  State& s = g_state;
+  cudaStream_t st = s.stream;
+  const int nn = k1 - k0;
+  std::vector<MapNode> nodes(nn);
+  std::vector<long long> first(nn);
+  std::vector<int2> blocks;
+  long long pt = 0;
+  for (int k = 0; k < nn; k++) {
+    float T[12];  // Eigen's Matrix4d::cast<float>(): every double entry rounded to float
+    for (int j = 0; j < 12; j++) T[j] = (float)transforms12[(size_t)(k0 + k) * 12 + j];
+    nodes[k] = map_node(nds[k0 + k], T);
+    const int P = nodes[k].cw * nodes[k].ch;
+    first[k] = pt;
+    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2(k, f));
+    pt += P;
+  }
+  const int nb = (int)blocks.size();
+  int rc;
+  if ((rc = m.nodes.ensure(sizeof(MapNode) * nn)) || (rc = m.blocks.ensure(sizeof(int2) * std::max(nb, 1))) ||
+      (rc = m.first.ensure(sizeof(long long) * nn)))
+    return rc;
+  NodeSlab* slab = new NodeSlab();
+  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max(points, 1ll));
+  if (e != cudaSuccess) {
+    delete slab;
+    return cuda_fail(e, "cudaMalloc(transformed clouds)");
+  }
+  slabs.push_back(slab);
+  RB200_CUDA(cudaMemcpyAsync(m.nodes.ptr, nodes.data(), sizeof(MapNode) * nn, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(cudaMemcpyAsync(m.first.ptr, first.data(), sizeof(long long) * nn, cudaMemcpyHostToDevice, st));
+  if (nb > 0) RB200_CUDA(cudaMemcpyAsync(m.blocks.ptr, blocks.data(), sizeof(int2) * nb, cudaMemcpyHostToDevice, st));
+  RB200_CUDA(launch_transform_clouds((const MapNode*)m.nodes.ptr, (const int2*)m.blocks.ptr, nb, (const long long*)m.first.ptr,
+                                     (float*)slab->base, st));
+  RB200_CUDA(cudaStreamSynchronize(st));  // the work buffers are the next chunk's
+  s.launches += nb > 0;
+  for (int k = 0; k < nn; k++) {
+    NodeDev* nd = nds[k0 + k];
+    CloudResult r{nd, nd->pc};
+    const long long P = (long long)nodes[k].cw * nodes[k].ch;
+    r.pc.x = (float*)slab->base + 4 * first[k];
+    r.pc.y = r.pc.x + P;
+    r.pc.z = r.pc.y + P;
+    r.pc.rgb = (uint32_t*)(r.pc.z + P);
+    r.pc.step = 0;
+    r.pc.slab = slab;
+    r.pc.point0_one = nd->pc.step > 0 || nd->pc.point0_one;
+    r.pc.transformed = true;
+    results.push_back(r);
+  }
+  return 0;
+}
+
 // ---- the ICP fallback of matchNodePair -------------------------------------------------------------------------------------
 
 constexpr long long kIcpChunkPoints = 1 << 24;  // raster points of the nodes one filter launch treats: 4 bytes of scratch each
@@ -478,6 +543,50 @@ int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter
   return 0;
 }
 
+int rgbdslam_b200_transform_clouds(int n, const uint64_t* nodes, const double* transforms12) {
+  RB200_ENTER_INITED();
+  if (n < 0 || (n > 0 && (!nodes || !transforms12))) {
+    set_error("transform_clouds: n >= 0 and non-null nodes and transforms are needed");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  for (size_t i = 0; i < (size_t)n * 12; i++)
+    if (!std::isfinite(transforms12[i])) {
+      set_error("transform_clouds: transform " + std::to_string(i / 12) + " has a non-finite entry");
+      return RGBDSLAM_B200_ERR_ARG;
+    }
+  std::vector<NodeDev*> nds(n);
+  for (int k = 0; k < n; k++) {
+    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
+    if (!nds[k]->pc.rgb) {
+      set_error("transform_clouds: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    }
+  }
+  std::vector<uint64_t> sorted(nodes, nodes + n);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
+    set_error("transform_clouds: a node is listed twice");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  std::vector<CloudResult> results;
+  std::vector<NodeSlab*> slabs;
+  int rc = 0;
+  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
+    int k1 = k0;
+    long long points = 0;
+    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
+    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= kXfChunkPoints);
+    rc = xf_chunk(nds, transforms12, k0, k1, points, results, slabs);
+    k0 = k1;
+  }
+  if (rc) {  // no node is changed
+    drop_slabs(slabs);
+    return rc;
+  }
+  adopt_clouds(results, slabs);
+  return 0;
+}
+
 int rgbdslam_b200_icp_align(int n, const uint64_t* source, const uint64_t* target, int max_cloud_size,
                             rgbdslam_b200_icp_result* out) {
   return rgbdslam_b200_icp_align_ex(n, source, target, max_cloud_size, RGBDSLAM_B200_ICP_METHOD_ICP, out);
@@ -515,6 +624,9 @@ int rgbdslam_b200_icp_align_ex(int n, const uint64_t* source, const uint64_t* ta
   for (size_t u = 0; u < nds.size(); u++)
     if (!nds[u]->pc.z) {
       set_error("icp_align: a node has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD or KEEP_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    } else if (nds[u]->pc.transformed) {
+      set_error("icp_align: a cloud moved into the map frame (rgbdslam_b200_transform_clouds) holds no camera points");
       return RGBDSLAM_B200_ERR_STATE;
     }
   if (n == 0) return 0;

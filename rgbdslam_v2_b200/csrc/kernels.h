@@ -65,6 +65,10 @@ cudaError_t launch_map_count(const MapNode* d_nodes, const int2* d_blocks, int n
 cudaError_t launch_map_scan(const int* d_counts, int nblocks, long long* d_offs, cudaStream_t st);
 cudaError_t launch_map_scatter(const MapNode* d_nodes, const int2* d_blocks, const long long* d_offs, int b0, int b1, long long lo,
                                long long hi, const MapArgs& a, void* d_out, cudaStream_t st);
+// pcl::transformPointCloud of the stored clouds of a chunk of nodes (rgbdslam_b200_transform_clouds), each by its MapNode::m:
+// node k's new planes [x | y | z | colour] of P_k points each start at word 4 * d_first[k] of slab
+cudaError_t launch_transform_clouds(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const long long* d_first, float* slab,
+                                    cudaStream_t st);
 // The voxel filter of the stored clouds, Node::reducePointCloud (voxel.cu).  A call works on a chunk of whole nodes whose
 // points lie back to back in the work buffers; the (node, first point) block table is the map's.
 struct VoxSeg {        // one node of the chunk

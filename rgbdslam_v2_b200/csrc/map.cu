@@ -8,6 +8,8 @@
 //   k_map_count           transformAndAppendPointCloud (misc.cpp:183-238): the points each 1024-point block keeps
 //   k_map_scan            exclusive scan of the block counts (output offsets, in node order then raster order)
 //   k_map_scatter         the kept points of the blocks that overlap one staging piece, transformed, as PCL records
+//   k_transform_clouds    pcl::transformPointCloud (PCL 1.7) of every stored point into new x / y / z / colour planes
+//                         (transform_individual_clouds, graph_mgr_io.cpp:372-374)
 // The float point chain is written with explicit _rn intrinsics: nvcc would otherwise contract it into FMAs, which the
 // reference (x86-64 without -mfma) does not do.
 #include "kernels.h"
@@ -189,6 +191,45 @@ __global__ void __launch_bounds__(kMapThreads) k_map_scatter(const MapNode* __re
     next += total;
     __syncthreads();
   }
+}
+
+// Every point of the blocks, read as stored; a point whose x, y and z are all finite becomes ((m0 x + m1 y) + m2 z) + m3 per
+// row (Eigen's Affine3f * Vector3f, no FMA), any other is left as it is -- PCL 1.7's test for a cloud that is not dense, stricter
+// than transformAndAppendPointCloud's NaN test: +-inf stays.  The colour word is copied; data[3] follows from point0_one.
+__global__ void __launch_bounds__(kMapThreads) k_transform_clouds(const MapNode* __restrict__ nodes, const int2* __restrict__ blocks,
+                                                                  const long long* __restrict__ first, float* __restrict__ slab) {
+  const int2 blk = blocks[blockIdx.x];
+  const MapNode& nd = nodes[blk.x];
+  const int P = nd.cw * nd.ch;
+  float* x = slab + 4 * first[blk.x];
+  float* y = x + P;
+  float* z = y + P;
+  uint32_t* rgb = reinterpret_cast<uint32_t*>(z + P);
+  const MapArgs as_stored{0.f, 0, 1, 0, 32};
+#pragma unroll
+  for (int k = 0; k < kMapBlockPoints / kMapThreads; k++) {
+    const int i = blk.y + k * kMapThreads + threadIdx.x;
+    if (i >= P) continue;
+    MapOut o;
+    map_point(nd, i, as_stored, o);
+    if (isfinite(o.x) && isfinite(o.y) && isfinite(o.z)) {
+      const float px = o.x, py = o.y, pz = o.z;
+      o.x = __fadd_rn(dot3_map(nd.m[0], px, nd.m[1], py, nd.m[2], pz), nd.m[3]);
+      o.y = __fadd_rn(dot3_map(nd.m[4], px, nd.m[5], py, nd.m[6], pz), nd.m[7]);
+      o.z = __fadd_rn(dot3_map(nd.m[8], px, nd.m[9], py, nd.m[10], pz), nd.m[11]);
+    }
+    x[i] = o.x;
+    y[i] = o.y;
+    z[i] = o.z;
+    rgb[i] = o.rgb;
+  }
+}
+
+cudaError_t launch_transform_clouds(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const long long* d_first, float* slab,
+                                    cudaStream_t st) {
+  if (nblocks <= 0) return cudaSuccess;
+  k_transform_clouds<<<nblocks, kMapThreads, 0, st>>>(d_nodes, d_blocks, d_first, slab);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_map_count(const MapNode* d_nodes, const int2* d_blocks, int nblocks, const MapArgs& a, int* d_counts,
