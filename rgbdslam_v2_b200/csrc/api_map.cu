@@ -68,7 +68,45 @@ MapNode map_node(const NodeDev* nd, const float* T) {
   return m;
 }
 
-void adopt_clouds(const std::vector<CloudResult>& results, const std::vector<NodeSlab*>& slabs) {
+int stored_cloud_nodes(const char* call, int n, const uint64_t* handles, bool distinct, std::vector<NodeDev*>* nds) {
+  nds->resize(n);
+  for (int k = 0; k < n; k++) {
+    if (!((*nds)[k] = get_node(handles[k]))) return RGBDSLAM_B200_ERR_ARG;
+    if (!(*nds)[k]->pc.rgb) {
+      set_error(std::string(call) + ": node " + std::to_string(k) +
+                " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
+      return RGBDSLAM_B200_ERR_STATE;
+    }
+  }
+  if (!distinct) return 0;
+  std::vector<uint64_t> sorted(handles, handles + n);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
+    set_error(std::string(call) + ": a node is listed twice");
+    return RGBDSLAM_B200_ERR_ARG;
+  }
+  return 0;
+}
+
+std::vector<int2> map_blocks(const std::vector<MapNode>& nodes, std::vector<int>* first) {
+  std::vector<int2> blocks;
+  if (first) first->resize(nodes.size() + 1);
+  for (size_t k = 0; k < nodes.size(); k++) {
+    if (first) (*first)[k] = (int)blocks.size();
+    const int P = nodes[k].cw * nodes[k].ch;
+    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2((int)k, f));
+  }
+  if (first) first->back() = (int)blocks.size();
+  return blocks;
+}
+
+long long chunk_limit(long long limit, const char* env_name) {
+  const char* env = std::getenv(env_name);
+  return env ? std::max(1ll, std::atoll(env)) : limit;
+}
+
+// Each node takes its new cloud and lets go of its old allocation; slabs no node took are freed.
+static void adopt_clouds(const std::vector<CloudResult>& results, const std::vector<NodeSlab*>& slabs) {
   for (const CloudResult& r : results) {
     release_slab(r.nd->pc.slab);
     r.nd->pc = r.pc;
@@ -81,12 +119,57 @@ void adopt_clouds(const std::vector<CloudResult>& results, const std::vector<Nod
     }
 }
 
-void drop_slabs(const std::vector<NodeSlab*>& slabs) {
+// After a failure: frees the call's new slabs (after the stream has drained).
+static void drop_slabs(const std::vector<NodeSlab*>& slabs) {
   cudaStreamSynchronize(g_state.stream);
   for (NodeSlab* sl : slabs) {
     cudaFree(sl->base);
     delete sl;
   }
+}
+
+int rebuild_clouds(const std::vector<NodeDev*>& nds, long long limit, const CloudChunk& chunk) {
+  const int n = (int)nds.size();
+  std::vector<CloudResult> results;
+  std::vector<NodeSlab*> slabs;
+  int rc = 0;
+  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
+    int k1 = k0;
+    long long points = 0;
+    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
+    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= limit);
+    rc = chunk(k0, k1, points, results, slabs);
+    k0 = k1;
+  }
+  if (rc) {  // no node is changed
+    drop_slabs(slabs);
+    return rc;
+  }
+  adopt_clouds(results, slabs);
+  return 0;
+}
+
+NodeSlab* new_slab(long long points, const char* what, std::vector<NodeSlab*>& slabs) {
+  NodeSlab* slab = new NodeSlab();
+  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max(points, 1ll));
+  if (e != cudaSuccess) {
+    delete slab;
+    cuda_fail(e, what);
+    return nullptr;
+  }
+  slabs.push_back(slab);
+  return slab;
+}
+
+NodeCloud slab_cloud(const NodeCloud& c, NodeSlab* slab, long long first, long long count) {
+  NodeCloud r = c;
+  r.x = (float*)slab->base + 4 * first;
+  r.y = r.x + count;
+  r.z = r.y + count;
+  r.rgb = (uint32_t*)(r.z + count);
+  r.step = 0;
+  r.slab = slab;
+  return r;
 }
 
 // Count, scan and (unless out is NULL) scatter the records of `nodes` into the host buffer out (capacity records).
@@ -96,11 +179,7 @@ static int map_emit(const std::vector<MapNode>& nodes, const MapArgs& a, void* o
   cudaStream_t st = s.stream;
   int rc;
   if ((rc = map_ensure_streams())) return rc;
-  std::vector<int2> blocks;
-  for (size_t k = 0; k < nodes.size(); k++) {
-    const int P = nodes[k].cw * nodes[k].ch;
-    for (int first = 0; first < P; first += kMapBlockPoints) blocks.push_back(make_int2((int)k, first));
-  }
+  const std::vector<int2> blocks = map_blocks(nodes, nullptr);
   const int nb = (int)blocks.size();
   std::vector<long long> offs(nb + 1);
   if ((rc = m.nodes.ensure(sizeof(MapNode) * std::max<size_t>(nodes.size(), 1))) ||
@@ -180,17 +259,13 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
   cudaStream_t st = s.stream;
   const int nn = k1 - k0;
   std::vector<MapNode> nodes(nn);
+  for (int k = 0; k < nn; k++) nodes[k] = map_node(nds[k0 + k], nullptr);
+  std::vector<int> first_block;
+  const std::vector<int2> blocks = map_blocks(nodes, &first_block);
   std::vector<VoxSeg> segs(nn);
-  std::vector<int2> blocks;
-  int pt = 0;
-  for (int k = 0; k < nn; k++) {
-    nodes[k] = map_node(nds[k0 + k], nullptr);
+  for (int k = 0, pt = 0; k < nn; k++) {
     const int P = nodes[k].cw * nodes[k].ch;
-    segs[k].pt0 = pt;
-    segs[k].npts = P;
-    segs[k].blk0 = (int)blocks.size();
-    for (int first = 0; first < P; first += kMapBlockPoints) blocks.push_back(make_int2(k, first));
-    segs[k].nblk = (int)blocks.size() - segs[k].blk0;
+    segs[k] = VoxSeg{pt, P, first_block[k], first_block[k + 1] - first_block[k]};
     pt += P;
   }
   const int nb = (int)blocks.size();
@@ -240,13 +315,8 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
   RB200_CUDA(cudaStreamSynchronize(st));
   s.launches += launches;
   const long long nvox = offs[nb];
-  NodeSlab* slab = new NodeSlab();
-  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max<long long>(nvox, 1));
-  if (e != cudaSuccess) {
-    delete slab;
-    return cuda_fail(e, "cudaMalloc(reduced clouds)");
-  }
-  slabs.push_back(slab);
+  NodeSlab* slab = new_slab(nvox, "cudaMalloc(reduced clouds)", slabs);
+  if (!slab) return RGBDSLAM_B200_ERR_CUDA;
   RB200_CUDA(launch_vox_centroids(b, passes, nvox, (float*)slab->base, st));
   RB200_CUDA(cudaStreamSynchronize(st));  // the work buffers are the next chunk's
   s.launches += nvox > 0;
@@ -255,16 +325,10 @@ static int vox_chunk(VoxCtx& v, const std::vector<NodeDev*>& nds, int k0, int k1
       n_points[k0 + k] = -1;
       continue;
     }
-    const long long first = offs[segs[k].blk0], count = offs[segs[k].blk0 + segs[k].nblk] - first;
-    CloudResult r{nds[k0 + k], nds[k0 + k]->pc};
-    r.pc.x = (float*)slab->base + 4 * first;
-    r.pc.y = r.pc.x + count;
-    r.pc.z = r.pc.y + count;
-    r.pc.rgb = (uint32_t*)(r.pc.z + count);
+    const long long first = offs[first_block[k]], count = offs[first_block[k + 1]] - first;
+    CloudResult r{nds[k0 + k], slab_cloud(nds[k0 + k]->pc, slab, first, count)};
     r.pc.w = (int32_t)count;
     r.pc.h = 1;
-    r.pc.step = 0;
-    r.pc.slab = slab;
     r.pc.unorganised = true;
     r.pc.point0_one = false;
     results.push_back(r);
@@ -287,29 +351,22 @@ static int xf_chunk(const std::vector<NodeDev*>& nds, const double* transforms12
   const int nn = k1 - k0;
   std::vector<MapNode> nodes(nn);
   std::vector<long long> first(nn);
-  std::vector<int2> blocks;
   long long pt = 0;
   for (int k = 0; k < nn; k++) {
     float T[12];  // Eigen's Matrix4d::cast<float>(): every double entry rounded to float
     for (int j = 0; j < 12; j++) T[j] = (float)transforms12[(size_t)(k0 + k) * 12 + j];
     nodes[k] = map_node(nds[k0 + k], T);
-    const int P = nodes[k].cw * nodes[k].ch;
     first[k] = pt;
-    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2(k, f));
-    pt += P;
+    pt += nodes[k].cw * nodes[k].ch;
   }
+  const std::vector<int2> blocks = map_blocks(nodes, nullptr);
   const int nb = (int)blocks.size();
   int rc;
   if ((rc = m.nodes.ensure(sizeof(MapNode) * nn)) || (rc = m.blocks.ensure(sizeof(int2) * std::max(nb, 1))) ||
       (rc = m.first.ensure(sizeof(long long) * nn)))
     return rc;
-  NodeSlab* slab = new NodeSlab();
-  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max(points, 1ll));
-  if (e != cudaSuccess) {
-    delete slab;
-    return cuda_fail(e, "cudaMalloc(transformed clouds)");
-  }
-  slabs.push_back(slab);
+  NodeSlab* slab = new_slab(points, "cudaMalloc(transformed clouds)", slabs);
+  if (!slab) return RGBDSLAM_B200_ERR_CUDA;
   RB200_CUDA(cudaMemcpyAsync(m.nodes.ptr, nodes.data(), sizeof(MapNode) * nn, cudaMemcpyHostToDevice, st));
   RB200_CUDA(cudaMemcpyAsync(m.first.ptr, first.data(), sizeof(long long) * nn, cudaMemcpyHostToDevice, st));
   if (nb > 0) RB200_CUDA(cudaMemcpyAsync(m.blocks.ptr, blocks.data(), sizeof(int2) * nb, cudaMemcpyHostToDevice, st));
@@ -319,14 +376,7 @@ static int xf_chunk(const std::vector<NodeDev*>& nds, const double* transforms12
   s.launches += nb > 0;
   for (int k = 0; k < nn; k++) {
     NodeDev* nd = nds[k0 + k];
-    CloudResult r{nd, nd->pc};
-    const long long P = (long long)nodes[k].cw * nodes[k].ch;
-    r.pc.x = (float*)slab->base + 4 * first[k];
-    r.pc.y = r.pc.x + P;
-    r.pc.z = r.pc.y + P;
-    r.pc.rgb = (uint32_t*)(r.pc.z + P);
-    r.pc.step = 0;
-    r.pc.slab = slab;
+    CloudResult r{nd, slab_cloud(nd->pc, slab, first[k], (long long)nodes[k].cw * nodes[k].ch)};
     r.pc.point0_one = nd->pc.step > 0 || nd->pc.point0_one;
     r.pc.transformed = true;
     results.push_back(r);
@@ -466,22 +516,16 @@ int rgbdslam_b200_render_cloud(int n, const uint64_t* nodes, const double* trans
     set_error("render_cloud: point_bytes must be 16 (PointXYZ) or 32 (PointXYZRGB)");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  for (size_t i = 0; i < (size_t)n * 12; i++)
-    if (!std::isfinite(transforms12[i])) {
-      set_error("render_cloud: transform " + std::to_string(i / 12) + " has a non-finite entry");
-      return RGBDSLAM_B200_ERR_ARG;
-    }
+  std::vector<NodeDev*> nds;
+  int rc;
+  if ((rc = check_finite("render_cloud", "transform", n, 12, transforms12)) ||
+      (rc = stored_cloud_nodes("render_cloud", n, nodes, false, &nds)))
+    return rc;
   std::vector<MapNode> table(n);
   for (int k = 0; k < n; k++) {
-    NodeDev* nd = get_node(nodes[k]);
-    if (!nd) return RGBDSLAM_B200_ERR_ARG;
-    if (!nd->pc.rgb) {
-      set_error("render_cloud: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
-      return RGBDSLAM_B200_ERR_STATE;
-    }
     float T[12];  // pcl_ros::transformAsMatrix: every double entry of the tf::Transform cast to float
     for (int j = 0; j < 12; j++) T[j] = (float)transforms12[(size_t)k * 12 + j];
-    table[k] = map_node(nd, T);
+    table[k] = map_node(nds[k], T);
     if (used16) {  // Eigen::Matrix4f, column-major
       float* M = used16 + (size_t)k * 16;
       for (int r = 0; r < 3; r++)
@@ -503,42 +547,18 @@ int rgbdslam_b200_reduce_clouds(int n, const uint64_t* nodes, double voxelfilter
     set_error("reduce_clouds: n >= 0, nodes non-null and a finite voxelfilter_size > 0 (as a float) are needed");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  std::vector<NodeDev*> nds(n);
-  for (int k = 0; k < n; k++) {
-    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
-    if (!nds[k]->pc.rgb) {
-      set_error("reduce_clouds: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
-      return RGBDSLAM_B200_ERR_STATE;
-    }
-  }
-  std::vector<uint64_t> sorted(nodes, nodes + n);
-  std::sort(sorted.begin(), sorted.end());
-  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
-    set_error("reduce_clouds: a node is listed twice");
-    return RGBDSLAM_B200_ERR_ARG;
-  }
-  long long limit = kVoxChunkPoints;
-  if (const char* env = std::getenv("RB200_VOX_CHUNK_POINTS")) limit = std::max(1ll, std::atoll(env));
+  std::vector<NodeDev*> nds;
+  int rc;
+  if ((rc = stored_cloud_nodes("reduce_clouds", n, nodes, true, &nds))) return rc;
   const float inv_leaf = 1.0f / leaf;
   std::vector<int32_t> counts(n);
-  std::vector<CloudResult> results;
-  std::vector<NodeSlab*> slabs;
   VoxCtx v;
-  int rc = 0;
-  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
-    int k1 = k0;
-    long long points = 0;
-    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
-    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= limit);
-    rc = vox_chunk(v, nds, k0, k1, points, inv_leaf, results, slabs, counts.data());
-    k0 = k1;
-  }
+  rc = rebuild_clouds(nds, chunk_limit(kVoxChunkPoints, "RB200_VOX_CHUNK_POINTS"),
+                      [&](int k0, int k1, long long points, auto& results, auto& slabs) {
+                        return vox_chunk(v, nds, k0, k1, points, inv_leaf, results, slabs, counts.data());
+                      });
   v.release();
-  if (rc) {  // no node is changed
-    drop_slabs(slabs);
-    return rc;
-  }
-  adopt_clouds(results, slabs);
+  if (rc) return rc;
   if (n_points) std::copy(counts.begin(), counts.end(), n_points);
   return 0;
 }
@@ -549,42 +569,14 @@ int rgbdslam_b200_transform_clouds(int n, const uint64_t* nodes, const double* t
     set_error("transform_clouds: n >= 0 and non-null nodes and transforms are needed");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  for (size_t i = 0; i < (size_t)n * 12; i++)
-    if (!std::isfinite(transforms12[i])) {
-      set_error("transform_clouds: transform " + std::to_string(i / 12) + " has a non-finite entry");
-      return RGBDSLAM_B200_ERR_ARG;
-    }
-  std::vector<NodeDev*> nds(n);
-  for (int k = 0; k < n; k++) {
-    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
-    if (!nds[k]->pc.rgb) {
-      set_error("transform_clouds: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
-      return RGBDSLAM_B200_ERR_STATE;
-    }
-  }
-  std::vector<uint64_t> sorted(nodes, nodes + n);
-  std::sort(sorted.begin(), sorted.end());
-  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
-    set_error("transform_clouds: a node is listed twice");
-    return RGBDSLAM_B200_ERR_ARG;
-  }
-  std::vector<CloudResult> results;
-  std::vector<NodeSlab*> slabs;
-  int rc = 0;
-  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
-    int k1 = k0;
-    long long points = 0;
-    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
-    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= kXfChunkPoints);
-    rc = xf_chunk(nds, transforms12, k0, k1, points, results, slabs);
-    k0 = k1;
-  }
-  if (rc) {  // no node is changed
-    drop_slabs(slabs);
+  std::vector<NodeDev*> nds;
+  int rc;
+  if ((rc = check_finite("transform_clouds", "transform", n, 12, transforms12)) ||
+      (rc = stored_cloud_nodes("transform_clouds", n, nodes, true, &nds)))
     return rc;
-  }
-  adopt_clouds(results, slabs);
-  return 0;
+  return rebuild_clouds(nds, kXfChunkPoints, [&](int k0, int k1, long long points, auto& results, auto& slabs) {
+    return xf_chunk(nds, transforms12, k0, k1, points, results, slabs);
+  });
 }
 
 int rgbdslam_b200_icp_align(int n, const uint64_t* source, const uint64_t* target, int max_cloud_size,

@@ -7,7 +7,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <unordered_map>
@@ -156,14 +155,8 @@ static int oct_insert(OctoMap& m, const std::vector<MapNode>& table) {
   State& s = g_state;
   cudaStream_t st = s.stream;
   const int n = (int)table.size();
-  std::vector<int2> blocks;
-  std::vector<int> first_block(n + 1);
-  for (int k = 0; k < n; k++) {
-    first_block[k] = (int)blocks.size();
-    const int P = table[k].cw * table[k].ch;
-    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2(k, f));
-  }
-  first_block[n] = (int)blocks.size();
+  std::vector<int> first_block;
+  const std::vector<int2> blocks = map_blocks(table, &first_block);
   const int nb = (int)blocks.size();
   if (nb == 0) return 0;
   int rc;
@@ -178,8 +171,7 @@ static int oct_insert(OctoMap& m, const std::vector<MapNode>& table) {
   RB200_CUDA(cudaMemcpyAsync(counts.data(), m.counts.ptr, 4 * (size_t)nb, cudaMemcpyDeviceToHost, st));
   RB200_CUDA(cudaStreamSynchronize(st));
   s.launches += 1;
-  long long limit = kOctBatchEntries;
-  if (const char* env = std::getenv("RB200_OCT_BATCH_ENTRIES")) limit = std::max(1ll, std::atoll(env));
+  const long long limit = chunk_limit(kOctBatchEntries, "RB200_OCT_BATCH_ENTRIES");
   // batches of whole nodes, at least one, in order
   for (int k0 = 0; k0 < n;) {
     long long E = 0;
@@ -239,16 +231,10 @@ static int ocf_chunk(OctoMap& m, const std::vector<NodeDev*>& nds, const float* 
   cudaStream_t st = s.stream;
   const int nn = k1 - k0;
   std::vector<MapNode> nodes(nn);
-  std::vector<int2> blocks;
-  std::vector<int> blk0(nn + 1);
-  for (int k = 0; k < nn; k++) {
-    nodes[k] = map_node(nds[k0 + k], nullptr);
-    blk0[k] = (int)blocks.size();
-    const int P = nodes[k].cw * nodes[k].ch;
-    for (int f = 0; f < P; f += kMapBlockPoints) blocks.push_back(make_int2(k, f));
-  }
+  for (int k = 0; k < nn; k++) nodes[k] = map_node(nds[k0 + k], nullptr);
+  std::vector<int> first_block;
+  const std::vector<int2> blocks = map_blocks(nodes, &first_block);
   const int nb = (int)blocks.size();
-  blk0[nn] = nb;
   int rc;
   if ((rc = m.nodes.ensure(sizeof(MapNode) * nn)) || (rc = m.blocks.ensure(sizeof(int2) * std::max(nb, 1))) ||
       (rc = m.counts.ensure(4 * (size_t)std::max(nb, 1))) || (rc = m.offs.ensure(8 * ((size_t)nb + 1))) ||
@@ -272,20 +258,15 @@ static int ocf_chunk(OctoMap& m, const std::vector<NodeDev*>& nds, const float* 
   std::vector<OcfOut> out(nn);
   long long dst = 0;
   for (int k = 0; k < nn; k++) {
-    const long long first = offs[blk0[k]], count = offs[blk0[k + 1]] - first;
+    const long long first = offs[first_block[k]], count = offs[first_block[k + 1]] - first;
     const bool changed = count < (long long)nodes[k].cw * nodes[k].ch;
     out[k] = OcfOut{changed ? dst : -1, first, count};
     if (changed) dst += count;
     n_points[k0 + k] = (int32_t)count;
   }
   if (std::none_of(out.begin(), out.end(), [](const OcfOut& o) { return o.dst >= 0; })) return 0;
-  NodeSlab* slab = new NodeSlab();
-  cudaError_t e = cudaMalloc(&slab->base, 16 * (size_t)std::max(dst, 1ll));
-  if (e != cudaSuccess) {
-    delete slab;
-    return cuda_fail(e, "cudaMalloc(occupancy-filtered clouds)");
-  }
-  slabs.push_back(slab);
+  NodeSlab* slab = new_slab(dst, "cudaMalloc(occupancy-filtered clouds)", slabs);
+  if (!slab) return RGBDSLAM_B200_ERR_CUDA;
   RB200_CUDA(cudaMemcpyAsync(m.outs.ptr, out.data(), sizeof(OcfOut) * nn, cudaMemcpyHostToDevice, st));
   RB200_CUDA(launch_ocf_scatter((const MapNode*)m.nodes.ptr, (const int2*)m.blocks.ptr, nb, (const uint8_t*)m.pflags.ptr,
                                 (const long long*)m.offs.ptr, (const OcfOut*)m.outs.ptr, (float*)slab->base, st));
@@ -294,16 +275,9 @@ static int ocf_chunk(OctoMap& m, const std::vector<NodeDev*>& nds, const float* 
   for (int k = 0; k < nn; k++) {
     if (out[k].dst < 0) continue;
     NodeDev* nd = nds[k0 + k];
-    CloudResult r{nd, nd->pc};
-    const long long c = out[k].count;
-    r.pc.x = (float*)slab->base + 4 * out[k].dst;
-    r.pc.y = r.pc.x + c;
-    r.pc.z = r.pc.y + c;
-    r.pc.rgb = (uint32_t*)(r.pc.z + c);
-    r.pc.w = (int32_t)c;
+    CloudResult r{nd, slab_cloud(nd->pc, slab, out[k].dst, out[k].count)};
+    r.pc.w = (int32_t)out[k].count;
     r.pc.h = 1;
-    r.pc.step = 0;
-    r.pc.slab = slab;
     r.pc.unorganised = true;
     r.pc.point0_one = (nd->pc.step > 0 || nd->pc.point0_one) && keep0[k];  // the kept point 0 stays point 0
     results.push_back(r);
@@ -408,21 +382,13 @@ int rgbdslam_b200_octomap_insert(uint64_t map, int n, const uint64_t* nodes, con
     set_error("octomap_insert: n >= 0, non-null nodes and transforms and a max_range that is not NaN are needed");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  for (size_t i = 0; i < (size_t)n * 12; i++)
-    if (!std::isfinite(transforms12[i])) {
-      set_error("octomap_insert: transform " + std::to_string(i / 12) + " has a non-finite entry");
-      return RGBDSLAM_B200_ERR_ARG;
-    }
+  std::vector<NodeDev*> nds;
+  int rc;
+  if ((rc = check_finite("octomap_insert", "transform", n, 12, transforms12)) ||
+      (rc = stored_cloud_nodes("octomap_insert", n, nodes, false, &nds)))
+    return rc;
   std::vector<MapNode> table(n);
-  for (int k = 0; k < n; k++) {
-    NodeDev* nd = get_node(nodes[k]);
-    if (!nd) return RGBDSLAM_B200_ERR_ARG;
-    if (!nd->pc.rgb) {
-      set_error("octomap_insert: node " + std::to_string(k) + " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
-      return RGBDSLAM_B200_ERR_STATE;
-    }
-    table[k] = map_node(nd, transforms12 + (size_t)k * 12);
-  }
+  for (int k = 0; k < n; k++) table[k] = map_node(nds[k], transforms12 + (size_t)k * 12);
   m->a.max_range = max_range;
   m->occ_ok = false;
   return oct_insert(*m, table);
@@ -437,49 +403,21 @@ int rgbdslam_b200_octomap_filter_clouds(uint64_t map, int n, const uint64_t* nod
     set_error("octomap_filter_clouds: n >= 0, non-null nodes and sensor poses and a threshold that is not NaN are needed");
     return RGBDSLAM_B200_ERR_ARG;
   }
-  for (size_t i = 0; i < (size_t)n * 7; i++)
-    if (!std::isfinite(sensor7[i])) {
-      set_error("octomap_filter_clouds: sensor pose " + std::to_string(i / 7) + " has a non-finite entry");
-      return RGBDSLAM_B200_ERR_ARG;
-    }
-  std::vector<NodeDev*> nds(n);
-  for (int k = 0; k < n; k++) {
-    if (!(nds[k] = get_node(nodes[k]))) return RGBDSLAM_B200_ERR_ARG;
-    if (!nds[k]->pc.rgb) {
-      set_error("octomap_filter_clouds: node " + std::to_string(k) +
-                " has no stored cloud (nodes_create_ex with RGBDSLAM_B200_STORE_CLOUD)");
-      return RGBDSLAM_B200_ERR_STATE;
-    }
-  }
-  std::vector<uint64_t> sorted(nodes, nodes + n);
-  std::sort(sorted.begin(), sorted.end());
-  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) {
-    set_error("octomap_filter_clouds: a node is listed twice");
-    return RGBDSLAM_B200_ERR_ARG;
-  }
-  if (n == 0) return 0;
+  std::vector<NodeDev*> nds;
   int rc;
+  if ((rc = check_finite("octomap_filter_clouds", "sensor pose", n, 7, sensor7)) ||
+      (rc = stored_cloud_nodes("octomap_filter_clouds", n, nodes, true, &nds)))
+    return rc;
+  if (n == 0) return 0;
   if ((rc = oct_occupancy(*m))) return rc;
   const OcfArgs a{m->p.resolution, m->a.rf, occupancy_threshold, (const unsigned long long*)m->lk[m->cur].ptr, (const double*)m->occ.ptr,
                   m->nleaves};
-  long long limit = kOcfChunkPoints;
-  if (const char* env = std::getenv("RB200_OCF_CHUNK_POINTS")) limit = std::max(1ll, std::atoll(env));
   std::vector<int32_t> counts(n);
-  std::vector<CloudResult> results;
-  std::vector<NodeSlab*> slabs;
-  for (int k0 = 0; k0 < n && rc == 0;) {  // chunks of whole nodes, at least one
-    int k1 = k0;
-    long long points = 0;
-    do points += (long long)nds[k1]->pc.w * nds[k1]->pc.h;
-    while (++k1 < n && points + (long long)nds[k1]->pc.w * nds[k1]->pc.h <= limit);
-    rc = ocf_chunk(*m, nds, sensor7, k0, k1, a, results, slabs, counts.data());
-    k0 = k1;
-  }
-  if (rc) {  // no node is changed
-    drop_slabs(slabs);
-    return rc;
-  }
-  adopt_clouds(results, slabs);
+  rc = rebuild_clouds(nds, chunk_limit(kOcfChunkPoints, "RB200_OCF_CHUNK_POINTS"),
+                      [&](int k0, int k1, long long, auto& results, auto& slabs) {
+                        return ocf_chunk(*m, nds, sensor7, k0, k1, a, results, slabs, counts.data());
+                      });
+  if (rc) return rc;
   if (n_points) std::copy(counts.begin(), counts.end(), n_points);
   return 0;
 }

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cmath>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -73,16 +75,22 @@ struct NodeDev {
 };
 
 // A new cloud that is not yet its node's: a call that rebuilds clouds (reduce_clouds, octomap_filter_clouds, transform_clouds)
-// hands them over
-// with adopt_clouds only when every chunk has succeeded, so that a failed call changes no node.
+// hands them over through rebuild_clouds only when every chunk has succeeded, so that a failed call changes no node.
 struct CloudResult {
   NodeDev* nd;
   NodeCloud pc;
 };
-// Each node takes its new cloud and lets go of its old allocation; slabs no node took are freed.
-void adopt_clouds(const std::vector<CloudResult>& results, const std::vector<NodeSlab*>& slabs);
-// After a failure: frees the call's new slabs (after the stream has drained).
-void drop_slabs(const std::vector<NodeSlab*>& slabs);
+// Builds the new clouds of nodes [k0, k1) of the call, `points` stored points in all, into new slabs registered in `slabs`.
+using CloudChunk = std::function<int(int k0, int k1, long long points, std::vector<CloudResult>& results, std::vector<NodeSlab*>& slabs)>;
+// Runs chunk over chunks of whole nodes (at least one) of at most `limit` points.  The nodes take their new clouds only when
+// every chunk has succeeded; otherwise the new slabs are freed (after the stream has drained) and no node changes.
+int rebuild_clouds(const std::vector<NodeDev*>& nds, long long limit, const CloudChunk& chunk);
+// A chunk's new slab of max(points, 1) 16-byte points, appended to slabs; nullptr (last_error: "CUDA error in <what>") on failure.
+NodeSlab* new_slab(long long points, const char* what, std::vector<NodeSlab*>& slabs);
+// c with its x / y / z / colour planes at point `first` of slab, `count` points apart, and no raster step.
+NodeCloud slab_cloud(const NodeCloud& c, NodeSlab* slab, long long first, long long count);
+// The chunk or batch size `limit`, or the environment variable env_name's value (at least 1) when it is set, for tests.
+long long chunk_limit(long long limit, const char* env_name);
 
 constexpr int kSlots = 8;  // independent in-flight match_pairs pipelines (stream + workspace each)
 
@@ -168,5 +176,22 @@ Workspace* get_slot(int slot);  // nullptr (and last_error set) unless 0 <= slot
 void free_node(NodeDev* nd);  // frees everything a (possibly half-built) node owns (api.cu)
 void release_slab(NodeSlab* slab);  // drops one node's reference to a shared allocation, freeing it with the last (api.cu)
 MapNode map_node(const NodeDev* nd, const float* T);  // nd's stored cloud as map_point reads it, transform T (api_map.cu)
+// The (node, first point) table of the kMapBlockPoints-point blocks of nodes' clouds; with `first`, node k's blocks are
+// [first[k], first[k + 1]) and first[n] is the block count.
+std::vector<int2> map_blocks(const std::vector<MapNode>& nodes, std::vector<int>* first);
+// The n handles of a stored-cloud call, resolved in order into nds: ERR_ARG for an unknown handle, ERR_STATE for a node
+// without a stored cloud, then, when `distinct`, ERR_ARG for a node listed twice.
+int stored_cloud_nodes(const char* call, int n, const uint64_t* handles, bool distinct, std::vector<NodeDev*>* nds);
+
+// ERR_ARG ("<call>: <noun> k has a non-finite entry") unless every entry of the n x stride values v is finite.
+template <typename T>
+int check_finite(const char* call, const char* noun, int n, int stride, const T* v) {
+  for (size_t i = 0; i < (size_t)n * stride; i++)
+    if (!std::isfinite(v[i])) {
+      set_error(std::string(call) + ": " + noun + " " + std::to_string(i / stride) + " has a non-finite entry");
+      return RGBDSLAM_B200_ERR_ARG;
+    }
+  return 0;
+}
 
 }  // namespace rb200
