@@ -16,6 +16,34 @@
 - `identity_planted_pair`: every hypothesis draws an outlier, so the pair ends in the identity fallback and rows planted near
   both cuts under T = I keep their margins in the transform the kernel returns.
 - `degenerate_pair`: hypothesis 0 draws a rank-deficient sample (many-to-one matches or collinear from-points).
+- `kabsch_f64`: the float64 weighted rigid fit (getTransformFromMatches): weights 1/(z_from z_to), NaN-depth rows skipped,
+  R = U diag(1, 1, d) V^T of the weighted centred covariance C = sum w (to - m2)(from - m1)^T, d = sign(det U det V).
+- `fit_f32`: a numpy emulation of the kernel's float32 fit (`fit_moments` + `fit_solve`, csrc/frontend_kernels.cu) in its
+  operation order: the centroid the fit is centred on, per-lane sequential fmaf sums, the butterfly of `wsum16`, the Jacobi
+  sweeps with their early exit, the column choice and the cross products.  MUFU steps (rsqrtf, __fdividef) are taken as IEEE
+  operations, and products nvcc may contract into an fma are rounded separately.
+- `fit_bound`: the error bound of that fit against `kabsch_f64`, derived below; `fit_cases`: the conditioning edges it is
+  checked on.
+
+The fit's error bound.  u = 2^-24.  The kernel centres every row on the pair's float centroid c (one rounding per coordinate,
+relative to the centred value) and sums the 16 moments per lane (ceil(M/32) sequential fmaf adds) and then over a 5-level
+butterfly, so with L = ceil(M/32) + 5 every moment carries at most L u of the sum of its terms' magnitudes.  The weight (two
+roundings), the weighted to-point (one) and the centring (two) add 5 u per term, and fit_solve's 1/W, means and the
+subtraction C = S/W - m2 m1^T add 5 u more.  With A = E_w[|b~| |a~|] + |m2~| |m1~| (a~, b~ the rows centred on c, E_w the
+weighted mean: A >= ||C||_F, and A is the size of the float sums C is formed from, which exceeds ||C||_F when the weighted
+mean lies far from c)
+    ||dC||_F <= (L + 10) u A.
+The one-sided Jacobi applies at most 6 sweeps x 3 rotations; a rotation from the 2-ulp rsqrtf / __fdividef and two rounded
+products is orthogonal to 6 u, so the sweeps add at most 18 x 6 u ||C||_F <= 108 u A of backward error.  The rotation factor
+of C moves by at most 2 ||dC||_F / (s2 + d s3) (s1 >= s2 >= s3 the singular values of C).  The exit test leaves columns at most
+4e-7 (7 u) from orthogonal, and the normalisation (2-ulp rsqrtf), the cross products and the three-term sums of R add about
+8 u more: 30 u in all, absolute, which is at most 60 u A / (s2 + d s3) because s2 + d s3 <= 2 s1 <= 2 A.  So
+    ||R_gpu - R64||_max <= K u A / (s2 + d s3),   K = 2 (L + 10 + 108) + 60 = 2 L + 296.
+The translation t = (m2 + c_to) - R (m1 + c_from) adds the means' error ((L + 3) u of E_w|a~|, E_w|b~|), the centroid add-back
+and the 3-term product (4 u of |g1|) and the final subtraction (u of |g2| + |g1|):
+    |t_gpu - t64 + (R_gpu - R64) g1| <= K u (|g2| + |g1| + E_w|a~| + E_w|b~|)
+with g1, g2 the weighted centroids: the translation is the one R_gpu implies (t64 = g2 - R64 g1), which bounds
+|t_gpu - t64| by ||R_gpu - R64||_2 |g1| plus the same term without letting a rotation error hide a translation error.  Separately, |det R - 1| and ||R^T R - I||_max stay below 1e-5 (SHAPE_TOL).
 """
 from __future__ import annotations
 
@@ -191,6 +219,203 @@ def screen_envelope(T, frm, to, band=3e-3, **kw):
     wrong = int((sc & (code == 1) & ~ref["inl"]).sum() + (sc & (code == -1) & ref["inl"]).sum())
     return dict(m_err=float(em.max(initial=0.0)), s_err=float(es.max(initial=0.0)), n_m=int(near_m.sum()),
                 n_s=int(near_s.sum()), wrong=wrong, undecided=int((sc & (code == 0)).sum()))
+
+
+# ---- the rigid fit --------------------------------------------------------------------------------------------------------
+
+U32 = 2.0 ** -24
+SHAPE_TOL = 1e-5
+
+
+def _fit_rows(frm, to, sel=None):
+    """float64 copies of the selected rows whose depth is finite on both sides (transformation_estimation_euclidean.cpp:22)."""
+    a = np.asarray(frm, F32).reshape(-1, 4).astype(F64)
+    b = np.asarray(to, F32).reshape(-1, 4).astype(F64)
+    keep = ~(np.isnan(a[:, 2]) | np.isnan(b[:, 2]))
+    if sel is not None:
+        m = np.zeros(len(a), bool)
+        m[sel] = True
+        keep &= m
+    return a[keep], b[keep]
+
+
+def kabsch_f64(frm, to, sel=None):
+    """The weighted rigid fit of getTransformFromMatches in float64: R, t minimising sum w |R from + t - to|^2 with
+    w = 1/(z_from z_to) over the rows (of `sel`, indices or a mask) with a finite depth on both sides.  Returns
+    (R, t, s, d): s the singular values of the weighted centred covariance C = sum w (to - m2)(from - m1)^T / W, descending,
+    and d = sign(det U det V), so R = U diag(1, 1, d) V^T."""
+    a, b = _fit_rows(frm, to, sel)
+    w = 1.0 / (a[:, 2] * b[:, 2])  # :25
+    w = w / w.sum()
+    m1, m2 = w @ a[:, :3], w @ b[:, :3]
+    Cm = ((b[:, :3] - m2) * w[:, None]).T @ (a[:, :3] - m1)
+    U, S, Vt = np.linalg.svd(Cm)
+    d = 1.0 if np.linalg.det(U) * np.linalg.det(Vt) >= 0 else -1.0
+    R = U @ np.diag([1.0, 1.0, d]) @ Vt
+    return R, m2 - R @ m1, S, d
+
+
+def _bfly(x):
+    """wsum / wsum16: the xor butterfly over 32 lanes (offsets 16, 8, 4, 2, 1); every lane ends with the same float."""
+    x = np.asarray(x, F32)
+    idx = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        x = (x + x[idx ^ o]).astype(F32)
+    return x[0]
+
+
+def centroid_f32(frm, to):
+    """The centroid ransac_hyp_kernel centres the fit on: kCenWarps = 8 virtual warps, virtual lane v sums rows v, v + 256
+    (rows with a NaN coordinate left out), each warp's butterfly, the 8 warp sums in order, divided by M."""
+    a = np.asarray(frm, F32).reshape(-1, 4)
+    b = np.asarray(to, F32).reshape(-1, 4)
+    M = len(a)
+    x = np.concatenate([a[:, :3], b[:, :3]], 1)
+    ok = ~np.isnan(x.sum(1))
+    cs = np.zeros((256, 6), F32)
+    for i in range(M):
+        if ok[i]:
+            cs[i % 256] = (cs[i % 256] + x[i]).astype(F32)
+    tot = np.zeros(6, F32)
+    for w in range(8):
+        part = np.array([_bfly(cs[w * 32:(w + 1) * 32, k]) for k in range(6)], F32)
+        tot = (tot + part).astype(F32)
+    return (tot / F32(M)).astype(F32)
+
+
+def _fmaf(a, b, c):
+    return F32(F64(a) * F64(b) + F64(c))
+
+
+def _rsq(x):
+    return F32(1.0 / np.sqrt(F64(x)))
+
+
+def fit_f32(frm, to, sel, *, sweeps=6):
+    """fit_moments + fit_solve in float32 on the pair's rows frm / to ((M, 4) float32, the fit's centroid is taken over all M
+    rows) for the rows of `sel` (indices or a mask).  Returns (R, t, ok) with R (3, 3) and t (3,) float32; ok is False where
+    the kernel reports a failed fit (no weight, rank < 2, or a non-finite result)."""
+    a = np.asarray(frm, F32).reshape(-1, 4)
+    b = np.asarray(to, F32).reshape(-1, 4)
+    M = len(a)
+    cen = centroid_f32(a, b)
+    ca = np.concatenate([(a[:, :3] - cen[:3]).astype(F32), a[:, 2:3]], 1)
+    cb = np.concatenate([(b[:, :3] - cen[3:]).astype(F32), b[:, 2:3]], 1)
+    mask = np.zeros(M, bool)
+    mask[sel] = True
+    # fit_moments: lane l adds rows l, l + 32, ... in order
+    acc = np.zeros((32, 16), F32)
+    for w in range((M + 31) // 32):
+        for lane in range(32):
+            i = w * 32 + lane
+            if i >= M or not mask[i]:
+                continue
+            p, q = ca[i], cb[i]
+            if np.isnan(p[3]) or np.isnan(q[3]):
+                continue
+            m = acc[lane]
+            wt = F32(F32(1.0) / F32(p[3] * q[3]))
+            m[0] = F32(m[0] + wt)
+            for k in range(3):
+                m[1 + k] = _fmaf(wt, p[k], m[1 + k])
+            bw = [F32(wt * q[k]) for k in range(3)]
+            for k in range(3):
+                m[4 + k] = F32(m[4 + k] + bw[k])
+            for r in range(3):
+                for k in range(3):
+                    m[7 + 3 * r + k] = _fmaf(bw[r], p[k], m[7 + 3 * r + k])
+    mom = np.array([_bfly(acc[:, j]) for j in range(16)], F32)
+    # fit_solve
+    W = mom[0]
+    if not W > 0:
+        return np.eye(3, dtype=F32), np.zeros(3, F32), False
+    iW = F32(F32(1.0) / W)
+    m1 = [F32(mom[1 + k] * iW) for k in range(3)]
+    m2 = [F32(mom[4 + k] * iW) for k in range(3)]
+    A = np.array([[F32(F32(mom[7 + 3 * r + k] * iW) - F32(m2[r] * m1[k])) for k in range(3)] for r in range(3)], F32)
+    V = np.eye(3, dtype=F32)
+
+    def dot(x, y):
+        return F32(F32(F32(x[0] * y[0]) + F32(x[1] * y[1])) + F32(x[2] * y[2]))
+
+    for _ in range(sweeps):
+        rotated = False
+        for pp, qq in ((0, 1), (0, 2), (1, 2)):
+            al, be, ga = dot(A[:, pp], A[:, pp]), dot(A[:, qq], A[:, qq]), dot(A[:, pp], A[:, qq])
+            if not F32(ga * ga) > F32(F32(1.6e-13) * F32(al * be)):
+                continue
+            if F32(ga * ga) > F32(F32(1e-7) * F32(al * be)):
+                rotated = True
+            dd, g2 = F32(be - al), F32(F32(2) * ga)
+            hh = F32(np.sqrt(_fmaf(dd, dd, F32(g2 * g2))))
+            sg = F32(-1) if (dd < 0) != (g2 < 0) else F32(1)
+            tt = F32(sg * F32(abs(g2) / F32(abs(dd) + hh)))
+            cs = _rsq(_fmaf(tt, tt, F32(1)))
+            sn = F32(cs * tt)
+            for X in (A, V):
+                x, y = X[:, pp].copy(), X[:, qq].copy()
+                X[:, pp] = (F32(cs) * x - F32(sn) * y).astype(F32)
+                X[:, qq] = (F32(sn) * x + F32(cs) * y).astype(F32)
+        if not rotated:
+            break
+    n = [dot(A[:, k], A[:, k]) for k in range(3)]
+    ip = 0
+    if n[1] > n[0]:
+        ip = 1
+    if n[2] > n[ip]:
+        ip = 2
+    iq = {0: 2 if n[2] > n[1] else 1, 1: 2 if n[2] > n[0] else 0, 2: 1 if n[1] > n[0] else 0}[ip]
+    if not (n[ip] > 0) or not (n[iq] > F32(F32(1e-24) * n[ip])):
+        return np.eye(3, dtype=F32), np.zeros(3, F32), False
+    p = (A[:, ip] * _rsq(n[ip])).astype(F32)
+    q = (A[:, iq] * _rsq(n[iq])).astype(F32)
+    vp, vq = V[:, ip], V[:, iq]
+
+    def cross(x, y):
+        return np.array([F32(x[1] * y[2]) - F32(x[2] * y[1]), F32(x[2] * y[0]) - F32(x[0] * y[2]),
+                         F32(x[0] * y[1]) - F32(x[1] * y[0])], F32)
+
+    u3, v3 = cross(p, q), cross(vp, vq)
+    R = np.array([[F32(F32(F32(p[r] * vp[k]) + F32(q[r] * vq[k])) + F32(u3[r] * v3[k])) for k in range(3)] for r in range(3)],
+                 F32)
+    g1 = [F32(m1[k] + cen[k]) for k in range(3)]
+    t = np.array([F32(F32(m2[r] + cen[3 + r]) - dot(R[r], g1)) for r in range(3)], F32)
+    ok = bool(np.isfinite(R).all() and np.isfinite(t).all())
+    return R, t, ok
+
+
+def fit_K(M):
+    """K of the rotation bound (module docstring) for a pair of M rows."""
+    return 2 * (-(-M // 32) + 5) + 296
+
+
+def fit_bound(frm, to, sel=None):
+    """The bound of the module docstring for the fit of the rows `sel` of a pair (frm, to: all M rows, which set the
+    centroid).  Returns a dict: rot and trans, the bounds on ||R_gpu - R64||_max and |t_gpu - t64 + (R_gpu - R64) g1|_max;
+    R, t, s, d of kabsch_f64, the conditioning ratio cond = A / (s2 + d s3), K and the weighted from-centroid g1."""
+    R, t, s, d = kabsch_f64(frm, to, sel)
+    M = len(np.asarray(frm).reshape(-1, 4))
+    c = centroid_f32(frm, to).astype(F64)
+    a, b = _fit_rows(frm, to, sel)
+    w = 1.0 / (a[:, 2] * b[:, 2])
+    w = w / w.sum()
+    at, bt = a[:, :3] - c[:3], b[:, :3] - c[3:]
+    na, nb = np.linalg.norm(at, axis=1), np.linalg.norm(bt, axis=1)
+    A = w @ (na * nb) + np.linalg.norm(w @ at) * np.linalg.norm(w @ bt)
+    K = fit_K(M)
+    cond = A / (s[1] + d * s[2])
+    g1, g2 = w @ a[:, :3], w @ b[:, :3]
+    tmag = np.linalg.norm(g1) + np.linalg.norm(g2) + w @ na + w @ nb
+    return dict(rot=K * U32 * cond, trans=K * U32 * tmag, R=R, t=t, s=s, d=d, cond=cond, K=K, g1=g1)
+
+
+def fit_errors(R, t, ref):
+    """(rotation error, translation error, shape error) of a fit (R, t) against fit_bound's ref: ||R - R64||_max,
+    |t - t64 + (R - R64) g1|_max (bounded by ref["trans"]) and max(|det R - 1|, ||R^T R - I||_max)."""
+    R64, t64 = np.asarray(R, F64), np.asarray(t, F64)
+    dR = R64 - ref["R"]
+    shape = max(abs(np.linalg.det(R64) - 1), np.abs(R64.T @ R64 - np.eye(3)).max())
+    return float(np.abs(dR).max()), float(np.abs(t64 - ref["t"] + dR @ ref["g1"]).max()), float(shape)
 
 
 # ---- generators -----------------------------------------------------------------------------------------------------------
@@ -557,3 +782,140 @@ def scenario_batches(oracle_mod, seed=7, names=None):
             meta.append((name, M, valid, M - n_out))
         out[cfg] = (concat_batch(pairs), meta, seed)
     return out
+
+
+# ---- conditioning edges of the rigid fit ----------------------------------------------------------------------------------
+
+def rot_axis(axis, deg):
+    """Rotation by `deg` degrees about `axis` (Rodrigues)."""
+    k = np.asarray(axis, F64) / np.linalg.norm(axis)
+    K = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    a = np.deg2rad(deg)
+    return np.eye(3) + np.sin(a) * K + (1 - np.cos(a)) * (K @ K)
+
+
+def _moved(P, R, shift=(0.0, 0.0, 0.0), zmin=0.3):
+    """R about the cloud's centre plus `shift`, and a z-shift that keeps every to-point at z >= zmin."""
+    c = P.mean(0)
+    Q = (P - c) @ R.T + c + np.asarray(shift, F64)
+    lo = Q[:, 2].min()
+    if lo < zmin:
+        Q[:, 2] += zmin + 0.2 - lo
+    return Q
+
+
+def _noisy(rng, Q, sd):
+    return Q + np.clip(rng.normal(scale=sd, size=Q.shape), -2.5 * sd, 2.5 * sd)
+
+
+def _case(family, name, P, Q, noisy=False, nan=None):
+    """One pair's rows: frm (from = query / newer side), to (train / older side), float32 (x, y, z, 1); nan: (rows, side)
+    with side 'from', 'to' or 'both' gets a NaN depth."""
+    frm, to = to4(P), to4(Q)
+    if nan is not None:
+        rows, side = nan
+        if side in ("from", "both"):
+            frm[rows, 2] = np.nan
+        if side in ("to", "both"):
+            to[rows, 2] = np.nan
+    return dict(family=family, name=name, frm=frm, to=to, noisy=noisy, M=len(frm))
+
+
+OBLIQUE = (1.0, -2.0, 0.7)
+
+
+def fit_cases():
+    """The fit's conditioning edges, one dict per pair (see `_case`; `noisy`: 0.5-2 mm of noise on every to-point, so that the
+    refit over all rows is a strictly better model than any 4-point sample's)."""
+    rng = np.random.default_rng(2024)
+    cases = []
+    # trivial motions
+    P4 = np.array([[-0.4, -0.3, 1.2], [0.5, -0.2, 1.9], [0.1, 0.45, 2.6], [-0.3, 0.35, 1.6]])
+    P40 = frustum_points(rng, 40, 1.0, 3.0)
+    for nm, sh in (("identity", (0, 0, 0)), ("t=1cm", (0.01, 0, 0)), ("t=5m-lateral", (3.0, -4.0, 0)), ("t=5m-depth", (0, 0, 5.0))):
+        cases.append(_case("trivial", f"{nm}-M4", P4, P4 + sh))
+        cases.append(_case("trivial", f"{nm}-M40", P40, P40 + sh))
+    # rotations about x, y, z and an oblique axis
+    for ax_name, ax in (("x", (1, 0, 0)), ("y", (0, 1, 0)), ("z", (0, 0, 1)), ("oblique", OBLIQUE)):
+        for deg in (1.0, 30.0, 90.0, 179.9, 180.0):
+            R = rot_axis(ax, deg)
+            cases.append(_case("rotation", f"{ax_name}{deg:g}-M4", P4, _moved(P4, R, (0.1, -0.05, 0.2))))
+            P = frustum_points(rng, 40, 1.0, 3.0)
+            cases.append(_case("rotation", f"{ax_name}{deg:g}-M40-noisy", P,
+                               _noisy(rng, _moved(P, R, (0.1, -0.05, 0.2)), rng.uniform(5e-4, 2e-3)), noisy=True))
+    # coplanar sets (exact rank 2): a fronto-parallel wall at z = 2 and an oblique plane; rotations about the normal and
+    # about in-plane axes
+    wall = lambda n: np.concatenate([rng.uniform(-1, 1, (n, 2)), np.full((n, 1), 2.0)], 1)
+    nrm = np.array([0.3, -0.5, 0.8]) / np.linalg.norm([0.3, -0.5, 0.8])
+    e1 = np.cross(nrm, [1.0, 0, 0]); e1 /= np.linalg.norm(e1)
+    e2 = np.cross(nrm, e1)
+    oblique = lambda n: np.array([0.0, 0.0, 2.5]) + rng.uniform(-1, 1, (n, 1)) * e1 + rng.uniform(-1, 1, (n, 1)) * e2
+    for pl_name, gen, normal, inplane in (("wall", wall, (0, 0, 1.0), (1.0, 0.3, 0)), ("oblique", oblique, nrm, e1)):
+        for rot_name, ax, deg in (("normal30", normal, 30.0), ("normal180", normal, 180.0), ("inplane30", inplane, 30.0),
+                                  ("inplane90", inplane, 90.0), ("inplane180", inplane, 180.0)):
+            R = rot_axis(ax, deg)
+            for M in (4, 40):
+                P = gen(M)
+                cases.append(_case("coplanar", f"{pl_name}-{rot_name}-M{M}", P, _moved(P, R, (0.05, 0.1, 0.3))))
+    # the reflection case: noisy coplanar sets whose unconstrained Kabsch has d = -1 (test_oracle's reflection case)
+    found = 0
+    while found < 4:
+        M = 4 if found < 2 else 6
+        P = np.concatenate([rng.uniform(-1, 1, (M, 2)), np.full((M, 1), 2.0)], 1)
+        Q = P + np.array([0.1, -0.05, 0.02]) + rng.normal(size=P.shape) * 1e-4
+        if kabsch_f64(to4(P), to4(Q))[3] < 0 and (M == 4 or kabsch_f64(to4(P), to4(Q), np.arange(4))[3] < 0):
+            cases.append(_case("reflection", f"reflection-{found}-M{M}", P, Q))
+            found += 1
+    # near-collinear strips: 1 m long, lateral spread 1e-2, 1e-3, 1e-4 of the length
+    u = np.array(OBLIQUE) / np.linalg.norm(OBLIQUE)
+    for s in (1e-2, 1e-3, 1e-4):
+        for M in (4, 40):
+            lat = rng.normal(size=(M, 3))
+            lat -= np.outer(lat @ u, u)
+            P = np.array([0.0, 0.0, 2.0]) + np.outer(np.linspace(-0.5, 0.5, M), u) + s * lat
+            cases.append(_case("collinear", f"strip{s:g}-M{M}", P, _moved(P, rot_axis((0.2, 1, 0.4), 20.0), (0.05, 0, 0.1))))
+    # isotropic sets: equal singular values (exact ties when the motion keeps C diagonal)
+    h = 0.25
+    cube = np.array([[x, y, z] for x in (-h, h) for y in (-h, h) for z in (-h, h)])
+    tetra = np.array([[1, 1, 1], [1, -1, -1], [-1, 1, -1], [-1, -1, 1]]) * (h / np.sqrt(3))
+    octa = np.concatenate([np.eye(3), -np.eye(3)]) * h
+    square = np.array([[h, 0, 0], [-h, 0, 0], [0, h, 0], [0, -h, 0]])
+    for nm, S in (("cube", cube), ("tetrahedron", tetra), ("octahedron", octa), ("square", square)):
+        P = S + np.array([0.0, 0.0, 2.5])
+        cases.append(_case("isotropic", f"{nm}-identity", P, P.copy()))
+        cases.append(_case("isotropic", f"{nm}-shift", P, P + np.array([0.25, -0.5, 0.5])))
+        cases.append(_case("isotropic", f"{nm}-rot", P, _moved(P, rot_axis(OBLIQUE, 30.0), (0.1, 0.0, 0.2))))
+    # scale: 4-point clouds of 0.1 mm to 1 cm, 10 m clouds, 2 cm clouds 8 m away
+    for size in (1e-4, 3e-4, 1e-3, 1e-2):
+        P = np.array([0.2, -0.1, 1.0]) + P4 / 0.9 * size
+        for z_name, zoff in (("z1", 0.0), ("z3", 2.0)):
+            Pz = P + np.array([0, 0, zoff])
+            cases.append(_case("scale", f"{size:g}m-{z_name}-M4", Pz, _moved(Pz, rot_axis(OBLIQUE, 10.0), (0.03, 0.01, 0.02))))
+    P = np.concatenate([rng.uniform(-5, 5, (40, 2)), rng.uniform(1.0, 11.0, (40, 1))], 1)
+    cases.append(_case("scale", "10m-M40-noisy", P, _noisy(rng, _moved(P, rot_axis(OBLIQUE, 10.0), (0.2, 0, 0.3)), 1e-3),
+                       noisy=True))
+    for M in (4, 40):
+        P = np.array([0.5, -0.3, 8.0]) + rng.uniform(-0.01, 0.01, (M, 3))
+        cases.append(_case("scale", f"2cm-at-8m-M{M}", P, _moved(P, rot_axis(OBLIQUE, 10.0), (0.05, 0.02, -0.1))))
+    # weight spread: depths from 0.3 m to 15 m on both sides (weights over four decades)
+    zz = np.array([0.3, 1.0, 5.0, 15.0])
+    P = np.stack([(np.array([100.0, 500.0, 250.0, 400.0]) - CX) * zz / FX, (np.array([300.0, 100.0, 400.0, 200.0]) - CY) * zz / FY, zz], 1)
+    cases.append(_case("weights", "z0.3-15-M4", P, P @ rot_axis((0, 1, 0), 0.5).T))
+    for k in range(2):
+        z = np.exp(rng.uniform(np.log(0.3), np.log(15.0), 40))
+        z[:2] = (0.3, 15.0)
+        P = np.stack([rng.uniform(-0.5, 0.5, 40) * z, rng.uniform(-0.4, 0.4, 40) * z, z], 1)
+        Q = P @ rot_axis((0.1, 1, 0.2), 0.5).T + np.array([0.0, 0.0, 0.01])
+        assert Q[:, 2].min() >= 0.3
+        cases.append(_case("weights", f"z0.3-15-M40-{k}", P, _noisy(rng, Q, 5e-4), noisy=True))
+    # NaN depths among finite rows
+    for side in ("from", "to", "both"):
+        P = frustum_points(rng, 40, 1.0, 3.0)
+        Q = _noisy(rng, _moved(P, rot_axis(OBLIQUE, 5.0), (0.05, 0.0, 0.02)), 1e-3)
+        cases.append(_case("nan", f"nan-{side}", P, Q, noisy=True, nan=(np.array([5, 17, 33]), side)))
+    # M around the mask words and the two kernel instantiations (10 words up to max_matches 320, 16 above)
+    for M in (4, 5, 31, 32, 33, 63, 64, 65, 300, 320, 321, 512):
+        P = frustum_points(rng, M, 1.0, 3.0)
+        Q = _noisy(rng, _moved(P, rot_axis(OBLIQUE, 3.0), (0.04, -0.02, 0.03)), 1e-3)
+        cases.append(_case("M", f"M{M}", P, Q, noisy=True))
+    return cases
