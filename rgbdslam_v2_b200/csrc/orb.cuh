@@ -13,11 +13,10 @@ namespace rb200 {
 
 constexpr int kOrbLevels = 8;
 constexpr int kOrbMaxCells = 16;       // detector_grid_resolution <= 4
-constexpr int kOrbCandCap = 12288;     // FAST/NMS candidates per (frame, cell), all levels, up to kOrbNarrowMax px per side
+constexpr int kOrbCandCap = 12288;     // FAST/NMS candidates per (frame, cell), all levels: the smallest buffer orb_prepare sizes
 constexpr int kOrbHalfPatch = 15;
-// Frames of up to kOrbNarrowMax px per side run the narrow kernels (10-bit level coordinates in k_cell_select's keys, kOrbCandCap
-// candidates per cell); larger frames, up to kOrbMaxSide, the wide ones (12-bit coordinates, a candidate buffer sized from the
-// largest cell, cv::ORB's per-level quotas).  DESIGN.md 4.5.5.
+// Frames wider or taller than kOrbNarrowMax px, up to kOrbMaxSide, take a candidate buffer sized from the largest cell's area and
+// need a grid whose per-cell maximum stays below cv::ORB's smallest quota (api_orb.cu).  DESIGN.md 4.5.5.
 constexpr int kOrbNarrowMax = 1023;
 constexpr int kOrbMaxSide = 4095;
 
@@ -38,7 +37,7 @@ struct OrbGeom {
   int32_t cell_bytes;           // packed bytes per frame for all cell pyramids (image; mask uses the same layout)
   OrbPlane full[kOrbLevels];    // extractor pyramid of the whole image
   int32_t full_bytes;
-  int32_t n_per_level[kOrbLevels];  // ORB feature quota per level for nfeatures = 10000 (applied by k_cell_select_wide)
+  int32_t n_per_level[kOrbLevels];  // ORB feature quota per level for nfeatures = 10000 (applied by k_cell_select)
 };
 
 // resize tables: for every destination column/row the first source index and the weight of the second tap (x256)

@@ -11,7 +11,7 @@ cudaError_t orb_upload_constants(const OrbGeom& g, const int* umax, cudaStream_t
 
 // d_depth_for_mask != nullptr: detection mask = depthToCV8UC1(depth) != 0 (misc.cpp:414-418), d_mask ignored.
 // detector: RGBDSLAM_B200_DETECTOR_ORB (8-level cell pyramids) or _FAST (level 0 only, cv::FAST's 3 px border).
-// cand_cap: candidates per (frame, cell) in d_cand, kOrbCandCap unless the frame is wider or taller than kOrbNarrowMax.
+// cand_cap: candidates per (frame, cell) in d_cand, as orb_prepare sizes it (at least kOrbCandCap).
 cudaError_t orb_run_detect(const OrbGeom& g, const OrbTables& tab, int nframes, const uint8_t* d_gray, const uint8_t* d_mask,
                            const float* d_depth_for_mask, int detector, uint8_t* d_cell_img, uint8_t* d_cell_mask, OrbCand* d_cand,
                            int* d_cand_count, int* d_hist, int* d_mask_any, int cand_cap, cudaStream_t st, int* launches);
@@ -94,7 +94,7 @@ struct OrbSurvivors {
   int stride;
 };
 
-// detector ORB: Harris responses, cv::ORB's per-level quotas (k_cell_select_wide), orientation, size 31 * scale; FAST:
+// detector ORB: Harris responses, cv::ORB's per-level quotas (k_cell_select), orientation, size 31 * scale; FAST:
 // response = corner score, angle -1, size 7.  all != NULL (one whole-frame cell): no keepStrongest, the survivors go through
 // `all` to k_frame_precap; d_err bit 1: a detector output (mode 0) of more than kOrbFrameCap keypoints.
 cudaError_t orb_run_select(const OrbGeom& g, int nframes, int detector, OrbPoints points, const OrbCandidates& c,

@@ -1,5 +1,5 @@
 """cv::ORB's per-level quotas (feature_adjuster.cpp:94: cv::ORB::create(10000, 1.2, 8, 15, 0, 2, HARRIS_SCORE, 31, t)) as
-k_cell_select_wide applies them, restated in numpy and pinned to cv2 4.13.
+k_cell_select applies them, restated in numpy and pinned to cv2 4.13.
 
 Per level l, with n_l = [2172, 1810, 1508, 1257, 1047, 873, 727, 606]: the FAST corners at threshold t inside the 15 px
 border and the mask, retainBest(2 n_l) by FAST score, then retainBest(n_l) by Harris response, where retainBest(n) keeps
