@@ -177,6 +177,61 @@ def posegraph_optimize(poses, fixed, ij, meas, info, stop=0.01, huber_delta=1.0)
     return x, chi2, it.value, cg.value
 
 
+TRIAL_FIELDS = ("lam", "tol", "iterations", "scale", "chi2", "rho", "accepted", "ok")
+
+
+def posegraph_lm_trace(poses, fixed, ij, meas, info, huber_delta=1.0):
+    """One LM iteration exactly as posegraph_optimize(stop=1) runs it, every trial traced.  Returns dict(poses, chi2,
+    cg_iterations, trials=[dict(lam, tol, iterations, scale, chi2, rho, accepted, ok, dx (nv, 6): the PCG step,
+    dn: r'M^-1 r before each PCG iteration, iterations + 1 values)])."""
+    x = np.array(poses, np.float64, order="C")
+    nv = len(x)
+    fixed = np.ascontiguousarray(fixed, np.uint8); ij = np.ascontiguousarray(ij, np.int32).reshape(-1, 2)
+    meas = np.ascontiguousarray(meas, np.float64); info = np.ascontiguousarray(info, np.float64)
+    tr = np.zeros((10, 8)); dx = np.zeros((10, nv, 6)); dn = np.zeros((10, 6 * nv + 1))
+    chi2 = C.c_double(0); cg = C.c_int(0)
+    n = lib().oracle_posegraph_lm_trace(C.c_int(nv), _p(x), _p(fixed), C.c_int(len(ij)), _p(ij), _p(meas), _p(info),
+                                        C.c_double(huber_delta), _p(tr), _p(dx), _p(dn), C.byref(chi2), C.byref(cg))
+    trials = []
+    for t in range(n):
+        d = dict(zip(TRIAL_FIELDS, tr[t].tolist()))
+        for k in ("iterations", "accepted", "ok"):
+            d[k] = int(d[k])
+        d["dx"] = dx[t].copy()
+        d["dn"] = dn[t, :d["iterations"] + 1].copy()
+        trials.append(d)
+    return dict(poses=x, chi2=chi2.value, cg_iterations=cg.value, trials=trials)
+
+
+def posegraph_damped_system(poses, fixed, ij, meas, info, lam, huber_delta=1.0):
+    """The system one PCG solve of the oracle works on at these poses and damping: dict(Hd (nv, 6, 6) with lam I on the free
+    vertices, Ho (ne, 6, 6) = Ji'WJj, b (nv, 6) and babs (nv, 6), the sums of |terms| of b, both 0 on the fixed vertices,
+    A: the free rows and columns of H + lam I as a
+    scipy CSR matrix (without the off-diagonal block of a self edge, like the PCG), free: the free vertices' indices)."""
+    import scipy.sparse as sp
+    x = np.ascontiguousarray(poses, np.float64)
+    nv = len(x)
+    fixed = np.ascontiguousarray(fixed, np.uint8); ij = np.ascontiguousarray(ij, np.int32).reshape(-1, 2)
+    meas = np.ascontiguousarray(meas, np.float64); info = np.ascontiguousarray(info, np.float64)
+    Hd = np.zeros((nv, 6, 6)); Ho = np.zeros((max(len(ij), 1), 6, 6)); b = np.zeros((nv, 6)); babs = np.zeros((nv, 6))
+    lib().oracle_posegraph_system(C.c_int(nv), _p(x), _p(fixed), C.c_int(len(ij)), _p(ij), _p(meas), _p(info),
+                                  C.c_double(huber_delta), C.c_double(lam), _p(Hd), _p(Ho), _p(b), _p(babs))
+    Ho = Ho[:len(ij)]
+    free = np.nonzero(fixed == 0)[0]
+    col = -np.ones(nv, np.int64); col[free] = np.arange(len(free))
+    keep = (col[ij[:, 0]] >= 0) & (col[ij[:, 1]] >= 0) & (ij[:, 0] != ij[:, 1]) if len(ij) else np.zeros(0, bool)
+    bi, bj = col[ij[keep, 0]], col[ij[keep, 1]]
+    nf = 6 * len(free)
+    r6, c6 = np.meshgrid(np.arange(6), np.arange(6), indexing="ij")  # element [r, c] of a block: C couples row r of i to c of j
+    rows = [(6 * col[free])[:, None, None] + r6, (6 * bi)[:, None, None] + r6, (6 * bj)[:, None, None] + c6]
+    cols = [(6 * col[free])[:, None, None] + c6, (6 * bj)[:, None, None] + c6, (6 * bi)[:, None, None] + r6]
+    vals = [Hd[free], Ho[keep], Ho[keep]]
+    A = sp.csr_matrix((np.concatenate([v.reshape(-1) for v in vals]),
+                       (np.concatenate([r.reshape(-1) for r in rows]), np.concatenate([c.reshape(-1) for c in cols]))),
+                      shape=(nf, nf))
+    return dict(Hd=Hd, Ho=Ho, b=b, babs=babs, A=A, free=free)
+
+
 def posegraph_chi2(poses, ij, meas, info, huber_delta=1.0):
     x = np.ascontiguousarray(poses, np.float64); ij = np.ascontiguousarray(ij, np.int32)
     meas = np.ascontiguousarray(meas, np.float64); info = np.ascontiguousarray(info, np.float64)

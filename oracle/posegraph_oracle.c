@@ -130,6 +130,12 @@ typedef struct {
   double* b;   /* nv x 6 */
   double* Minv; /* nv x 36 block-Jacobi */
   double pcg_residual; /* LinearSolverPCG::_residual (-1 initially) */
+  /* trace of one LM iteration (oracle_posegraph_lm_trace; NULL elsewhere), per trial t: tr_trial[8 t ..] = lambda, PCG
+   * tolerance, PCG iterations, computeScale, trial chi2 (robust), rho, accepted, PCG ok; tr_dx[6 nv t ..] the PCG step;
+   * tr_dn[(6 nv + 1) t + k] = r^T M^-1 r before PCG iteration k (k = 0 .. iterations) */
+  double *tr_trial, *tr_dx, *tr_dn;
+  int tr_n;
+  double* babs; /* nv x 6: sum of |terms| of b (oracle_posegraph_system; NULL elsewhere) */
 } pg_t;
 
 static void mat6_AtWB(const double* A, const double* W, const double* B, double s, double* out /* += s*A^T W B */) {
@@ -190,6 +196,10 @@ static void pg_build(pg_t* g, const double* x) {
       for (int a = 0; a < 6; a++) { si += Ji[6 * a + c] * We[a]; sj += Jj[6 * a + c] * We[a]; }
       g->b[6 * i + c] -= w * si;
       g->b[6 * j + c] -= w * sj;
+      if (g->babs) {
+        g->babs[6 * i + c] += fabs(w * si);
+        g->babs[6 * j + c] += fabs(w * sj);
+      }
     }
   }
 }
@@ -256,7 +266,10 @@ static int pg_pcg(pg_t* g, double lambda, double* x, int* iters_out) {
   const double tol = (g->pcg_residual > 0.0 && g->pcg_residual > 1e-6) ? g->pcg_residual : 1e-6;
   int it = 0, maxit = n;
   int ok = 1;
+  double* trace = g->tr_dn ? g->tr_dn + (size_t)g->tr_n * (n + 1) : NULL;
+  if (g->tr_trial) g->tr_trial[8 * g->tr_n + 1] = tol;
   for (; it < maxit; it++) {
+    if (trace) trace[it] = dn;
     if (dn <= tol) break;
     pg_spmv(g, lambda, d, q);
     double dq = 0;
@@ -277,6 +290,7 @@ static int pg_pcg(pg_t* g, double lambda, double* x, int* iters_out) {
     double beta = dn / dold;
     for (int i = 0; i < n; i++) d[i] = s[i] + beta * d[i];
   }
+  if (trace && it == maxit) trace[it] = dn;
   free(r);
   g->pcg_residual = 0.5 * dn;
   if (iters_out) *iters_out += it;
@@ -307,6 +321,8 @@ static int pg_lm_solve(pg_t* g, double* x, int iteration, lm_state_t* st, int* c
   int qmax = 0;
   do {
     memcpy(backup, x, sizeof(double) * 7 * g->nv);
+    const double lambda = st->lambda;
+    const int cg0 = *cg_iters;
     int ok2 = pg_pcg(g, st->lambda, dx, cg_iters);
     for (int i = 0; i < g->nv; i++) if (!g->fixed[i]) oracle_vertex_oplus(x + 7 * i, dx + 6 * i);
     pg_errors(g, x, &temp, &plain);
@@ -314,6 +330,13 @@ static int pg_lm_solve(pg_t* g, double* x, int iteration, lm_state_t* st, int* c
     rho = cur - temp;
     double scale = 0;
     for (int i = 0; i < n; i++) if (!g->fixed[i / 6]) scale += dx[i] * (st->lambda * dx[i] + g->b[i]);
+    if (g->tr_trial) {
+      double* t = g->tr_trial + 8 * g->tr_n;
+      t[0] = lambda; t[2] = *cg_iters - cg0; t[3] = scale; t[4] = temp; t[5] = rho / (scale + 1e-3);
+      t[6] = rho / (scale + 1e-3) > 0 && isfinite(temp); t[7] = ok2;
+      memcpy(g->tr_dx + (size_t)n * g->tr_n, dx, sizeof(double) * n);
+      g->tr_n++;
+    }
     scale += 1e-3;
     rho /= scale;
     if (rho > 0 && isfinite(temp)) {
@@ -348,18 +371,25 @@ static int pg_optimize(pg_t* g, double* x, int iterations, int* cg_iters) { /* S
   return cj;
 }
 
+static void pg_init(pg_t* g, int nv, const uint8_t* fixed, int ne, const int32_t* ij, const double* meas, const double* info,
+                    double huber_delta) {
+  memset(g, 0, sizeof(*g));
+  g->nv = nv; g->ne = ne; g->fixed = fixed; g->ij = ij; g->meas = meas; g->info = info; g->delta = huber_delta;
+  g->Hd = (double*)malloc(sizeof(double) * 36 * (nv > 0 ? nv : 1));
+  g->Ho = (double*)malloc(sizeof(double) * 36 * (ne > 0 ? ne : 1));
+  g->b = (double*)malloc(sizeof(double) * 6 * (nv > 0 ? nv : 1));
+  g->Minv = (double*)malloc(sizeof(double) * 36 * (nv > 0 ? nv : 1));
+  g->pcg_residual = -1.0;
+}
+static void pg_free(pg_t* g) { free(g->Hd); free(g->Ho); free(g->b); free(g->Minv); }
+
 /* GraphManager::optimizeGraphImpl stop rule (graph_manager.cpp:998-1014).
  * poses: nv x 7 in/out.  stop >= 1: iteration budget; 0 < stop < 1: relative chi2 convergence in chunks of 5.
  * Returns chi2 (sum e^T Omega e, optimizer_->chi2()). */
 double oracle_posegraph_optimize(int nv, double* poses, const uint8_t* fixed, int ne, const int32_t* ij, const double* meas,
                                  const double* info, double stop, double huber_delta, int* iters_out, int* cg_iters_out) {
   pg_t g;
-  g.nv = nv; g.ne = ne; g.fixed = fixed; g.ij = ij; g.meas = meas; g.info = info; g.delta = huber_delta;
-  g.Hd = (double*)malloc(sizeof(double) * 36 * nv);
-  g.Ho = (double*)malloc(sizeof(double) * 36 * (ne > 0 ? ne : 1));
-  g.b = (double*)malloc(sizeof(double) * 6 * nv);
-  g.Minv = (double*)malloc(sizeof(double) * 36 * nv);
-  g.pcg_residual = -1.0;
+  pg_init(&g, nv, fixed, ne, ij, meas, info, huber_delta);
   int it = 0, cg = 0;
   double chi2 = DBL_MAX, robust;
   if (stop >= 1.0) {
@@ -374,10 +404,46 @@ double oracle_posegraph_optimize(int nv, double* poses, const uint8_t* fixed, in
       pg_errors(&g, poses, &robust, &chi2);
     } while (chi2 / prev < (1.0 - stop));
   }
-  free(g.Hd); free(g.Ho); free(g.b); free(g.Minv);
+  pg_free(&g);
   if (iters_out) *iters_out = it;
   if (cg_iters_out) *cg_iters_out = cg;
   return chi2;
+}
+
+/* One LM iteration exactly as oracle_posegraph_optimize(stop = 1) runs it (ceil(1 / 10) = 1: one pg_optimize(1)), with every
+ * trial traced (pg_t.tr_*): trials[10 x 8], dx[10 x 6 nv], dn[10 x (6 nv + 1)] (layouts at pg_t).  poses: nv x 7 in/out.
+ * Returns the number of trials; *chi2_out = chi2 of the returned poses, *cg_iters_out = PCG iterations of all trials. */
+int oracle_posegraph_lm_trace(int nv, double* poses, const uint8_t* fixed, int ne, const int32_t* ij, const double* meas,
+                              const double* info, double huber_delta, double* trials, double* dx, double* dn, double* chi2_out,
+                              int* cg_iters_out) {
+  pg_t g;
+  pg_init(&g, nv, fixed, ne, ij, meas, info, huber_delta);
+  g.tr_trial = trials; g.tr_dx = dx; g.tr_dn = dn;
+  int cg = 0;
+  double robust;
+  pg_optimize(&g, poses, 1, &cg);
+  pg_errors(&g, poses, &robust, chi2_out);
+  pg_free(&g);
+  *cg_iters_out = cg;
+  return g.tr_n;
+}
+
+/* The damped system one PCG solves at the poses: Hd[nv x 36] = H_vv + lambda I for a free vertex (H_vv for a fixed one),
+ * Ho[ne x 36] = Ji^T W Jj (Huber-weighted) of every edge, b[nv x 6] = -sum J^T W e and babs[nv x 6] = sum |J^T W e| (both 0 for
+ * a fixed vertex).  The PCG's operator is the free rows and columns of that matrix, without the off-diagonal block of a self
+ * edge (pg_spmv). */
+void oracle_posegraph_system(int nv, const double* poses, const uint8_t* fixed, int ne, const int32_t* ij, const double* meas,
+                             const double* info, double huber_delta, double lambda, double* Hd, double* Ho, double* b, double* babs) {
+  pg_t g;
+  memset(&g, 0, sizeof(g));
+  g.nv = nv; g.ne = ne; g.fixed = fixed; g.ij = ij; g.meas = meas; g.info = info; g.delta = huber_delta;
+  g.Hd = Hd; g.Ho = Ho; g.b = b; g.babs = babs;
+  memset(babs, 0, sizeof(double) * 6 * nv);
+  pg_build(&g, poses);
+  for (int i = 0; i < nv; i++) {
+    if (fixed[i]) { memset(b + 6 * i, 0, 6 * sizeof(double)); memset(babs + 6 * i, 0, 6 * sizeof(double)); continue; }
+    for (int k = 0; k < 6; k++) Hd[36 * i + 7 * k] += lambda;
+  }
 }
 
 /* chi2 only (optimizer_->computeActiveErrors(); chi2()) */

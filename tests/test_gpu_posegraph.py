@@ -111,8 +111,9 @@ def _hub_graph(nv, seed):
 
 
 def test_resident_solver_matches_general_kernel_on_hub_graph(fe, monkeypatch):
-    """700 vertices on 148 CTAs = 5 per CTA; the hub's 699 incidences exceed the 568 a CTA stages in shared memory, so the
-    resident kernel takes its global-memory path for the tail -- same solution as the general kernel (RB200_PG_RESIDENT=0)"""
+    """700 vertices on one CTA per SM (132 on an H100 SXM: 6 per CTA); the hub's incidences exceed the 568 a CTA stages in
+    shared memory, so the resident kernel takes its global-memory path for the tail -- same solution as the general kernel
+    (RB200_PG_RESIDENT=0)"""
     g = _hub_graph(700, seed=5)
     monkeypatch.setenv("RB200_PG_RESIDENT", "1")
     x1, c1, it1, cg1 = fe.optimize_graph(g["init"], g["fixed"], g["ij"], g["meas"], g["info"], stop=0.01)
