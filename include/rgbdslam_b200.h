@@ -151,8 +151,8 @@ int rgbdslam_b200_set_stream(void* cuda_stream);
 /* Block until all work queued by the library has finished. */
 int rgbdslam_b200_synchronize(void);
 
-/* Which kernel computes the Hamming brute-force stage: 0 = SIMT popcount kernel (cross-check); 1 (default) = wgmma s8
- * tensor-core GEMM with arg-max epilogue, the 32-byte descriptors expanded to int8 operands inside the kernel.  Both are exact
+/* Which kernel computes the Hamming brute-force stage: 0 = SIMT popcount kernel (cross-check); 1 (default) = wgmma binary
+ * tensor-core GEMM (AND-popcount of the raw 32-byte descriptors) with arg-max epilogue.  Both are exact
  * and give identical results (DESIGN.md 4.1); other values are rejected. */
 int rgbdslam_b200_set_hamming_path(int path);
 
@@ -266,7 +266,7 @@ int rgbdslam_b200_match_pairs_wait(int slot);
 int rgbdslam_b200_last_timing(float* hamming_ms, float* total_device_ms);
 int rgbdslam_b200_last_timing_slot(int slot, float* hamming_ms, float* total_device_ms);
 /* CUDA-event stage times (ms) of the last finished call on a slot: [0] host->device copies, [1] float-descriptor operand
- * preparation (0 for ORB: descriptors are expanded inside the match kernel), [2] Hamming kernel, [3] match selection + RANSAC, [4] device->host copies, [5] whole call on the stream. */
+ * preparation (0 for ORB: the match kernel reads the descriptors themselves), [2] Hamming kernel, [3] match selection + RANSAC, [4] device->host copies, [5] whole call on the stream. */
 int rgbdslam_b200_slot_stage_times(int slot, float* ms6);
 /* Pipeline diagnostics: timeline_epoch() marks t = 0 on the device; slot_timeline() returns, for the last finished
  * call on a slot, the device time (ms since the epoch) of [0] submit, [1] uploads done, [2] operand expansion done,

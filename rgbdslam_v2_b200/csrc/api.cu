@@ -207,8 +207,8 @@ static int stage_match_items(Workspace& w, const PairDesc* h_pairs, int npairs, 
     if ((rc = w.d_knn.ensure(sizeof(float4) * (size_t)npairs * stride))) return rc;
   }
   // work items: 256 queries of one pair against 128-row train tiles (every tensor-core kernel).  The ORB kernel gets the 32-byte
-  // descriptors themselves (expanded to int8 operands inside the kernel); the float-descriptor matchers read the bf16 / u8
-  // operand tiles their nodes keep resident.
+  // descriptors themselves (its binary GEMM's operands); the float-descriptor matchers read the bf16 / u8 operand tiles their
+  // nodes keep resident.
   const bool raw = kind == 0;
   const int mblk = 256, nblk = 128;
   std::vector<HamItem> items;
@@ -281,7 +281,7 @@ static int launch_hamming(Workspace& w, const PairDesc* d_pairs, int npairs, int
       if (e != cudaSuccess) return cuda_fail(e, "zero the match kernel's claim counter");
       w.claim = ClaimCounter{(unsigned long long*)w.d_claim.ptr, 0};
     }
-    e = launch_hamming_tc_expand((const HamItem*)w.d_items.ptr, n_items, s.sm_count, w.claim, w.stream);
+    e = launch_hamming_tc_b1((const HamItem*)w.d_items.ptr, n_items, s.sm_count, w.claim, w.stream);
   } else {
     cudaEventRecord(w.ev[kEvMatchEnd], w.stream);
     return 0;
@@ -788,7 +788,7 @@ int rgbdslam_b200_set_sift_matcher(int matcher) {
 int rgbdslam_b200_set_hamming_path(int path) {
   std::lock_guard<std::mutex> lk(g_state.mu);
   if (path < 0 || path > 1) {
-    set_error("set_hamming_path: 0 = SIMT popcount (cross-check), 1 = wgmma int8 GEMM (default)");
+    set_error("set_hamming_path: 0 = SIMT popcount (cross-check), 1 = wgmma binary AND-popcount GEMM (default)");
     return RGBDSLAM_B200_ERR_ARG;
   }
   g_state.hamming_path = path;

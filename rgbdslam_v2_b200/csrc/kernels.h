@@ -19,10 +19,9 @@ struct ClaimCounter {
   unsigned long long base = 0;
 };
 
-// Hamming brute force on the tensor cores, 32-byte descriptors expanded to int8 operands inside the kernel (HamItem::a / b =
-// descriptor rows); same output as launch_hamming_simt.  Advances claim.base past the tickets the launch takes.
-cudaError_t launch_hamming_tc_expand(const HamItem* d_items, int n_items, int sm_count, ClaimCounter& claim,
-                                     cudaStream_t stream);
+// Hamming brute force on the tensor cores as a binary GEMM (popcount(a & b) of the raw 32-byte descriptor rows, HamItem::a /
+// b = descriptor rows); same output as launch_hamming_simt.  Advances claim.base past the tickets the launch takes.
+cudaError_t launch_hamming_tc_b1(const HamItem* d_items, int n_items, int sm_count, ClaimCounter& claim, cudaStream_t stream);
 cudaError_t launch_l2_tc256(const HamItem* d_items, int n_items, int sm_count, cudaStream_t stream);
 
 // SIFT-128 path (sift_l2.cu / hamming_tc.cu MODE 1)

@@ -146,7 +146,7 @@ struct State {
   Workspace ws[kSlots];
   DevBuf d_f32_a, d_f32_b, d_root_a, d_root_b, d_norm_a, d_norm_b, d_i8_a, d_i8_b;  // SIFT staging of the synchronous calls
   int sift_matcher = 0;  // float-descriptor nodes created from now on: 0 = exact 2-NN ratio matcher (FLANN branch), 1 = SiftGPU matcher
-  int hamming_path = 1;  // 1 = wgmma int8 GEMM, operands expanded inside the kernel (default); 0 = SIMT popcount (cross-check)
+  int hamming_path = 1;  // 1 = wgmma binary GEMM (AND-popcount of the raw descriptors, default); 0 = SIMT popcount (cross-check)
   void release_workspaces() {
     for (Workspace& w : ws) w.release();
     DevBuf* all[] = {&d_f32_a, &d_f32_b, &d_root_a, &d_root_b, &d_norm_a, &d_norm_b, &d_i8_a, &d_i8_b};
